@@ -1,7 +1,7 @@
 """ctypes binding of the C-ABI in include/b200bt.h (libb200bt.so, built in-tree).
 
 There is no fallback: if the shared library is missing, or a compute entry
-point is called without an sm_100 device, this module raises.
+point is called without an sm_90 device, this module raises.
 """
 from __future__ import annotations
 

@@ -13,7 +13,7 @@ __all__ = ["BacktestEngine", "HistoricalDataManager", "ResultAnalyzer", "Strateg
 
 def install_as_backtesting() -> None:
     """Make `import backtesting` (and `backtesting.data_manager`, ... as run_backtest.py:11-12 imports them) resolve to
-    this package, so that the reference's CLI runs unmodified on the B200 path:
+    this package, so that the reference's CLI runs unmodified on the H100 path:
 
         import ai_crypto_trader_b200.backtesting as b; b.install_as_backtesting(); runpy.run_path("run_backtest.py")
     """

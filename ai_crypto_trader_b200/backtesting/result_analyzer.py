@@ -149,11 +149,11 @@ class ResultAnalyzer:
             return None
 
     def plot_equity_curve(self, result: Dict, save_path: Optional[str] = None) -> Optional[str]:
-        logger.error("Error plotting equity curve: matplotlib is not part of the B200 drop-in")
+        logger.error("Error plotting equity curve: matplotlib is not part of the H100 drop-in")
         return None
 
     def plot_trade_analysis(self, result: Dict, save_path: Optional[str] = None) -> Optional[str]:
-        logger.error("Error plotting trade analysis: matplotlib is not part of the B200 drop-in")
+        logger.error("Error plotting trade analysis: matplotlib is not part of the H100 drop-in")
         return None
 
     def save_summary_report(self, summary: Dict, filename: str = "backtest_summary.json") -> Optional[str]:

@@ -15,7 +15,7 @@ void set_error(const char* fmt, ...) {
     va_end(ap);
 }
 
-// The library is compiled for sm_100a only; anything else cannot run its kernels.
+// The library is compiled for sm_90a (H100) only; anything else cannot run its kernels.
 int check_device() {
     int dev = 0;
     cudaError_t e = cudaGetDevice(&dev);
@@ -28,13 +28,23 @@ int check_device() {
     if (ok_dev == dev) return B200BT_OK;
     int major = 0;
     e = cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
-    if (e != cudaSuccess || major != 10) {
-        set_error("device %d is not sm_100 (compute capability major %d); this library has no other code path", dev, major);
+    if (e != cudaSuccess || major != 9) {
+        set_error("device %d is not sm_90 (compute capability major %d); this library has no other code path", dev, major);
         cudaGetLastError();
         return B200BT_ENODEVICE;
     }
     ok_dev = dev;
     return B200BT_OK;
+}
+
+int device_sm_count() {
+    int dev = 0, sms = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
+        sms <= 0) {
+        cudaGetLastError();
+        return 132;
+    }
+    return sms;
 }
 
 }  // namespace b200bt

@@ -1,4 +1,4 @@
-// Shared helpers for the b200bt kernels (sm_100a only).
+// Shared helpers for the b200bt kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -10,6 +10,7 @@ namespace b200bt {
 
 void set_error(const char* fmt, ...);
 int check_device();
+int device_sm_count();     // SMs of the current device (132 on an H100 SXM)
 extern std::atomic<int64_t> g_launches;
 
 inline int cuda_status(cudaError_t e, const char* what) {

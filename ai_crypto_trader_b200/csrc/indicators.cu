@@ -1,4 +1,4 @@
-// Family 1: rolling indicators over fp32 OHLCV (sm_100a).
+// Family 1: rolling indicators over fp32 OHLCV (sm_90a).
 //
 // Data layout: every series is a row of a row-major [S][N] fp32 matrix; a bank
 // is [S][P][N].  One CTA owns one (symbol, time-tile): it stages the close tile

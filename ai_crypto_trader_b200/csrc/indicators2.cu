@@ -1,5 +1,5 @@
 // Family 1 (continued): EMA / MACD / SMA / Bollinger / stochastic / Williams %R /
-// Ichimoku / ATR / VWAP over fp32 OHLCV, plus the TechnicalAnalyzer NaN policy (sm_100a).
+// Ichimoku / ATR / VWAP over fp32 OHLCV, plus the TechnicalAnalyzer NaN policy (sm_90a).
 //
 // Reference call sites: binance_ml_strategy.py:63-182 (TechnicalAnalyzer, via the third-party
 // `ta` package, whose definitions are restated in oracle/indicators_ref.py) and

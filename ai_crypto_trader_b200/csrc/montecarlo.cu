@@ -1,5 +1,5 @@
 // Family 3: Monte-Carlo price paths (GBM / bootstrap) with a Philox4x32-10
-// counter-based RNG, plus the exact order statistics the risk report needs (sm_100a).
+// counter-based RNG, plus the exact order statistics the risk report needs (sm_90a).
 //
 // Reference semantics: MonteCarloService.run_monte_carlo_simulation,
 // services/monte_carlo_service.py:197-394.
@@ -281,7 +281,8 @@ extern "C" int b200bt_select(const float* x, int64_t n, const int64_t* ranks_dev
     unsigned* hist_lo = rem_of + 64;
     cudaError_t e = cudaMemsetAsync(workspace, 0, (size_t)need, st);
     if (e != cudaSuccess) return cuda_status(e, "select: memset");
-    const int blocks = (int)((n + 255) / 256 < 148 * 8 ? (n + 255) / 256 : 148 * 8);
+    const int64_t grid = (int64_t)device_sm_count() * 8;
+    const int blocks = (int)((n + 255) / 256 < grid ? (n + 255) / 256 : grid);
     sel_hist_hi<<<blocks, 256, 0, st>>>(x, n, hist);
     B200BT_LAUNCH_CHECK("select hist_hi");
     sel_find_hi<<<1, 1024, 0, st>>>(hist, ranks_dev, n_ranks, bin_of, rem_of);
@@ -305,7 +306,8 @@ extern "C" int b200bt_mc_moments(const float* finals, const float* maxdd, int64_
     cudaStream_t st = (cudaStream_t)stream;
     cudaError_t e = cudaMemsetAsync(out7, 0, 7 * sizeof(double), st);
     if (e != cudaSuccess) return cuda_status(e, "mc_moments: memset");
-    const int blocks = (int)((n + 255) / 256 < 148 * 4 ? (n + 255) / 256 : 148 * 4);
+    const int64_t grid = (int64_t)device_sm_count() * 4;
+    const int blocks = (int)((n + 255) / 256 < grid ? (n + 255) / 256 : grid);
     mc_moments<<<blocks, 256, 0, st>>>(finals, maxdd, n, s0, var_threshold, out7);
     B200BT_LAUNCH_CHECK("mc_moments");
     return B200BT_OK;

@@ -1,4 +1,4 @@
-// Portfolio risk reductions (sm_100a): simple returns, tail statistics for historical VaR / CVaR,
+// Portfolio risk reductions (sm_90a): simple returns, tail statistics for historical VaR / CVaR,
 // and the pairwise-complete Pearson correlation matrix of the asset return series.
 //
 // Reference: services/portfolio_risk_service.py

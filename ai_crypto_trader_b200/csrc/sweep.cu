@@ -1,6 +1,6 @@
 // Family 2: the per-bar entry/exit/stop/PnL state machine over
 // (GA-individual x symbol) lanes, with calculate_metrics and the strategy score
-// reduced in-kernel (sm_100a).
+// reduced in-kernel (sm_90a).
 //
 // Reference semantics: services/strategy_evaluation.py:746-878 (_simulate_trades),
 // :32-228 (calculate_metrics), :579-633 (_calculate_strategy_score).

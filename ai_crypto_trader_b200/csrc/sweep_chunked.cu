@@ -1,5 +1,5 @@
 // Family 2, time-parallel form: the population sweep with every expensive lane split into
-// TIME CHUNKS that are scanned concurrently (sm_100a).
+// TIME CHUNKS that are scanned concurrently (sm_90a).
 //
 // The trade state machine (strategy_evaluation.py:746-878) is serial in time, and the lanes of a
 // GA population differ by two to three orders of magnitude in trade count, so at moderate
@@ -1254,9 +1254,7 @@ int finish_chunks(const ChunkScanArgs& A, const ChunkWorkspace& w, const b200bt_
     B200BT_REQUIRE(lanes < (1ll << 30), B200BT_ELIMIT, "sweep_chunked: too many lanes");
 
     // Both repair kernels run a persistent grid (3 CTAs per SM) whose warps take work from a counter (n_repair[0], [1]).
-    int dev = 0, sms = 148;
-    if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    const unsigned repair_grid = 3u * (unsigned)sms;
+    const unsigned repair_grid = 3u * (unsigned)device_sm_count();
     auto repair_pass = [&](cudaStream_t rs, int pass, unsigned char* redo) -> int {
         ChunkScanArgs R = A;
         R.redo = redo;

@@ -204,7 +204,7 @@ class DeviceGeneticAlgorithm:
         from . import _lib
         self._torch, self._lib = torch, _lib
         if not torch.cuda.is_available():
-            raise RuntimeError("DeviceGeneticAlgorithm needs a CUDA device (sm_100); use GeneticAlgorithm on the host")
+            raise RuntimeError("DeviceGeneticAlgorithm needs a CUDA device (sm_90); use GeneticAlgorithm on the host")
         self.param_ranges = param_ranges
         self.batch_fitness_function = getattr(batch_fitness_function, "batch", batch_fitness_function)
         self.population_size, self.generations = int(population_size), int(generations)

@@ -8,7 +8,7 @@ return {} -- never raise, :392-394).  Differences, all deliberate (SURVEY.md 5, 
     caches them at :223-227, or `set_returns`); holdings are passed in;
   * the constructor never rewrites config.json (the reference does, :98-101);
   * path generation, per-path drawdown, order statistics and moments run in the
-    sm_100a kernels of csrc/montecarlo.cu (Philox4x32-10 instead of NumPy's MT19937:
+    sm_90a kernels of csrc/montecarlo.cu (Philox4x32-10 instead of NumPy's MT19937:
     same distribution, different stream; `seed` makes runs reproducible);
   * `block_len` > 1 turns the 'historical' method into a block bootstrap (north-star
     extension; 1 reproduces the reference's iid resampling).
@@ -71,7 +71,7 @@ class PathEngine:
 
     def __init__(self, device: Optional[torch.device] = None):
         if not torch.cuda.is_available():
-            raise RuntimeError("Monte-Carlo engine needs a CUDA device (sm_100); there is no CPU path")
+            raise RuntimeError("Monte-Carlo engine needs a CUDA device (sm_90); there is no CPU path")
         self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
         self._ws = None
 

@@ -14,7 +14,7 @@ cross_validate_strategy :682-691; the mean over symbols mirrors its mean over
 folds, :1030-1060.)
 
 PyTorch is used for device memory and streams only; all arithmetic happens in
-the hand-written sm_100a kernels behind the C-ABI.
+the hand-written sm_90a kernels behind the C-ABI.
 """
 from __future__ import annotations
 
@@ -62,7 +62,7 @@ class MarketData:
                  minute0: int = EPOCH_2024_MINUTES, bar_minutes: int = 1,
                  device: Optional[torch.device] = None, pinned_source: bool = False):
         if not torch.cuda.is_available():
-            raise RuntimeError("MarketData needs a CUDA device (sm_100); this engine has no CPU path")
+            raise RuntimeError("MarketData needs a CUDA device (sm_90); this engine has no CPU path")
         self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
         if isinstance(ohlcv, torch.Tensor):
             host = ohlcv

@@ -33,14 +33,7 @@ POP_PER_GPU = 1024
 N_SYMBOLS = 10
 N_BARS = 1_000_000
 BYTES_PER_EVAL = 8  # SURVEY 8(d): price 4 B + RSI 4 B per (individual, symbol, bar), reference RSI rule
-# ncu figures of the dominant kernel per launch on the configs[1] workload (pop 1024 x 10 x 1M, seed-42 population), from
-# the committed `ncu --set full` capture named in "source"; "scan_share" = the kernel's share of the sweep's kernel time in
-# the committed launch list of this bench command.  Valid for exactly that workload (the kernels are deterministic).
-NCU_C2 = {
-    "tiled": {"warp_inst": 3.2099e9, "threads_per_inst": 13.70, "dram_bytes": 4.613e9 + 1.032e9, "scan_share": 0.579,
-              "issue_active_pct": 69.4, "alu_pipe_pct": 54.7,
-              "source": "profiles/r2_lane_scan_ncu.txt (ncu --set full), profiles/r2_launches.csv (launch list of `bench.py --steps 2 --warmup 3 --skip-extras`)"},
-}
+DUMP_BYTES_MAX = 64 << 20   # --dump-outputs: at most this much in all (a fixed, seeded sample of lanes beyond it)
 
 
 def measured_hbm_peak():
@@ -50,7 +43,7 @@ def measured_hbm_peak():
             return float(json.loads(p.read_text())["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3)"
 
 
 _T0 = time.perf_counter()
@@ -112,8 +105,7 @@ class ClockSampler:
 # CPU arms.  `--impl reference` and the inline `cpu_baseline` leg use ONE recipe (same pool, same sample shape, the
 # timer started after the pool is warm), so the two agree:
 #   kind "reference": the reference's own _simulate_trades + calculate_metrics + _calculate_strategy_score, imported
-#                     unmodified from oracle/_ref (placed there by oracle/make_ref.py in the build container; it
-#                     travels to the GPU box with the snapshot, where /root/reference does not exist)
+#                     unmodified from oracle/_ref (placed there by oracle/make_ref.py where the reference tree exists)
 #   kind "port"     : the float64 Python restatement (oracle/simulate_ref.py) when oracle/_ref is not populated
 # plus the same algorithm as compiled C (oracle/sim_oracle.c) under the same pool: the strong CPU baseline.
 # --------------------------------------------------------------------------
@@ -329,6 +321,39 @@ def cpu_baseline_child(timeout_s: float = 420.0, attempts: int = 2):
     return {"value": None, "unit": UNIT, "cores": 0, "kind": "reference", "sample": "", "unavailable": why}
 
 
+# fields the reference lets be infinite (no losing trade, no negative day): each gets a <name>_nonfinite.npy
+MAY_BE_NONFINITE = ("profit_factor", "sortino_ratio", "score", "fitness")
+
+
+def dump_outputs(out_dir, fitness, stats):
+    """fitness [pop] and every lane statistic [pop][S] as float64 .npy (trade hash as two exact 32-bit halves).  A
+    non-finite value is written as 0 plus its kind in <name>_nonfinite.npy (1 +inf, -1 -inf, 2 NaN).  Beyond DUMP_BYTES_MAX
+    a fixed, seeded sample of individuals is kept, listed in lane_sample.npy."""
+    import numpy as np
+    out = Path(out_dir)
+    out.mkdir(parents=True, exist_ok=True)
+    arrays = {name: v.astype(np.float64) for name, v in stats.items() if name != "trade_hash"}
+    h = stats["trade_hash"].astype(np.uint64)
+    arrays["trade_hash_hi"] = (h >> np.uint64(32)).astype(np.float64)
+    arrays["trade_hash_lo"] = (h & np.uint64(0xFFFFFFFF)).astype(np.float64)
+    pop = len(fitness)
+    per_individual = sum(a[0].nbytes for a in arrays.values()) * 2 + 16
+    if 2 * fitness.nbytes + pop * per_individual > DUMP_BYTES_MAX:
+        keep = np.sort(np.random.default_rng(0).choice(pop, (DUMP_BYTES_MAX - 2 * fitness.nbytes) // per_individual, replace=False))
+        arrays = {k: a[keep] for k, a in arrays.items()}
+        arrays["lane_sample"] = keep.astype(np.float64)
+    arrays["fitness"] = np.asarray(fitness, dtype=np.float64)
+    for name, a in list(arrays.items()):
+        finite = np.isfinite(a)
+        if name in MAY_BE_NONFINITE or not finite.all():
+            if name not in MAY_BE_NONFINITE:
+                _phase(f"dump-outputs: {name} holds {int((~finite).sum())} non-finite value(s)")
+            arrays[name + "_nonfinite"] = np.where(np.isnan(a), 2.0, np.where(np.isinf(a), np.sign(a), 0.0))
+            arrays[name] = np.where(finite, a, 0.0)
+    for name, a in arrays.items():
+        np.save(out / f"{name}.npy", np.ascontiguousarray(a))
+
+
 def configs0_frame():
     """10 000 synthetic 1-minute bars ending in a sell-off (the constant technical signal then trades, as in the parity
     fixtures tests/golden/bt_reference.*)."""
@@ -502,6 +527,7 @@ def main():
     ap.add_argument("--cpu-baseline-only", action="store_true", help="(internal) print the cpu_baseline dict and exit")
     ap.add_argument("--reference-child", action="store_true", help="(internal) the worker of --impl reference")
     ap.add_argument("--mode", default="auto", choices=["auto", "fused", "chunked", "tiled"], help="sweep kernel path (auto = product default)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs as DIR/<name>.npy")
     args = ap.parse_args()
     if args.cpu_baseline_only:
         print(json.dumps(cpu_baseline_inline()), flush=True)
@@ -571,11 +597,6 @@ def main():
     path = "fused" if plan is None else ("tiled" if type(plan[0]).__name__ == "TilePlan" else "chunked")
     path_kernels = {"fused": "sweep_kernel", "chunked": "chunk_scan_kernel + chunk_sums/partial/lane_combine",
                     "tiled": "lane_scan_kernel + chunk_sums/partial/lane_combine"}[path]
-    # DRAM bytes (read + write) of the dominant kernel per launch on THIS workload, from the committed
-    # `ncu --set full` captures (profiles/r1_tiled_final_ncu.txt, r1_chunk_scan_ncu.txt, r1_sweep_v2_ncu.txt);
-    # null for any other workload size
-    ncu_traffic = {"tiled": 5.222e9 + 1.006e9, "chunked": 45.6e9, "fused": 3.3e9}[path] \
-        if (pop_local, S, N) == (POP_PER_GPU, N_SYMBOLS, N_BARS) else None
 
     def barrier():
         if world > 1:
@@ -638,6 +659,8 @@ def main():
     evals_per_step_global = pop_global * S * N
     value = evals_per_step_global * args.steps / (ms_total * 1e-3)
     fit_random = fit_local.clone()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, fit_random.cpu().numpy(), sweep.lane_stats())
 
     # ---- parity spot check of the timed population (rank 0): 64 lanes against the C oracle ----
     parity = None
@@ -702,34 +725,18 @@ def main():
         peak, peak_src = measured_hbm_peak()
         lanes_evals = pop_local * S * N
         algorithmic_gbps = lanes_evals * BYTES_PER_EVAL / (ms_kernel * 1e-3) / 1e9
-        # What binds the sweep is instruction issue, not HBM (profiles/: DRAM 10-15 % of peak, issue slots ~60 % busy,
-        # the RSI rows are shared by every lane of a symbol so most of SURVEY 8(d)'s 8 B/eval never leaves L1/L2).
-        # The roofline is therefore stated against the issue rate: warp-instructions of the dominant kernel per launch
-        # (ncu, committed under profiles/, valid for exactly this workload) / its share of the live kernel time, against
-        # 148 SMs x 4 schedulers x the SM clock sampled during the timed region.
-        ncu = NCU_C2.get(path) if (pop_local, S, N) == (POP_PER_GPU, N_SYMBOLS, N_BARS) else None
-        sm_mhz = (clocks or {}).get("sm_mhz") or 1965.0
-        issue_peak = 148 * 4 * sm_mhz * 1e6 / 1e9                     # G warp-instructions / s
+        # issue-bound (DESIGN.md 3.1); "achieved" needs the scan kernel's warp-instruction count from a profiler capture
+        sms = torch.cuda.get_device_properties(dev).multi_processor_count
+        sm_mhz = (clocks or {}).get("sm_mhz")
+        issue_peak = sms * 4 * sm_mhz * 1e6 / 1e9 if sm_mhz else None        # G warp-instructions / s
         roofline = {"bound": "issue", "kernel": path_kernels, "sweep_mode": path, "kernel_ms": ms_kernel,
-                    "peak": issue_peak, "unit": "Ginst/s", "peak_source": f"148 SMs x 4 warp schedulers x {sm_mhz:.0f} MHz (sampled under load)",
+                    "peak": issue_peak, "unit": "Ginst/s",
+                    "peak_source": f"{sms} SMs x 4 warp schedulers x {sm_mhz:.0f} MHz (sampled under load)" if sm_mhz else "SM clock not sampled",
                     "algorithmic_gbps": algorithmic_gbps, "bytes_per_eval": BYTES_PER_EVAL,
-                    "hbm_peak_gbs": peak, "hbm_peak_source": peak_src}
-        if ncu:
-            scan_ms = scan_ms_live if scan_ms_live else ms_kernel * ncu["scan_share"]
-            achieved = ncu["warp_inst"] / (scan_ms * 1e-3) / 1e9
-            roofline.update({
-                "achieved": achieved, "frac": achieved / issue_peak,
-                "warp_inst_per_launch": ncu["warp_inst"], "warp_inst_per_eval": ncu["warp_inst"] / lanes_evals,
-                "threads_per_inst": ncu["threads_per_inst"], "dominant_kernel_ms": scan_ms,
-                "dominant_kernel_share_of_step": scan_ms / ms_kernel, "dominant_kernel_share_in_launch_list": ncu["scan_share"],
-                "issue_active_pct_ncu": ncu["issue_active_pct"], "alu_pipe_pct_ncu": ncu["alu_pipe_pct"],
-                "traffic": ncu["dram_bytes"], "traffic_unit": "DRAM bytes per launch of the dominant kernel (ncu dram__bytes_read.sum + dram__bytes_write.sum)",
-                "dram_frac": ncu["dram_bytes"] / (scan_ms * 1e-3) / 1e9 / peak, "compulsory_bytes": (S * N * 4 + sweep.bank.numel() * 4),
-                "source": ncu["source"],
-                "note": "achieved = warp-instructions of lane_scan_kernel per launch (ncu, this workload) / its mean duration in the timed region (CUDA events recorded by the library around the kernel, on its stream); algorithmic_gbps = SURVEY 8(d)'s 8 B x evals / kernel time, a throughput figure, not a bound"})
-        else:
-            roofline.update({"achieved": None, "frac": None, "traffic": None,
-                             "note": "no committed ncu capture for this workload size: only the algorithmic throughput is reported"})
+                    "hbm_peak_gbs": peak, "hbm_peak_source": peak_src,
+                    "dominant_kernel_ms": scan_ms_live, "compulsory_bytes": (S * N * 4 + sweep.bank.numel() * 4),
+                    "achieved": None, "frac": None, "traffic": None,
+                    "note": "dominant_kernel_ms = lane_scan_kernel's mean duration (CUDA events around it); algorithmic_gbps is a throughput scale, not a bound"}
         line = {
             "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": ms_total / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
@@ -750,9 +757,12 @@ def main():
             if "configs0_backtest" in cpu_baseline and not abandoned:
                 # the same configs[0] backtest through the GPU path (indicators, backtest_ref kernel, stats dict)
                 import asyncio
-                from ai_crypto_trader_b200.backtesting import StrategyTester
+                import tempfile
+                from ai_crypto_trader_b200.backtesting import HistoricalDataManager, StrategyTester
                 df0 = configs0_frame()
-                tester = StrategyTester(config={}, data_manager=None, results_dir=os.path.join(os.path.dirname(os.path.abspath(__file__)), "gpurun_out", "bench_results"), config_path=None)
+                scratch = tempfile.mkdtemp(prefix="b200bt_bench_")        # (the tree may be read-only)
+                tester = StrategyTester(config={}, data_manager=HistoricalDataManager(None, data_dir=os.path.join(scratch, "data")),
+                                        results_dir=os.path.join(scratch, "results"), config_path=None)
                 asyncio.run(tester.backtest_frame(df0, "SYNUSDC"))
                 t0 = time.perf_counter()
                 st0 = asyncio.run(tester.backtest_frame(df0, "SYNUSDC"))

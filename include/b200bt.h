@@ -1,5 +1,5 @@
 /*
- * b200bt.h -- C-ABI of the B200-native backtest / evolution / Monte-Carlo engine.
+ * b200bt.h -- C-ABI of the H100-native backtest / evolution / Monte-Carlo engine.
  *
  * This is the drop-in boundary below the reference's Python call surface
  * (zd87pl/ai-crypto-trader; SURVEY.md section 8b).  The reference has no FFI
@@ -13,7 +13,7 @@
  * throws across the boundary.  `b200bt_last_error()` returns a thread-local,
  * human-readable description of the last failure.
  *
- * There is NO CPU fallback behind this ABI.  If no sm_100 device is present
+ * There is NO CPU fallback behind this ABI.  If no sm_90 device is present
  * the compute entry points return B200BT_ENODEVICE.
  */
 #ifndef B200BT_H_

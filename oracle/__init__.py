@@ -11,8 +11,8 @@ Pinning status (see DESIGN.md "Oracle"):
   * simulate / metrics / advanced metrics / score / cross-validation / GA operators / Monte-Carlo statistics /
     StrategyTester backtest / portfolio VaR, CVaR and correlation are
     pinned by golden fixtures produced by EXECUTING the reference's own code
-    (tests/golden/make_golden.py, run in the build container where
-    /root/reference exists; fixtures committed under tests/golden/).
+    (tests/golden/make_golden.py, run where a copy of the reference tree
+    exists; fixtures committed under tests/golden/).
   * the `ta` indicator arithmetic is restated from the published definitions of
     the third-party `ta` package (unpinned `ta>=0.7.0`, requirements.txt:5; not
     vendored in the reference tree, not installed here): PARITY UNPINNED for

@@ -1,11 +1,12 @@
 """Recipe for oracle/_ref/: the reference's OWN hot-path modules, placed (not committed) next to the oracle so that the
 CPU baseline legs of bench.py can time the real `_simulate_trades` / `calculate_metrics` / `_calculate_strategy_score`
 (services/strategy_evaluation.py:746-878, :32-228, :579-633) and the real `GeneticAlgorithm` operators
-(services/genetic_algorithm.py:135-252) on the GPU box, where /root/reference does not exist.
+(services/genetic_algorithm.py:135-252) on a machine that has no copy of the reference tree.
 
-TEST / MEASUREMENT INFRASTRUCTURE.  oracle/_ref/ is git-ignored (no reference source enters the history) and NOT
-gpurun-ignored, so it travels to the GPU box with the snapshot like the built .so files.  `__graft_entry__.build()` runs
-this in the build container; on the GPU box the placed files are used as they are.  The modules are Python (the reference
+TEST / MEASUREMENT INFRASTRUCTURE.  oracle/_ref/ is git-ignored (no reference source enters the history); it goes with
+the working tree like the built .so files.  `__graft_entry__.build()` places the files where the reference tree is found:
+a checkout named `reference` beside this repository, or the tree B200BT_REFERENCE_ROOT names; elsewhere placed files
+are used as they are.  The modules are Python (the reference
 has no compiled code), so "building" the reference is placing these files unmodified; `load()` imports them with
 matplotlib stubbed (used for plots only) and with the cwd-relative paths the modules open at import time
 (`logs/*.log`, `config.json`; strategy_evaluation.py:23,513) provided in a scratch directory.
@@ -20,13 +21,17 @@ from pathlib import Path
 
 HERE = Path(__file__).resolve().parent
 REF_DIR = HERE / "_ref"
-REFERENCE_ROOT = Path(os.environ.get("B200BT_REFERENCE_ROOT", "/root/reference"))
+REFERENCE_ROOT = Path(os.environ.get("B200BT_REFERENCE_ROOT", HERE.parents[1] / "reference"))
 FILES = ("services/strategy_evaluation.py", "services/genetic_algorithm.py", "config.json")
 
 
 def place(force: bool = False) -> bool:
-    """Copy FILES from the reference tree into oracle/_ref/ (build container).  -> True when oracle/_ref is complete."""
-    if (REFERENCE_ROOT / FILES[0]).exists():
+    """Copy FILES from the reference tree into oracle/_ref/.  -> True when oracle/_ref is complete."""
+    try:
+        found = (REFERENCE_ROOT / FILES[0]).exists()
+    except OSError:             # (a tree this user may not read is no tree)
+        found = False
+    if found:
         for rel in FILES:
             dst = REF_DIR / rel
             if force or not dst.exists() or dst.stat().st_mtime < (REFERENCE_ROOT / rel).stat().st_mtime:
@@ -49,7 +54,7 @@ def load():
     if _loaded is not None:
         return _loaded
     if not available():
-        raise RuntimeError("oracle/_ref is not populated (run oracle/make_ref.py where /root/reference exists)")
+        raise RuntimeError(f"oracle/_ref is not populated (no reference tree at {REFERENCE_ROOT})")
     import tempfile
     for name in ("matplotlib", "matplotlib.pyplot"):
         if name not in sys.modules:

@@ -1,9 +1,9 @@
-"""Run the REFERENCE's own code as the oracle of record (build container only).
+"""Run the REFERENCE's own code as the oracle of record (where a copy of the reference tree exists).
 
-TEST INFRASTRUCTURE.  /root/reference exists only in the build container, so
-this module is imported only by tests/golden/make_golden.py (which writes the
-committed fixtures) and by tests that skip when the reference tree is absent.
-Nothing on the GPU box imports it.
+TEST INFRASTRUCTURE.  The reference tree is a checkout named `reference` beside this
+repository, or the tree B200BT_REFERENCE_ROOT names; this
+module is imported only by tests/golden/make_golden.py, which writes the
+committed fixtures.  No test, smoke() or bench.py imports it.
 
 The reference's numeric code runs UNMODIFIED; only modules it imports for
 plotting / networking (matplotlib, seaborn, redis, binance) are replaced by
@@ -21,7 +21,7 @@ import tempfile
 import types
 from pathlib import Path
 
-REFERENCE_ROOT = Path(os.environ.get("B200BT_REFERENCE_ROOT", "/root/reference"))
+REFERENCE_ROOT = Path(os.environ.get("B200BT_REFERENCE_ROOT", Path(__file__).resolve().parents[2] / "reference"))
 
 
 def available() -> bool:

@@ -12,7 +12,7 @@ GOLDEN = Path(__file__).resolve().parent / "golden"
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run by the driver with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (select with -m gpu)")
 
 
 @pytest.fixture(scope="session")

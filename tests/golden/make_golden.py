@@ -1,6 +1,7 @@
 """Generate the committed golden fixtures by EXECUTING the reference's own code.
 
-Run in the build container (where /root/reference exists):
+Run where a copy of the reference tree exists (a checkout named `reference` beside this repository, or
+B200BT_REFERENCE_ROOT=<reference tree>):
 
     python tests/golden/make_golden.py
 

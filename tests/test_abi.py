@@ -1,4 +1,4 @@
-"""CPU-side checks of the drop-in boundary: the library builds for sm_100a, loads,
+"""CPU-side checks of the drop-in boundary: the library builds for sm_90a, loads,
 exports every symbol include/b200bt.h declares, and refuses to compute without a GPU."""
 import ctypes as C
 import re
@@ -18,6 +18,19 @@ def test_library_exports_every_declared_symbol(native_lib):
     for name in declared:
         assert hasattr(native_lib, name), name
     assert native_lib.b200bt_abi_version() == 1
+
+
+def test_library_holds_sm90a_code_only(native_lib):
+    import shutil
+    import subprocess
+    import __graft_entry__
+    nvcc = shutil.which(__graft_entry__._nvcc())          # cuobjdump sits beside the nvcc the build uses
+    tool = Path(nvcc).with_name("cuobjdump") if nvcc else None
+    if tool is None or not tool.exists():
+        pytest.skip("cuobjdump not available")
+    from ai_crypto_trader_b200 import _lib
+    out = subprocess.run([tool, "--list-elf", str(_lib.LIB_PATH)], capture_output=True, text=True, check=True).stdout
+    assert set(re.findall(r"\.(sm_\w+)\.cubin", out)) == {"sm_90a"}, out
 
 
 def test_struct_layouts_match_header(native_lib):

@@ -10,7 +10,7 @@ import torch
 from ai_crypto_trader_b200 import synth
 from ai_crypto_trader_b200.indicators import TechnicalAnalyzer
 from ai_crypto_trader_b200.sweep import MarketData
-peak = json.load(open(ROOT / "MEASURED_PEAKS.json"))["hbm_gbs"] if (ROOT / "MEASURED_PEAKS.json").exists() else 6583.5
+peak = json.load(open(ROOT / "MEASURED_PEAKS.json"))["hbm_gbs"] if (ROOT / "MEASURED_PEAKS.json").exists() else 3350.0     # H100 SXM data sheet
 for S in [int(x) for x in sys.argv[1:]] or [10, 50]:
     m = MarketData(synth.synth_ohlcv(S, 1_000_000)).materialise()
     torch.cuda.synchronize()

@@ -14,7 +14,7 @@ for src in sorted(ge.CSRC.glob("*.cu")):
     obj = bd / (src.stem + ".o"); objs.append(obj)
     procs.append(subprocess.Popen([ge._nvcc(), *ge.NVCC_FLAGS, *flags, "-c", str(src), "-o", str(obj)]))
 assert all(p.wait() == 0 for p in procs)
-subprocess.check_call([ge._nvcc(), "-shared", "-gencode", "arch=compute_100a,code=sm_100a", *map(str, objs), "-o", str(out / (name + ".so"))])
+subprocess.check_call([ge._nvcc(), "-shared", *ge.ARCH, *map(str, objs), "-o", str(out / (name + ".so"))])
 for o in objs: o.unlink()
 bd.rmdir()
 print(out / (name + ".so"))

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """BASELINE configs[3]: the strategy-evolution loop -- 100 generations, population 4096, 20 symbols x 1M 1-minute bars,
-RSI indicators on the 1m / 5m / 15m timeframes, on 1..8 B200 (torchrun: individuals sharded by rank, one all-gather per
+RSI indicators on the 1m / 5m / 15m timeframes, on 1..8 H100 (torchrun: individuals sharded by rank, one all-gather per
 generation, GA operators on the device).
 
     python tools/evolution_c4.py [--generations 100] [--population 4096] [--symbols 20] [--bars 1000000]

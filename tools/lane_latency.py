@@ -27,5 +27,6 @@ for name, p in (("heavy", heavy), ("mid", mid), ("light", light)):
     ms = t([p]); n = sw.lane_stats()["n_records"][0, 0]
     print(f"{name:6s} single lane {ms:7.2f} ms  records {int(n):7d}  {ms * 1e6 / max(n, 1):7.1f} ns/event")
 print("8 heavy lanes (1 CTA)      %.2f ms" % t([heavy] * 8))
-print("148*16 heavy lanes (1 wave) %.2f ms" % t([heavy] * (148 * 16)))
-print("148*16 light lanes (1 wave) %.2f ms" % t([light] * (148 * 16)))
+sms = torch.cuda.get_device_properties(0).multi_processor_count
+print("%d*16 heavy lanes (1 wave) %.2f ms" % (sms, t([heavy] * (sms * 16))))
+print("%d*16 light lanes (1 wave) %.2f ms" % (sms, t([light] * (sms * 16))))

@@ -4,7 +4,7 @@
     python tools/sass_digest.py lane_scan_kernel [lib.so] > profiles/r2_lane_scan_sass.txt
 
 Prints, per instantiation of the kernel: total SASS instructions, the count per mnemonic class, and the presence of the
-data-movement mnemonics the Blackwell guides name (LDGSTS = cp.async, UBLKCP / UTMALDG = TMA bulk copies, SYNCS = mbarrier).
+data-movement mnemonics Hopper's SASS uses (LDGSTS = cp.async, UBLKCP / UTMALDG = TMA bulk copies, SYNCS = mbarrier).
 """
 import collections
 import re
@@ -29,7 +29,7 @@ for line in txt.splitlines():
         m = re.match(r"\s*/\*[0-9a-f]+\*/\s+(?:@!?U?P\d+\s+)?([A-Z0-9_.]+)", line)
         if m:
             counts[fn][m.group(1).split(".")[0]] += 1
-print(f"# SASS digest of `{kernel}` in {Path(lib).name} (cuobjdump -sass, sm_100a)")
+print(f"# SASS digest of `{kernel}` in {Path(lib).name} (cuobjdump -sass, sm_90a)")
 for fn in order:
     c = counts[fn]
     tot = sum(c.values())
