@@ -140,6 +140,11 @@ _SIGNATURES = {
     "b200bt_select_workspace_bytes": (C.c_int64, [_i]),
     "b200bt_select": (C.c_int, [_vp, _i64, _vp, _i, _vp, _vp, _i64, _vp]),
     "b200bt_mc_moments": (C.c_int, [_vp, _vp, _i64, C.c_double, C.c_double, _vp, _vp]),
+    "b200bt_mc_portfolio_gbm": (C.c_int, [_i, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double),
+                                          C.POINTER(C.c_double), C.POINTER(C.c_float), _i64, _i, C.c_uint64, C.c_uint64,
+                                          _vp, _vp, _vp, _vp]),
+    "b200bt_mc_portfolio_bootstrap": (C.c_int, [_i, _vp, _i, _i, _i, C.POINTER(C.c_double), C.POINTER(C.c_double), _i64,
+                                                _i, C.c_uint64, C.c_uint64, _vp, _vp, _vp, _vp]),
     "b200bt_ga_init": (C.c_int, [_vp, _i, _i, _i, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_int),
                                  C.c_uint64, _vp]),
     "b200bt_ga_next_generation": (C.c_int, [_vp, _vp, _vp, _i, _i, C.POINTER(C.c_double), C.POINTER(C.c_double),

@@ -16,6 +16,7 @@
 // Randomness is a pure function of (seed, path index, step): results do not
 // depend on the launch geometry or on how paths are sharded across GPUs.
 #include <math.h>
+#include <string.h>
 #include "common.cuh"
 #include "philox.cuh"
 
@@ -110,6 +111,147 @@ mc_paths_kernel(double s0, double drift, double vol, const float* __restrict__ r
     const double logS = base;
     finals[p] = (float)(s0 * exp(logS));
     maxdd[p] = (float)(1.0 - exp(worst));
+}
+
+// ---- joint paths of S <= 32 assets (portfolio value V_t = sum_i q_i s0_i exp(logS_i,t)) ----------
+// One thread per path.  Each asset's log-price is kept as in mc_paths_kernel (fp32 within a Philox block of four steps,
+// relative to an fp64 base), so asset i of a joint run computes exactly what the single-asset kernel computes from the
+// same increments.  Counter = (path lo, hi, step/4, (factor << 8) | MODE): GBM factor 0 is mc_paths_kernel<0>'s stream,
+// the bootstrap's one day-index stream is mc_paths_kernel<1>'s.
+// Per-asset constants live in the parameter space (constant bank) and are indexed with compile-time offsets after
+// unrolling, so every FMA of the mat-vec reads its Cholesky entry as an operand.  The fp64 bases live in shared memory
+// (thread-private columns, touched once per block of four steps), which leaves the registers to z, l and A.
+constexpr int JOINT_THREADS = 128;
+constexpr int JOINT_MAX_ASSETS = 32;
+constexpr int JOINT_MAX_TABLE = 12288;   // R * S floats of the bootstrap table (48 KB, the single-asset table's limit)
+
+template <int SMAX>
+struct JointParams {
+    float L[SMAX * (SMAX + 1) / 2];   // Cholesky factor of the correlation, lower triangle packed by rows (GBM)
+    float drift[SMAX], vol[SMAX];     // per-step drift / volatility, rounded to fp32 as mc_paths_kernel rounds them
+    float w[SMAX];                    // q_i s0_i / V_0: the portfolio value is tracked relative to V_0
+    double a[SMAX];                   // q_i s0_i
+    double s0[SMAX];
+    int S;
+};
+
+// V_t / V_0 = sum_i A_i exp(l_i), A_i = w_i exp(base_i); four partial sums shorten the dependent chain
+template <int SMAX>
+__device__ __forceinline__ float joint_value(const float (&A)[SMAX], const float (&l)[SMAX], int S) {
+    float acc[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+    for (int i = 0; i < SMAX; ++i)
+        if (i < S) acc[i & 3] = fmaf(A[i], __expf(l[i]), acc[i & 3]);
+    return (acc[0] + acc[1]) + (acc[2] + acc[3]);
+}
+
+// (min. 1 block per SM: without it ptxas caps the 16-asset instances a few registers short and spills)
+template <int MODE, int SMAX>
+__global__ void __launch_bounds__(JOINT_THREADS, 1)
+mc_joint_kernel(const __grid_constant__ JointParams<SMAX> P, const float* __restrict__ returns, int R, int block_len,
+                int log_returns, int64_t n_paths, int steps, uint64_t seed, uint64_t path_offset,
+                float* __restrict__ finals, float* __restrict__ maxdd, float* __restrict__ asset_finals) {
+    extern __shared__ double s_joint[];
+    double* s_base = s_joint;                                            // [SMAX][JOINT_THREADS]
+    float* s_ret = reinterpret_cast<float*>(s_joint + SMAX * JOINT_THREADS);   // [R][S] bootstrap table
+    const int S = P.S;
+    if (MODE == 1) {
+        for (int i = threadIdx.x; i < R * S; i += blockDim.x) {
+            const float r = returns[i];
+            s_ret[i] = log_returns ? r : log1pf(r);
+        }
+        __syncthreads();
+    }
+    const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= n_paths) return;
+    const uint64_t gid = path_offset + (uint64_t)p;
+    const uint32_t k0 = (uint32_t)seed, k1 = (uint32_t)(seed >> 32);
+    const uint32_t c0 = (uint32_t)gid, c1 = (uint32_t)(gid >> 32);
+
+    float l[SMAX], A[SMAX];
+#pragma unroll
+    for (int i = 0; i < SMAX; ++i) {
+        l[i] = 0.f;
+        A[i] = P.w[i];
+        if (i < S) s_base[i * JOINT_THREADS + threadIdx.x] = 0.0;
+    }
+    float runmax = joint_value<SMAX>(A, l, S), dd = 0.f;
+    int boot_idx = 0, boot_left = 0;
+    for (int t0 = 0; t0 < steps; t0 += 4) {
+        float z[SMAX][4];   // GBM: four normals per factor, then (L z) in place
+        int day[4];         // bootstrap: one day (row of the table) per step
+        if (MODE == 0) {
+#pragma unroll
+            for (int k = 0; k < SMAX; ++k) {
+                if (k < S) {
+                    uint32_t x[4];
+                    philox4x32_10(c0, c1, (uint32_t)(t0 >> 2), ((uint32_t)k << 8) | (uint32_t)MODE, k0, k1, x);
+                    box_muller(x[0], x[1], z[k][0], z[k][1]);
+                    box_muller(x[2], x[3], z[k][2], z[k][3]);
+                }
+            }
+            // bottom row first: row i reads z_0..z_i, which rows above it have not overwritten yet
+#pragma unroll
+            for (int i = SMAX - 1; i >= 0; --i) {
+                if (i < S) {
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) {
+                        float y = P.L[i * (i + 1) / 2] * z[0][j];
+#pragma unroll
+                        for (int k = 1; k <= i; ++k) y = fmaf(P.L[i * (i + 1) / 2 + k], z[k][j], y);
+                        z[i][j] = y;
+                    }
+                }
+            }
+        } else {
+            uint32_t x[4];
+            philox4x32_10(c0, c1, (uint32_t)(t0 >> 2), (uint32_t)MODE, k0, k1, x);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                if (boot_left == 0) {
+                    boot_idx = (int)__umulhi(x[j], (uint32_t)R);
+                    boot_left = block_len;
+                } else {
+                    boot_idx = boot_idx + 1 == R ? 0 : boot_idx + 1;
+                }
+                --boot_left;
+                day[j] = boot_idx * S;
+            }
+        }
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            if (t0 + j < steps) {
+#pragma unroll
+                for (int i = 0; i < SMAX; ++i)
+                    if (i < S) l[i] += MODE == 0 ? fmaf(P.vol[i], z[i][j], P.drift[i]) : s_ret[day[j] + i];
+                const float v = joint_value<SMAX>(A, l, S);
+                runmax = fmaxf(runmax, v);
+                dd = fmaxf(dd, 1.0f - __fdividef(v, runmax));   // (runmax_t - V_t) / runmax_t
+            }
+        }
+#pragma unroll
+        for (int i = 0; i < SMAX; ++i) {
+            if (i < S) {
+                double& b = s_base[i * JOINT_THREADS + threadIdx.x];
+                const double nb = b + (double)l[i];
+                b = nb;
+                const float hi = (float)nb;   // exp(nb) = exp(hi) (1 + (nb - hi)) to fp32 accuracy
+                A[i] = P.w[i] * expf(hi) * (1.0f + (float)(nb - (double)hi));
+                l[i] = 0.f;
+            }
+        }
+    }
+    double v = 0.0;
+#pragma unroll
+    for (int i = 0; i < SMAX; ++i) {
+        if (i < S) {
+            const double e = exp(s_base[i * JOINT_THREADS + threadIdx.x]);
+            v += P.a[i] * e;
+            if (asset_finals) asset_finals[(int64_t)i * n_paths + p] = (float)(P.s0[i] * e);
+        }
+    }
+    finals[p] = (float)v;
+    maxdd[p] = dd;
 }
 
 // ---- exact order statistics: two-level radix select over fp32 keys ----------
@@ -311,4 +453,100 @@ extern "C" int b200bt_mc_moments(const float* finals, const float* maxdd, int64_
     mc_moments<<<blocks, 256, 0, st>>>(finals, maxdd, n, s0, var_threshold, out7);
     B200BT_LAUNCH_CHECK("mc_moments");
     return B200BT_OK;
+}
+
+// ---- joint (portfolio) paths -----------------------------------------------------------------------
+template <int SMAX>
+static int joint_launch_bucket(int mode, int S, const double* s0, const double* qty, const double* drift,
+                               const double* vol, const float* chol, const float* returns, int R, int block_len,
+                               int log_returns, int64_t n_paths, int steps, uint64_t seed, uint64_t path_offset,
+                               float* finals, float* maxdd, float* asset_finals, cudaStream_t st) {
+    JointParams<SMAX> P;
+    memset(&P, 0, sizeof(P));
+    P.S = S;
+    double v0 = 0.0;
+    for (int i = 0; i < S; ++i) v0 += qty[i] * s0[i];
+    for (int i = 0; i < S; ++i) {
+        P.a[i] = qty[i] * s0[i];
+        P.s0[i] = s0[i];
+        P.w[i] = (float)(P.a[i] / v0);
+        if (mode == 0) {
+            P.drift[i] = (float)drift[i];
+            P.vol[i] = (float)vol[i];
+            for (int k = 0; k <= i; ++k) P.L[i * (i + 1) / 2 + k] = chol[i * S + k];
+        }
+    }
+    const unsigned blocks = (unsigned)((n_paths + JOINT_THREADS - 1) / JOINT_THREADS);
+    size_t smem = (size_t)SMAX * JOINT_THREADS * sizeof(double);
+    if (mode == 0) {
+        mc_joint_kernel<0, SMAX><<<blocks, JOINT_THREADS, smem, st>>>(P, nullptr, 0, 1, 1, n_paths, steps, seed,
+                                                                       path_offset, finals, maxdd, asset_finals);
+    } else {
+        smem += (size_t)R * S * sizeof(float);
+        cudaError_t e = cudaFuncSetAttribute(mc_joint_kernel<1, SMAX>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return cuda_status(e, "mc_portfolio_bootstrap: shared memory attribute");
+        mc_joint_kernel<1, SMAX><<<blocks, JOINT_THREADS, smem, st>>>(P, returns, R, block_len, log_returns, n_paths,
+                                                                       steps, seed, path_offset, finals, maxdd,
+                                                                       asset_finals);
+    }
+    B200BT_LAUNCH_CHECK(mode == 0 ? "mc_portfolio_gbm" : "mc_portfolio_bootstrap");
+    return B200BT_OK;
+}
+
+// Checks shared by both entry points, then dispatch on the smallest bucket that holds S assets.
+static int joint_launch(int mode, int S, const double* s0, const double* qty, const double* drift, const double* vol,
+                        const float* chol, const float* returns, int R, int block_len, int log_returns, int64_t n_paths,
+                        int steps, uint64_t seed, uint64_t path_offset, float* finals, float* maxdd, float* asset_finals,
+                        b200bt_stream_t stream) {
+    B200BT_REQUIRE(S >= 1, B200BT_EINVAL, "mc_portfolio: need at least one asset (S = %d)", S);
+    B200BT_REQUIRE(S <= JOINT_MAX_ASSETS, B200BT_ELIMIT, "mc_portfolio: at most %d assets (S = %d)", JOINT_MAX_ASSETS, S);
+    B200BT_REQUIRE(s0 && qty && finals && maxdd, B200BT_EINVAL, "mc_portfolio: null pointer");
+    B200BT_REQUIRE(n_paths > 0 && steps >= 0, B200BT_EINVAL, "mc_portfolio: bad sizes");
+    double v0 = 0.0;
+    for (int i = 0; i < S; ++i) {
+        B200BT_REQUIRE(s0[i] > 0.0 && isfinite(s0[i]), B200BT_EINVAL, "mc_portfolio: initial price %d must be positive", i);
+        B200BT_REQUIRE(qty[i] >= 0.0 && isfinite(qty[i]), B200BT_EINVAL, "mc_portfolio: quantity %d must be >= 0", i);
+        v0 += qty[i] * s0[i];
+    }
+    B200BT_REQUIRE(v0 > 0.0 && isfinite(v0), B200BT_EINVAL, "mc_portfolio: initial portfolio value must be positive");
+    if (mode == 0) {
+        B200BT_REQUIRE(drift && vol && chol, B200BT_EINVAL, "mc_portfolio_gbm: null pointer");
+        for (int i = 0; i < S; ++i) {
+            B200BT_REQUIRE(isfinite(drift[i]) && isfinite(vol[i]), B200BT_EINVAL, "mc_portfolio_gbm: drift / vol %d", i);
+            for (int k = 0; k <= i; ++k)
+                B200BT_REQUIRE(isfinite(chol[i * S + k]), B200BT_EINVAL, "mc_portfolio_gbm: Cholesky entry (%d, %d)", i, k);
+        }
+    } else {
+        B200BT_REQUIRE(returns && R > 0 && block_len > 0, B200BT_EINVAL, "mc_portfolio_bootstrap: bad return table");
+        B200BT_REQUIRE((int64_t)R * S <= JOINT_MAX_TABLE, B200BT_ELIMIT,
+                       "mc_portfolio_bootstrap: at most %d table entries (R x S = %lld)", JOINT_MAX_TABLE,
+                       (long long)R * S);
+    }
+    int rc = check_device();
+    if (rc) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+#define B200BT_JOINT_BUCKET(N)                                                                                          \
+    joint_launch_bucket<N>(mode, S, s0, qty, drift, vol, chol, returns, R, block_len, log_returns, n_paths, steps, seed, \
+                           path_offset, finals, maxdd, asset_finals, st)
+    if (S <= 4) return B200BT_JOINT_BUCKET(4);
+    if (S <= 8) return B200BT_JOINT_BUCKET(8);
+    if (S <= 16) return B200BT_JOINT_BUCKET(16);
+    return B200BT_JOINT_BUCKET(32);
+#undef B200BT_JOINT_BUCKET
+}
+
+extern "C" int b200bt_mc_portfolio_gbm(int S, const double* s0_host, const double* qty_host, const double* drift_host,
+                                       const double* vol_host, const float* chol_host, int64_t n_paths, int steps,
+                                       uint64_t seed, uint64_t path_offset, float* finals, float* maxdd,
+                                       float* asset_finals_or_null, b200bt_stream_t stream) {
+    return joint_launch(0, S, s0_host, qty_host, drift_host, vol_host, chol_host, nullptr, 0, 1, 1, n_paths, steps, seed,
+                        path_offset, finals, maxdd, asset_finals_or_null, stream);
+}
+
+extern "C" int b200bt_mc_portfolio_bootstrap(int S, const float* returns, int R, int block_len, int log_returns,
+                                             const double* s0_host, const double* qty_host, int64_t n_paths, int steps,
+                                             uint64_t seed, uint64_t path_offset, float* finals, float* maxdd,
+                                             float* asset_finals_or_null, b200bt_stream_t stream) {
+    return joint_launch(1, S, s0_host, qty_host, nullptr, nullptr, nullptr, returns, R, block_len, log_returns, n_paths,
+                        steps, seed, path_offset, finals, maxdd, asset_finals_or_null, stream);
 }

@@ -129,3 +129,19 @@ def gather_paths(local_finals: torch.Tensor, local_maxdd: torch.Tensor, n_total:
     finals = torch.cat([recv[r, 0, :counts[r]] for r in range(world)])
     maxdd = torch.cat([recv[r, 1, :counts[r]] for r in range(world)])
     return finals, maxdd
+
+
+def gather_path_rows(local_rows: torch.Tensor, n_total: int, group=None) -> torch.Tensor:
+    """gather_paths for a [K][n_local] block of per-path rows (the per-asset finals of a joint run): one collective,
+    and the gathered [K][n_total] equals a single-GPU run bit for bit."""
+    if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size(group) == 1:
+        return local_rows
+    world = dist.get_world_size(group)
+    per = -(-n_total // world)
+    K = local_rows.shape[0]
+    send = torch.full((K, per), float("nan"), dtype=local_rows.dtype, device=local_rows.device)
+    send[:, :local_rows.shape[1]] = local_rows
+    recv = torch.empty((world, K, per), dtype=local_rows.dtype, device=local_rows.device)
+    dist.all_gather_into_tensor(recv.view(-1), send.view(-1), group=group)
+    counts = [shard_bounds(n_total, world, r)[1] - shard_bounds(n_total, world, r)[0] for r in range(world)]
+    return torch.cat([recv[r, :, :counts[r]] for r in range(world)], dim=1)

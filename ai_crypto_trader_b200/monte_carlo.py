@@ -66,6 +66,67 @@ def _virtual_index(n: int, q_percent: float):
     return lo, hi, float(h - math.floor(h))
 
 
+def _f64(x) -> np.ndarray:
+    return np.atleast_1d(np.asarray(x, dtype=np.float64))
+
+
+def _c_doubles(x: np.ndarray):
+    return (C.c_double * len(x))(*x.tolist())
+
+
+def joint_factor(corr: np.ndarray):
+    """(correlation used, its float64 Cholesky factor, fallback taken) for a joint simulation.
+
+    A matrix with a NaN entry (an asset without variance or without a common observation) or an eigenvalue <= 0 is
+    replaced by the identity -- the policy of portfolio_risk_service.py:377-381 -- and the fallback is reported.  The
+    diagonal is set to exactly 1, so that L_00 = 1 and asset 0 follows the single-asset generator's path."""
+    c = np.array(corr, dtype=np.float64)
+    S = c.shape[0]
+    fallback = not np.all(np.isfinite(c))
+    if not fallback:
+        c = 0.5 * (c + c.T)
+        np.fill_diagonal(c, 1.0)
+        fallback = not np.all(np.linalg.eigvalsh(c) > 0)
+    if not fallback:
+        try:
+            return c, np.linalg.cholesky(c), False
+        except np.linalg.LinAlgError:
+            fallback = True
+    logger.warning("Correlation matrix is not positive definite, using identity matrix")
+    return np.eye(S), np.eye(S), True
+
+
+def joint_assets(holdings: Dict, historical_data: Dict):
+    """The holdings a joint simulation can use: non-USDC assets with a current price and a return sample
+    (historical_data[f"{asset}USDC"]), in holdings order.  -> [(asset, current_price, quantity, value_usdc, returns)]
+    with quantity = value_usdc / current_price; the others are skipped with a warning (as :520-527 does)."""
+    out = []
+    for asset, h in holdings["assets"].items():
+        if asset == "USDC":
+            continue
+        price = h.get("current_price", 0)
+        if price == 0:
+            logger.warning("No current price available for %s, skipping simulation", asset)
+            continue
+        df = historical_data.get(f"{asset}USDC")
+        returns = df["returns"].dropna() if df is not None and not df.empty else None
+        if returns is None or len(returns) < 2:
+            logger.warning("No historical data available for %sUSDC, skipping simulation", asset)
+            continue
+        value = h.get("value_usdc", 0)
+        out.append((asset, float(price), value / price, float(value), returns))
+    return out
+
+
+def _var_pct(engine: "PathEngine", finals: torch.Tensor, initial: float, confidence: float) -> float:
+    """risk_statistics' VaR (:316-317) alone: the (1 - confidence) percentile of the percentage change."""
+    lo, hi, g = _virtual_index(int(finals.numel()), 100 * (1 - confidence))
+    ranks = sorted({lo, hi})
+    vals = dict(zip(ranks, engine.select(finals, ranks)))
+    pct = lambda v: (v / initial - 1) * 100
+    return _lerp(pct(vals[lo]), pct(vals[hi]), g)
+
+
 class PathEngine:
     """Device-side Monte-Carlo primitives (one instance per GPU)."""
 
@@ -104,6 +165,50 @@ class PathEngine:
                       float(s0), int(n_paths), int(steps), int(seed) & (2**64 - 1), int(path_offset),
                       finals.data_ptr(), maxdd.data_ptr(), _lib.ptr(paths), _lib.current_stream())
         return finals, maxdd, paths
+
+    def _joint_outputs(self, S, n_paths, asset_finals):
+        dev = self.device
+        finals = torch.empty(n_paths, dtype=torch.float32, device=dev)
+        maxdd = torch.empty(n_paths, dtype=torch.float32, device=dev)
+        af = torch.empty((S, n_paths), dtype=torch.float32, device=dev) if asset_finals else None
+        return finals, maxdd, af
+
+    def portfolio_gbm(self, s0, qty, mu, sigma, dt, chol, n_paths, steps, seed, path_offset=0, asset_finals=False):
+        """Joint GBM of S assets: per-asset s0 / qty / mu / sigma (length S), `chol` the [S][S] lower Cholesky factor
+        of their correlation.  -> (portfolio finals V_T [n], portfolio max drawdown [n], asset finals [S][n] or None)."""
+        s0, qty = _f64(s0), _f64(qty)
+        mu, sigma = _f64(mu), _f64(sigma)
+        S = len(s0)
+        drift = (mu - 0.5 * sigma * sigma) * dt     # as b200bt_mc_gbm derives them (:273)
+        vol = sigma * np.sqrt(dt)
+        L = np.ascontiguousarray(chol, dtype=np.float32).reshape(S, S)
+        finals, maxdd, af = self._joint_outputs(S, n_paths, asset_finals)
+        if n_paths == 0:          # a rank without paths (more ranks than paths), as in gbm()
+            return finals, maxdd, af
+        with torch.cuda.device(self.device):
+            _lib.call("b200bt_mc_portfolio_gbm", S, _c_doubles(s0), _c_doubles(qty), _c_doubles(drift), _c_doubles(vol),
+                      (C.c_float * L.size)(*L.ravel().tolist()), int(n_paths), int(steps), int(seed) & (2**64 - 1),
+                      int(path_offset), finals.data_ptr(), maxdd.data_ptr(), _lib.ptr(af), _lib.current_stream())
+        return finals, maxdd, af
+
+    def portfolio_bootstrap(self, returns: np.ndarray, log_returns: bool, s0, qty, n_paths, steps, seed, path_offset=0,
+                            block_len=1, asset_finals=False):
+        """Joint bootstrap of whole days: `returns` [R][S], one row per day with a return for every asset."""
+        s0, qty = _f64(s0), _f64(qty)
+        S = len(s0)
+        table = np.ascontiguousarray(returns, dtype=np.float32)
+        if table.ndim != 2 or table.shape[1] != S:
+            raise ValueError(f"return table of shape {table.shape} for {S} assets")
+        finals, maxdd, af = self._joint_outputs(S, n_paths, asset_finals)
+        if n_paths == 0:
+            return finals, maxdd, af
+        r = torch.from_numpy(table).to(self.device)
+        with torch.cuda.device(self.device):
+            _lib.call("b200bt_mc_portfolio_bootstrap", S, r.data_ptr(), int(table.shape[0]), int(block_len),
+                      1 if log_returns else 0, _c_doubles(s0), _c_doubles(qty), int(n_paths), int(steps),
+                      int(seed) & (2**64 - 1), int(path_offset), finals.data_ptr(), maxdd.data_ptr(), _lib.ptr(af),
+                      _lib.current_stream())
+        return finals, maxdd, af
 
     def select(self, x: torch.Tensor, ranks) -> np.ndarray:
         """Exact order statistics x_(k) for ascending 0-based ranks (float32 values as float64)."""
@@ -292,6 +397,130 @@ class MonteCarloService:
                     "asset_simulations": portfolio_simulations, "portfolio_stats": stats}
         except Exception as e:
             logger.error("Error running portfolio Monte Carlo simulations: %s", e, exc_info=True)
+            return {}
+
+    def run_joint_portfolio_monte_carlo(self, holdings: Optional[Dict] = None, scenarios=None, days: int = None,
+                                        num_simulations: int = None) -> Dict:
+        """Simulate the holdings JOINTLY and read the risk off the distribution of the portfolio value.
+
+        run_portfolio_monte_carlo simulates each asset on its own and _calculate_portfolio_stats adds up the weighted
+        per-asset VaR / CVaR (:630-631 "ignores correlations"): the comonotone worst case, without diversification and
+        without a portfolio drawdown.  Here the assets move together -- GBM with the assets' correlation (device
+        b200bt_correlation on the return series aligned on their index, Cholesky factor on the host) or a bootstrap of
+        whole days -- and the statistics of run_monte_carlo_simulation are taken on V_t = sum_i q_i P_i,t.
+        Per scenario, `undiversified_var` is the weighted sum of the per-asset VaRs of the same run (what
+        _calculate_portfolio_stats reports) and `diversification_benefit` is that minus the joint VaR.  `portfolio_stats`
+        has the keys of _calculate_portfolio_stats, from the joint distribution.  Never raises: logs and returns {}."""
+        try:
+            if not holdings or not holdings.get("assets"):
+                logger.debug("No holdings to analyze")
+                return {}
+            if days is None:
+                days = self.mc_params["time_horizon_days"]
+            if num_simulations is None:
+                num_simulations = self.mc_params["num_simulations"]
+            if scenarios is None:
+                scenarios = list(self.mc_params["scenarios"].keys())
+            used = joint_assets(holdings, self.historical_data)
+            if not used:
+                logger.warning("No assets with a price and historical data to simulate")
+                return {}
+            import pandas as pd
+            from .dist import gather_path_rows, gather_paths, shard_bounds
+            from .portfolio_risk import PortfolioRiskService, ReturnBank
+            assets = [u[0] for u in used]
+            s0 = np.array([u[1] for u in used])
+            qty = np.array([u[2] for u in used])
+            values = np.array([u[3] for u in used])
+            v0 = sum(q * p for q, p in zip(qty.tolist(), s0.tolist()))    # V_0 as the kernel sums it
+            if not values.sum() > 0:
+                logger.warning("No non-USDC assets with value in portfolio")
+                return {}
+            weights = values / values.sum()
+            frame = pd.DataFrame({u[0]: u[4] for u in used})             # aligned on the index (portfolio_risk_service.py:307)
+            eng = self.engine
+            x = torch.from_numpy(np.ascontiguousarray(frame.to_numpy(dtype=np.float64).T, dtype=np.float32)).to(eng.device)
+            corr = PortfolioRiskService(ReturnBank(assets, x), device=eng.device).correlation_matrix()
+            corr, chol, fallback = joint_factor(corr)
+            method = self.mc_params["simulation_method"]
+            if method == "historical":
+                table = frame.dropna().to_numpy(dtype=np.float64)         # days with a return for every asset
+                if len(table) == 0:
+                    logger.error("No day with a return for every asset: cannot bootstrap the portfolio")
+                    return {}
+            elif method != "geometric_brownian_motion":
+                logger.error("Unknown simulation method: %s", method)
+                return {}
+            periods_per_year, confidence = 252, self.mc_params["confidence_level"]
+            steps = int(days) - 1
+            world, rank = 1, 0
+            if torch.distributed.is_available() and torch.distributed.is_initialized():
+                world, rank = torch.distributed.get_world_size(), torch.distributed.get_rank()
+            lo, hi, _ = shard_bounds(int(num_simulations), world, rank)
+            results = {}
+            for scenario in scenarios:
+                scenario_params = self.mc_params["scenarios"].get(scenario, {})
+                drift_factor = scenario_params.get("drift_factor", 1.0)
+                volatility_factor = scenario_params.get("volatility_factor", 1.0)
+                mu = np.array([u[4].mean() * periods_per_year * drift_factor for u in used])                # :243
+                sigma = np.array([u[4].std() * np.sqrt(periods_per_year) * volatility_factor for u in used])  # :244
+                seed = self.seed + self._sim_counter
+                self._sim_counter += 1
+                if method == "geometric_brownian_motion":
+                    finals, maxdd, af = eng.portfolio_gbm(s0, qty, mu, sigma, 1 / periods_per_year, chol.astype(np.float32),
+                                                          hi - lo, steps, seed, path_offset=lo, asset_finals=True)
+                else:
+                    finals, maxdd, af = eng.portfolio_bootstrap(table, self.mc_params["return_method"] == "log", s0, qty,
+                                                                hi - lo, steps, seed, path_offset=lo,
+                                                                block_len=self.block_len, asset_finals=True)
+                if world > 1:
+                    finals, maxdd = gather_paths(finals, maxdd, int(num_simulations))
+                    af = gather_path_rows(af, int(num_simulations))
+                st = risk_statistics(eng, finals, maxdd, v0, confidence)
+                asset_var = [abs(_var_pct(eng, af[i], s0[i], confidence)) for i in range(len(assets))]
+                undiversified = float(sum(w * v for w, v in zip(weights.tolist(), asset_var)))
+                var = float(abs(st["var"]))
+                results[scenario] = {
+                    "scenario": scenario, "time_horizon_days": days, "num_simulations": num_simulations,
+                    "simulation_method": method, "initial_value": v0,
+                    "drift_factor": drift_factor, "volatility_factor": volatility_factor,
+                    "mu": dict(zip(assets, mu.tolist())), "sigma": dict(zip(assets, sigma.tolist())),
+                    "percentiles": {str(p): {"price": float(v), "pct_change": float((v / v0 - 1) * 100)}
+                                    for p, v in zip(PERCENTILES, st["percentile_values"])},
+                    "expected": {"price": float(st["expected_price"]), "pct_change": float(st["expected_pct"])},
+                    "risk_metrics": {
+                        "var": var, "cvar": float(abs(st["cvar"])),
+                        "prob_profit": float(st["prob_profit"]), "prob_loss": float(1 - st["prob_profit"]),
+                        "max_drawdown": {"mean": float(st["mdd_mean"]), "median": float(st["mdd_median"]),
+                                         "max": float(st["mdd_max"])},
+                    },
+                    "undiversified_var": undiversified,
+                    "diversification_benefit": undiversified - var,
+                }
+            # _calculate_portfolio_stats' keys and conventions (:577-659), from the joint distribution
+            scenario_stats = {s: {"expected_return": r["expected"]["pct_change"] / 100, "var": r["risk_metrics"]["var"] / 100,
+                                  "cvar": r["risk_metrics"]["cvar"] / 100} for s, r in results.items()}
+            base = scenario_stats.get("base", {})
+            current = holdings["total_value"]
+            return {
+                "timestamp": datetime.now().isoformat(), "portfolio_value": current,
+                "assets": assets, "weights": dict(zip(assets, weights.tolist())),
+                "quantities": dict(zip(assets, qty.tolist())),
+                "correlation": {a: {b: float(corr[i, j]) for j, b in enumerate(assets)} for i, a in enumerate(assets)},
+                "correlation_fallback": bool(fallback),
+                "scenarios": results,
+                "portfolio_stats": {
+                    "current_value": current,
+                    "expected_value": current * (1 + base.get("expected_return", 0)),
+                    "expected_change": base.get("expected_return", 0) * 100,
+                    "var": base.get("var", 0) * 100,
+                    "cvar": base.get("cvar", 0) * 100,
+                    "var_loss_value": current * base.get("var", 0),
+                    "scenario_stats": scenario_stats,
+                },
+            }
+        except Exception as e:  # reference convention: log, return {}
+            logger.error("Error running joint portfolio Monte Carlo simulation: %s", e, exc_info=True)
             return {}
 
     def _calculate_portfolio_stats(self, holdings: Dict, simulations: Dict) -> Dict:

@@ -413,6 +413,32 @@ int b200bt_select(const float* x, int64_t n, const int64_t* ranks_dev, int n_ran
 int b200bt_mc_moments(const float* finals, const float* maxdd, int64_t n, double s0,
                       double var_threshold, double* out7, b200bt_stream_t stream);
 
+/* Joint paths of a portfolio of 1 <= S <= 32 assets (B200BT_ELIMIT above), simulated together instead of one
+ * asset at a time.  Replaces the per-asset loop of MonteCarloService.run_portfolio_monte_carlo
+ * (services/monte_carlo_service.py:492-575) and the correlation-free sums of _calculate_portfolio_stats (:577-659,
+ * "Simplified approach - ignores correlations", :630-631).  Portfolio value V_t = sum_i qty_i s0_i exp(logS_i,t)
+ * (qty_i >= 0, V_0 > 0).  Outputs: finals[n] = V_T, maxdd[n] = max_t (runmax_t - V_t)/runmax_t (the :327-336 rule
+ * on V_t), optional asset_finals[S][n] = s0_i exp(logS_i,T); finals / maxdd feed b200bt_select and b200bt_mc_moments
+ * with s0 = V_0.  Randomness: counter = (path index lo, hi, step/4, (factor << 8) | mode), key = seed.
+ *
+ * GBM (:266-273 per asset): every step draws S standard normals z; asset i moves by drift_i + vol_i (L z)_i with the
+ * per-step drift_i = (mu_i - sigma_i^2/2) dt and vol_i = sigma_i sqrt(dt).  chol_host: [S][S] row-major, the
+ * lower-triangular Cholesky factor L of the correlation matrix (the upper triangle is not read).  Factor 0 draws
+ * b200bt_mc_gbm's stream: with L_00 = 1, asset 0 equals b200bt_mc_gbm's path for the same (seed, path, s0, drift, vol). */
+int b200bt_mc_portfolio_gbm(int S, const double* s0_host, const double* qty_host, const double* drift_host,
+                            const double* vol_host, const float* chol_host, int64_t n_paths, int steps, uint64_t seed,
+                            uint64_t path_offset, float* finals, float* maxdd, float* asset_finals_or_null,
+                            b200bt_stream_t stream);
+
+/* Historical bootstrap (:277-298) of whole days: `returns` is a device table [R][S] fp32 (one row per day that has a
+ * return for every asset, R x S <= 12288), each step draws ONE row and applies it to every asset, which keeps the
+ * cross-asset dependence.  block_len and log_returns as in b200bt_mc_bootstrap, whose index stream this one is:
+ * asset i equals b200bt_mc_bootstrap on column i. */
+int b200bt_mc_portfolio_bootstrap(int S, const float* returns, int R, int block_len, int log_returns,
+                                  const double* s0_host, const double* qty_host, int64_t n_paths, int steps,
+                                  uint64_t seed, uint64_t path_offset, float* finals, float* maxdd,
+                                  float* asset_finals_or_null, b200bt_stream_t stream);
+
 /* ---- portfolio risk (SURVEY 8-f4) -------------------------------------------------------------------
  * Replaces the numeric core of services/portfolio_risk_service.py. */
 

@@ -1,0 +1,64 @@
+"""Status codes of the joint (portfolio) Monte-Carlo entry points: argument checks come before the device check, so
+EINVAL and ELIMIT are exercised with or without a GPU; ENODEVICE without one."""
+import ctypes as C
+
+import pytest
+
+EINVAL, ENODEVICE, ELIMIT = 10001, 10002, 10003
+
+
+def _d(*v):
+    return (C.c_double * len(v))(*v)
+
+
+def _gbm(S=2, s0=None, qty=None, chol=None, n_paths=8, steps=4, finals=True):
+    buf = (C.c_float * 64)()
+    out = C.addressof(buf) if finals else None
+    s0 = s0 if s0 is not None else _d(*[1.0] * S)
+    qty = qty if qty is not None else _d(*[1.0] * S)
+    chol = chol if chol is not None else (C.c_float * (S * S))(*[1.0 if i % (S + 1) == 0 else 0.0 for i in range(S * S)])
+    return ("b200bt_mc_portfolio_gbm", S, s0, qty, _d(*[0.0] * S), _d(*[0.01] * S), chol, n_paths, steps, 1, 0,
+            out, out, None, None)
+
+
+def _boot(S=2, R=16, block_len=1, returns=True, n_paths=8):
+    buf = (C.c_float * 64)()
+    return ("b200bt_mc_portfolio_bootstrap", S, C.addressof(buf) if returns else None, R, block_len, 1,
+            _d(*[1.0] * S), _d(*[1.0] * S), n_paths, 4, 1, 0, C.addressof(buf), C.addressof(buf), None, None)
+
+
+def _status(args):
+    from ai_crypto_trader_b200 import _lib
+    try:
+        _lib.call(*args)
+    except _lib.B200btError as e:
+        return e.status
+    return 0
+
+
+def test_portfolio_entry_points_refuse_without_device(native_lib):
+    import torch
+    if torch.cuda.is_available():
+        pytest.skip("GPU present: the no-device path cannot be exercised")
+    assert _status(_gbm()) == ENODEVICE
+    assert _status(_boot()) == ENODEVICE
+
+
+def test_portfolio_entry_points_validate_arguments(native_lib):
+    assert _status(_gbm(S=0)) == EINVAL
+    assert _status(_gbm(n_paths=0)) == EINVAL
+    assert _status(_gbm(steps=-1)) == EINVAL
+    assert _status(_gbm(finals=False)) == EINVAL
+    assert _status(_gbm(s0=_d(1.0, 0.0))) == EINVAL                  # a price must be positive
+    assert _status(_gbm(qty=_d(1.0, -1.0))) == EINVAL                # no short positions
+    assert _status(_gbm(qty=_d(0.0, 0.0))) == EINVAL                 # V_0 = 0
+    assert _status(_gbm(chol=(C.c_float * 4)(1.0, 0.0, float("nan"), 1.0))) == EINVAL
+    assert _status(_boot(returns=False)) == EINVAL
+    assert _status(_boot(R=0)) == EINVAL
+    assert _status(_boot(block_len=0)) == EINVAL
+
+
+def test_portfolio_entry_points_limits(native_lib):
+    assert _status(_gbm(S=33)) == ELIMIT
+    assert _status(_boot(S=33)) == ELIMIT
+    assert _status(_boot(S=4, R=3073)) == ELIMIT                      # R x S > 12288 table entries

@@ -2,10 +2,13 @@
 """Monte-Carlo throughput (BASELINE configs[2]): 1M GBM paths x 10k steps, VaR + max drawdown.
 
     python tools/mc_bench.py [--paths 1000000] [--steps 10000] [--store-steps 1000]
+    python tools/mc_bench.py --assets [1 4 16 32]
 
 Prints one JSON object: risk-only path-steps/s (compute-bound: Philox + Box-Muller per step),
 path-store mode GB/s against the measured HBM peak (4 B per path-step written), the statistics
 stage time, and the reference's NumPy GBM timed on the host on a bounded sample.
+With --assets: the joint (portfolio) GBM for each asset count S, in path-asset-steps/s, next to the
+single-asset kernel on the same paths and steps, with the card's name and power limit.
 """
 import argparse, json, sys, time
 from pathlib import Path
@@ -21,7 +24,11 @@ def main():
     ap.add_argument("--steps", type=int, default=10_000)
     ap.add_argument("--store-steps", type=int, default=1000)
     ap.add_argument("--reps", type=int, default=5)
+    ap.add_argument("--assets", type=int, nargs="*", default=None,
+                    help="time the joint GBM for these asset counts (no value: 1 4 16 32)")
     a = ap.parse_args()
+    if a.assets is not None:
+        return joint(a, a.assets or [1, 4, 16, 32])
     from ai_crypto_trader_b200.monte_carlo import PathEngine, risk_statistics
     import os
     world, rank = int(os.environ.get("WORLD_SIZE", 1)), int(os.environ.get("RANK", 0))
@@ -80,6 +87,52 @@ def main():
                        "frac": store_bytes / (ms_store * 1e-3) / 1e9 / peak},
         "statistics_ms": ms_stats, "var_pct": abs(st["var"]), "mdd_mean": st["mdd_mean"],
         "cpu_reference_numpy": {"path_steps_per_s": n_ref * (days_ref - 1) / ref_s, "sample": f"{n_ref} paths x {days_ref - 1} steps, 1 core"},
+    }))
+
+
+def _card():
+    """(name, power limit) of the card the numbers were taken on (read-only query)."""
+    import subprocess
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i",
+                              str(torch.cuda.current_device())], capture_output=True, text=True, timeout=30).stdout
+        name, power = [x.strip() for x in out.strip().splitlines()[0].split(",")]
+        return name, power
+    except Exception:
+        return torch.cuda.get_device_name(), "unknown"
+
+
+def joint(a, assets):
+    from ai_crypto_trader_b200.monte_carlo import PathEngine
+    torch.cuda.set_device(0)
+    eng = PathEngine()
+    reps = max(1, min(a.reps, 3))
+
+    def timed(fn):
+        fn(); torch.cuda.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(reps): fn()
+        e1.record(); torch.cuda.synchronize()
+        return e0.elapsed_time(e1) / reps
+
+    ms1 = timed(lambda: eng.gbm(100.0, 0.08, 0.35, 1 / 252, a.paths, a.steps, 2024))
+    rows = []
+    for S in assets:
+        rng = np.random.default_rng(S)
+        A = rng.normal(size=(S, S + 2)); c = A @ A.T; c /= np.sqrt(np.outer(np.diag(c), np.diag(c)))
+        L = np.linalg.cholesky(c).astype(np.float32)
+        s0, qty = rng.uniform(1, 100, S), rng.uniform(0.1, 10, S)
+        mu, sigma = rng.uniform(-0.1, 0.2, S), rng.uniform(0.2, 0.8, S)
+        ms = timed(lambda: eng.portfolio_gbm(s0, qty, mu, sigma, 1 / 252, L, a.paths, a.steps, 2024))
+        rows.append({"assets": S, "ms": ms, "path_asset_steps_per_s": a.paths * a.steps * S / (ms * 1e-3),
+                     "vs_single_asset_per_asset_step": (ms1 / ms) * S})
+    name, power = _card()
+    print(json.dumps({
+        "workload": f"joint GBM {a.paths} paths x {a.steps} steps, portfolio value + drawdown every step",
+        "card": name, "power_limit": power, "reps": reps,
+        "single_asset": {"ms": ms1, "path_steps_per_s": a.paths * a.steps / (ms1 * 1e-3)},
+        "joint": rows,
     }))
 
 

@@ -19,7 +19,7 @@ from ai_crypto_trader_b200.monte_carlo import PathEngine, risk_statistics
 from ai_crypto_trader_b200.sweep import MarketData, PopulationSweep
 from oracle import indicators_ref, sim_oracle
 
-legs = sys.argv[1:] or ["sweep", "mc", "indicators"]
+legs = sys.argv[1:] or ["sweep", "mc", "joint", "indicators"]
 torch.cuda.set_device(0)
 
 if "sweep" in legs:
@@ -56,6 +56,21 @@ if "mc" in legs:
     eng.bootstrap(ret, True, 100.0, 3000, 45, 77, block_len=5)
     st = risk_statistics(eng, f, d, 100.0, 0.95)
     print("mc ok", st["var"], flush=True)
+
+if "joint" in legs:
+    # joint portfolio paths: every asset bucket (4 / 8 / 16 / 32), the bootstrap table staged in shared memory
+    eng = PathEngine()
+    for S in (3, 8, 13, 32):
+        rng = np.random.default_rng(S)
+        A = rng.normal(size=(S, S + 2)); c = A @ A.T; c /= np.sqrt(np.outer(np.diag(c), np.diag(c)))
+        L = np.linalg.cholesky(c).astype(np.float32)
+        s0, qty = rng.uniform(1, 100, S), rng.uniform(0.1, 10, S)
+        f, d, af = eng.portfolio_gbm(s0, qty, rng.uniform(-0.1, 0.2, S), rng.uniform(0.2, 0.8, S), 1 / 252, L, 1000, 37,
+                                     2024, path_offset=5, asset_finals=True)
+        table = rng.normal(0, 0.02, (12288 // S, S)).astype(np.float32)
+        fb, db, _ = eng.portfolio_bootstrap(table, False, s0, qty, 1000, 37, 7, block_len=3, asset_finals=True)
+        assert bool(torch.isfinite(f).all() and torch.isfinite(fb).all() and (d >= 0).all() and (db >= 0).all())
+    print("joint ok", float(f.mean()), float(fb.mean()), flush=True)
 
 if "indicators" in legs:
     m = MarketData(synth.synth_ohlcv(2, 9000))
