@@ -754,12 +754,16 @@ lane_scan_kernel(const LaneScanArgs A, const bool vec16) {   // by value, not __
 
 // ---- metrics, chunk-parallel -------------------------------------------------------------------------
 // The trade-record metrics are a fold over the lane's events in time order, but every piece of it is
-// either a sum / max / xor (associative) or depends on the past only through three scalars: the equity
-// and running equity peak at the chunk's start, and the index of the chunk's first record.  So:
-//   chunk_sums_kernel    warp per (chunk, symbol): sum of record pnls and the largest prefix sum.
-//   chunk_partial_kernel warp per (chunk, symbol): exclusive scan of those over the lane's earlier chunks
-//                        -> starting equity / peak / record index, then the ordinary batch arithmetic
-//                        (batch_core) over the chunk's own events into a ChunkPartial.
+// either a sum / max / xor (associative) or depends on the past only through the index of the chunk's
+// first record -- except the max drawdown, which needs the equity and the running equity peak at the
+// chunk's start (E0, P0).  A chunk whose equity never rises above the peak it inherits has drawdown
+// (P0 - (E0 + smallest prefix)) / P0, so only the chunks that set a new peak need their records again:
+//   chunk_partial_kernel warp per (chunk, symbol): exclusive sum of the record counts of the lane's earlier
+//                        chunks -> record index, then the batch arithmetic (batch_core) over the chunk's own
+//                        events into a ChunkPartial, plus the chunk's PnL sum and largest / smallest prefix sum.
+//   chunk_prefix_kernel  thread per (individual, symbol): E0 / P0 of every chunk in time order; the drawdown of
+//                        a chunk below its inherited peak in closed form, the others listed.
+//   chunk_peak_kernel    warp per listed chunk: equity, running peak and drawdown record by record from E0 / P0.
 //   lane_combine_kernel  thread per (individual, symbol): verifies the boundaries, merges the partials
 //                        (calendar days that straddle a chunk boundary are re-joined) and finalises.
 struct ChunkPartial {
@@ -769,7 +773,8 @@ struct ChunkPartial {
     unsigned n_win, n_loss, n_days, count;
     int first_done, first_day, day_cur;
     unsigned n_neg;
-    double npivot, ns1, ns2, pad;     // the chunk's finished negative days (DayAcc)
+    double npivot, ns1, ns2;          // the chunk's finished negative days (DayAcc)
+    double min_prefix;                // smallest equity of the chunk relative to its start (+inf: no records)
 };
 static_assert(sizeof(ChunkPartial) == 160, "ChunkPartial layout");
 
@@ -782,72 +787,15 @@ __device__ __forceinline__ void chunk_carry(const int2 in, const float* __restri
     }
 }
 
-__global__ void __launch_bounds__(128)
-chunk_sums_kernel(const float* __restrict__ price, int64_t ld_price, const b200bt_individual* __restrict__ indiv,
-                  const b200bt_chunk_item* __restrict__ items, int n_items, int S, int n_seg,
-                  const uint2* __restrict__ pool, const int* __restrict__ next, const int* __restrict__ seg_first,
-                  const unsigned* __restrict__ seg_count, const int2* __restrict__ seg_in,
-                  double* __restrict__ seg_sum, double* __restrict__ seg_max, const int* __restrict__ n_items_dev,
-                  int pool_blocks) {
-    const int lane = threadIdx.x & 31;
-    const int sym = (int)(blockIdx.x % (unsigned)S);
-    const int it = (int)(blockIdx.x / (unsigned)S) * 4 + (threadIdx.x >> 5);
-    if (it >= (n_items_dev ? *n_items_dev : n_items)) return;
-    const b200bt_chunk_item item = items[it];
-    const int seg = sym * n_seg + item.segment;
-    const double size = indiv[item.individual].position_size;
-    const double fee1 = __dmul_rn(size, 0.001), fee2 = __dmul_rn(size, 0.002);
-    unsigned left = seg_count[seg];
-    if (left == 0xffffffffu) left = 0;
-    unsigned w_carry; float p_carry;
-    chunk_carry(seg_in[seg], price + (int64_t)sym * ld_price, w_carry, p_carry);
-    int b = left ? seg_first[seg] : -1, off = 0;
-    if ((unsigned)b >= (unsigned)pool_blocks) left = 0;   // (a segment being re-scanned on the side stream)
-    double run = 0.0, best = -INFINITY;
-    // 64 records per step, two consecutive ones per lane (one 16-byte load): half the shuffles per record
-    while (left) {
-        const int cnt = (int)min(64u, left);
-        const bool a0 = 2 * lane < cnt, a1 = 2 * lane + 1 < cnt;
-        uint4 ev = make_uint4(0u, 0u, 0u, 0u);
-        if (a0) ev = *reinterpret_cast<const uint4*>(pool + (int64_t)b * CK_BLOCK + off + 2 * lane);   // (slot 2l+1 may be unused: in-block)
-        const float pf0 = __uint_as_float(ev.y), pf1 = __uint_as_float(ev.w);
-        float p_prev = __shfl_up_sync(FULL, pf1, 1);
-        unsigned w_prev = __shfl_up_sync(FULL, ev.z, 1);
-        if (lane == 0) { p_prev = p_carry; w_prev = w_carry; }
-        int dur;
-        const double pnl0 = record_pnl(a0, ev.x, pf0, w_prev, p_prev, size, fee1, fee2, dur);
-        const double pnl1 = record_pnl(a1, ev.z, pf1, ev.x, pf0, size, fee1, fee2, dur);
-        const double s2 = pnl0 + pnl1;
-        double cs = s2;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-            const double up = shfl_up_d(cs, d);
-            if (lane >= d) cs += up;
-        }
-        const double after0 = run + (cs - s2) + pnl0, after1 = run + cs;
-        best = fmax(best, warp_max_d(fmax(a0 ? after0 : -INFINITY, a1 ? after1 : -INFINITY)));
-        run += shfl_d(cs, 31);
-        const int last = (cnt - 1) >> 1;
-        const unsigned wl = (cnt & 1) ? ev.x : ev.z;
-        const float pl = (cnt & 1) ? pf0 : pf1;
-        w_carry = __shfl_sync(FULL, wl, last);
-        p_carry = __shfl_sync(FULL, pl, last);
-        left -= cnt;
-        off += 64;
-        if (off == CK_BLOCK && left) { b = next[b]; off = 0; if ((unsigned)b >= (unsigned)pool_blocks) break; }
-    }
-    if (lane == 0) { seg_sum[seg] = run; seg_max[seg] = best; }
-}
-
 #ifndef B200BT_M2_MIN_BLOCKS
-#define B200BT_M2_MIN_BLOCKS 8
+#define B200BT_M2_MIN_BLOCKS 5      // 96 registers, no spills (nvcc 12.9, sm_90a); at 6 CTAs/SM (80) it spills 64 B
 #endif
 __global__ void __launch_bounds__(128, B200BT_M2_MIN_BLOCKS)
 chunk_partial_kernel(const float* __restrict__ price, int64_t ld_price, const b200bt_individual* __restrict__ indiv,
                      const b200bt_chunk_item* __restrict__ items, int n_items, int S, int n_seg,
                      const uint2* __restrict__ pool, const int* __restrict__ next, const int* __restrict__ seg_first,
                      const unsigned* __restrict__ seg_count, const int2* __restrict__ seg_in,
-                     const double* __restrict__ seg_sum, const double* __restrict__ seg_max,
+                     double* __restrict__ seg_sum, double* __restrict__ seg_max,
                      const b200bt_sweep_config cfg, uint32_t* __restrict__ events, int64_t ev_cap,
                      ChunkPartial* __restrict__ partial, const int* __restrict__ n_items_dev, int pool_blocks) {
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -859,33 +807,20 @@ chunk_partial_kernel(const float* __restrict__ price, int64_t ld_price, const b2
     const int base = seg - item.chunk;
     const b200bt_individual iv = indiv[item.individual];
 
-    // state at the chunk's start: equity, running peak, record index -- exclusive scan over earlier chunks
-    double e0 = cfg.initial_capital, p0 = cfg.initial_capital;
+    // index of the chunk's first record: exclusive sum over the lane's earlier chunks
     unsigned first_index = 0;
     for (int c0 = 0; c0 < item.chunk; c0 += 32) {
         const int c = c0 + lane;
-        const bool in = c < item.chunk;
-        const double s = in ? seg_sum[base + c] : 0.0;
-        const double mx = in ? seg_max[base + c] : -INFINITY;
-        unsigned n = in ? seg_count[base + c] : 0u;
+        unsigned n = c < item.chunk ? seg_count[base + c] : 0u;
         if (n == 0xffffffffu) n = 0;
-        double incl = s;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-            const double up = shfl_up_d(incl, d);
-            if (lane >= d) incl += up;
-        }
-        const double start = e0 + (incl - s);            // equity at the start of chunk c
-        p0 = fmax(p0, warp_max_d(start + mx));
-        e0 += shfl_d(incl, 31);
         first_index += __reduce_add_sync(FULL, n);
     }
 
-    // Order-dependent state (equity, peak, drawdown, calendar day) is warp-uniform and lives in registers; what
-    // is a plain sum / max / xor over the records is accumulated PER LANE and reduced once at the end of the chunk.
+    // Order-dependent state (equity relative to the chunk's start, calendar day) is warp-uniform and lives in registers;
+    // what is a plain sum / max / min / xor over the records is accumulated PER LANE and reduced once at the end of the chunk.
     const double size = iv.position_size;
     const double fee1 = __dmul_rn(size, 0.001), fee2 = __dmul_rn(size, 0.002);
-    double equity = e0, peak = p0, maxdd = 0.0;
+    double equity = 0.0, l_top = -INFINITY, l_bottom = INFINITY;
     DayAcc da{0.0, 0.0, 0.0, 0u, 0};
     int day_valid = 0, day_cur = 0, first_done = 0, first_id = 0;
     double day_sum = 0.0, first_sum = 0.0;
@@ -942,7 +877,7 @@ chunk_partial_kernel(const float* __restrict__ price, int64_t ld_price, const b2
             if (ev_out && (int64_t)i0 + 1 < ev_cap) ev_out[i0 + 1] = w1;
         }
 
-        // equity curve: inclusive scan of the lane sums, running peak, drawdown (cf. batch_core, sweep_dev.cuh)
+        // equity relative to the chunk's start: inclusive scan of the lane sums; its extremes per lane
         const double s2 = pnl0 + pnl1;
         double cs = s2;
 #pragma unroll
@@ -951,28 +886,8 @@ chunk_partial_kernel(const float* __restrict__ price, int64_t ld_price, const b2
             if (lane >= d) cs += up;
         }
         const double eq0 = equity + (cs - s2) + pnl0, eq1 = equity + cs;
-        const double m2 = fmax(a0 ? eq0 : -INFINITY, a1 ? eq1 : -INFINITY);
-        double pk0 = peak, pk1 = peak;
-        if (__any_sync(FULL, m2 > peak)) {
-            double pk = m2;
-#pragma unroll
-            for (int d = 1; d < 32; d <<= 1) {
-                const double up = shfl_up_d(pk, d);
-                if (lane >= d) pk = fmax(pk, up);
-            }
-            double before = shfl_up_d(pk, 1);          // peak over the records of the lanes in front
-            before = fmax(lane == 0 ? peak : before, peak);
-            pk0 = fmax(before, eq0);
-            pk1 = fmax(pk0, eq1);
-            peak = fmax(peak, shfl_d(pk, 31));
-        }
-        {
-            const double gap0 = __dsub_rn(pk0, eq0), gap1 = __dsub_rn(pk1, eq1);
-            const double lim = maxdd * (1.0 - 1e-12);
-            const bool c0 = a0 && gap0 > 0.0 && gap0 >= lim * pk0, c1 = a1 && gap1 > 0.0 && gap1 >= lim * pk1;
-            if (__any_sync(FULL, c0 || c1))
-                maxdd = fmax(maxdd, warp_max_d(fmax(c0 ? __ddiv_rn(gap0, pk0) : 0.0, c1 ? __ddiv_rn(gap1, pk1) : 0.0)));
-        }
+        if (a0) { l_top = fmax(l_top, eq0); l_bottom = fmin(l_bottom, eq0); }
+        if (a1) { l_top = fmax(l_top, eq1); l_bottom = fmin(l_bottom, eq1); }
         const double batch_sum = shfl_d(cs, 31);
         equity += batch_sum;
 
@@ -1041,15 +956,125 @@ chunk_partial_kernel(const float* __restrict__ price, int64_t ld_price, const b2
     for (int m = 16; m > 0; m >>= 1) sum_dur += __shfl_xor_sync(FULL, sum_dur, m);
     hlo = __reduce_xor_sync(FULL, hlo);
     hhi = __reduce_xor_sync(FULL, hhi);
+    const double top = warp_max_d(l_top), bottom = warp_min_d(l_bottom);
     if (lane == 0) {
         ChunkPartial q;
         q.tot_profit = tot_profit; q.tot_loss = tot_loss; q.largest_p = largest_p; q.largest_l = largest_l;
-        q.maxdd = maxdd; q.first_sum = first_sum; q.pivot = da.pivot; q.s1 = da.s1; q.s2 = da.s2; q.day_sum = day_sum;
+        q.maxdd = 0.0; q.first_sum = first_sum; q.pivot = da.pivot; q.s1 = da.s1; q.s2 = da.s2; q.day_sum = day_sum;
         q.sum_dur = sum_dur; q.hash = ((unsigned long long)hhi << 32) | hlo;
         q.n_win = n_win; q.n_loss = n_loss; q.n_days = da.n_days; q.count = count;
         q.first_done = first_done; q.first_day = first_id; q.day_cur = day_cur;
-        q.n_neg = da.n_neg; q.npivot = da.npivot; q.ns1 = da.ns1; q.ns2 = da.ns2; q.pad = 0.0;
+        q.n_neg = da.n_neg; q.npivot = da.npivot; q.ns1 = da.ns1; q.ns2 = da.ns2; q.min_prefix = bottom;
         partial[seg] = q;
+        seg_sum[seg] = equity;
+        seg_max[seg] = top;
+    }
+}
+
+// Drawdown, thread per (individual, symbol): the chunks' PnL sums and largest prefixes give every chunk's starting equity E0
+// and inherited peak P0, in time order.  A chunk that does not rise above P0 (E0 + largest prefix <= P0: the strict > of the
+// running peak's update) has drawdown (P0 - (E0 + smallest prefix)) / P0 when positive -- division by a fixed P0 is monotone,
+// so that is the largest of its records' values.  A chunk that sets a new peak is listed for chunk_peak_kernel, its seg_sum /
+// seg_max overwritten with E0 / P0.
+__global__ void __launch_bounds__(128)
+chunk_prefix_kernel(int pop, int S, const int32_t* __restrict__ seg_base, const int32_t* __restrict__ n_chunks, int n_seg,
+                    double* __restrict__ seg_sum, double* __restrict__ seg_max, ChunkPartial* __restrict__ partial,
+                    double initial_capital, int4* __restrict__ peaks, unsigned* __restrict__ n_peaks) {
+    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= (int64_t)pop * S) return;
+    const int ind = (int)(t / S), sym = (int)(t % S);
+    const int K = n_chunks[ind];
+    const int base = sym * n_seg + seg_base[ind];
+    double e0 = initial_capital, p0 = initial_capital;
+    for (int c = 0; c < K; ++c) {
+        const int seg = base + c;
+        const double sum = seg_sum[seg], top = __dadd_rn(e0, seg_max[seg]);   // (a chunk without records: 0, -inf)
+        if (top > p0) {
+            seg_sum[seg] = e0;
+            seg_max[seg] = p0;
+            peaks[atomicAdd(n_peaks, 1u)] = make_int4(seg, ind, sym, 0);
+        } else {
+            const double gap = __dsub_rn(p0, __dadd_rn(e0, partial[seg].min_prefix));
+            partial[seg].maxdd = gap > 0.0 ? __ddiv_rn(gap, p0) : 0.0;
+        }
+        p0 = fmax(p0, top);
+        e0 = __dadd_rn(e0, sum);
+    }
+}
+
+// Drawdown of the listed chunks (chunk_prefix_kernel), one warp per chunk over a device-side count: equity from E0, running
+// peak from P0 and the drawdown candidates record by record (the arithmetic of batch_core, two records per lane).
+__global__ void __launch_bounds__(128)
+chunk_peak_kernel(const float* __restrict__ price, int64_t ld_price, const b200bt_individual* __restrict__ indiv,
+                  const uint2* __restrict__ pool, const int* __restrict__ next, const int* __restrict__ seg_first,
+                  const unsigned* __restrict__ seg_count, const int2* __restrict__ seg_in, const double* __restrict__ seg_e0,
+                  const double* __restrict__ seg_p0, const int4* __restrict__ peaks, const unsigned* __restrict__ n_peaks,
+                  ChunkPartial* __restrict__ partial, int pool_blocks) {
+    const int lane = threadIdx.x & 31;
+    const unsigned n = *n_peaks, warps = (gridDim.x * blockDim.x) >> 5;
+    for (unsigned i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n; i += warps) {
+        const int4 pk = peaks[i];
+        const int seg = pk.x;
+        const double size = indiv[pk.y].position_size;
+        const double fee1 = __dmul_rn(size, 0.001), fee2 = __dmul_rn(size, 0.002);
+        unsigned left = seg_count[seg];
+        if (left == 0xffffffffu) left = 0;
+        unsigned w_carry; float p_carry;
+        chunk_carry(seg_in[seg], price + (int64_t)pk.z * ld_price, w_carry, p_carry);
+        int b = left ? seg_first[seg] : -1, off = 0;
+        if ((unsigned)b >= (unsigned)pool_blocks) left = 0;
+        double equity = seg_e0[seg], peak = seg_p0[seg], maxdd = 0.0;
+        while (left) {
+            const int cnt = (int)min(64u, left);
+            const bool a0 = 2 * lane < cnt, a1 = 2 * lane + 1 < cnt;
+            uint4 ev = make_uint4(0u, 0u, 0u, 0u);
+            if (a0) ev = *reinterpret_cast<const uint4*>(pool + (int64_t)b * CK_BLOCK + off + 2 * lane);
+            const float pf0 = __uint_as_float(ev.y), pf1 = __uint_as_float(ev.w);
+            float p_prev = __shfl_up_sync(FULL, pf1, 1);
+            unsigned w_prev = __shfl_up_sync(FULL, ev.z, 1);
+            if (lane == 0) { p_prev = p_carry; w_prev = w_carry; }
+            int dur;
+            const double pnl0 = record_pnl(a0, ev.x, pf0, w_prev, p_prev, size, fee1, fee2, dur);
+            const double pnl1 = record_pnl(a1, ev.z, pf1, ev.x, pf0, size, fee1, fee2, dur);
+            const double s2 = pnl0 + pnl1;
+            double cs = s2;
+#pragma unroll
+            for (int d = 1; d < 32; d <<= 1) {
+                const double up = shfl_up_d(cs, d);
+                if (lane >= d) cs += up;
+            }
+            const double eq0 = equity + (cs - s2) + pnl0, eq1 = equity + cs;
+            const double m2 = fmax(a0 ? eq0 : -INFINITY, a1 ? eq1 : -INFINITY);
+            double pk0 = peak, pk1 = peak;
+            if (__any_sync(FULL, m2 > peak)) {
+                double p = m2;
+#pragma unroll
+                for (int d = 1; d < 32; d <<= 1) {
+                    const double up = shfl_up_d(p, d);
+                    if (lane >= d) p = fmax(p, up);
+                }
+                double before = shfl_up_d(p, 1);           // peak over the records of the lanes in front
+                before = fmax(lane == 0 ? peak : before, peak);
+                pk0 = fmax(before, eq0);
+                pk1 = fmax(pk0, eq1);
+                peak = fmax(peak, shfl_d(p, 31));
+            }
+            {
+                const double gap0 = __dsub_rn(pk0, eq0), gap1 = __dsub_rn(pk1, eq1);
+                const double lim = maxdd * (1.0 - 1e-12);
+                const bool c0 = a0 && gap0 > 0.0 && gap0 >= lim * pk0, c1 = a1 && gap1 > 0.0 && gap1 >= lim * pk1;
+                if (__any_sync(FULL, c0 || c1))
+                    maxdd = fmax(maxdd, warp_max_d(fmax(c0 ? __ddiv_rn(gap0, pk0) : 0.0, c1 ? __ddiv_rn(gap1, pk1) : 0.0)));
+            }
+            equity += shfl_d(cs, 31);
+            const int last = (cnt - 1) >> 1;
+            w_carry = __shfl_sync(FULL, (cnt & 1) ? ev.x : ev.z, last);
+            p_carry = __shfl_sync(FULL, (cnt & 1) ? pf0 : pf1, last);
+            left -= cnt;
+            off += 64;
+            if (off == CK_BLOCK && left) { b = next[b]; off = 0; if ((unsigned)b >= (unsigned)pool_blocks) break; }
+        }
+        if (lane == 0) partial[seg].maxdd = maxdd;
     }
 }
 
@@ -1159,7 +1184,7 @@ using namespace b200bt;
 
 namespace {
 
-constexpr int REPAIR_COUNTERS = 130;   // work counters: [0] bounded repair pass, [1] overlapped pass, [last] the scan; 2 + REPAIR_COUNTERS a multiple of 4 (alignment)
+constexpr int REPAIR_COUNTERS = 130;   // work counters: [0] bounded repair pass, [1] overlapped pass, [2] listed peak chunks, [last] the scan; 2 + REPAIR_COUNTERS a multiple of 4 (alignment)
 struct ChunkWorkspace {
     uint2* pool; int2* seg_in; int2* seg_out; int* seg_first; unsigned* seg_count; unsigned* alloc; int* overflow;
     unsigned* n_repair; int4* repair; int* next; ChunkPartial* partial; double* seg_sum; double* seg_max;
@@ -1168,7 +1193,7 @@ struct ChunkWorkspace {
 };
 
 // pool[pool_blocks][256] uint2 | seg_in[segs] int2 | seg_out[segs] int2 | seg_first[segs] | seg_count[segs] |
-// alloc, overflow, n_repair[REPAIR_COUNTERS] (work counters) | repair[segs] int4 (reserved) | next[pool_blocks] | (16-byte aligned) partial[segs] (128 B) |
+// alloc, overflow, n_repair[REPAIR_COUNTERS] (work counters) | repair[segs] int4 (chunks that set a new equity peak) | next[pool_blocks] | (16-byte aligned) partial[segs] (160 B) |
 // seg_sum[segs] | seg_max[segs] | fix_items[n_seg] (16 B) | n_fix (16 B) | redo[pop]
 // (wide types first: the base must be 16-byte aligned)
 ChunkWorkspace carve(void* workspace, int pool_blocks, int64_t segs, int n_seg, int pop) {
@@ -1265,9 +1290,6 @@ int finish_chunks(const ChunkScanArgs& A, const ChunkWorkspace& w, const b200bt_
     };
     // (the fix-up pass reuses the full-size grid with a device-side item count: CTAs beyond it leave at once)
     auto metrics = [&](const b200bt_chunk_item* its, const int* n_dev) -> int {
-        chunk_sums_kernel<<<(unsigned)mblocks, 128, 0, st>>>(A.price, A.ld_price, A.indiv, its, n_items, S, n_seg, w.pool, w.next,
-                                                              w.seg_first, w.seg_count, w.seg_in, w.seg_sum, w.seg_max, n_dev, A.pool_blocks);
-        B200BT_LAUNCH_CHECK("chunk_sums launch");
         chunk_partial_kernel<<<(unsigned)mblocks, 128, 0, st>>>(A.price, A.ld_price, A.indiv, its, n_items, S, n_seg, w.pool, w.next,
                                                                  w.seg_first, w.seg_count, w.seg_in, w.seg_sum, w.seg_max,
                                                                  *cfg_host, events, event_cap, w.partial, n_dev, A.pool_blocks);
@@ -1299,6 +1321,15 @@ int finish_chunks(const ChunkScanArgs& A, const ChunkWorkspace& w, const b200bt_
         B200BT_LAUNCH_CHECK("fix_items launch");
         if ((rc = metrics(w.fix_items, w.n_fix))) return rc;
     }
+    // drawdown: chunks below their inherited peak in closed form, the chunks that set a new peak record by record
+    // (n_repair[2] = number of those; a persistent grid walks the list)
+    chunk_prefix_kernel<<<(unsigned)((lanes + 127) / 128), 128, 0, st>>>(pop, S, seg_base, A.n_chunks, n_seg, w.seg_sum, w.seg_max,
+                                                                        w.partial, cfg_host->initial_capital, w.repair, w.n_repair + 2);
+    B200BT_LAUNCH_CHECK("chunk_prefix launch");
+    chunk_peak_kernel<<<8u * (unsigned)device_sm_count(), 128, 0, st>>>(A.price, A.ld_price, A.indiv, w.pool, w.next, w.seg_first,
+                                                                       w.seg_count, w.seg_in, w.seg_sum, w.seg_max, w.repair,
+                                                                       w.n_repair + 2, w.partial, A.pool_blocks);
+    B200BT_LAUNCH_CHECK("chunk_peak launch");
     lane_combine_kernel<<<(unsigned)((lanes + 127) / 128), 128, 0, st>>>(A.indiv, pop, S, seg_base, A.n_chunks, n_seg, w.seg_count,
                                                                         w.seg_in, w.seg_out, w.partial, *cfg_host, stats,
                                                                         lane_invalid);
@@ -1313,11 +1344,13 @@ int finish_chunks(const ChunkScanArgs& A, const ChunkWorkspace& w, const b200bt_
         return rc;
     if (overflow_host_or_null) {
         // [0] = the event pool overflowed, [1] = lanes that went through the fallback, [2] = pool blocks handed out, [3] = tiles
-        // of the thread-per-lane scan that did not arrive in time (read by the host after its next sync)
+        // of the thread-per-lane scan that did not arrive in time, [4] = chunks that set a new equity peak (read by the host
+        // after its next sync)
         e = cudaMemcpyAsync(overflow_host_or_null, w.overflow, sizeof(int), cudaMemcpyDeviceToHost, st);
         if (e == cudaSuccess) e = cudaMemcpyAsync(overflow_host_or_null + 1, w.n_fix + 2, sizeof(int), cudaMemcpyDeviceToHost, st);
         if (e == cudaSuccess) e = cudaMemcpyAsync(overflow_host_or_null + 2, w.alloc, sizeof(int), cudaMemcpyDeviceToHost, st);
         if (e == cudaSuccess) e = cudaMemcpyAsync(overflow_host_or_null + 3, w.n_repair + 64, sizeof(int), cudaMemcpyDeviceToHost, st);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(overflow_host_or_null + 4, w.n_repair + 2, sizeof(int), cudaMemcpyDeviceToHost, st);
         if (e != cudaSuccess) return cuda_status(e, "sweep_chunked: overflow readback");
     }
     if (trace_launches()) {

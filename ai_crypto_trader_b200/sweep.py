@@ -309,12 +309,13 @@ _FLAG_SLOTS = 256
 
 
 def _pinned_flags() -> torch.Tensor:
-    """Pinned int32 [256][4]: per plan (slice) of a sweep, [0] = the event pool overflowed, [1] = lanes that went through
-    the exact fallback, [2] = pool blocks handed out, [3] = scan tiles that timed out.  The kernels' flags are copied here asynchronously; the host looks at them only after a stream
+    """Pinned int32 [256][5]: per plan (slice) of a sweep, [0] = the event pool overflowed, [1] = lanes that went through
+    the exact fallback, [2] = pool blocks handed out, [3] = scan tiles that timed out, [4] = time chunks that set a new
+    equity peak.  The kernels' flags are copied here asynchronously; the host looks at them only after a stream
     synchronisation it does anyway (page-locking memory is slow: one table shared by every plan)."""
     global _PINNED_FLAGS
     if _PINNED_FLAGS is None:
-        _PINNED_FLAGS = torch.zeros((_FLAG_SLOTS, 4), dtype=torch.int32).pin_memory()
+        _PINNED_FLAGS = torch.zeros((_FLAG_SLOTS, 5), dtype=torch.int32).pin_memory()
     return _PINNED_FLAGS
 
 
@@ -681,6 +682,12 @@ class PopulationSweep:
         """Tiles of the last thread-per-lane scan whose bulk copy did not complete in time (their chunks were re-scanned by the
         repair pass or their lanes re-run by the exact fallback; 0 in normal operation)."""
         return int(sum(int(f[3]) for f in self._sync_flags()))
+
+    @property
+    def last_peak_chunks(self) -> int:
+        """(individual, symbol, chunk) time chunks of the last time-chunked evaluation that set a new equity peak: only those
+        take the record-by-record drawdown pass (chunk_peak_kernel); the others' drawdown comes from three per-chunk sums."""
+        return int(sum(int(f[4]) for f in self._sync_flags()))
 
     @property
     def last_pool_overflow(self) -> bool:

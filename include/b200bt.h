@@ -280,11 +280,12 @@ int b200bt_sweep(const float* price, int64_t ld_price,
  *  items      [n_items] device      seg_base, n_chunks  [pop] device int32      n_seg = sum of n_chunks
  *  pool_blocks  event pool size in blocks of 256 events; a chunk that cannot get a block flags its lane
  *  workspace  b200bt_sweep_chunked_workspace_bytes(pool_blocks, S, n_seg) device bytes
- *  overflow_host_or_null  optional PINNED host int[4], written asynchronously on `stream` (read after synchronising it):
+ *  overflow_host_or_null  optional PINNED host int[5], written asynchronously on `stream` (read after synchronising it):
  *                         [0] = 1 if the event pool ran out (grow it next time), [1] = number of (individual, symbol)
  *                         lanes that were flagged and re-evaluated by the exact fallback, [2] = pool blocks handed out
  *                         (what the next sweep of a similar population needs), [3] = tiles of the thread-per-lane scan
- *                         whose bulk copy did not complete in time (b200bt_sweep_tiled; their work was redone, see there).
+ *                         whose bulk copy did not complete in time (b200bt_sweep_tiled; their work was redone, see there),
+ *                         [4] = time chunks that set a new equity peak (their drawdown took the record-by-record pass).
  * Flagged lanes are re-evaluated by the fused kernel (b200bt_sweep's) inside this call, from a device-side list: the call
  * reads nothing back and never synchronises; lane_invalid reports which lanes took that path. */
 typedef struct b200bt_chunk_item {

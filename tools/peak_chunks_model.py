@@ -1,12 +1,14 @@
 #!/usr/bin/env python
-"""CPU model behind DESIGN.md section 8, item 2: how many time chunks of a lane set a NEW EQUITY PEAK?
+"""CPU model behind the sparse drawdown pass of the time-chunked sweeps (DESIGN.md section 3.1): how many time chunks of a
+lane set a NEW EQUITY PEAK?
 
-chunk_sums_kernel exists only to hand chunk_partial_kernel the equity and the running peak at the start of every chunk, and
-those are needed for one number, the drawdown.  A chunk in which the equity never exceeds the peak it inherits has
-max drawdown (P0 - E0 - min prefix) / P0, which lane_combine could form from three per-chunk scalars; only chunks that set a
-new peak need the record-by-record pass.  This script counts them on the bench workload (configs[1]: population 1024, symbol
-0, 1M bars, K = 28 chunks) for the random seed-42 population and for the generation-3 population of the GA run bench.py
-times (`evolved`: the GA is run on the C oracle over all 10 symbols, ~40 s on 8 cores).
+The equity and the running peak at the start of a chunk are needed for one metric, the max drawdown.  A chunk in which the
+equity never exceeds the peak it inherits has max drawdown (P0 - E0 - min prefix) / P0, which chunk_prefix_kernel forms from
+three per-chunk scalars; only the chunks that set a new peak take the record-by-record pass (chunk_peak_kernel).  This
+script counts them on the bench workload (configs[1]: population 1024, symbol 0, 1M bars, K = 28 chunks) for the random
+seed-42 population and for the generation-3 population of the GA run bench.py times (`evolved`: the GA is run on the C
+oracle over all 10 symbols, ~40 s on 8 cores).  The GPU's count is PopulationSweep.last_peak_chunks
+(tools/sweep_kernels.py prints it).
 
     python tools/peak_chunks_model.py [random|evolved]
 
