@@ -23,26 +23,73 @@
 //                   of chunk c for every boundary and merges the chunks' partial metrics.
 // A lane with any mismatching boundary is flagged; the host re-evaluates flagged lanes with the
 // fused (serial) kernel, so results never depend on the speculation being right.
-#include <stdlib.h>
+#include <stddef.h>
 #include "sweep_dev.cuh"
 
 namespace b200bt {
 
 constexpr int CK_BLOCK = 256;   // events per pool block
 constexpr unsigned EVENT_BAR_MASK = ~(B200BT_EVENT_EXIT | B200BT_EVENT_SELL);   // event word = bar | flags
+constexpr unsigned SEG_LOST = 0xffffffffu;   // seg_count of a chunk whose events were lost (full pool, tile given up, unpacked warp)
 
-struct ChunkScanArgs {
+// Device-side counters of one sweep (a workspace section, zeroed at the start of the sweep); the first five are the flags
+// the caller reads back, in the order of the C-ABI's overflow_host int[5].  The scan and repair kernels are given pointers
+// to the fields they use: an address computed from the struct's base stays in registers the scan loops cannot spare.
+struct SweepCounters {
+    int overflow;            // [0] the event pool ran out
+    int fallback_lanes;      // [1] (individual, symbol) lanes re-run by the exact fallback
+    unsigned alloc;          // [2] pool blocks handed out (the pool's bump allocator)
+    int stalls;              // [3] tiles of the thread-per-lane scan that did not arrive in time
+    unsigned peak_chunks;    // [4] chunks that set a new equity peak (length of the peak list)
+    int stall[8];            // the first stall: block, warp, item, tile, tiles, stage * 2 + parity, first tile, rows
+    unsigned scan_work, chunk_repair_work, lane_repair_work;   // work counters of the persistent grids
+    int n_fix_items;         // fix-up work items (individuals the overlapped repair touched)
+    int n_redo;              // individuals listed for the exact fallback
+};
+constexpr int SWEEP_FLAGS = 5;
+static_assert(offsetof(SweepCounters, peak_chunks) == (SWEEP_FLAGS - 1) * sizeof(int), "flags are the ABI's int[5]");
+
+// The event pool and the per-chunk tables the scan kernels write and the repair / metrics kernels read.  Events live in
+// blocks of CK_BLOCK (event word, price bits) pairs, bump-allocated; a chunk's blocks are linked from seg_first[seg]
+// through next[].
+struct ChunkTables {
+    uint2* pool; int pool_blocks; int* next;
+    unsigned* alloc; int* overflow;        // &SweepCounters::alloc, ::overflow
+    int* seg_first; unsigned* seg_count;   // first block, number of events (SEG_LOST: dropped)
+    int2* seg_in; int2* seg_out;           // assumed state at the chunk's start, state at its end: (side, entry bar or -1)
+};
+
+struct ChunkScanArgs : ChunkTables {
     const float* price; int64_t ld_price;
     const float* rsi; int64_t ld_rsi;
     int P, S; int64_t N;
     const b200bt_individual* indiv;
     const b200bt_chunk_item* items; int n_items; int n_seg;   // n_seg = segments per symbol
     int warm;
-    uint2* pool; int pool_blocks; int* next; unsigned* alloc;
-    int* seg_first; unsigned* seg_count; int2* seg_in; int2* seg_out; int* overflow;
     const int32_t* n_chunks;
     unsigned char* redo;  // repair pass of the overlapped tail: individuals whose metrics must be recomputed
 };
+
+__device__ __forceinline__ unsigned seg_records(unsigned count) { return count == SEG_LOST ? 0u : count; }
+
+// links a new pool block behind chunk `seg`'s last one, `block` (-1: none yet), and moves `block` to it; false when the
+// pool is full (flagged)
+__device__ __forceinline__ bool pool_take_block(const ChunkTables& T, const int seg, int& block) {
+    const int b = (int)atomicAdd(T.alloc, 1u);
+    if (b >= T.pool_blocks) { atomicExch(T.overflow, 1); return false; }
+    T.next[b] = -1;
+    if (block < 0) T.seg_first[seg] = b; else T.next[block] = b;
+    block = b;
+    return true;
+}
+
+// the chunk is not scanned: it is marked as having lost its events, which sends it to a repair pass or its lane to the
+// exact fallback
+__device__ __forceinline__ void mark_lost(const ChunkTables& T, const int seg) {
+    T.seg_in[seg] = make_int2(0, -1);
+    T.seg_out[seg] = make_int2(0, -1);
+    T.seg_count[seg] = SEG_LOST;
+}
 
 __device__ __forceinline__ int64_t chunk_begin(int64_t N, int c, int K) {
     if (c >= K) return N;
@@ -106,8 +153,8 @@ __device__ __forceinline__ bool chunk_scan_item(const ChunkScanArgs& A, const b2
     if (REPAIR) {
         const unsigned oc = A.seg_count[seg];
         const int2 oin = A.seg_in[seg];
-        old_ok = oc != 0xffffffffu;     // (a chunk whose events were dropped has no chain to splice)
-        old_left = old_ok ? oc : 0u;
+        old_ok = oc != SEG_LOST;     // (a chunk whose events were dropped has no chain to splice)
+        old_left = seg_records(oc);
         old_block = A.seg_first[seg];
         old_pos = oin.x; old_ebar = oin.x != 0 ? oin.y : -1;
     }
@@ -116,15 +163,8 @@ __device__ __forceinline__ bool chunk_scan_item(const ChunkScanArgs& A, const b2
     int cur_block = -1, fill = CK_BLOCK, dead = 0;
     auto flush = [&](int cnt) {
         if (fill == CK_BLOCK && !dead) {
-            int b = 0;
-            if (lane == 0) {
-                b = (int)atomicAdd(A.alloc, 1u);
-                if (b >= A.pool_blocks) { atomicExch(A.overflow, 1); b = -1; }
-                else {
-                    A.next[b] = -1;
-                    if (cur_block < 0) A.seg_first[seg] = b; else A.next[cur_block] = b;
-                }
-            }
+            int b = cur_block;
+            if (lane == 0 && !pool_take_block(A, seg, b)) b = -1;
             b = __shfl_sync(FULL, b, 0);
             if (b < 0) dead = 1; else { cur_block = b; fill = 0; }
         }
@@ -250,7 +290,7 @@ __device__ __forceinline__ bool chunk_scan_item(const ChunkScanArgs& A, const b2
     }
     __syncwarp();
     while (m.qhead != qtail) flush((int)min(32u, m.qhead - qtail));
-    if (lane == 0) A.seg_count[seg] = dead ? 0xffffffffu : m.qhead;
+    if (lane == 0) A.seg_count[seg] = dead ? SEG_LOST : m.qhead;
     __syncwarp();
     return spliced;      // REPAIR: the chunk's recorded end state stands
 }
@@ -292,7 +332,7 @@ chunk_repair_kernel(const ChunkScanArgs A, unsigned* __restrict__ work) {
         if (item.chunk == 0) continue;
         const int seg = sym * A.n_seg + item.segment;
         const int2 a = A.seg_in[seg], z = A.seg_out[seg - 1];
-        if ((a.x != z.x || a.y != z.y) && A.seg_count[seg - 1] != 0xffffffffu) chunk_scan_item<VEC16, true>(A, item, sym, ws);
+        if ((a.x != z.x || a.y != z.y) && A.seg_count[seg - 1] != SEG_LOST) chunk_scan_item<VEC16, true>(A, item, sym, ws);
     }
 }
 
@@ -318,7 +358,7 @@ lane_repair_kernel(const ChunkScanArgs A, const int pop, const int32_t* __restri
         const int sb = seg_base[ind];
         const int base = sym * A.n_seg + sb;
         int2 prev = A.seg_out[base];
-        bool usable = A.seg_count[base] != 0xffffffffu;      // (a chunk that lost events to a full pool ends the walk: the lane is flagged later)
+        bool usable = A.seg_count[base] != SEG_LOST;      // (a chunk that lost events to a full pool ends the walk: the lane is flagged later)
         for (int c = 1; c < K && usable; ++c) {
             const int2 a = A.seg_in[base + c];
             if (a.x != prev.x || a.y != prev.y) {
@@ -328,7 +368,7 @@ lane_repair_kernel(const ChunkScanArgs A, const int pop, const int32_t* __restri
                 chunk_scan_item<VEC16, true>(A, item, sym, ws);      // (ends with a __syncwarp: its stores are visible to the warp)
             }
             prev = A.seg_out[base + c];
-            usable = A.seg_count[base + c] != 0xffffffffu;
+            usable = A.seg_count[base + c] != SEG_LOST;
         }
     }
 }
@@ -388,17 +428,15 @@ zone_map_kernel(const float* __restrict__ price, int64_t ld_price, const float* 
     }
 }
 
-struct LaneScanArgs {
+struct LaneScanArgs : ChunkTables {
     const float* price; int64_t ld_price;
     const float* rsi; int64_t ld_rsi;
     const float2* zones; int64_t n_zone_blocks;   // zone map (coarse part; n_zone_blocks = its row stride) or NULL
     const float2* fine; int64_t n_fine;           // 4-bar ranges and their row stride
     int P, S; int64_t N;
     const b200bt_individual* indiv; const int32_t* slots; int n_slots; int pop; int K; int warm;
-    uint2* pool; int pool_blocks; int* next; unsigned* alloc;
-    int* seg_first; unsigned* seg_count; int2* seg_in; int2* seg_out; int* overflow;
-    unsigned* work;      // work-item counter of the persistent scan (zero at launch)
-    int* stalls;         // [0] tiles that did not arrive in time (their items go to the exact fallback), [1..8] the first one's details
+    unsigned* work;          // &SweepCounters::scan_work
+    SweepCounters* ctr;      // (stalls, stall)
     long long wait_cycles;   // bound of a tile wait in SM clocks (LS_WAIT_CYCLES; b200bt_sweep_scan_wait_cycles overrides, for tests)
 };
 
@@ -420,7 +458,7 @@ __global__ void lane_tables_kernel(int pop, int K, const int32_t* __restrict__ o
 }
 
 #ifndef B200BT_LS_MIN_BLOCKS
-#define B200BT_LS_MIN_BLOCKS 3      // 85 registers: at 4 CTAs/SM (64) the scan loop spilled 18 words and ran 3 % slower
+#define B200BT_LS_MIN_BLOCKS 3      // 80 registers, 4 / 28 B spilled without / with zones (nvcc 12.9); at 4 CTAs/SM (64) 3 % slower
 #endif
 #ifndef B200BT_LS_STAGES
 #define B200BT_LS_STAGES 2
@@ -447,16 +485,11 @@ static_assert(LS_ZONE == ZONE_BLOCK && LS_T == ZONE_TILE, "zone map layout (comm
 // One work item: the 32 machines of warp-slot `wslot` (thread slots wslot * 32 ...) on symbol `sym`, chunk `c`.
 constexpr long long LS_WAIT_CYCLES = 40ll * 1000 * 1000;     // ~20 ms at 1.9 GHz; a tile normally lands within microseconds
 
-// the 32 machines of (warp-slot, symbol, chunk) are not scanned: their chunk is marked as having lost its events, which sends
-// the chunk to the repair pass or the lane to the exact fallback
+// the 32 machines of (warp-slot, symbol, chunk) are not scanned: their chunks are marked lost
 __device__ __forceinline__ void lane_scan_give_up(const LaneScanArgs& A, const int wslot, const int sym, const int c) {
     const int k = wslot * 32 + (int)(threadIdx.x & 31);
     const int slot = k < A.n_slots ? (A.slots ? A.slots[k] : (k < A.pop ? k : -1)) : -1;
-    if (slot < 0) return;
-    const int seg = sym * (A.pop * A.K) + slot * A.K + c;
-    A.seg_in[seg] = make_int2(0, -1);
-    A.seg_out[seg] = make_int2(0, -1);
-    A.seg_count[seg] = 0xffffffffu;
+    if (slot >= 0) mark_lost(A, sym * (A.pop * A.K) + slot * A.K + c);
 }
 
 // -> false: a tile of this item did not arrive (see the wait below); the warp must not take another item
@@ -509,11 +542,7 @@ __device__ __forceinline__ bool lane_scan_item(const LaneScanArgs& A, const bool
     const int my_row = 1 + __popc(heads & ((1u << leader) - 1u));       // staged row this machine reads
     if (n_rsi > LS_RSI_ROWS) {
         // not packed for this schedule: the lanes are flagged and re-run by the caller's exact fallback (fused kernel)
-        if (active) {
-            A.seg_in[seg] = make_int2(0, -1);
-            A.seg_out[seg] = make_int2(0, -1);
-            A.seg_count[seg] = 0xffffffffu;
-        }
+        if (active) mark_lost(A, seg);
         return true;
     }
     // lane L <= n_rsi issues the copies of staged row L (0 = price)
@@ -576,6 +605,14 @@ __device__ __forceinline__ bool lane_scan_item(const LaneScanArgs& A, const bool
     unsigned count = 0;
     bool rec = false, dead = false;
     uint2* wptr = A.pool;
+    auto record = [&](unsigned word, float p) {
+        if (fill == CK_BLOCK && !dead) {
+            if (!pool_take_block(A, seg, cur_block)) dead = true;
+            else { fill = 0; wptr = A.pool + (int64_t)cur_block * CK_BLOCK; }
+        }
+        if (!dead) { *wptr++ = make_uint2(word, __float_as_uint(p)); ++fill; }
+        ++count;
+    };
 
     // one bar of the state machine; same decisions as scan_window (sweep_dev.cuh).  Written as straight-line
     // selects: the threads of a warp that fire on the same bar (entries and exits alike) share one pass.
@@ -606,20 +643,7 @@ __device__ __forceinline__ bool lane_scan_item(const LaneScanArgs& A, const bool
         plo = flat ? p * mc[LS_THREADS] : -INFINITY;
         e_px = flat ? p : e_px;
         entry_bar = flat ? t : entry_bar;
-        if (rec) {
-            if (fill == CK_BLOCK && !dead) {
-                const int b = (int)atomicAdd(A.alloc, 1u);
-                if (b >= A.pool_blocks) { atomicExch(A.overflow, 1); dead = true; }
-                else {
-                    A.next[b] = -1;
-                    if (cur_block < 0) A.seg_first[seg] = b; else A.next[cur_block] = b;
-                    cur_block = b; fill = 0;
-                    wptr = A.pool + (int64_t)b * CK_BLOCK;
-                }
-            }
-            if (!dead) { *wptr++ = make_uint2(word, __float_as_uint(p)); ++fill; }
-            ++count;
-        }
+        if (rec) record(word, p);
     };
 
     int stage = ring_stage;
@@ -634,9 +658,10 @@ __device__ __forceinline__ bool lane_scan_item(const LaneScanArgs& A, const bool
                                             : !mbar_wait_bounded(&full[stage], parity, A.wait_cycles);
         if (__any_sync(FULL, lost)) {
             lane_scan_give_up(A, wslot, sym, c);
-            if (lane == 0 && A.stalls && atomicAdd(A.stalls, 1) == 0) {
-                A.stalls[1] = (int)blockIdx.x; A.stalls[2] = (int)(threadIdx.x >> 5); A.stalls[3] = wslot * 65536 + sym * 256 + c;
-                A.stalls[4] = it; A.stalls[5] = n_tiles; A.stalls[6] = stage * 2 + (int)parity; A.stalls[7] = tl_begin; A.stalls[8] = n_rsi;
+            if (lane == 0 && atomicAdd(&A.ctr->stalls, 1) == 0) {
+                int* const d = A.ctr->stall;
+                d[0] = (int)blockIdx.x; d[1] = (int)(threadIdx.x >> 5); d[2] = wslot * 65536 + sym * 256 + c;
+                d[3] = it; d[4] = n_tiles; d[5] = stage * 2 + (int)parity; d[6] = tl_begin; d[7] = n_rsi;
             }
             return false;
         }
@@ -691,23 +716,9 @@ __device__ __forceinline__ bool lane_scan_item(const LaneScanArgs& A, const bool
     ring_parity = parity;
     if (!active) return true;
     A.seg_out[seg] = make_int2(pos, pos != 0 ? entry_bar : -1);
-    if (c == A.K - 1 && pos != 0)   // force-close at the last bar (:849-876)
-    {
-        rec = true;   // (the last chunk always records: T0 < N)
-        const unsigned word = (unsigned)(n - 1) | B200BT_EVENT_EXIT | (pos > 0 ? B200BT_EVENT_SELL : 0u);
-        if (fill == CK_BLOCK && !dead) {
-            const int b = (int)atomicAdd(A.alloc, 1u);
-            if (b >= A.pool_blocks) { atomicExch(A.overflow, 1); dead = true; }
-            else {
-                A.next[b] = -1;
-                if (cur_block < 0) A.seg_first[seg] = b; else A.next[cur_block] = b;
-                wptr = A.pool + (int64_t)b * CK_BLOCK;
-            }
-        }
-        if (!dead) *wptr = make_uint2(word, __float_as_uint(__ldg(A.price + (int64_t)sym * A.ld_price + (n - 1))));
-        ++count;
-    }
-    A.seg_count[seg] = dead ? 0xffffffffu : count;
+    if (c == A.K - 1 && pos != 0)   // force-close at the last bar (:849-876; the last chunk always records: T0 < N)
+        record((unsigned)(n - 1) | B200BT_EVENT_EXIT | (pos > 0 ? B200BT_EVENT_SELL : 0u), __ldg(A.price + (int64_t)sym * A.ld_price + (n - 1)));
+    A.seg_count[seg] = dead ? SEG_LOST : count;
     return true;
 }
 
@@ -778,13 +789,69 @@ struct ChunkPartial {
 };
 static_assert(sizeof(ChunkPartial) == 160, "ChunkPartial layout");
 
-// entry record a chunk's first exit is priced against, from the chunk's (verified) start state
-__device__ __forceinline__ void chunk_carry(const int2 in, const float* __restrict__ pr, unsigned& w_carry, float& p_carry) {
-    w_carry = 0u; p_carry = 0.f;
+// One step of walk_records, per lane: records 2 lane and 2 lane + 1 of the step (a0 / a1: they exist), priced.
+struct RecordPair {
+    int cnt;                             // records in the step (<= 64)
+    bool a0, a1;
+    unsigned w0, w1; float pf0, pf1;     // event words, prices
+    double pnl0, pnl1, s2, eq0, eq1;     // PnL of each record (0 for an entry), pnl0 + pnl1, equity after each record
+    int dur0, dur1;
+};
+
+// The records of chunk `seg` in time order, 64 per step, two per lane (one 16-byte load): every record is priced against
+// the one before it (the first against the entry the chunk's verified start state holds), the equity runs on from `equity`
+// by an inclusive warp scan, and body(pair, step's PnL sum) consumes the step.  -> the chunk's record count (0: lost).
+template <class Body>
+__device__ __forceinline__ unsigned walk_records(const uint2* __restrict__ pool, const int* __restrict__ next, const int pool_blocks,
+                                                 const int* __restrict__ seg_first, const unsigned* __restrict__ seg_count,
+                                                 const int2* __restrict__ seg_in, const float* __restrict__ pr, const int seg,
+                                                 const double size, double& equity, Body&& body) {
+    const int lane = threadIdx.x & 31;
+    const double fee1 = __dmul_rn(size, 0.001), fee2 = __dmul_rn(size, 0.002);
+    const unsigned count = seg_records(seg_count[seg]);
+    unsigned left = count;
+    const int2 in = seg_in[seg];
+    unsigned w_carry = 0u;
+    float p_carry = 0.f;
     if (in.x != 0) {
         w_carry = (unsigned)in.y | (in.x < 0 ? B200BT_EVENT_SELL : 0u);
         p_carry = __ldg(pr + in.y);
     }
+    int b = left ? seg_first[seg] : -1, off = 0;
+    if ((unsigned)b >= (unsigned)pool_blocks) left = 0;
+    while (left) {
+        RecordPair r;
+        r.cnt = (int)min(64u, left);
+        r.a0 = 2 * lane < r.cnt; r.a1 = 2 * lane + 1 < r.cnt;
+        uint4 ev = make_uint4(0u, 0u, 0u, 0u);
+        if (r.a0) ev = *reinterpret_cast<const uint4*>(pool + (int64_t)b * CK_BLOCK + off + 2 * lane);
+        r.w0 = ev.x; r.w1 = ev.z;
+        r.pf0 = __uint_as_float(ev.y); r.pf1 = __uint_as_float(ev.w);
+        float p_prev = __shfl_up_sync(FULL, r.pf1, 1);
+        unsigned w_prev = __shfl_up_sync(FULL, r.w1, 1);
+        if (lane == 0) { p_prev = p_carry; w_prev = w_carry; }
+        r.pnl0 = record_pnl(r.a0, r.w0, r.pf0, w_prev, p_prev, size, fee1, fee2, r.dur0);
+        r.pnl1 = record_pnl(r.a1, r.w1, r.pf1, r.w0, r.pf0, size, fee1, fee2, r.dur1);
+        r.s2 = r.pnl0 + r.pnl1;
+        double cs = r.s2;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const double up = shfl_up_d(cs, d);
+            if (lane >= d) cs += up;
+        }
+        r.eq0 = equity + (cs - r.s2) + r.pnl0;
+        r.eq1 = equity + cs;
+        const double step_sum = shfl_d(cs, 31);
+        equity += step_sum;
+        body(r, step_sum);
+        const int last = (r.cnt - 1) >> 1;
+        w_carry = __shfl_sync(FULL, (r.cnt & 1) ? r.w0 : r.w1, last);
+        p_carry = __shfl_sync(FULL, (r.cnt & 1) ? r.pf0 : r.pf1, last);
+        left -= r.cnt;
+        off += 64;
+        if (off == CK_BLOCK && left) { b = next[b]; off = 0; if ((unsigned)b >= (unsigned)pool_blocks) break; }
+    }
+    return count;
 }
 
 #ifndef B200BT_M2_MIN_BLOCKS
@@ -811,15 +878,11 @@ chunk_partial_kernel(const float* __restrict__ price, int64_t ld_price, const b2
     unsigned first_index = 0;
     for (int c0 = 0; c0 < item.chunk; c0 += 32) {
         const int c = c0 + lane;
-        unsigned n = c < item.chunk ? seg_count[base + c] : 0u;
-        if (n == 0xffffffffu) n = 0;
-        first_index += __reduce_add_sync(FULL, n);
+        first_index += __reduce_add_sync(FULL, c < item.chunk ? seg_records(seg_count[base + c]) : 0u);
     }
 
     // Order-dependent state (equity relative to the chunk's start, calendar day) is warp-uniform and lives in registers;
     // what is a plain sum / max / min / xor over the records is accumulated PER LANE and reduced once at the end of the chunk.
-    const double size = iv.position_size;
-    const double fee1 = __dmul_rn(size, 0.001), fee2 = __dmul_rn(size, 0.002);
     double equity = 0.0, l_top = -INFINITY, l_bottom = INFINITY;
     DayAcc da{0.0, 0.0, 0.0, 0u, 0};
     int day_valid = 0, day_cur = 0, first_done = 0, first_id = 0;
@@ -841,32 +904,18 @@ chunk_partial_kernel(const float* __restrict__ price, int64_t ld_price, const b2
         else day_complete(da, x);
     };
 
-    unsigned left = seg_count[seg];
-    if (left == 0xffffffffu) left = 0;
-    const unsigned count = left;
-    unsigned w_carry; float p_carry;
-    chunk_carry(seg_in[seg], price + (int64_t)sym * ld_price, w_carry, p_carry);
-    int b = left ? seg_first[seg] : -1, off = 0;
-    if ((unsigned)b >= (unsigned)pool_blocks) left = 0;
-    // 64 records per step, two consecutive ones per lane (record 2l and 2l+1 of the step: one 16-byte load)
-    while (left) {
-        const int cnt = (int)min(64u, left);
-        const bool a0 = 2 * lane < cnt, a1 = 2 * lane + 1 < cnt;
-        uint4 ev = make_uint4(0u, 0u, 0u, 0u);
-        if (a0) ev = *reinterpret_cast<const uint4*>(pool + (int64_t)b * CK_BLOCK + off + 2 * lane);
-        const unsigned w0 = ev.x, w1 = ev.z;
-        const float pf0 = __uint_as_float(ev.y), pf1 = __uint_as_float(ev.w);
-        float p_prev = __shfl_up_sync(FULL, pf1, 1);
-        unsigned w_prev = __shfl_up_sync(FULL, w1, 1);
-        if (lane == 0) { p_prev = p_carry; w_prev = w_carry; }
-        int dur0, dur1;
-        const double pnl0 = record_pnl(a0, w0, pf0, w_prev, p_prev, size, fee1, fee2, dur0);
-        const double pnl1 = record_pnl(a1, w1, pf1, w0, pf0, size, fee1, fee2, dur1);
+    // equity relative to the chunk's start
+    const unsigned count = walk_records(pool, next, pool_blocks, seg_first, seg_count, seg_in, price + (int64_t)sym * ld_price, seg,
+                                        iv.position_size, equity, [&](const RecordPair& r, const double batch_sum) {
+        const int cnt = r.cnt;
+        const bool a0 = r.a0, a1 = r.a1;
+        const unsigned w0 = r.w0, w1 = r.w1;
+        const double pnl0 = r.pnl0, pnl1 = r.pnl1, s2 = r.s2;
         if (pnl0 > 0.0) { l_gain += pnl0; ++l_win; l_maxp = fmax(l_maxp, pnl0); }
         else if (pnl0 < 0.0) { l_loss += pnl0; ++l_los; l_minl = fmin(l_minl, pnl0); }
         if (pnl1 > 0.0) { l_gain += pnl1; ++l_win; l_maxp = fmax(l_maxp, pnl1); }
         else if (pnl1 < 0.0) { l_loss += pnl1; ++l_los; l_minl = fmin(l_minl, pnl1); }
-        l_dur += dur0 + dur1;
+        l_dur += r.dur0 + r.dur1;
         const unsigned i0 = index + 2 * lane;
         if (a0) {
             l_hash ^= event_hash(i0, w0);
@@ -876,20 +925,8 @@ chunk_partial_kernel(const float* __restrict__ price, int64_t ld_price, const b2
             l_hash ^= event_hash(i0 + 1, w1);
             if (ev_out && (int64_t)i0 + 1 < ev_cap) ev_out[i0 + 1] = w1;
         }
-
-        // equity relative to the chunk's start: inclusive scan of the lane sums; its extremes per lane
-        const double s2 = pnl0 + pnl1;
-        double cs = s2;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-            const double up = shfl_up_d(cs, d);
-            if (lane >= d) cs += up;
-        }
-        const double eq0 = equity + (cs - s2) + pnl0, eq1 = equity + cs;
-        if (a0) { l_top = fmax(l_top, eq0); l_bottom = fmin(l_bottom, eq0); }
-        if (a1) { l_top = fmax(l_top, eq1); l_bottom = fmin(l_bottom, eq1); }
-        const double batch_sum = shfl_d(cs, 31);
-        equity += batch_sum;
+        if (a0) { l_top = fmax(l_top, r.eq0); l_bottom = fmin(l_bottom, r.eq0); }
+        if (a1) { l_top = fmax(l_top, r.eq1); l_bottom = fmin(l_bottom, r.eq1); }
 
         // calendar-day buckets
         const int last_lane = (cnt - 1) >> 1;
@@ -938,14 +975,8 @@ chunk_partial_kernel(const float* __restrict__ price, int64_t ld_price, const b2
         }
         day_cur = last_day;
         day_valid = 1;
-
         index += cnt;
-        w_carry = __shfl_sync(FULL, (cnt & 1) ? w0 : w1, last_lane);
-        p_carry = __shfl_sync(FULL, (cnt & 1) ? pf0 : pf1, last_lane);
-        left -= cnt;
-        off += 64;
-        if (off == CK_BLOCK && left) { b = next[b]; off = 0; if ((unsigned)b >= (unsigned)pool_blocks) break; }
-    }
+    });
     // per-lane accumulators -> chunk totals
     const double tot_profit = warp_sum_d(l_gain), tot_loss = warp_sum_d(l_loss);
     const double largest_p = warp_max_d(l_maxp), largest_l = warp_min_d(l_minl);
@@ -1015,35 +1046,11 @@ chunk_peak_kernel(const float* __restrict__ price, int64_t ld_price, const b200b
     for (unsigned i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n; i += warps) {
         const int4 pk = peaks[i];
         const int seg = pk.x;
-        const double size = indiv[pk.y].position_size;
-        const double fee1 = __dmul_rn(size, 0.001), fee2 = __dmul_rn(size, 0.002);
-        unsigned left = seg_count[seg];
-        if (left == 0xffffffffu) left = 0;
-        unsigned w_carry; float p_carry;
-        chunk_carry(seg_in[seg], price + (int64_t)pk.z * ld_price, w_carry, p_carry);
-        int b = left ? seg_first[seg] : -1, off = 0;
-        if ((unsigned)b >= (unsigned)pool_blocks) left = 0;
         double equity = seg_e0[seg], peak = seg_p0[seg], maxdd = 0.0;
-        while (left) {
-            const int cnt = (int)min(64u, left);
-            const bool a0 = 2 * lane < cnt, a1 = 2 * lane + 1 < cnt;
-            uint4 ev = make_uint4(0u, 0u, 0u, 0u);
-            if (a0) ev = *reinterpret_cast<const uint4*>(pool + (int64_t)b * CK_BLOCK + off + 2 * lane);
-            const float pf0 = __uint_as_float(ev.y), pf1 = __uint_as_float(ev.w);
-            float p_prev = __shfl_up_sync(FULL, pf1, 1);
-            unsigned w_prev = __shfl_up_sync(FULL, ev.z, 1);
-            if (lane == 0) { p_prev = p_carry; w_prev = w_carry; }
-            int dur;
-            const double pnl0 = record_pnl(a0, ev.x, pf0, w_prev, p_prev, size, fee1, fee2, dur);
-            const double pnl1 = record_pnl(a1, ev.z, pf1, ev.x, pf0, size, fee1, fee2, dur);
-            const double s2 = pnl0 + pnl1;
-            double cs = s2;
-#pragma unroll
-            for (int d = 1; d < 32; d <<= 1) {
-                const double up = shfl_up_d(cs, d);
-                if (lane >= d) cs += up;
-            }
-            const double eq0 = equity + (cs - s2) + pnl0, eq1 = equity + cs;
+        walk_records(pool, next, pool_blocks, seg_first, seg_count, seg_in, price + (int64_t)pk.z * ld_price, seg,
+                     indiv[pk.y].position_size, equity, [&](const RecordPair& r, double) {
+            const bool a0 = r.a0, a1 = r.a1;
+            const double eq0 = r.eq0, eq1 = r.eq1;
             const double m2 = fmax(a0 ? eq0 : -INFINITY, a1 ? eq1 : -INFINITY);
             double pk0 = peak, pk1 = peak;
             if (__any_sync(FULL, m2 > peak)) {
@@ -1059,21 +1066,12 @@ chunk_peak_kernel(const float* __restrict__ price, int64_t ld_price, const b200b
                 pk1 = fmax(pk0, eq1);
                 peak = fmax(peak, shfl_d(p, 31));
             }
-            {
-                const double gap0 = __dsub_rn(pk0, eq0), gap1 = __dsub_rn(pk1, eq1);
-                const double lim = maxdd * (1.0 - 1e-12);
-                const bool c0 = a0 && gap0 > 0.0 && gap0 >= lim * pk0, c1 = a1 && gap1 > 0.0 && gap1 >= lim * pk1;
-                if (__any_sync(FULL, c0 || c1))
-                    maxdd = fmax(maxdd, warp_max_d(fmax(c0 ? __ddiv_rn(gap0, pk0) : 0.0, c1 ? __ddiv_rn(gap1, pk1) : 0.0)));
-            }
-            equity += shfl_d(cs, 31);
-            const int last = (cnt - 1) >> 1;
-            w_carry = __shfl_sync(FULL, (cnt & 1) ? ev.x : ev.z, last);
-            p_carry = __shfl_sync(FULL, (cnt & 1) ? pf0 : pf1, last);
-            left -= cnt;
-            off += 64;
-            if (off == CK_BLOCK && left) { b = next[b]; off = 0; if ((unsigned)b >= (unsigned)pool_blocks) break; }
-        }
+            const double gap0 = __dsub_rn(pk0, eq0), gap1 = __dsub_rn(pk1, eq1);
+            const double lim = maxdd * (1.0 - 1e-12);
+            const bool c0 = a0 && gap0 > 0.0 && gap0 >= lim * pk0, c1 = a1 && gap1 > 0.0 && gap1 >= lim * pk1;
+            if (__any_sync(FULL, c0 || c1))
+                maxdd = fmax(maxdd, warp_max_d(fmax(c0 ? __ddiv_rn(gap0, pk0) : 0.0, c1 ? __ddiv_rn(gap1, pk1) : 0.0)));
+        });
         if (lane == 0) partial[seg].maxdd = maxdd;
     }
 }
@@ -1120,7 +1118,7 @@ __global__ void lane_combine_kernel(const b200bt_individual* __restrict__ indiv,
             const int2 z = seg_out[base + c - 1];
             ok = ok && (a.x == z.x) && (a.y == z.y);
         }
-        ok = ok && (seg_count[base + c] != 0xffffffffu);
+        ok = ok && (seg_count[base + c] != SEG_LOST);
     }
     invalid[t] = ok ? 0 : 1;
     if (!ok) return;
@@ -1184,43 +1182,75 @@ using namespace b200bt;
 
 namespace {
 
-constexpr int REPAIR_COUNTERS = 130;   // work counters: [0] bounded repair pass, [1] overlapped pass, [2] listed peak chunks, [last] the scan; 2 + REPAIR_COUNTERS a multiple of 4 (alignment)
-struct ChunkWorkspace {
-    uint2* pool; int2* seg_in; int2* seg_out; int* seg_first; unsigned* seg_count; unsigned* alloc; int* overflow;
-    unsigned* n_repair; int4* repair; int* next; ChunkPartial* partial; double* seg_sum; double* seg_max;
-    b200bt_chunk_item* fix_items; int* n_fix; unsigned char* redo;   // overlapped repair tail (n_seg items, pop flags)
-    unsigned char* end;
+// The sweep workspace: byte offsets of its sections, each 16-byte aligned (so must the base be), and its size.  segs =
+// S x n_seg chunks; `tables`: b200bt_sweep_tiled's work items, seg_base and n_chunks of its uniform chunks.  The sections
+// in front of `cleared` are zeroed at the start of every sweep.
+struct ChunkLayout {
+    int64_t seg_in, seg_out, seg_first, seg_count, counters, redo, cleared;
+    int64_t pool, next, peaks, partial, seg_sum, seg_max, fix_items, items, seg_base, n_chunks, bytes;
 };
 
-// pool[pool_blocks][256] uint2 | seg_in[segs] int2 | seg_out[segs] int2 | seg_first[segs] | seg_count[segs] |
-// alloc, overflow, n_repair[REPAIR_COUNTERS] (work counters) | repair[segs] int4 (chunks that set a new equity peak) | next[pool_blocks] | (16-byte aligned) partial[segs] (160 B) |
-// seg_sum[segs] | seg_max[segs] | fix_items[n_seg] (16 B) | n_fix (16 B) | redo[pop]
-// (wide types first: the base must be 16-byte aligned)
-ChunkWorkspace carve(void* workspace, int pool_blocks, int64_t segs, int n_seg, int pop) {
+ChunkLayout chunk_layout(int pool_blocks, int64_t segs, int n_seg, int pop, bool tables) {
+    ChunkLayout L;
+    int64_t at = 0;
+    auto section = [&](int64_t bytes) { const int64_t o = at; at += (bytes + 15) & ~(int64_t)15; return o; };
+    L.seg_in = section(segs * sizeof(int2));
+    L.seg_out = section(segs * sizeof(int2));
+    L.seg_first = section(segs * sizeof(int));
+    L.seg_count = section(segs * sizeof(unsigned));
+    L.counters = section(sizeof(SweepCounters));
+    L.redo = section(pop);                                            // individuals the overlapped repair touched
+    L.cleared = at;
+    L.pool = section((int64_t)pool_blocks * CK_BLOCK * sizeof(uint2));
+    L.next = section((int64_t)pool_blocks * sizeof(int));
+    L.peaks = section(segs * sizeof(int4));                           // chunks that set a new equity peak
+    L.partial = section(segs * sizeof(ChunkPartial));
+    L.seg_sum = section(segs * sizeof(double));
+    L.seg_max = section(segs * sizeof(double));
+    L.fix_items = section((int64_t)n_seg * sizeof(b200bt_chunk_item));   // fix-up items, then the exact fallback's list
+    L.items = section(tables ? (int64_t)n_seg * sizeof(b200bt_chunk_item) : 0);
+    L.seg_base = section(tables ? (int64_t)pop * sizeof(int32_t) : 0);
+    L.n_chunks = section(tables ? (int64_t)pop * sizeof(int32_t) : 0);
+    L.bytes = at;
+    return L;
+}
+
+struct ChunkWorkspace : ChunkTables {
+    SweepCounters* ctr; int4* peaks; ChunkPartial* partial; double* seg_sum; double* seg_max;
+    b200bt_chunk_item* fix_items; unsigned char* redo;
+    b200bt_chunk_item* items; int32_t* seg_base; int32_t* n_chunks;
+};
+
+ChunkWorkspace carve(void* workspace, const ChunkLayout& L, int pool_blocks) {
+    unsigned char* const at = (unsigned char*)workspace;
     ChunkWorkspace w;
-    w.pool = (uint2*)workspace;
-    w.seg_in = (int2*)(w.pool + (int64_t)pool_blocks * CK_BLOCK);
-    w.seg_out = w.seg_in + segs;
-    w.seg_first = (int*)(w.seg_out + segs);
-    w.seg_count = (unsigned*)(w.seg_first + segs);
-    w.alloc = w.seg_count + segs;
-    w.overflow = (int*)(w.alloc + 1);
-    w.n_repair = (unsigned*)(w.overflow + 1);
-    w.repair = (int4*)(((uintptr_t)(w.n_repair + REPAIR_COUNTERS) + 15) & ~(uintptr_t)15);
-    w.next = (int*)(w.repair + segs);
-    w.partial = (ChunkPartial*)(((uintptr_t)(w.next + pool_blocks) + 15) & ~(uintptr_t)15);
-    w.seg_sum = (double*)(w.partial + segs);
-    w.seg_max = w.seg_sum + segs;
-    w.fix_items = (b200bt_chunk_item*)(w.seg_max + segs);
-    w.n_fix = (int*)(w.fix_items + n_seg);
-    w.redo = (unsigned char*)(w.n_fix + 4);
-    w.end = w.redo + ((pop + 15) & ~15);
+    w.pool = (uint2*)(at + L.pool); w.pool_blocks = pool_blocks; w.next = (int*)(at + L.next);
+    w.seg_first = (int*)(at + L.seg_first); w.seg_count = (unsigned*)(at + L.seg_count);
+    w.seg_in = (int2*)(at + L.seg_in); w.seg_out = (int2*)(at + L.seg_out);
+    w.ctr = (SweepCounters*)(at + L.counters);
+    w.alloc = &w.ctr->alloc; w.overflow = &w.ctr->overflow;
+    w.peaks = (int4*)(at + L.peaks); w.partial = (ChunkPartial*)(at + L.partial);
+    w.seg_sum = (double*)(at + L.seg_sum); w.seg_max = (double*)(at + L.seg_max);
+    w.fix_items = (b200bt_chunk_item*)(at + L.fix_items); w.redo = at + L.redo;
+    w.items = (b200bt_chunk_item*)(at + L.items); w.seg_base = (int32_t*)(at + L.seg_base); w.n_chunks = (int32_t*)(at + L.n_chunks);
     return w;
 }
 
-int64_t chunk_workspace_bytes(int pool_blocks, int64_t segs, int n_seg, int pop) {
-    return (int64_t)pool_blocks * CK_BLOCK * 8 + segs * 16 + (segs * 2 + 2 + REPAIR_COUNTERS) * 4 + 16 + segs * 16 + (int64_t)pool_blocks * 4 + 16 +
-           segs * (int64_t)(sizeof(ChunkPartial) + 16) + (int64_t)n_seg * 16 + 16 + ((pop + 15) & ~15);
+// price and RSI rows that allow 16-byte copies
+bool vec16_rows(const float* price, int64_t ld_price, const float* rsi, int64_t ld_rsi) {
+    return (((uintptr_t)price | (uintptr_t)rsi) & 15) == 0 && ld_price % 4 == 0 && ld_rsi % 4 == 0;
+}
+
+// arguments of the warp-per-chunk scan and of the repair and metrics kernels both schedules share
+ChunkScanArgs scan_args(const float* price, int64_t ld_price, const float* rsi, int64_t ld_rsi, int P, int S, int64_t N,
+                        const b200bt_individual* indiv, const b200bt_chunk_item* items, int n_items, int n_seg,
+                        const int32_t* n_chunks, int warm, const ChunkWorkspace& w) {
+    ChunkScanArgs A;
+    static_cast<ChunkTables&>(A) = w;
+    A.price = price; A.ld_price = ld_price; A.rsi = rsi; A.ld_rsi = ld_rsi; A.P = P; A.S = S; A.N = N;
+    A.indiv = indiv; A.items = items; A.n_items = n_items; A.n_seg = n_seg; A.warm = warm;
+    A.n_chunks = n_chunks; A.redo = nullptr;
+    return A;
 }
 
 // second stream + events for the overlapped repair tail, one set per device
@@ -1244,16 +1274,6 @@ int side_stream(SideStream** out) {
     return B200BT_OK;
 }
 
-// the bounded repair pass on the critical path can be switched off (B200BT_MAIN_REPAIR=0: everything in the overlapped pass)
-int main_repair_rounds() {
-    static int v = -1;
-    if (v < 0) {
-        const char* e = getenv("B200BT_MAIN_REPAIR");
-        v = e ? atoi(e) : 1;
-    }
-    return v;
-}
-
 // Everything after the speculative scan: verify + repair (lane_repair_kernel) -> chunk-parallel metrics.
 //
 // chunk_repair_kernel on the critical path makes almost every lane consistent; what it leaves is a handful of lanes whose
@@ -1261,12 +1281,11 @@ int main_repair_rounds() {
 // after chunk by a single warp each.  That is lane_repair_kernel, on another stream BESIDE the metrics kernels of all
 // lanes; the individuals it touches are flagged and only their metrics are recomputed afterwards.
 // max_repair_rounds: 0 = no repair (every inconsistent lane takes the exact fallback), 1 = chunk_repair_kernel only, >= 2 = both.
-int finish_chunks(const ChunkScanArgs& A, const ChunkWorkspace& w, const b200bt_chunk_item* items, int n_items,
-                  const int32_t* seg_base, int pop, int max_repair_rounds, const b200bt_sweep_config* cfg_host,
-                  b200bt_lane_stats* stats, uint32_t* events, int64_t event_cap, unsigned char* lane_invalid,
-                  int* overflow_host_or_null, cudaStream_t st) {
-    const int S = A.S, n_seg = A.n_seg;
-    const bool vec16 = (((uintptr_t)A.price | (uintptr_t)A.rsi) & 15) == 0 && A.ld_price % 4 == 0 && A.ld_rsi % 4 == 0;
+int finish_chunks(const ChunkScanArgs& A, const ChunkWorkspace& w, const bool vec16, const int32_t* seg_base, int pop,
+                  int max_repair_rounds, const b200bt_sweep_config* cfg_host, b200bt_lane_stats* stats, uint32_t* events,
+                  int64_t event_cap, unsigned char* lane_invalid, int* overflow_host_or_null, cudaStream_t st) {
+    const int S = A.S, n_seg = A.n_seg, n_items = A.n_items;
+    const b200bt_chunk_item* const items = A.items;
     auto kern_fix = vec16 ? chunk_repair_kernel<true> : chunk_repair_kernel<false>;
     auto kern_walk = vec16 ? lane_repair_kernel<true> : lane_repair_kernel<false>;
     const size_t smem = sizeof(WarpShared) * SW_WARPS;
@@ -1278,13 +1297,13 @@ int finish_chunks(const ChunkScanArgs& A, const ChunkWorkspace& w, const b200bt_
     B200BT_REQUIRE(mblocks < (1ll << 31), B200BT_ELIMIT, "sweep_chunked: too many work items");
     B200BT_REQUIRE(lanes < (1ll << 30), B200BT_ELIMIT, "sweep_chunked: too many lanes");
 
-    // Both repair kernels run a persistent grid (3 CTAs per SM) whose warps take work from a counter (n_repair[0], [1]).
+    // Both repair kernels run a persistent grid (3 CTAs per SM) whose warps take work from a counter.
     const unsigned repair_grid = 3u * (unsigned)device_sm_count();
     auto repair_pass = [&](cudaStream_t rs, int pass, unsigned char* redo) -> int {
         ChunkScanArgs R = A;
         R.redo = redo;
-        if (pass == 0) kern_fix<<<repair_grid, SW_WARPS * 32, smem, rs>>>(R, w.n_repair);
-        else kern_walk<<<repair_grid, SW_WARPS * 32, smem, rs>>>(R, pop, seg_base, w.n_repair + 1);
+        if (pass == 0) kern_fix<<<repair_grid, SW_WARPS * 32, smem, rs>>>(R, &w.ctr->chunk_repair_work);
+        else kern_walk<<<repair_grid, SW_WARPS * 32, smem, rs>>>(R, pop, seg_base, &w.ctr->lane_repair_work);
         B200BT_LAUNCH_CHECK("repair launch");
         return B200BT_OK;
     };
@@ -1298,12 +1317,9 @@ int finish_chunks(const ChunkScanArgs& A, const ChunkWorkspace& w, const b200bt_
     };
 
     int rc = B200BT_OK;
-    const bool main_pass = max_repair_rounds >= 1 && main_repair_rounds() != 0;
-    const bool tail = max_repair_rounds >= 2 || (max_repair_rounds >= 1 && !main_pass);
-    if (main_pass && (rc = repair_pass(st, 0, nullptr))) return rc;
+    const bool tail = max_repair_rounds >= 2;
+    if (max_repair_rounds >= 1 && (rc = repair_pass(st, 0, nullptr))) return rc;
     SideStream* side = nullptr;
-    e = cudaMemsetAsync(w.n_fix, 0, 16 + ((pop + 15) & ~15), st);   // n_fix, redo-list length, flagged lanes + redo flags
-    if (e != cudaSuccess) return cuda_status(e, "sweep_chunked: memset");
     if (tail) {
         if ((rc = side_stream(&side))) return rc;
         e = cudaEventRecord(side->fork, st);
@@ -1317,47 +1333,42 @@ int finish_chunks(const ChunkScanArgs& A, const ChunkWorkspace& w, const b200bt_
         e = cudaEventRecord(side->join, side->stream);
         if (e == cudaSuccess) e = cudaStreamWaitEvent(st, side->join, 0);
         if (e != cudaSuccess) return cuda_status(e, "sweep_chunked: join");
-        fix_items_kernel<<<(n_items + 255) / 256, 256, 0, st>>>(items, n_items, w.redo, w.fix_items, w.n_fix);
+        fix_items_kernel<<<(n_items + 255) / 256, 256, 0, st>>>(items, n_items, w.redo, w.fix_items, &w.ctr->n_fix_items);
         B200BT_LAUNCH_CHECK("fix_items launch");
-        if ((rc = metrics(w.fix_items, w.n_fix))) return rc;
+        if ((rc = metrics(w.fix_items, &w.ctr->n_fix_items))) return rc;
     }
     // drawdown: chunks below their inherited peak in closed form, the chunks that set a new peak record by record
-    // (n_repair[2] = number of those; a persistent grid walks the list)
+    // (a persistent grid walks their list)
     chunk_prefix_kernel<<<(unsigned)((lanes + 127) / 128), 128, 0, st>>>(pop, S, seg_base, A.n_chunks, n_seg, w.seg_sum, w.seg_max,
-                                                                        w.partial, cfg_host->initial_capital, w.repair, w.n_repair + 2);
+                                                                        w.partial, cfg_host->initial_capital, w.peaks,
+                                                                        &w.ctr->peak_chunks);
     B200BT_LAUNCH_CHECK("chunk_prefix launch");
     chunk_peak_kernel<<<8u * (unsigned)device_sm_count(), 128, 0, st>>>(A.price, A.ld_price, A.indiv, w.pool, w.next, w.seg_first,
-                                                                       w.seg_count, w.seg_in, w.seg_sum, w.seg_max, w.repair,
-                                                                       w.n_repair + 2, w.partial, A.pool_blocks);
+                                                                       w.seg_count, w.seg_in, w.seg_sum, w.seg_max, w.peaks,
+                                                                       &w.ctr->peak_chunks, w.partial, A.pool_blocks);
     B200BT_LAUNCH_CHECK("chunk_peak launch");
     lane_combine_kernel<<<(unsigned)((lanes + 127) / 128), 128, 0, st>>>(A.indiv, pop, S, seg_base, A.n_chunks, n_seg, w.seg_count,
                                                                         w.seg_in, w.seg_out, w.partial, *cfg_host, stats,
                                                                         lane_invalid);
     B200BT_LAUNCH_CHECK("lane_combine launch");
     // exact fallback, driven from the device: the flagged individuals are listed and re-evaluated by the fused (serial)
-    // kernel; with nothing flagged its warps leave at once.  [n_fix + 1] = list length, [n_fix + 2] = flagged lanes.
+    // kernel; with nothing flagged its warps leave at once.
     int32_t* redo_list = reinterpret_cast<int32_t*>(w.fix_items);      // (the fix-up item list is no longer needed)
-    redo_list_kernel<<<(pop + 127) / 128, 128, 0, st>>>(pop, S, lane_invalid, redo_list, w.n_fix + 1, w.n_fix + 2);
+    redo_list_kernel<<<(pop + 127) / 128, 128, 0, st>>>(pop, S, lane_invalid, redo_list, &w.ctr->n_redo, &w.ctr->fallback_lanes);
     B200BT_LAUNCH_CHECK("redo_list launch");
-    if ((rc = launch_sweep(A.price, A.ld_price, A.rsi, A.ld_rsi, A.P, S, A.N, A.indiv, redo_list, pop, w.n_fix + 1, cfg_host, stats,
-                           events, event_cap, st)))
+    if ((rc = launch_sweep(A.price, A.ld_price, A.rsi, A.ld_rsi, A.P, S, A.N, A.indiv, redo_list, pop, &w.ctr->n_redo, cfg_host,
+                           stats, events, event_cap, st)))
         return rc;
-    if (overflow_host_or_null) {
-        // [0] = the event pool overflowed, [1] = lanes that went through the fallback, [2] = pool blocks handed out, [3] = tiles
-        // of the thread-per-lane scan that did not arrive in time, [4] = chunks that set a new equity peak (read by the host
-        // after its next sync)
-        e = cudaMemcpyAsync(overflow_host_or_null, w.overflow, sizeof(int), cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(overflow_host_or_null + 1, w.n_fix + 2, sizeof(int), cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(overflow_host_or_null + 2, w.alloc, sizeof(int), cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(overflow_host_or_null + 3, w.n_repair + 64, sizeof(int), cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(overflow_host_or_null + 4, w.n_repair + 2, sizeof(int), cudaMemcpyDeviceToHost, st);
+    if (overflow_host_or_null) {   // (read by the host after its next sync)
+        e = cudaMemcpyAsync(overflow_host_or_null, w.ctr, SWEEP_FLAGS * sizeof(int), cudaMemcpyDeviceToHost, st);
         if (e != cudaSuccess) return cuda_status(e, "sweep_chunked: overflow readback");
     }
     if (trace_launches()) {
-        int d[9];
-        if (cudaMemcpy(d, w.n_repair + 64, sizeof(d), cudaMemcpyDeviceToHost) == cudaSuccess && d[0])
+        SweepCounters c;
+        const int* d = c.stall;
+        if (cudaMemcpy(&c, w.ctr, sizeof(c), cudaMemcpyDeviceToHost) == cudaSuccess && c.stalls)
             fprintf(stderr, "[b200bt] lane_scan: %d tile(s) timed out; first: block %d warp %d item(wslot,sym,c) %d,%d,%d tile %d of %d stage %d parity %d tl_begin %d rows %d\n",
-                    d[0], d[1], d[2], d[3] >> 16, (d[3] >> 8) & 255, d[3] & 255, d[4], d[5], d[6] >> 1, d[6] & 1, d[7], d[8]);
+                    c.stalls, d[0], d[1], d[2] >> 16, (d[2] >> 8) & 255, d[2] & 255, d[3], d[4], d[5] >> 1, d[5] & 1, d[6], d[7]);
     }
     return B200BT_OK;
 }
@@ -1378,7 +1389,7 @@ int check_sweep_args(const char* who, const float* price, int64_t ld_price, cons
 }  // namespace
 
 extern "C" int64_t b200bt_sweep_chunked_workspace_bytes(int pool_blocks, int S, int n_seg) {
-    return chunk_workspace_bytes(pool_blocks, (int64_t)S * n_seg, n_seg, n_seg);   // pop <= n_seg
+    return chunk_layout(pool_blocks, (int64_t)S * n_seg, n_seg, n_seg, false).bytes;   // pop <= n_seg
 }
 
 extern "C" int b200bt_sweep_chunked(const float* price, int64_t ld_price, const float* rsi, int64_t ld_rsi, int P, int S,
@@ -1400,19 +1411,14 @@ extern "C" int b200bt_sweep_chunked(const float* price, int64_t ld_price, const 
     rc = check_device();
     if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    const int64_t segs = (int64_t)S * n_seg;
     B200BT_REQUIRE(pop <= n_seg, B200BT_EINVAL, "sweep_chunked: fewer segments than individuals");
-    const ChunkWorkspace w = carve(workspace, pool_blocks, segs, n_seg, pop);
-    cudaError_t e = cudaMemsetAsync(w.seg_in, 0, (size_t)(segs * 6 + 2 + REPAIR_COUNTERS) * 4, st);
+    const ChunkLayout L = chunk_layout(pool_blocks, (int64_t)S * n_seg, n_seg, pop, false);
+    const ChunkWorkspace w = carve(workspace, L, pool_blocks);
+    cudaError_t e = cudaMemsetAsync(workspace, 0, (size_t)L.cleared, st);
     if (e != cudaSuccess) return cuda_status(e, "sweep_chunked: memset");
 
-    ChunkScanArgs A;
-    A.price = price; A.ld_price = ld_price; A.rsi = rsi; A.ld_rsi = ld_rsi; A.P = P; A.S = S; A.N = N;
-    A.indiv = indiv; A.items = items; A.n_items = n_items; A.n_seg = n_seg; A.warm = warm;
-    A.pool = w.pool; A.pool_blocks = pool_blocks; A.next = w.next; A.alloc = w.alloc;
-    A.seg_first = w.seg_first; A.seg_count = w.seg_count; A.seg_in = w.seg_in; A.seg_out = w.seg_out; A.overflow = w.overflow;
-    A.n_chunks = n_chunks; A.redo = nullptr;
-    const bool vec16 = (((uintptr_t)price | (uintptr_t)rsi) & 15) == 0 && ld_price % 4 == 0 && ld_rsi % 4 == 0;
+    const ChunkScanArgs A = scan_args(price, ld_price, rsi, ld_rsi, P, S, N, indiv, items, n_items, n_seg, n_chunks, warm, w);
+    const bool vec16 = vec16_rows(price, ld_price, rsi, ld_rsi);
     auto kern = vec16 ? chunk_scan_kernel<true> : chunk_scan_kernel<false>;
     const size_t smem = sizeof(WarpShared) * SW_WARPS;
     e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -1421,8 +1427,8 @@ extern "C" int b200bt_sweep_chunked(const float* price, int64_t ld_price, const 
     B200BT_REQUIRE(blocks < (1ll << 31), B200BT_ELIMIT, "sweep_chunked: too many work items");
     kern<<<(unsigned)blocks, SW_WARPS * 32, smem, st>>>(A);
     B200BT_LAUNCH_CHECK("chunk_scan launch");
-    return finish_chunks(A, w, items, n_items, seg_base, pop, max_repair_rounds, cfg_host, stats, events, event_cap,
-                         lane_invalid, overflow_host_or_null, st);
+    return finish_chunks(A, w, vec16, seg_base, pop, max_repair_rounds, cfg_host, stats, events, event_cap, lane_invalid,
+                         overflow_host_or_null, st);
 }
 
 extern "C" int64_t b200bt_zone_map_floats(int P, int S, int64_t N) {
@@ -1450,7 +1456,7 @@ extern "C" int b200bt_zone_map(const float* price, int64_t ld_price, const float
 
 extern "C" int64_t b200bt_sweep_tiled_workspace_bytes(int pool_blocks, int S, int pop, int K) {
     const int64_t n_seg = (int64_t)pop * K;
-    return chunk_workspace_bytes(pool_blocks, S * n_seg, (int)n_seg, pop) + 16 + n_seg * 16 + (int64_t)pop * 8;
+    return chunk_layout(pool_blocks, S * n_seg, (int)n_seg, pop, true).bytes;
 }
 
 // measurement hook: a pair of caller-owned CUDA events recorded around the scan kernel of the next b200bt_sweep_tiled calls
@@ -1490,32 +1496,27 @@ extern "C" int b200bt_sweep_tiled(const float* price, int64_t ld_price, const fl
     if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     const int n_seg = pop * K;
-    const int64_t segs = (int64_t)S * n_seg;
-    const ChunkWorkspace w = carve(workspace, pool_blocks, segs, n_seg, pop);
-    b200bt_chunk_item* items = (b200bt_chunk_item*)(((uintptr_t)w.end + 15) & ~(uintptr_t)15);
-    int32_t* seg_base = (int32_t*)(items + n_seg);
-    int32_t* n_chunks = seg_base + pop;
-    cudaError_t e = cudaMemsetAsync(w.seg_in, 0, (size_t)(segs * 6 + 2 + REPAIR_COUNTERS) * 4, st);
+    const ChunkLayout lay = chunk_layout(pool_blocks, (int64_t)S * n_seg, n_seg, pop, true);
+    const ChunkWorkspace w = carve(workspace, lay, pool_blocks);
+    cudaError_t e = cudaMemsetAsync(workspace, 0, (size_t)lay.cleared, st);
     if (e != cudaSuccess) return cuda_status(e, "sweep_tiled: memset");
-    lane_tables_kernel<<<(n_seg + 255) / 256, 256, 0, st>>>(pop, K, order, items, seg_base, n_chunks);
+    lane_tables_kernel<<<(n_seg + 255) / 256, 256, 0, st>>>(pop, K, order, w.items, w.seg_base, w.n_chunks);
     B200BT_LAUNCH_CHECK("lane_tables launch");
 
     LaneScanArgs L;
+    static_cast<ChunkTables&>(L) = w;
     L.price = price; L.ld_price = ld_price; L.rsi = rsi; L.ld_rsi = ld_rsi; L.P = P; L.S = S; L.N = N;
     L.zones = (const float2*)zones_or_null; L.n_zone_blocks = zone_row_stride(N);    // (row stride of the zone map)
     L.fine = zones_or_null ? L.zones + (int64_t)S * (P + 1) * zone_row_stride(N) : nullptr; L.n_fine = zone_fine_stride(N);
     L.indiv = indiv; L.slots = slots; L.n_slots = n_slots; L.pop = pop; L.K = K; L.warm = warm;
-    L.pool = w.pool; L.pool_blocks = pool_blocks; L.next = w.next; L.alloc = w.alloc;
-    L.seg_first = w.seg_first; L.seg_count = w.seg_count; L.seg_in = w.seg_in; L.seg_out = w.seg_out; L.overflow = w.overflow;
-    const bool vec16 = (((uintptr_t)price | (uintptr_t)rsi) & 15) == 0 && ld_price % 4 == 0 && ld_rsi % 4 == 0;
+    L.work = &w.ctr->scan_work; L.ctr = w.ctr;
+    const bool vec16 = vec16_rows(price, ld_price, rsi, ld_rsi);
     auto kern = zones_or_null ? lane_scan_kernel<true> : lane_scan_kernel<false>;
     e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
     if (e != cudaSuccess) return cuda_status(e, "sweep_tiled: cudaFuncSetAttribute");
     const int64_t n_items = (int64_t)(n_slots / 32) * K * S;
     B200BT_REQUIRE(n_items < (1ll << 30), B200BT_ELIMIT, "sweep_tiled: too many work items");
-    L.work = w.n_repair + REPAIR_COUNTERS - 1;      // (a counter no repair round uses; zeroed with the rest above)
-    L.stalls = reinterpret_cast<int*>(w.n_repair + 64);   // (counters 64..72, zeroed with the rest)
     L.wait_cycles = g_wait_cycles != 0 ? g_wait_cycles : LS_WAIT_CYCLES;
     // persistent grid: one resident set of CTAs (warps take work items from the counter), no more CTAs than items need
     int dev = 0, sms = 0, per_sm = 0;
@@ -1530,12 +1531,7 @@ extern "C" int b200bt_sweep_tiled(const float* price, int64_t ld_price, const fl
     if (g_scan_ev[1]) cudaEventRecord(g_scan_ev[1], st);
     B200BT_LAUNCH_CHECK("lane_scan launch");
 
-    ChunkScanArgs A;   // for the shared repair / metrics kernels
-    A.price = price; A.ld_price = ld_price; A.rsi = rsi; A.ld_rsi = ld_rsi; A.P = P; A.S = S; A.N = N;
-    A.indiv = indiv; A.items = items; A.n_items = n_seg; A.n_seg = n_seg; A.warm = warm;
-    A.pool = w.pool; A.pool_blocks = pool_blocks; A.next = w.next; A.alloc = w.alloc;
-    A.seg_first = w.seg_first; A.seg_count = w.seg_count; A.seg_in = w.seg_in; A.seg_out = w.seg_out; A.overflow = w.overflow;
-    A.n_chunks = n_chunks; A.redo = nullptr;
-    return finish_chunks(A, w, items, n_seg, seg_base, pop, max_repair_rounds, cfg_host, stats, events, event_cap, lane_invalid,
+    const ChunkScanArgs A = scan_args(price, ld_price, rsi, ld_rsi, P, S, N, indiv, w.items, n_seg, n_seg, w.n_chunks, warm, w);
+    return finish_chunks(A, w, vec16, w.seg_base, pop, max_repair_rounds, cfg_host, stats, events, event_cap, lane_invalid,
                          overflow_host_or_null, st);
 }
