@@ -70,6 +70,8 @@ EVENT_EXIT = 0x40000000
 EVENT_SELL = 0x80000000
 EVENT_BAR_MASK = 0x3FFFFFFF
 
+TRADE_MC_METHODS = {"bootstrap": 0, "shuffle": 1}     # B200BT_TRADE_MC_*
+
 PRIMARY = {"sharpe_ratio": 0, "return_pct": 1, "profit_factor": 2, "win_rate": 3, "net_profit": 4, "total_trades": 5,
            "max_drawdown": 6, "total_profit": 7, "total_loss": 8, "largest_profit": 9, "largest_loss": 10,
            "average_profit": 11, "average_loss": 12}
@@ -145,6 +147,9 @@ _SIGNATURES = {
                                           _vp, _vp, _vp, _vp]),
     "b200bt_mc_portfolio_bootstrap": (C.c_int, [_i, _vp, _i, _i, _i, C.POINTER(C.c_double), C.POINTER(C.c_double), _i64,
                                                 _i, C.c_uint64, C.c_uint64, _vp, _vp, _vp, _vp]),
+    "b200bt_trade_pnl": (C.c_int, [_vp, _i64, _i, _i64, _vp, _i, _vp, _vp, _i64, _vp, _i64, _vp, _vp, _vp]),
+    "b200bt_trade_mc": (C.c_int, [_vp, _i64, C.POINTER(C.c_int32), C.POINTER(C.c_double), C.POINTER(C.c_uint32), _i, _i,
+                                  _i, C.c_double, _i64, C.c_uint64, C.c_uint64, _vp, _vp, _vp]),
     "b200bt_ga_init": (C.c_int, [_vp, _i, _i, _i, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_int),
                                  C.c_uint64, _vp]),
     "b200bt_ga_next_generation": (C.c_int, [_vp, _vp, _vp, _i, _i, C.POINTER(C.c_double), C.POINTER(C.c_double),

@@ -154,9 +154,8 @@ class StrategyEvaluationSystem:
         self.performance_metrics = self.config.get("evolution", {}).get("performance_metrics", {})
 
     # -- reference-compatible single-strategy call -----------------------------------
-    def _simulate_trades(self, strategy_id: str, parameters: Dict, market_data: List[Dict]) -> List[Dict]:
-        if not market_data:
-            return []
+    def _lane_sweep(self, parameters: Dict, market_data: List[Dict], event_cap: int):
+        """(one-lane sweep over the points' own price and rsi fields, fp32 prices) for one parameter set."""
         n = len(market_data)
         price = np.array([d.get("price", 50000) for d in market_data], dtype=np.float32)
         rsi = np.array([d.get("rsi", 50) for d in market_data], dtype=np.float32)
@@ -165,7 +164,14 @@ class StrategyEvaluationSystem:
         market = MarketData(ohlcv)
         period = int(parameters.get("rsi_period", 14))
         sweep = PopulationSweep.from_bank(market, torch.from_numpy(rsi).to(market.device).view(1, 1, n), [period],
-                                          self.optimization_goals, event_cap=n + 1)
+                                          self.optimization_goals, event_cap=event_cap)
+        return sweep, price
+
+    def _simulate_trades(self, strategy_id: str, parameters: Dict, market_data: List[Dict]) -> List[Dict]:
+        if not market_data:
+            return []
+        n = len(market_data)
+        sweep, price = self._lane_sweep(parameters, market_data, event_cap=n + 1)
         sweep.evaluate([dict(parameters)])
         n_rec = int(sweep.lane_stats()["n_records"][0, 0])
         ev = sweep.events()[0, 0, :n_rec]
@@ -317,6 +323,93 @@ class StrategyEvaluationSystem:
         if per_day < floor:
             score *= per_day / floor
         return score
+
+    # -- trade-sequence Monte-Carlo (BACKLOG.md:194 "BACK-04") --------------------------------------------------------
+    def monte_carlo_trades(self, strategy_id: str, parameters: Dict, market_data: List[Dict],
+                           num_simulations: int = 1000, simulation_method: str = "bootstrap", block_len: int = 1,
+                           confidence_level: float = 0.95, seed: int = 2024) -> Dict:
+        """How much of a strategy's result is the luck of its trade order: the round trips of _simulate_trades'
+        records on `market_data` (same flat list of points) are resampled `num_simulations` times on the GPU
+        ("bootstrap": with replacement, in circular blocks of `block_len` trips; "shuffle": every trip once, in a keyed
+        pseudo-random order) and the equity walked as calculate_metrics walks it.  Returns a dict shaped like
+        run_monte_carlo_simulation's (monte_carlo_service.py:339-374) with equity in place of price; `original` holds
+        the unresampled sequence's values, `num_trades` counts round trips (two records each).  Logs and returns {} on
+        failure (:392)."""
+        from .trade_monte_carlo import TradeMonteCarlo, result_blocks
+        try:
+            if not market_data:
+                logger.error("No market data for the trade Monte-Carlo of %s", strategy_id)
+                return {}
+            if simulation_method not in _lib.TRADE_MC_METHODS:
+                logger.error("Unknown trade simulation method: %s", simulation_method)
+                return {}
+            sweep, _ = self._lane_sweep(parameters, market_data, event_cap=0)
+            trip, n_trips, fee = sweep.trade_pnl([dict(parameters)])
+            st = sweep.lane_stats()
+            capital = float(sweep.cfg.initial_capital)
+            mc = TradeMonteCarlo(sweep.market.device)
+            finals, maxdd = mc.simulate(trip, n_trips, fee, num_simulations, simulation_method, block_len, capital, seed)
+            blocks = result_blocks(mc.statistics(finals[0], maxdd[0], capital, confidence_level), capital)
+            net = float(st["net_profit"][0, 0])
+            return {
+                "strategy_id": strategy_id, "symbol": market_data[0].get("symbol", "BTCUSDT"),
+                "initial_capital": capital, "num_trades": int(n_trips[0, 0].item()),
+                "num_simulations": int(num_simulations), "simulation_method": simulation_method,
+                "block_len": int(block_len), "seed": int(seed), "timestamp": datetime.now().isoformat(),
+                "original": {"final_equity": capital + net, "return_pct": net / capital * 100,
+                             "max_drawdown": float(st["max_drawdown"][0, 0])},
+                **blocks,
+            }
+        except Exception as e:  # reference convention: log, return {}
+            logger.error("Error running trade Monte-Carlo simulation for %s: %s", strategy_id, e, exc_info=True)
+            return {}
+
+    MC_POPULATION_FIELDS = ("expected_equity", "expected_pct_change", "var", "cvar", "prob_profit", "prob_loss",
+                            "mdd_mean", "mdd_median", "mdd_p95", "mdd_max")
+
+    def monte_carlo_population(self, population: List[Dict], market: MarketData,
+                               sweep: Optional[PopulationSweep] = None, num_simulations: int = 1000,
+                               simulation_method: str = "bootstrap", block_len: int = 1,
+                               confidence_level: float = 0.95, seed: int = 2024,
+                               max_path_bytes: int = 1 << 30) -> Dict[str, np.ndarray]:
+        """monte_carlo_trades for every (individual, symbol) lane of a population -- meant for its top, e.g. to rank it
+        by the 5th-percentile return or the 95th-percentile drawdown.  Lane id of (i, s) = i * S + s.  Returns [pop][S]
+        arrays of the scalars of monte_carlo_trades' dict: num_trades, original_final_equity / return_pct / max_drawdown,
+        MC_POPULATION_FIELDS, and [pop][S][9] arrays percentile_equity / percentile_pct_change at `percentiles`."""
+        from .monte_carlo import PERCENTILES
+        from .trade_monte_carlo import TradeMonteCarlo
+        sweep = sweep or PopulationSweep(market, optimization_goals=self.optimization_goals)
+        trip, n_trips, fee = sweep.trade_pnl(population)
+        st = sweep.lane_stats()
+        P, S = len(population), market.S
+        capital = float(sweep.cfg.initial_capital)
+        net = st["net_profit"]
+        out = {"num_trades": n_trips.cpu().numpy().astype(np.int64), "original_final_equity": capital + net,
+               "original_return_pct": net / capital * 100, "original_max_drawdown": st["max_drawdown"].copy(),
+               "percentiles": np.array(PERCENTILES),
+               "percentile_equity": np.zeros((P, S, len(PERCENTILES))),
+               "percentile_pct_change": np.zeros((P, S, len(PERCENTILES)))}
+        for k in self.MC_POPULATION_FIELDS:
+            out[k] = np.zeros((P, S))
+        mc = TradeMonteCarlo(market.device)
+        rows = trip.view(P * S, -1)
+        per_call = max(1, int(max_path_bytes) // (8 * int(num_simulations)))     # finals + maxdd fp32 per lane
+        for lo in range(0, P * S, per_call):
+            hi = min(P * S, lo + per_call)
+            finals, maxdd = mc.simulate(rows[lo:hi], n_trips.view(-1)[lo:hi], fee.view(-1)[lo:hi], num_simulations,
+                                        simulation_method, block_len, capital, seed, lane_ids=np.arange(lo, hi))
+            for r in range(hi - lo):
+                i, s = divmod(lo + r, S)
+                q = mc.statistics(finals[r], maxdd[r], capital, confidence_level)
+                pv = np.asarray(q["percentile_values"])
+                out["percentile_equity"][i, s] = pv
+                out["percentile_pct_change"][i, s] = (pv / capital - 1) * 100
+                out["expected_equity"][i, s], out["expected_pct_change"][i, s] = q["expected_price"], q["expected_pct"]
+                out["var"][i, s], out["cvar"][i, s] = abs(q["var"]), abs(q["cvar"])
+                out["prob_profit"][i, s], out["prob_loss"][i, s] = q["prob_profit"], 1 - q["prob_profit"]
+                for k in ("mdd_mean", "mdd_median", "mdd_p95", "mdd_max"):
+                    out[k][i, s] = q[k]
+        return out
 
     # -- batched form -------------------------------------------------------------
     def evaluate_population(self, population: List[Dict], market: MarketData,

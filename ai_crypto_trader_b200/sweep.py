@@ -842,6 +842,58 @@ class PopulationSweep:
         res = out.numpy().copy()
         return res if self._inverse is None else res[self._inverse]
 
+    TRADE_PNL_MAX_BYTES = 4 << 30
+
+    def trade_pnl(self, population: List[Dict], max_bytes: int = TRADE_PNL_MAX_BYTES):
+        """Round-trip PnL of every (individual, symbol) lane, on the device, in the order of `population`:
+        (trip_pnl float64 [pop][S][T_max], n_trips int32 [pop][S], fee float64 [pop][S]).  Lane (i, s) holds n_trips[i, s]
+        round trips; its records are, in time order, an entry with pnl -fee and an exit with pnl trip_pnl[i, s, j] --
+        bit-identical to the pnl of StrategyEvaluationSystem._simulate_trades' records (b200bt_trade_pnl).
+
+        Two sweeps of this bank under this schedule: the first counts each lane's records, the second writes their event
+        words with event_cap = the largest count.  Individuals that decode alike are swept once.  Meant for the top of a
+        population: a ValueError names the bytes when the event and PnL buffers would exceed `max_bytes`.  Afterwards
+        lane_stats() / events() describe this population (the next evaluate() allocates its own buffers)."""
+        if not population:
+            raise ValueError("trade_pnl needs at least one individual")
+        m = self.market
+        packed = decode_population(population, self.period_row, len(self.timeframes))
+        dup = _duplicate_classes(packed)
+        if dup is not None:                                     # evaluate() sweeps these, in this order
+            packed = np.ascontiguousarray(packed[np.sort(dup[0])])
+        U, P, S = len(packed), len(population), m.S
+        saved_cap = self.event_cap
+        try:
+            self.event_cap, self._stats = 0, None
+            self.evaluate(population)
+            cap = int(self._stats[:, :, 0].max().item())           # n_records of the busiest lane (always even)
+            cap = max(2, cap + (cap & 1))
+            T = cap // 2
+            need = U * S * cap * 4 + (U + P) * S * T * 8
+            if need > max_bytes:
+                raise ValueError(f"trade_pnl: {need} bytes of event and trip PnL buffers for {P} individuals x {S} symbols "
+                                 f"(up to {cap} records per lane) exceed the budget of {max_bytes} bytes; pass the top "
+                                 f"of the population, not all of it")
+            self.event_cap, self._stats = cap, None
+            self.evaluate(population)
+            indiv = torch.from_numpy(packed.view(np.uint8)).to(m.device)
+            trip = torch.empty((U, S, T), dtype=torch.float64, device=m.device)
+            n_trips = torch.empty((U, S), dtype=torch.int32, device=m.device)
+            fee = torch.empty((U, S), dtype=torch.float64, device=m.device)
+            with torch.cuda.device(m.device):
+                _lib.call("b200bt_trade_pnl", m.close.data_ptr(), _lib.ld(m.close), S, m.N, indiv.data_ptr(), U,
+                          self._stats.data_ptr(), self._events.data_ptr(), cap, trip.data_ptr(), T, n_trips.data_ptr(),
+                          fee.data_ptr(), _lib.current_stream())
+        finally:
+            self.event_cap = saved_cap
+            self._pop = -1                 # the next evaluation allocates stats / events for its own event_cap
+        if self._inverse is not None:
+            inv = torch.from_numpy(self._inverse).to(m.device)
+            trip, n_trips, fee = trip.index_select(0, inv), n_trips.index_select(0, inv), fee.index_select(0, inv)
+        if bool((n_trips < 0).any()):
+            raise RuntimeError("trade_pnl: a lane wrote more records than its event buffer held")
+        return trip, n_trips, fee
+
     def lane_stats(self) -> Dict[str, np.ndarray]:
         """Per-lane metrics of the last evaluation: dict field -> [pop][S] array."""
         raw = self._stats.cpu().numpy()

@@ -440,6 +440,55 @@ int b200bt_mc_portfolio_bootstrap(int S, const float* returns, int R, int block_
                                   uint64_t seed, uint64_t path_offset, float* finals, float* maxdd,
                                   float* asset_finals_or_null, b200bt_stream_t stream);
 
+/* ---- trade-sequence Monte-Carlo of backtested strategies --------------------------------------------
+ * The reference's open backtesting item "BACK-04: Add Monte Carlo simulations" (BACKLOG.md:194): resample the round
+ * trips of a strategy's own trade records many times and report the spread of final equity and maximum drawdown.
+ * Records as _simulate_trades emits them (services/strategy_evaluation.py:746-878): an entry record with pnl -fee and an
+ * exit record with the trip's pnl; equity walk and drawdown rule of calculate_metrics (:119-139), resampling rule of
+ * MonteCarloService (services/monte_carlo_service.py:277-298), statistics block as :339-374 with equity for price. */
+
+/* Round-trip PnL from a sweep's event words.  For every lane = i * S + s of a sweep with an event buffer:
+ *  n_trips[lane] (device int32) = n_records / 2, or -1 when n_records > event_cap (records were lost)
+ *  fee[lane]     (device float64) = position_size * 0.001, the pnl of every entry record is -fee (:796-797, :810-811)
+ *  trip_pnl[lane][j] (device float64, row stride ld_trip >= event_cap / 2) = pnl of the j-th exit record,
+ *                qty * (price - entry) - position_size * 0.002 for a long trip, qty * (entry - price) - ... for a short
+ *                one (entry word's B200BT_EVENT_SELL bit), qty = position_size / entry, prices = the fp32 closes widened
+ *                to float64 (:819-820, :836-837, :852-853, :866-867); bit-identical to those float64 expressions.
+ * price [S][ld] fp32, indiv [pop], stats [pop][S] and events [pop][S][event_cap] are the sweep's (device). */
+int b200bt_trade_pnl(const float* price, int64_t ld, int S, int64_t N, const b200bt_individual* indiv, int pop,
+                     const b200bt_lane_stats* stats, const uint32_t* events, int64_t event_cap, double* trip_pnl,
+                     int64_t ld_trip, int32_t* n_trips, double* fee, b200bt_stream_t stream);
+
+/* Monte-Carlo over the round trips of L lanes.  Unit of resampling: the round trip (entry and exit records stay
+ * paired, so every path is again a valid record sequence).  Per path, T = n_trips_host[r] trip indices are drawn and the
+ * equity walks in float64: E = initial_capital, peak = initial_capital; per drawn trip j, E += -fee, then
+ * E += trip_pnl[r][j]; after each record a new peak needs E > peak, otherwise the record's drawdown is
+ * (peak - E) / peak.  finals[r][p] = fp32(E_T), maxdd[r][p] = fp32(largest drawdown, 0 if none), each rounded once from
+ * float64 (rows of n_paths; they feed b200bt_select / b200bt_mc_moments with s0 = initial_capital).  T = 0 gives
+ * initial_capital and 0.
+ * method B200BT_TRADE_MC_BOOTSTRAP: T draws with replacement, index __umulhi(u, T) (b200bt_mc_bootstrap's draw); with
+ *        block_len > 1 circular blocks of consecutive trips by b200bt_mc_bootstrap's block rule.
+ * method B200BT_TRADE_MC_SHUFFLE: every trip exactly once; position j holds pi(j), pi a balanced four-round Feistel
+ *        bijection over the smallest even bit width 2h >= 8 with 2^2h >= T, six rounds, cycle-walked into [0, T); round
+ *        keys = the first six words of the path's Philox blocks 0xFFFFFFFE and 0xFFFFFFFF (on fewer than 8 bits
+ *        the position marginals were visibly skewed even with eight rounds).  This order is NOT uniform over
+ *        all T! permutations (a keyed family of them, O(1) state per index); its position marginals pass chi-square
+ *        tests and positions 0 and 1 are uncorrelated beyond the -1/(T-1) of a uniform permutation.
+ * Randomness: Philox4x32-10, key = seed, counter = (gid lo, gid hi, block, lane id) with block = trip / 4 (bootstrap)
+ * or 0xFFFFFFFE / 0xFFFFFFFF (shuffle),
+ * gid = path_offset + p and lane id = lane_ids_host[r] (NULL = r).  A path is a pure function of (seed, lane id, gid, the
+ * lane's trips): it does not depend on path sharding or on the other lanes of the call; lane id 1's bootstrap index
+ * stream is b200bt_mc_bootstrap's for a table of T entries.
+ * n_trips_host, fee_host, lane_ids_host: HOST arrays of L entries; trip_pnl: device [L][ld_trip] float64; finals, maxdd:
+ * device [L][n_paths] fp32.  Limits: 0 <= T < 2^30 (ELIMIT above), T <= ld_trip, n_paths >= 1 (<= 2^38), block_len
+ * >= 1, initial_capital > 0.  Lanes with T <= 6144 are staged in shared memory, larger ones read through L2. */
+#define B200BT_TRADE_MC_BOOTSTRAP 0
+#define B200BT_TRADE_MC_SHUFFLE 1
+int b200bt_trade_mc(const double* trip_pnl, int64_t ld_trip, const int32_t* n_trips_host, const double* fee_host,
+                    const uint32_t* lane_ids_host, int L, int method, int block_len, double initial_capital,
+                    int64_t n_paths, uint64_t seed, uint64_t path_offset, float* finals, float* maxdd,
+                    b200bt_stream_t stream);
+
 /* ---- portfolio risk (SURVEY 8-f4) -------------------------------------------------------------------
  * Replaces the numeric core of services/portfolio_risk_service.py. */
 
