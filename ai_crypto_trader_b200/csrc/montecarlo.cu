@@ -43,6 +43,15 @@ __device__ __forceinline__ void box_muller(uint32_t a, uint32_t b, float& z0, fl
 
 constexpr int MC_THREADS = 256;
 
+// The n entries of a bootstrap table into shared memory as log returns: paths compound in log space either way.
+__device__ __forceinline__ void stage_log_returns(float* s_ret, const float* __restrict__ returns, int n, int log_returns) {
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        const float r = returns[i];
+        s_ret[i] = log_returns ? r : log1pf(r);
+    }
+    __syncthreads();
+}
+
 // mode 0: GBM.  mode 1: bootstrap of `returns` (R values, staged in shared memory),
 // blocks of `block_len` consecutive returns (circular), log_returns selects compounding.
 template <int MODE>
@@ -51,28 +60,19 @@ mc_paths_kernel(double s0, double drift, double vol, const float* __restrict__ r
                 int log_returns, int64_t n_paths, int steps, uint64_t seed, uint64_t path_offset,
                 float* __restrict__ finals, float* __restrict__ maxdd, float* __restrict__ paths) {
     extern __shared__ float s_ret[];
-    if (MODE == 1) {
-        for (int i = threadIdx.x; i < R; i += blockDim.x) {
-            const float r = returns[i];
-            s_ret[i] = log_returns ? r : log1pf(r);  // compounding in log space either way
-        }
-        __syncthreads();
-    }
+    if (MODE == 1) stage_log_returns(s_ret, returns, R, log_returns);
     const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= n_paths) return;
-    const uint64_t gid = path_offset + (uint64_t)p;
-    const uint32_t k0 = (uint32_t)seed, k1 = (uint32_t)(seed >> 32);
-    const uint32_t c0 = (uint32_t)gid, c1 = (uint32_t)(gid >> 32);
 
     // log-price relative to log(s0): block base `base` and running maximum `runmax` in fp64, the four
     // steps of a Philox block in fp32 relative to the base (their sum is folded into the base exactly)
     double base = 0.0, runmax = 0.0, worst = 0.0;
     const float fs0 = (float)s0, fdrift = (float)drift, fvol = (float)vol;
     if (paths) paths[p] = fs0;
-    int boot_idx = 0, boot_left = 0;
+    BlockBootstrap boot;
     for (int t0 = 0; t0 < steps; t0 += 4) {
         uint32_t x[4];
-        philox4x32_10(c0, c1, (uint32_t)(t0 >> 2), (uint32_t)MODE, k0, k1, x);
+        philox_path(seed, path_offset, p, (uint32_t)(t0 >> 2), (uint32_t)MODE, x);
         float inc[4];
         if (MODE == 0) {
             float z[4];
@@ -82,16 +82,7 @@ mc_paths_kernel(double s0, double drift, double vol, const float* __restrict__ r
             for (int j = 0; j < 4; ++j) inc[j] = fmaf(fvol, z[j], fdrift);
         } else {
 #pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                if (boot_left == 0) {
-                    boot_idx = (int)__umulhi(x[j], (uint32_t)R);  // uniform start in [0, R)
-                    boot_left = block_len;
-                } else {
-                    boot_idx = boot_idx + 1 == R ? 0 : boot_idx + 1;
-                }
-                --boot_left;
-                inc[j] = s_ret[boot_idx];
-            }
+            for (int j = 0; j < 4; ++j) inc[j] = s_ret[boot.next(x[j], R, block_len)];
         }
         const float d0 = (float)(runmax - base);   // running maximum seen from the block base (>= 0)
         float l = 0.f, mx = d0, wmin = 0.f;
@@ -155,18 +146,9 @@ mc_joint_kernel(const __grid_constant__ JointParams<SMAX> P, const float* __rest
     double* s_base = s_joint;                                            // [SMAX][JOINT_THREADS]
     float* s_ret = reinterpret_cast<float*>(s_joint + SMAX * JOINT_THREADS);   // [R][S] bootstrap table
     const int S = P.S;
-    if (MODE == 1) {
-        for (int i = threadIdx.x; i < R * S; i += blockDim.x) {
-            const float r = returns[i];
-            s_ret[i] = log_returns ? r : log1pf(r);
-        }
-        __syncthreads();
-    }
+    if (MODE == 1) stage_log_returns(s_ret, returns, R * S, log_returns);
     const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= n_paths) return;
-    const uint64_t gid = path_offset + (uint64_t)p;
-    const uint32_t k0 = (uint32_t)seed, k1 = (uint32_t)(seed >> 32);
-    const uint32_t c0 = (uint32_t)gid, c1 = (uint32_t)(gid >> 32);
 
     float l[SMAX], A[SMAX];
 #pragma unroll
@@ -176,7 +158,7 @@ mc_joint_kernel(const __grid_constant__ JointParams<SMAX> P, const float* __rest
         if (i < S) s_base[i * JOINT_THREADS + threadIdx.x] = 0.0;
     }
     float runmax = joint_value<SMAX>(A, l, S), dd = 0.f;
-    int boot_idx = 0, boot_left = 0;
+    BlockBootstrap boot;
     for (int t0 = 0; t0 < steps; t0 += 4) {
         float z[SMAX][4];   // GBM: four normals per factor, then (L z) in place
         int day[4];         // bootstrap: one day (row of the table) per step
@@ -185,7 +167,7 @@ mc_joint_kernel(const __grid_constant__ JointParams<SMAX> P, const float* __rest
             for (int k = 0; k < SMAX; ++k) {
                 if (k < S) {
                     uint32_t x[4];
-                    philox4x32_10(c0, c1, (uint32_t)(t0 >> 2), ((uint32_t)k << 8) | (uint32_t)MODE, k0, k1, x);
+                    philox_path(seed, path_offset, p, (uint32_t)(t0 >> 2), ((uint32_t)k << 8) | (uint32_t)MODE, x);
                     box_muller(x[0], x[1], z[k][0], z[k][1]);
                     box_muller(x[2], x[3], z[k][2], z[k][3]);
                 }
@@ -205,18 +187,9 @@ mc_joint_kernel(const __grid_constant__ JointParams<SMAX> P, const float* __rest
             }
         } else {
             uint32_t x[4];
-            philox4x32_10(c0, c1, (uint32_t)(t0 >> 2), (uint32_t)MODE, k0, k1, x);
+            philox_path(seed, path_offset, p, (uint32_t)(t0 >> 2), (uint32_t)MODE, x);
 #pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                if (boot_left == 0) {
-                    boot_idx = (int)__umulhi(x[j], (uint32_t)R);
-                    boot_left = block_len;
-                } else {
-                    boot_idx = boot_idx + 1 == R ? 0 : boot_idx + 1;
-                }
-                --boot_left;
-                day[j] = boot_idx * S;
-            }
+            for (int j = 0; j < 4; ++j) day[j] = boot.next(x[j], R, block_len) * S;
         }
 #pragma unroll
         for (int j = 0; j < 4; ++j) {

@@ -31,4 +31,31 @@ __host__ __device__ __forceinline__ void philox4x32_10(uint32_t c0, uint32_t c1,
     out[0] = c0; out[1] = c1; out[2] = c2; out[3] = c3;
 }
 
+// One Philox block of Monte-Carlo path p: key = seed, counter words 0 and 1 = the global path index path_offset + p, so a
+// path does not depend on the launch geometry or on how the paths are sharded.  Words 2 and 3 are the caller's.
+__device__ __forceinline__ void philox_path(uint64_t seed, uint64_t path_offset, int64_t p, uint32_t c2, uint32_t c3,
+                                            uint32_t out[4]) {
+    const uint64_t gid = path_offset + (uint64_t)p;
+    const uint32_t k0 = (uint32_t)seed, k1 = (uint32_t)(seed >> 32);
+    const uint32_t c0 = (uint32_t)gid, c1 = (uint32_t)(gid >> 32);
+    philox4x32_10(c0, c1, c2, c3, k0, k1, out);
+}
+
+// Circular block bootstrap over a table of R entries, one index per random word u: a block starts at the uniform index
+// __umulhi(u, R) and continues with the next entries, wrapping at R, for block_len draws.  Words drawn inside a block
+// are not used.  The single-asset, joint and trade bootstraps all draw through this, so their index streams agree.
+struct BlockBootstrap {
+    int idx = 0, left = 0;
+    __device__ __forceinline__ int next(uint32_t u, int R, int block_len) {
+        if (left == 0) {
+            idx = (int)__umulhi(u, (uint32_t)R);
+            left = block_len;
+        } else {
+            idx = idx + 1 == R ? 0 : idx + 1;
+        }
+        --left;
+        return idx;
+    }
+};
+
 }  // namespace b200bt

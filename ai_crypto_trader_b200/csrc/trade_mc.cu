@@ -124,27 +124,20 @@ __device__ __forceinline__ double trip_at(const double* __restrict__ pnl, int j)
 
 template <bool STAGED>
 __device__ __forceinline__ void walk(const double* __restrict__ pnl, const TradeLane& ln, int method, int block_len,
-                                     uint32_t c0, uint32_t c1, uint32_t k0, uint32_t k1, double& E, double& dd) {
+                                     uint64_t seed, uint64_t path_offset, int64_t path, double& E, double& dd) {
     const int T = ln.T;
     const double nfee = -ln.fee;
     double P = E, m = E;
     if (method == 0) {
-        // bootstrap: b200bt_mc_bootstrap's block rule on the trip table (start __umulhi(u, T), then circular steps)
-        int idx = 0, left = 0;
+        // bootstrap: b200bt_mc_bootstrap's block rule on the trip table
+        BlockBootstrap boot;
         for (int t0 = 0; t0 < T; t0 += 4) {
             uint32_t x[4];
-            philox4x32_10(c0, c1, (uint32_t)(t0 >> 2), ln.lane_id, k0, k1, x);
+            philox_path(seed, path_offset, path, (uint32_t)(t0 >> 2), ln.lane_id, x);
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
                 if (t0 + j < T) {
-                    if (left == 0) {
-                        idx = (int)__umulhi(x[j], (uint32_t)T);
-                        left = block_len;
-                    } else {
-                        idx = idx + 1 == T ? 0 : idx + 1;
-                    }
-                    --left;
-                    const double p = trip_at<STAGED>(pnl, idx);
+                    const double p = trip_at<STAGED>(pnl, boot.next(x[j], T, block_len));
                     equity_record(nfee, E, P, m, dd);
                     equity_record(p, E, P, m, dd);
                 }
@@ -153,8 +146,8 @@ __device__ __forceinline__ void walk(const double* __restrict__ pnl, const Trade
     } else if (T > 0) {
         // shuffle: position j holds trip pi(j), pi = the keyed Feistel bijection cycle-walked into [0, T)
         uint32_t x[8], k[FEISTEL_ROUNDS];
-        philox4x32_10(c0, c1, TMC_SHUFFLE_BLOCK, ln.lane_id, k0, k1, x);
-        philox4x32_10(c0, c1, TMC_SHUFFLE_BLOCK + 1, ln.lane_id, k0, k1, x + 4);
+        philox_path(seed, path_offset, path, TMC_SHUFFLE_BLOCK, ln.lane_id, x);
+        philox_path(seed, path_offset, path, TMC_SHUFFLE_BLOCK + 1, ln.lane_id, x + 4);
 #pragma unroll
         for (int r = 0; r < FEISTEL_ROUNDS; ++r) k[r] = x[r];
         const int h = feistel_half_bits(T);
@@ -187,14 +180,11 @@ trade_mc_kernel(const __grid_constant__ TradeMcBatch B, const double* __restrict
         __syncthreads();
     }
     if (p >= n_paths) return;
-    const uint64_t gid = path_offset + (uint64_t)p;
-    const uint32_t c0 = (uint32_t)gid, c1 = (uint32_t)(gid >> 32);
-    const uint32_t k0 = (uint32_t)seed, k1 = (uint32_t)(seed >> 32);
     double E = initial_capital, dd = 0.0;
     if (ln.staged)
-        walk<true>(s_pnl, ln, method, block_len, c0, c1, k0, k1, E, dd);
+        walk<true>(s_pnl, ln, method, block_len, seed, path_offset, p, E, dd);
     else
-        walk<false>(src, ln, method, block_len, c0, c1, k0, k1, E, dd);
+        walk<false>(src, ln, method, block_len, seed, path_offset, p, E, dd);
     const int64_t o = (int64_t)ln.row * n_paths + p;
     finals[o] = (float)E;
     maxdd[o] = (float)dd;

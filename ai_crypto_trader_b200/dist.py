@@ -117,23 +117,13 @@ def gather_paths(local_finals: torch.Tensor, local_maxdd: torch.Tensor, n_total:
     8 bytes per path; every rank then holds all finals / drawdowns and computes the same order statistics."""
     if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size(group) == 1:
         return local_finals, local_maxdd
-    world = dist.get_world_size(group)
-    per = -(-n_total // world)
-    send = torch.full((2 * per,), float("nan"), dtype=torch.float32, device=local_finals.device)
-    send[:local_finals.numel()] = local_finals
-    send[per:per + local_maxdd.numel()] = local_maxdd
-    recv = torch.empty((world * 2 * per,), dtype=torch.float32, device=local_finals.device)
-    dist.all_gather_into_tensor(recv, send, group=group)
-    recv = recv.view(world, 2, per)
-    counts = [shard_bounds(n_total, world, r)[1] - shard_bounds(n_total, world, r)[0] for r in range(world)]
-    finals = torch.cat([recv[r, 0, :counts[r]] for r in range(world)])
-    maxdd = torch.cat([recv[r, 1, :counts[r]] for r in range(world)])
+    finals, maxdd = gather_path_rows(torch.stack([local_finals, local_maxdd]), n_total, group)
     return finals, maxdd
 
 
 def gather_path_rows(local_rows: torch.Tensor, n_total: int, group=None) -> torch.Tensor:
-    """gather_paths for a [K][n_local] block of per-path rows (the per-asset finals of a joint run): one collective,
-    and the gathered [K][n_total] equals a single-GPU run bit for bit."""
+    """All-gather a [K][n_local] block of per-path rows (finals and drawdowns, the per-asset finals of a joint run),
+    sharded as gather_paths' arrays: one collective, and the gathered [K][n_total] equals a single-GPU run bit for bit."""
     if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size(group) == 1:
         return local_rows
     world = dist.get_world_size(group)

@@ -20,6 +20,7 @@ import json
 import logging
 import math
 from datetime import datetime
+from functools import partial
 from typing import Dict, Optional
 
 import numpy as np
@@ -64,6 +65,16 @@ def _virtual_index(n: int, q_percent: float):
     lo = min(max(lo, 0), n - 1)
     hi = min(lo + 1, n - 1)
     return lo, hi, float(h - math.floor(h))
+
+
+def percentile_points(select, n: int, percentiles):
+    """[(x_lo, x_hi, g)] for each percentile: numpy's linear percentile of n values is _lerp(x_lo, x_hi, g) of two exact
+    order statistics.  `select(ranks)` returns the order statistics at ascending 0-based ranks; it is called once, over
+    the union of the ranks every percentile needs."""
+    idx = [_virtual_index(n, q) for q in percentiles]
+    ranks = sorted({i for lo, hi, _ in idx for i in (lo, hi)})
+    vals = dict(zip(ranks, select(ranks)))
+    return [(vals[lo], vals[hi], g) for lo, hi, g in idx]
 
 
 def _f64(x) -> np.ndarray:
@@ -118,15 +129,6 @@ def joint_assets(holdings: Dict, historical_data: Dict):
     return out
 
 
-def _var_pct(engine: "PathEngine", finals: torch.Tensor, initial: float, confidence: float) -> float:
-    """risk_statistics' VaR (:316-317) alone: the (1 - confidence) percentile of the percentage change."""
-    lo, hi, g = _virtual_index(int(finals.numel()), 100 * (1 - confidence))
-    ranks = sorted({lo, hi})
-    vals = dict(zip(ranks, engine.select(finals, ranks)))
-    pct = lambda v: (v / initial - 1) * 100
-    return _lerp(pct(vals[lo]), pct(vals[hi]), g)
-
-
 class PathEngine:
     """Device-side Monte-Carlo primitives (one instance per GPU)."""
 
@@ -136,42 +138,29 @@ class PathEngine:
         self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
         self._ws = None
 
+    def _generate(self, fn: str, args, n_paths, steps, seed, path_offset, rows=None):
+        """Run the path generator `fn`(*args, n_paths, steps, seed, path_offset, finals, maxdd, block, stream) into new
+        outputs: finals [n], maxdd [n] and, when `rows` is given, a [rows][n] block (stored paths or asset finals).
+        A rank without paths (more ranks than paths) gets empty outputs and no launch."""
+        out = lambda *shape: torch.empty(shape, dtype=torch.float32, device=self.device)
+        finals, maxdd = out(n_paths), out(n_paths)
+        block = out(rows, n_paths) if rows is not None else None
+        if n_paths > 0:
+            with torch.cuda.device(self.device):
+                _lib.call(fn, *args, int(n_paths), int(steps), int(seed) & (2**64 - 1), int(path_offset),
+                          finals.data_ptr(), maxdd.data_ptr(), _lib.ptr(block), _lib.current_stream())
+        return finals, maxdd, block
+
     def gbm(self, s0, mu, sigma, dt, n_paths, steps, seed, path_offset=0, store_paths=False):
-        dev = self.device
-        if n_paths == 0:          # a rank without paths (more ranks than paths)
-            e = torch.empty(0, dtype=torch.float32, device=dev)
-            return e, e.clone(), None
-        finals = torch.empty(n_paths, dtype=torch.float32, device=dev)
-        maxdd = torch.empty(n_paths, dtype=torch.float32, device=dev)
-        paths = torch.empty((steps + 1, n_paths), dtype=torch.float32, device=dev) if store_paths else None
-        with torch.cuda.device(dev):
-            _lib.call("b200bt_mc_gbm", float(s0), float(mu), float(sigma), float(dt), int(n_paths), int(steps),
-                      int(seed) & (2**64 - 1), int(path_offset), finals.data_ptr(), maxdd.data_ptr(), _lib.ptr(paths),
-                      _lib.current_stream())
-        return finals, maxdd, paths
+        return self._generate("b200bt_mc_gbm", (float(s0), float(mu), float(sigma), float(dt)), n_paths, steps, seed,
+                              path_offset, steps + 1 if store_paths else None)
 
     def bootstrap(self, returns: np.ndarray, log_returns: bool, s0, n_paths, steps, seed, path_offset=0,
                   block_len=1, store_paths=False):
-        dev = self.device
-        if n_paths == 0:          # a rank without paths (more ranks than paths), as in gbm()
-            e = torch.empty(0, dtype=torch.float32, device=dev)
-            return e, e.clone(), None
-        r = torch.from_numpy(np.ascontiguousarray(returns, dtype=np.float32)).to(dev)
-        finals = torch.empty(n_paths, dtype=torch.float32, device=dev)
-        maxdd = torch.empty(n_paths, dtype=torch.float32, device=dev)
-        paths = torch.empty((steps + 1, n_paths), dtype=torch.float32, device=dev) if store_paths else None
-        with torch.cuda.device(dev):
-            _lib.call("b200bt_mc_bootstrap", r.data_ptr(), int(r.numel()), int(block_len), 1 if log_returns else 0,
-                      float(s0), int(n_paths), int(steps), int(seed) & (2**64 - 1), int(path_offset),
-                      finals.data_ptr(), maxdd.data_ptr(), _lib.ptr(paths), _lib.current_stream())
-        return finals, maxdd, paths
-
-    def _joint_outputs(self, S, n_paths, asset_finals):
-        dev = self.device
-        finals = torch.empty(n_paths, dtype=torch.float32, device=dev)
-        maxdd = torch.empty(n_paths, dtype=torch.float32, device=dev)
-        af = torch.empty((S, n_paths), dtype=torch.float32, device=dev) if asset_finals else None
-        return finals, maxdd, af
+        r = torch.from_numpy(np.ascontiguousarray(returns, dtype=np.float32)).to(self.device)
+        return self._generate("b200bt_mc_bootstrap", (r.data_ptr(), int(r.numel()), int(block_len),
+                                                      1 if log_returns else 0, float(s0)),
+                              n_paths, steps, seed, path_offset, steps + 1 if store_paths else None)
 
     def portfolio_gbm(self, s0, qty, mu, sigma, dt, chol, n_paths, steps, seed, path_offset=0, asset_finals=False):
         """Joint GBM of S assets: per-asset s0 / qty / mu / sigma (length S), `chol` the [S][S] lower Cholesky factor
@@ -182,14 +171,9 @@ class PathEngine:
         drift = (mu - 0.5 * sigma * sigma) * dt     # as b200bt_mc_gbm derives them (:273)
         vol = sigma * np.sqrt(dt)
         L = np.ascontiguousarray(chol, dtype=np.float32).reshape(S, S)
-        finals, maxdd, af = self._joint_outputs(S, n_paths, asset_finals)
-        if n_paths == 0:          # a rank without paths (more ranks than paths), as in gbm()
-            return finals, maxdd, af
-        with torch.cuda.device(self.device):
-            _lib.call("b200bt_mc_portfolio_gbm", S, _c_doubles(s0), _c_doubles(qty), _c_doubles(drift), _c_doubles(vol),
-                      (C.c_float * L.size)(*L.ravel().tolist()), int(n_paths), int(steps), int(seed) & (2**64 - 1),
-                      int(path_offset), finals.data_ptr(), maxdd.data_ptr(), _lib.ptr(af), _lib.current_stream())
-        return finals, maxdd, af
+        return self._generate("b200bt_mc_portfolio_gbm", (S, _c_doubles(s0), _c_doubles(qty), _c_doubles(drift),
+                                                          _c_doubles(vol), (C.c_float * L.size)(*L.ravel().tolist())),
+                              n_paths, steps, seed, path_offset, S if asset_finals else None)
 
     def portfolio_bootstrap(self, returns: np.ndarray, log_returns: bool, s0, qty, n_paths, steps, seed, path_offset=0,
                             block_len=1, asset_finals=False):
@@ -199,16 +183,10 @@ class PathEngine:
         table = np.ascontiguousarray(returns, dtype=np.float32)
         if table.ndim != 2 or table.shape[1] != S:
             raise ValueError(f"return table of shape {table.shape} for {S} assets")
-        finals, maxdd, af = self._joint_outputs(S, n_paths, asset_finals)
-        if n_paths == 0:
-            return finals, maxdd, af
         r = torch.from_numpy(table).to(self.device)
-        with torch.cuda.device(self.device):
-            _lib.call("b200bt_mc_portfolio_bootstrap", S, r.data_ptr(), int(table.shape[0]), int(block_len),
-                      1 if log_returns else 0, _c_doubles(s0), _c_doubles(qty), int(n_paths), int(steps),
-                      int(seed) & (2**64 - 1), int(path_offset), finals.data_ptr(), maxdd.data_ptr(), _lib.ptr(af),
-                      _lib.current_stream())
-        return finals, maxdd, af
+        return self._generate("b200bt_mc_portfolio_bootstrap", (S, r.data_ptr(), int(table.shape[0]), int(block_len),
+                                                                1 if log_returns else 0, _c_doubles(s0), _c_doubles(qty)),
+                              n_paths, steps, seed, path_offset, S if asset_finals else None)
 
     def select(self, x: torch.Tensor, ranks) -> np.ndarray:
         """Exact order statistics x_(k) for ascending 0-based ranks (float32 values as float64)."""
@@ -234,28 +212,55 @@ class PathEngine:
 
 
 def risk_statistics(engine: PathEngine, finals: torch.Tensor, maxdd: torch.Tensor, initial_price: float,
-                    confidence: float) -> Dict:
-    """The statistics block of run_monte_carlo_simulation (:305-336) from device arrays."""
+                    confidence: float, mdd_percentiles=()) -> Dict:
+    """The statistics block of run_monte_carlo_simulation (:305-336) from device arrays, plus `mdd_p<q>`, the q-th
+    percentile of the maximum drawdown, for each q in `mdd_percentiles`."""
     n = int(finals.numel())
-    var_percentile = 100 * (1 - confidence)                       # :316
-    idx = [_virtual_index(n, p) for p in PERCENTILES] + [_virtual_index(n, var_percentile)]
-    ranks = sorted({i for lo, hi, _ in idx for i in (lo, hi)})
-    vals = dict(zip(ranks, engine.select(finals, ranks)))
-    percentile_values = [_lerp(vals[lo], vals[hi], g) for lo, hi, g in idx[:-1]]
-    lo, hi, g = idx[-1]
+    *points, (v_lo, v_hi, g) = percentile_points(partial(engine.select, finals), n,
+                                                 PERCENTILES + [100 * (1 - confidence)])   # :308, :316
     pct = lambda v: (v / initial_price - 1) * 100                 # :312
-    var = _lerp(pct(vals[lo]), pct(vals[hi]), g)                  # :317 on pct_changes (monotone in S_T)
-    mid = sorted({(n - 1) // 2, n // 2})
-    dd_mid = engine.select(maxdd, mid)
+    var = _lerp(pct(v_lo), pct(v_hi), g)                          # :317 on pct_changes (monotone in S_T)
+    # the median is 50's order statistics: the middle one (g = 0, n odd) or the middle two (g = 0.5, n even)
+    (d_lo, d_hi, d_g), *dd_points = percentile_points(partial(engine.select, maxdd), n, [50, *mdd_percentiles])
     m = engine.moments(finals, maxdd, initial_price, var)
     cvar = m[5] / m[6] if m[6] > 0 else float("nan")              # :320
     prob_profit = m[2] / n                                        # :323
-    return {
-        "percentile_values": percentile_values,
+    st = {
+        "percentile_values": [_lerp(lo, hi, g) for lo, hi, g in points],
         "expected_price": m[0] / n, "expected_pct": m[1] / n,
         "var": var, "cvar": cvar, "prob_profit": prob_profit,
-        "mdd_mean": m[3] / n, "mdd_median": float(np.mean(dd_mid)), "mdd_max": float(m[4]),
+        "mdd_mean": m[3] / n, "mdd_median": float(np.mean([d_lo, d_hi] if d_g else [d_lo])), "mdd_max": float(m[4]),
     }
+    for q, (lo, hi, g) in zip(mdd_percentiles, dd_points):
+        st[f"mdd_p{q}"] = _lerp(lo, hi, g)
+    return st
+
+
+def statistics_blocks(st: Dict, initial: float, value_key: str) -> Dict:
+    """The percentiles / expected / risk_metrics blocks of run_monte_carlo_simulation's result (:339-374) from
+    risk_statistics' dict, the value under `value_key` ("price", or "equity" for a trade Monte-Carlo).  The drawdown
+    block has `p95` when the statistics do."""
+    drawdown = {"mean": float(st["mdd_mean"]), "median": float(st["mdd_median"])}
+    if "mdd_p95" in st:
+        drawdown["p95"] = float(st["mdd_p95"])
+    drawdown["max"] = float(st["mdd_max"])
+    return {
+        "percentiles": {str(p): {value_key: float(v), "pct_change": float((v / initial - 1) * 100)}
+                        for p, v in zip(PERCENTILES, st["percentile_values"])},
+        "expected": {value_key: float(st["expected_price"]), "pct_change": float(st["expected_pct"])},
+        "risk_metrics": {
+            "var": float(abs(st["var"])), "cvar": float(abs(st["cvar"])),
+            "prob_profit": float(st["prob_profit"]), "prob_loss": float(1 - st["prob_profit"]),
+            "max_drawdown": drawdown,
+        },
+    }
+
+
+def _world_rank():
+    """(world size, rank) under torch.distributed, (1, 0) without it."""
+    if torch.distributed.is_available() and torch.distributed.is_initialized():
+        return torch.distributed.get_world_size(), torch.distributed.get_rank()
+    return 1, 0
 
 
 class MonteCarloService:
@@ -308,9 +313,7 @@ class MonteCarloService:
             periods_per_year = 252
             mu = returns.mean() * periods_per_year                       # :243
             sigma = returns.std() * np.sqrt(periods_per_year)            # :244 (pandas ddof=1)
-            scenario_params = self.mc_params["scenarios"].get(scenario, {})
-            drift_factor = scenario_params.get("drift_factor", 1.0)
-            volatility_factor = scenario_params.get("volatility_factor", 1.0)
+            drift_factor, volatility_factor = self._scenario_factors(scenario)
             mu = mu * drift_factor
             sigma = sigma * volatility_factor
             dt = 1 / periods_per_year
@@ -323,9 +326,7 @@ class MonteCarloService:
             # under torch.distributed the paths are sharded over the ranks (Philox is keyed by the global path index:
             # the result does not depend on the number of GPUs) and gathered once for the statistics
             from .dist import gather_paths, shard_bounds
-            world, rank = 1, 0
-            if torch.distributed.is_available() and torch.distributed.is_initialized() and not store:
-                world, rank = torch.distributed.get_world_size(), torch.distributed.get_rank()
+            world, rank = (1, 0) if store else _world_rank()
             lo, hi, _ = shard_bounds(int(num_simulations), world, rank)
             if method == "geometric_brownian_motion":
                 finals, maxdd, paths = eng.gbm(initial_price, mu, sigma, dt, hi - lo, steps, seed, path_offset=lo,
@@ -345,15 +346,7 @@ class MonteCarloService:
                 "num_simulations": num_simulations, "mu": mu, "sigma": sigma,
                 "drift_factor": drift_factor, "volatility_factor": volatility_factor,
                 "simulation_method": method, "scenario": scenario, "timestamp": datetime.now().isoformat(),
-                "percentiles": {str(p): {"price": float(v), "pct_change": float((v / initial_price - 1) * 100)}
-                                for p, v in zip(PERCENTILES, st["percentile_values"])},
-                "expected": {"price": float(st["expected_price"]), "pct_change": float(st["expected_pct"])},
-                "risk_metrics": {
-                    "var": float(abs(st["var"])), "cvar": float(abs(st["cvar"])),
-                    "prob_profit": float(st["prob_profit"]), "prob_loss": float(1 - st["prob_profit"]),
-                    "max_drawdown": {"mean": float(st["mdd_mean"]), "median": float(st["mdd_median"]),
-                                     "max": float(st["mdd_max"])},
-                },
+                **statistics_blocks(st, initial_price, "price"),
                 "paths": paths.cpu().numpy().astype(np.float64).tolist() if store else None,
             }
             self.simulation_results[symbol] = results
@@ -453,15 +446,11 @@ class MonteCarloService:
                 return {}
             periods_per_year, confidence = 252, self.mc_params["confidence_level"]
             steps = int(days) - 1
-            world, rank = 1, 0
-            if torch.distributed.is_available() and torch.distributed.is_initialized():
-                world, rank = torch.distributed.get_world_size(), torch.distributed.get_rank()
+            world, rank = _world_rank()
             lo, hi, _ = shard_bounds(int(num_simulations), world, rank)
             results = {}
             for scenario in scenarios:
-                scenario_params = self.mc_params["scenarios"].get(scenario, {})
-                drift_factor = scenario_params.get("drift_factor", 1.0)
-                volatility_factor = scenario_params.get("volatility_factor", 1.0)
+                drift_factor, volatility_factor = self._scenario_factors(scenario)
                 mu = np.array([u[4].mean() * periods_per_year * drift_factor for u in used])                # :243
                 sigma = np.array([u[4].std() * np.sqrt(periods_per_year) * volatility_factor for u in used])  # :244
                 seed = self.seed + self._sim_counter
@@ -476,24 +465,20 @@ class MonteCarloService:
                 if world > 1:
                     finals, maxdd = gather_paths(finals, maxdd, int(num_simulations))
                     af = gather_path_rows(af, int(num_simulations))
-                st = risk_statistics(eng, finals, maxdd, v0, confidence)
-                asset_var = [abs(_var_pct(eng, af[i], s0[i], confidence)) for i in range(len(assets))]
+                blocks = statistics_blocks(risk_statistics(eng, finals, maxdd, v0, confidence), v0, "price")
+                asset_var = []
+                for row, p0 in zip(af, s0):                              # risk_statistics' VaR (:316-317) of each asset
+                    [(x_lo, x_hi, g)] = percentile_points(partial(eng.select, row), int(row.numel()),
+                                                          [100 * (1 - confidence)])
+                    asset_var.append(abs(_lerp((x_lo / p0 - 1) * 100, (x_hi / p0 - 1) * 100, g)))
                 undiversified = float(sum(w * v for w, v in zip(weights.tolist(), asset_var)))
-                var = float(abs(st["var"]))
+                var = blocks["risk_metrics"]["var"]
                 results[scenario] = {
                     "scenario": scenario, "time_horizon_days": days, "num_simulations": num_simulations,
                     "simulation_method": method, "initial_value": v0,
                     "drift_factor": drift_factor, "volatility_factor": volatility_factor,
                     "mu": dict(zip(assets, mu.tolist())), "sigma": dict(zip(assets, sigma.tolist())),
-                    "percentiles": {str(p): {"price": float(v), "pct_change": float((v / v0 - 1) * 100)}
-                                    for p, v in zip(PERCENTILES, st["percentile_values"])},
-                    "expected": {"price": float(st["expected_price"]), "pct_change": float(st["expected_pct"])},
-                    "risk_metrics": {
-                        "var": var, "cvar": float(abs(st["cvar"])),
-                        "prob_profit": float(st["prob_profit"]), "prob_loss": float(1 - st["prob_profit"]),
-                        "max_drawdown": {"mean": float(st["mdd_mean"]), "median": float(st["mdd_median"]),
-                                         "max": float(st["mdd_max"])},
-                    },
+                    **blocks,
                     "undiversified_var": undiversified,
                     "diversification_benefit": undiversified - var,
                 }
@@ -522,6 +507,11 @@ class MonteCarloService:
         except Exception as e:  # reference convention: log, return {}
             logger.error("Error running joint portfolio Monte Carlo simulation: %s", e, exc_info=True)
             return {}
+
+    def _scenario_factors(self, scenario: str):
+        """(drift_factor, volatility_factor) of a configured scenario, 1.0 for a factor it leaves out."""
+        params = self.mc_params["scenarios"].get(scenario, {})
+        return params.get("drift_factor", 1.0), params.get("volatility_factor", 1.0)
 
     def _calculate_portfolio_stats(self, holdings: Dict, simulations: Dict) -> Dict:
         """Value-weighted sums per scenario, correlations ignored (:577-659)."""

@@ -12,13 +12,14 @@ VaR / CVaR agree with the float64 reference to ~1e-6 relative, the correlation t
 from __future__ import annotations
 
 import logging
+from functools import partial
 from typing import Dict, List, Optional, Sequence
 
 import numpy as np
 import torch
 
 from . import _lib
-from .monte_carlo import PathEngine, _lerp, _virtual_index
+from .monte_carlo import PathEngine, _lerp, percentile_points
 
 logger = logging.getLogger("b200bt.portfolio_risk")
 
@@ -73,10 +74,8 @@ class PortfolioRiskService:
         return self._ws
 
     def _percentile(self, x: torch.Tensor, q: float) -> float:
-        lo, hi, g = _virtual_index(int(x.numel()), q)
-        ranks = sorted({lo, hi})
-        vals = dict(zip(ranks, self._engine.select(x, ranks)))
-        return _lerp(vals[lo], vals[hi], g)
+        [(lo, hi, g)] = percentile_points(partial(self._engine.select, x), int(x.numel()), [q])
+        return _lerp(lo, hi, g)
 
     def _tail(self, x: torch.Tensor, threshold: float) -> np.ndarray:
         n = int(x.numel())

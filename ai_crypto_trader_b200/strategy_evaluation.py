@@ -335,7 +335,8 @@ class StrategyEvaluationSystem:
         run_monte_carlo_simulation's (monte_carlo_service.py:339-374) with equity in place of price; `original` holds
         the unresampled sequence's values, `num_trades` counts round trips (two records each).  Logs and returns {} on
         failure (:392)."""
-        from .trade_monte_carlo import TradeMonteCarlo, result_blocks
+        from .monte_carlo import risk_statistics, statistics_blocks
+        from .trade_monte_carlo import TradeMonteCarlo
         try:
             if not market_data:
                 logger.error("No market data for the trade Monte-Carlo of %s", strategy_id)
@@ -349,7 +350,8 @@ class StrategyEvaluationSystem:
             capital = float(sweep.cfg.initial_capital)
             mc = TradeMonteCarlo(sweep.market.device)
             finals, maxdd = mc.simulate(trip, n_trips, fee, num_simulations, simulation_method, block_len, capital, seed)
-            blocks = result_blocks(mc.statistics(finals[0], maxdd[0], capital, confidence_level), capital)
+            blocks = statistics_blocks(risk_statistics(mc.engine, finals[0], maxdd[0], capital, confidence_level,
+                                                       mdd_percentiles=(95,)), capital, "equity")
             net = float(st["net_profit"][0, 0])
             return {
                 "strategy_id": strategy_id, "symbol": market_data[0].get("symbol", "BTCUSDT"),
@@ -376,7 +378,7 @@ class StrategyEvaluationSystem:
         by the 5th-percentile return or the 95th-percentile drawdown.  Lane id of (i, s) = i * S + s.  Returns [pop][S]
         arrays of the scalars of monte_carlo_trades' dict: num_trades, original_final_equity / return_pct / max_drawdown,
         MC_POPULATION_FIELDS, and [pop][S][9] arrays percentile_equity / percentile_pct_change at `percentiles`."""
-        from .monte_carlo import PERCENTILES
+        from .monte_carlo import PERCENTILES, risk_statistics
         from .trade_monte_carlo import TradeMonteCarlo
         sweep = sweep or PopulationSweep(market, optimization_goals=self.optimization_goals)
         trip, n_trips, fee = sweep.trade_pnl(population)
@@ -400,7 +402,7 @@ class StrategyEvaluationSystem:
                                         simulation_method, block_len, capital, seed, lane_ids=np.arange(lo, hi))
             for r in range(hi - lo):
                 i, s = divmod(lo + r, S)
-                q = mc.statistics(finals[r], maxdd[r], capital, confidence_level)
+                q = risk_statistics(mc.engine, finals[r], maxdd[r], capital, confidence_level, mdd_percentiles=(95,))
                 pv = np.asarray(q["percentile_values"])
                 out["percentile_equity"][i, s] = pv
                 out["percentile_pct_change"][i, s] = (pv / capital - 1) * 100

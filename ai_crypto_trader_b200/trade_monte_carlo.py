@@ -9,22 +9,22 @@ item "BACK-04: Add Monte Carlo simulations", BACKLOG.md:194).
     StrategyEvaluationSystem._simulate_trades' records);
   * the paths: TradeMonteCarlo.simulate (kernel b200bt_trade_mc: bootstrap, block bootstrap or keyed shuffle of the
     round trips, float64 equity walk in calculate_metrics' record order, strategy_evaluation.py:119-139);
-  * the statistics: TradeMonteCarlo.statistics = monte_carlo.risk_statistics (the statistics block of
-    run_monte_carlo_simulation, monte_carlo_service.py:305-336) on one lane with equity for price, plus the 95th
-    percentile of the maximum drawdown through the same exact select.
+  * the statistics: monte_carlo.risk_statistics (the statistics block of run_monte_carlo_simulation,
+    monte_carlo_service.py:305-336) on one lane with equity for price and mdd_percentiles=(95,), and
+    monte_carlo.statistics_blocks(..., "equity") for the result blocks.
 
 StrategyEvaluationSystem.monte_carlo_trades / monte_carlo_population are the user-facing calls.
 """
 from __future__ import annotations
 
 import ctypes as C
-from typing import Dict, Optional
+from typing import Optional
 
 import numpy as np
 import torch
 
 from . import _lib
-from .monte_carlo import PERCENTILES, PathEngine, _lerp, _virtual_index, risk_statistics
+from .monte_carlo import PathEngine
 
 
 def _host(x, dtype) -> np.ndarray:
@@ -66,30 +66,3 @@ class TradeMonteCarlo:
                       int(seed) & (2**64 - 1), int(path_offset), finals.data_ptr(), maxdd.data_ptr(),
                       _lib.current_stream())
         return finals, maxdd
-
-    def statistics(self, finals: torch.Tensor, maxdd: torch.Tensor, initial_capital: float = 10000.0,
-                   confidence: float = 0.95) -> Dict:
-        """risk_statistics of one lane's rows (initial price = initial capital) and `mdd_p95`, the 95th percentile of
-        the maximum drawdown (np.percentile's linear rule on exact order statistics)."""
-        st = risk_statistics(self.engine, finals, maxdd, initial_capital, confidence)
-        lo, hi, g = _virtual_index(int(maxdd.numel()), 95)
-        ranks = sorted({lo, hi})
-        vals = dict(zip(ranks, self.engine.select(maxdd, ranks)))
-        st["mdd_p95"] = _lerp(vals[lo], vals[hi], g)
-        return st
-
-
-def result_blocks(st: Dict, initial_capital: float) -> Dict:
-    """The percentiles / expected / risk_metrics blocks of run_monte_carlo_simulation's result (:339-374), with equity
-    in place of price and the maximum drawdown's 95th percentile added."""
-    return {
-        "percentiles": {str(p): {"equity": float(v), "pct_change": float((v / initial_capital - 1) * 100)}
-                        for p, v in zip(PERCENTILES, st["percentile_values"])},
-        "expected": {"equity": float(st["expected_price"]), "pct_change": float(st["expected_pct"])},
-        "risk_metrics": {
-            "var": float(abs(st["var"])), "cvar": float(abs(st["cvar"])),
-            "prob_profit": float(st["prob_profit"]), "prob_loss": float(1 - st["prob_profit"]),
-            "max_drawdown": {"mean": float(st["mdd_mean"]), "median": float(st["mdd_median"]),
-                             "p95": float(st["mdd_p95"]), "max": float(st["mdd_max"])},
-        },
-    }

@@ -82,8 +82,14 @@ def test_joint_bootstrap_matches_oracle(engine, S, log_returns, block_len):
     np.testing.assert_allclose(d.cpu().numpy(), do, rtol=2e-4, atol=2e-6)
 
 
-def test_comonotone_quantiles_add(engine):
-    from ai_crypto_trader_b200.monte_carlo import _var_pct
+def test_comonotone_var_percentile_points_add(engine):
+    from functools import partial
+    from ai_crypto_trader_b200.monte_carlo import _lerp, percentile_points
+
+    def var_pct(x, initial):                        # risk_statistics' VaR: the 5th percentile of the percentage change
+        [(lo, hi, g)] = percentile_points(partial(engine.select, x), int(x.numel()), [100 * (1 - 0.95)])
+        return _lerp((lo / initial - 1) * 100, (hi / initial - 1) * 100, g)
+
     S = 4
     s0 = np.array([100.0, 20.0, 3.0, 0.7])
     qty = np.array([1.0, 4.0, 10.0, 50.0])
@@ -93,8 +99,8 @@ def test_comonotone_quantiles_add(engine):
     L[:, 0] = 1.0                                   # every asset driven by the same normal
     f, _, af = engine.portfolio_gbm(s0, qty, mu, sigma, DT, L, 200_001, 29, 5, asset_finals=True)
     v0 = float(np.sum(qty * s0))
-    joint = _var_pct(engine, f, v0, 0.95)
-    per_asset = [_var_pct(engine, af[i].contiguous(), s0[i], 0.95) for i in range(S)]
+    joint = var_pct(f, v0)
+    per_asset = [var_pct(af[i].contiguous(), s0[i]) for i in range(S)]
     assert all(v < 0 for v in per_asset)
     w = qty * s0 / v0
     assert joint == pytest.approx(float(np.dot(w, per_asset)), rel=1e-5)

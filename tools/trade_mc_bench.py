@@ -8,7 +8,8 @@ swept once; the `--top` individuals by fitness x all symbols are the lanes.  Tim
   * extraction: PopulationSweep.trade_pnl (two sweeps of the top individuals + b200bt_trade_pnl), host clock;
   * the Monte-Carlo kernel (b200bt_trade_mc) for `bootstrap` (block 1) and `shuffle`: CUDA events, warmed up, `--reps`
     repetitions; round-trip steps/s = paths x sum(T) / kernel time;
-  * the statistics of every lane (TradeMonteCarlo.statistics: a few launches and a read-back per lane), host clock.
+  * the statistics of every lane (risk_statistics with the drawdown's p95: a few launches and a read-back per lane),
+    host clock.
 Prints one JSON line with the card's name, power limit and the SM clock sampled during the kernel timing, the trip
 counts (min / median / max / sum) and the registers / local memory of the new kernels.  Needs an H100; no fallback.
 """
@@ -72,6 +73,7 @@ def main():
     from bench import ClockSampler
     from ai_crypto_trader_b200 import synth
     from ai_crypto_trader_b200.sweep import MarketData, PopulationSweep
+    from ai_crypto_trader_b200.monte_carlo import risk_statistics
     from ai_crypto_trader_b200.trade_monte_carlo import TradeMonteCarlo
     torch.cuda.set_device(0)
     market = MarketData(synth.synth_ohlcv(a.symbols, a.bars))
@@ -112,7 +114,8 @@ def main():
         w1 = time.time()
         ms = e0.elapsed_time(e1) / a.reps
         t0 = time.perf_counter()
-        p5 = [mc.statistics(finals[r], maxdd[r], 10000.0, 0.95)["percentile_values"][1] for r in range(len(nt))]
+        p5 = [risk_statistics(mc.engine, finals[r], maxdd[r], 10000.0, 0.95, mdd_percentiles=(95,))["percentile_values"][1]
+              for r in range(len(nt))]
         stats_ms = (time.perf_counter() - t0) * 1e3
         legs[method] = {"kernel_ms": ms, "round_trip_steps_per_s": a.paths * sum_t / (ms * 1e-3),
                         "statistics_ms_all_lanes": stats_ms, "statistics_ms_per_lane": stats_ms / len(nt),
