@@ -249,12 +249,17 @@ def predicted_events(population: List[Dict], n_bars: int) -> np.ndarray:
     return EVENTS_PER_COST_BAR * lane_costs(population) * n_bars
 
 
+def _band_costs(period: np.ndarray, oversold: np.ndarray, overbought: np.ndarray) -> np.ndarray:
+    """lane_cost's band model on arrays of RSI windows and float64 thresholds."""
+    from scipy.special import ndtr
+    sd = 44.0 / np.sqrt(np.maximum(period, 1))
+    return ndtr((oversold - 50.0) / sd) + 1.0 - ndtr((overbought - 50.0) / sd)
+
+
 def lane_costs(population: List[Dict]) -> np.ndarray:
     """lane_cost for a whole population (vectorised)."""
-    from scipy.special import ndtr
     g = lambda key, default: np.array([float(p.get(key, default)) for p in population], dtype=np.float64)
-    sd = 44.0 / np.sqrt(np.maximum(g("rsi_period", 14).astype(np.int64), 1))
-    return ndtr((g("rsi_oversold", 30) - 50.0) / sd) + 1.0 - ndtr((g("rsi_overbought", 70) - 50.0) / sd)
+    return _band_costs(g("rsi_period", 14).astype(np.int64), g("rsi_oversold", 30), g("rsi_overbought", 70))
 
 
 _HASH_MULTIPLIERS = np.array([0x9E3779B97F4A7C15, 0xC2B2AE3D27D4EB4F, 0x165667B19E3779F9, 0x27D4EB2F165667C5,
@@ -281,11 +286,9 @@ def _duplicate_classes(packed: np.ndarray):
 def costs_from_packed(packed: np.ndarray, periods: Sequence[int], timeframes: Sequence[int] = (1,)) -> np.ndarray:
     """lane_cost of already decoded individuals (b200bt_individual records): no second pass over the dicts.  An RSI row
     of a k-times slower clock changes every k bars: its threshold crossings (events) are rarer by about sqrt(k)."""
-    from scipy.special import ndtr
     P = len(periods)
     w = np.asarray(periods, dtype=np.float64)[packed["rsi_row"] % P]
-    sd = 44.0 / np.sqrt(np.maximum(w, 1.0))
-    c = ndtr((packed["rsi_lo"].astype(np.float64) - 50.0) / sd) + 1.0 - ndtr((packed["rsi_hi"].astype(np.float64) - 50.0) / sd)
+    c = _band_costs(w, packed["rsi_lo"].astype(np.float64), packed["rsi_hi"].astype(np.float64))
     if len(timeframes) > 1:
         k = np.asarray(timeframes, dtype=np.float64)[packed["rsi_row"] // P] / float(timeframes[0])
         c = c / np.sqrt(k)
@@ -304,7 +307,6 @@ def _sm_count(device) -> int:
 
 
 _PINNED_FLAGS = None
-DEFERRED = torch.empty(0, dtype=torch.uint8)      # sentinel: the caller assigns plan.workspace (plan_batches)
 _FLAG_SLOTS = 256
 
 
@@ -327,54 +329,76 @@ def _flag_slot() -> torch.Tensor:
     return _pinned_flags()[i]
 
 
-class ChunkPlan:
-    """Host-side plan of the time-chunked sweep for one population (device tensors inside)."""
+class _Plan:
+    """What the plans of both time-chunked schedules share.  A plan covers the slice [lo, lo + pop) of the caller's
+    population (individual indices inside it are slice-relative); `pred` = predicted_events of that slice when the caller
+    already has it.  A plan sizes its workspace (`ws_bytes`); _allocate_plans gives it its device buffers."""
+
+    def _start(self, population: List[Dict], n_bars: int, lo: int, pred: Optional[np.ndarray]) -> np.ndarray:
+        self.lo, self.pop = int(lo), len(population)
+        self.workspace = self.invalid = self.overflow = None
+        return predicted_events(population, n_bars) if pred is None else np.asarray(pred, dtype=np.float64)
+
+    def _size_pool(self, pred: np.ndarray, n_symbols: int, pool_scale: float, pool_blocks: Optional[int]) -> None:
+        """Event pool in blocks of 256 events, once n_seg is known."""
+        self.pred_blocks = float(pred.sum()) * n_symbols / 256
+        # every segment owns at least one block, and a repaired segment abandons its first chain
+        self.pool_blocks = (int(pool_scale * self.pred_blocks) + 2 * self.n_seg * n_symbols + 1024 if pool_blocks is None
+                            else int(pool_blocks))
+
+
+def _allocate_plans(plans: List[_Plan], n_symbols: int, device) -> List[_Plan]:
+    """The device buffers of the plans of one call: one workspace, of the largest size any of them needs (their slices run
+    one after the other on the same stream), then every plan's lane fallback flags and pinned flag row."""
+    # keep this order: with the small buffers allocated before the workspace, the same lane_scan_kernel took 1.3 % longer
+    # on the configs[1] workload (H100 80GB HBM3, 400 W power limit), from where the allocations landed in device memory
+    shared = torch.empty(max(pl.ws_bytes for pl in plans), dtype=torch.uint8, device=device)
+    for pl in plans:
+        pl.workspace = shared
+        pl.invalid = torch.zeros((pl.pop, n_symbols), dtype=torch.uint8, device=device)
+        pl.overflow = _flag_slot()
+    return plans
+
+
+class ChunkPlan(_Plan):
+    """Host-side plan of the time-chunked sweep for one population slice (device tensors inside)."""
 
     def __init__(self, population: List[Dict], n_bars: int, n_symbols: int, device, target_events: int = 16384,
                  warm: int = 8192, max_chunks: int = 64, pool_scale: float = 1.5, pool_blocks: Optional[int] = None,
-                 max_repair_rounds: int = 8, lo: int = 0, workspace: Optional[torch.Tensor] = None,
-                 pred: Optional[np.ndarray] = None):
-        """`population` is the slice [lo, lo + len) of the caller's population (individual indices inside the
-        plan are slice-relative); `workspace` may be shared between the plans of successive slices; `pred` =
-        predicted_events(population, n_bars) when the caller already has it."""
-        pop = len(population)
-        self.lo = int(lo)
-        pred = predicted_events(population, n_bars) if pred is None else np.asarray(pred, dtype=np.float64)
+                 max_repair_rounds: int = 8, lo: int = 0, pred: Optional[np.ndarray] = None):
+        pred = self._start(population, n_bars, lo, pred)
         kmax = max(1, min(max_chunks, n_bars // max(8 * warm, 2048)))
         k = np.clip(np.ceil(pred / target_events), 1, kmax).astype(np.int32)
         self.n_chunks = k
         self.seg_base = np.concatenate([[0], np.cumsum(k)[:-1]]).astype(np.int32)
         self.n_seg = int(k.sum())
-        self.order = np.argsort(-pred, kind="stable").astype(np.int32)      # (b200bt_sweep_chunked ignores it)
         items = np.zeros((self.n_seg, 4), dtype=np.int32)
         # most expensive work first (per-chunk cost), keeping one individual's chunks together
         per_chunk = pred / k
         row = 0
-        for i in sorted(range(pop), key=lambda j: (-per_chunk[j], int(population[j].get("rsi_period", 14)))):
+        for i in sorted(range(self.pop), key=lambda j: (-per_chunk[j], int(population[j].get("rsi_period", 14)))):
             for c in range(int(k[i])):
                 items[row] = (i, c, k[i], self.seg_base[i] + c)
                 row += 1
         self.warm = int(warm)
         self.max_repair_rounds = int(max_repair_rounds)
-        self.pred_blocks = float(pred.sum()) * n_symbols / 256
-        self.pool_blocks = int(pool_scale * self.pred_blocks) + 2 * self.n_seg * n_symbols + 1024
-        if pool_blocks is not None:
-            self.pool_blocks = int(pool_blocks)
+        self._size_pool(pred, n_symbols, pool_scale, pool_blocks)
         self.items = torch.from_numpy(items).to(device)
         self.seg_base_dev = torch.from_numpy(self.seg_base).to(device)
         self.n_chunks_dev = torch.from_numpy(self.n_chunks).to(device)
-        self.order_dev = torch.from_numpy(self.order).to(device)
         self.ws_bytes = int(_lib.load().b200bt_sweep_chunked_workspace_bytes(self.pool_blocks, n_symbols, self.n_seg))
-        if workspace is not None and workspace.numel() >= self.ws_bytes:
-            self.workspace = workspace
-        else:
-            self.workspace = None if workspace is DEFERRED else torch.empty(self.ws_bytes, dtype=torch.uint8, device=device)
-        self.invalid = torch.zeros((pop, n_symbols), dtype=torch.uint8, device=device)
-        self.overflow = _flag_slot()
-        self.pop = pop
+
+    def launch(self, sweep: "PopulationSweep", data: tuple, indiv: int, stats: torch.Tensor,
+               events: Optional[torch.Tensor], event_cap: int, stream) -> None:
+        """b200bt_sweep_chunked on this slice: `data` = PopulationSweep._data_args(), `indiv` = address of the slice's first
+        record, `stats` / `events` = the slice's rows."""
+        _lib.call("b200bt_sweep_chunked", *data, indiv, None, self.pop, self.items.data_ptr(), self.n_seg,
+                  self.seg_base_dev.data_ptr(), self.n_chunks_dev.data_ptr(), self.n_seg, self.warm, self.max_repair_rounds,
+                  self.pool_blocks, self.workspace.data_ptr(), self.workspace.numel(), C.byref(sweep.cfg), stats.data_ptr(),
+                  _lib.ptr(events), event_cap, self.invalid.data_ptr(), self.overflow.data_ptr(), stream)
 
 
-class TilePlan:
+class TilePlan(_Plan):
     """Host-side plan of the thread-per-lane sweep (b200bt_sweep_tiled) for one population slice: every
     individual gets the same K time chunks, chosen so that the CTAs fill whole waves of the GPU."""
 
@@ -400,34 +424,30 @@ class TilePlan:
     def __init__(self, population: List[Dict], n_bars: int, n_symbols: int, device, warm: int = WARM,
                  max_chunks: int = 64, chunks: Optional[int] = None, pool_scale: float = 1.5,
                  pool_blocks: Optional[int] = None, max_repair_rounds: Optional[int] = None, lo: int = 0,
-                 workspace: Optional[torch.Tensor] = None, order_by: str = "row_cost", pred: Optional[np.ndarray] = None,
-                 rows: Optional[np.ndarray] = None):
-        pop = len(population)
-        self.lo, self.pop = int(lo), pop
+                 order_by: str = "row_cost", pred: Optional[np.ndarray] = None, rows: Optional[np.ndarray] = None):
+        pred = self._start(population, n_bars, lo, pred)
         self.warm = int(warm)
-        pred = predicted_events(population, n_bars) if pred is None else np.asarray(pred, dtype=np.float64)
         # thread slots: 32 consecutive slots = one warp, which stages its own tiles and may read two distinct RSI rows
         self.slots = pack_warps(population, pred, order_by, rows)
         if chunks is None:
-            chunks = self.chunks_for(pop, n_bars, n_symbols, device, warm, max_chunks, n_slots=len(self.slots))
+            chunks = self.chunks_for(self.pop, n_bars, n_symbols, device, warm, max_chunks, n_slots=len(self.slots))
         self.K = int(chunks)
         # 0 = no repair, 1 = the bounded pass on the critical path, 2 = that and the unbounded pass beside the metrics
         self.max_repair_rounds = int(max_repair_rounds) if max_repair_rounds is not None else 2
-        self.n_seg = pop * self.K
-        # every segment owns at least one block, and a repaired segment abandons its first chain
-        self.pred_blocks = float(pred.sum()) * n_symbols / 256
-        self.pool_blocks = int(pool_scale * self.pred_blocks) + 2 * self.n_seg * n_symbols + 1024
-        if pool_blocks is not None:
-            self.pool_blocks = int(pool_blocks)
+        self.n_seg = self.pop * self.K
+        self._size_pool(pred, n_symbols, pool_scale, pool_blocks)
         self.order = np.ascontiguousarray(self.slots[self.slots >= 0])      # individuals in dispatch order
         self.slots_dev = torch.from_numpy(np.concatenate([self.slots, self.order])).to(device)     # [slots | order]
-        self.ws_bytes = int(_lib.load().b200bt_sweep_tiled_workspace_bytes(self.pool_blocks, n_symbols, pop, self.K))
-        if workspace is not None and workspace.numel() >= self.ws_bytes:
-            self.workspace = workspace
-        else:
-            self.workspace = None if workspace is DEFERRED else torch.empty(self.ws_bytes, dtype=torch.uint8, device=device)
-        self.invalid = torch.zeros((pop, n_symbols), dtype=torch.uint8, device=device)
-        self.overflow = _flag_slot()
+        self.ws_bytes = int(_lib.load().b200bt_sweep_tiled_workspace_bytes(self.pool_blocks, n_symbols, self.pop, self.K))
+
+    def launch(self, sweep: "PopulationSweep", data: tuple, indiv: int, stats: torch.Tensor,
+               events: Optional[torch.Tensor], event_cap: int, stream) -> None:
+        """b200bt_sweep_tiled on this slice (arguments as ChunkPlan.launch)."""
+        n_slots = len(self.slots)
+        _lib.call("b200bt_sweep_tiled", *data, _lib.ptr(sweep._zones_if_amortised()), indiv, self.slots_dev.data_ptr(),
+                  n_slots, self.slots_dev.data_ptr() + 4 * n_slots, self.pop, self.K, self.warm, self.max_repair_rounds,
+                  self.pool_blocks, self.workspace.data_ptr(), self.workspace.numel(), C.byref(sweep.cfg), stats.data_ptr(),
+                  _lib.ptr(events), event_cap, self.invalid.data_ptr(), self.overflow.data_ptr(), stream)
 
 
 WARP_RSI_ROWS = 2       # distinct RSI rows the machines of one warp may read (csrc/sweep_chunked.cu LS_RSI_ROWS)
@@ -507,8 +527,15 @@ class PopulationSweep:
         mode: "fused" (one warp per lane, serial in time), "chunked" (expensive lanes split into verified
         time chunks, one warp per chunk), "tiled" (every lane split into the same K verified chunks, one THREAD
         per chunk; csrc/sweep_chunked.cu) or "auto" (tiled from 131072 bars up, fused below)."""
+        self._setup(market, sorted(set(int(p) for p in rsi_periods)), optimization_goals, initial_capital, event_cap, mode,
+                    chunk_options, score_on_advanced, timeframes)
+
+    def _setup(self, market: MarketData, periods: List[int], optimization_goals: Optional[Dict], initial_capital: float,
+               event_cap: int, mode: str, chunk_options: Optional[Dict], score_on_advanced: bool, timeframes: Sequence[int],
+               bank: Optional[torch.Tensor] = None) -> None:
+        """The initialisation of both constructors: `periods` in bank-row order, `bank` = None computes the bank."""
         self.market = market
-        self.periods = sorted(set(int(p) for p in rsi_periods))
+        self.periods = periods
         self.period_row = {p: i for i, p in enumerate(self.periods)}
         goals = optimization_goals or DEFAULT_GOALS
         primary, mask = _lib.score_codes(goals, advanced=score_on_advanced)
@@ -522,26 +549,33 @@ class PopulationSweep:
         self.timeframes = tuple(int(k) for k in timeframes) or (market.bar_minutes,)
         if self.timeframes[0] != market.bar_minutes or any(k % market.bar_minutes for k in self.timeframes):
             raise ValueError("timeframes must start with the market's own bar spacing and be multiples of it")
-        self.bank = self._bank_behind_the_upload(market) if len(self.timeframes) == 1 else self._multi_timeframe_bank(market)
         self.mode, self.chunk_min_bars, self.chunk_options = mode, 131072, dict(chunk_options or {})
-        self._stats = None
-        self._events = None
-        self._pop = 0
-        self._pinned_in = None
-        self._pinned_out = None
+        self._zones = None             # zone map of the bank: made with a computed one-clock bank, else on first use
+        if bank is not None:
+            self.bank = bank
+        elif len(self.timeframes) == 1:
+            self.bank, self._zones = self._bank_behind_the_upload(market)
+        else:
+            self.bank = self._multi_timeframe_bank(market)
+        self._stats = self._events = None      # lane stats / event words of the last evaluation (_buffers)
+        self._buffer_key = None                # (pop, event_cap) they were allocated for
+        self._inverse = None                   # last evaluate(): its population -> row of its unique individuals
+        self._last_plans = []                  # plans of the last evaluation, whose pinned flags _flags reads
+        self._pool_factor = 1.0                # event-pool scale learnt from earlier sweeps (_pool_options)
+        self._tiled_sweeps = 0                 # thread-per-lane slices swept so far (_zones_if_amortised)
+        self._pinned_in = self._pinned_out = None
+        self.last_unique = self.h2d_bytes = self.d2h_bytes = 0      # of the last evaluate()
 
-    def _bank_behind_the_upload(self, market: MarketData) -> torch.Tensor:
-        """RSI bank of the market.  While the close prices are still arriving in quarter copies (MarketData from a
-        pinned host tensor), each quarter's rows are computed on that quarter's copy stream, so the bank is ready one
+    def _bank_behind_the_upload(self, market: MarketData) -> Tuple[torch.Tensor, torch.Tensor]:
+        """RSI bank of the market and its zone map.  While the close prices are still arriving in quarter copies (MarketData
+        from a pinned host tensor), each quarter's rows are computed on that quarter's copy stream, so the bank is ready one
         quarter of its kernel time after the last byte instead of one whole kernel."""
         parts = market._close_parts
         P = len(self.periods)
         # the zone map of the bank (ranges of every 32-bar block and 4-bar group) comes out of the same pass
         zones = torch.empty(int(_lib.load().b200bt_zone_map_floats(P, market.S, market.N)), dtype=torch.float32, device=market.device)
         if not parts:
-            bank = rsi_bank(market.close, self.periods, zones=zones, zones_symbols=market.S)
-            self._zones = zones
-            return bank
+            return rsi_bank(market.close, self.periods, zones=zones, zones_symbols=market.S), zones
         bank = torch.empty((market.S, P, market.N), dtype=torch.float32, device=market.device)
         cur = torch.cuda.current_stream(market.device)
         for lo, hi, st in parts:
@@ -549,8 +583,7 @@ class PopulationSweep:
             with torch.cuda.stream(st):
                 rsi_bank(market._ohlcv[3, lo:hi], self.periods, out=bank[lo:hi], zones=zones, zones_symbols=market.S, first_symbol=lo)
         market._join_close()                           # the current stream now waits for copies AND bank rows
-        self._zones = zones
-        return bank
+        return bank, zones
 
     def _multi_timeframe_bank(self, market: MarketData) -> torch.Tensor:
         """[S][T * P][N] bank: block 0 = RSI of the base clock, block i = RSI of the clock-aligned timeframes[i]-minute bars
@@ -575,124 +608,89 @@ class PopulationSweep:
                   score_on_advanced: bool = False) -> "PopulationSweep":
         """Sweep over a caller-supplied RSI bank [S][P][N] (e.g. the 'rsi' field of the reference's
         market-data points) instead of one computed from the close prices."""
+        periods = [int(p) for p in periods]
+        assert bank.is_cuda and bank.dtype == torch.float32 and tuple(bank.shape) == (market.S, len(periods), market.N)
         self = cls.__new__(cls)
-        self.market = market
-        self.periods = [int(p) for p in periods]
-        self.period_row = {p: i for i, p in enumerate(self.periods)}
-        goals = optimization_goals or DEFAULT_GOALS
-        primary, mask = _lib.score_codes(goals, advanced=score_on_advanced)
-        self.cfg = _lib.SweepConfig(initial_capital=float(initial_capital), minute0=market.minute0,
-                                    bar_minutes=market.bar_minutes, primary=primary, secondary_mask=mask, variant=0)
-        self.event_cap = int(event_cap)
-        self.timeframes = (market.bar_minutes,)
-        assert bank.is_cuda and bank.dtype == torch.float32 and tuple(bank.shape) == (market.S, len(self.periods), market.N)
-        self.bank = bank.contiguous()
-        self.mode, self.chunk_min_bars, self.chunk_options = mode, 131072, {}
-        self._stats = self._events = None
-        self._pop = 0
-        self._pinned_in = self._pinned_out = None
+        self._setup(market, periods, optimization_goals, initial_capital, event_cap, mode, None, score_on_advanced, (),
+                    bank=bank.contiguous())
         return self
 
     # -- device-side evaluation (inputs already resident) -------------------
     def evaluate_device(self, indiv_dev: torch.Tensor, order_dev: Optional[torch.Tensor], pop: int,
-                        fitness_dev: torch.Tensor, plan: Optional["ChunkPlan"] = None) -> None:
-        """Sweep + fitness reduction on the current stream.  With a ChunkPlan the time-chunked kernels
-        run first and only lanes whose chunk boundaries failed verification go through the fused kernel."""
+                        fitness_dev: torch.Tensor, plan: Optional[List[_Plan]] = None,
+                        event_cap: Optional[int] = None) -> None:
+        """Sweep + fitness reduction on the current stream.  Without a plan the fused kernel runs (in `order_dev` order);
+        with the TilePlan / ChunkPlan slices of `plan` the time-chunked kernels run, and lanes whose chunk boundaries failed
+        verification go through the fused kernel inside the same call.  `event_cap`: event words kept per lane (default:
+        the instance's)."""
+        m = self.market
+        cap = self.event_cap if event_cap is None else int(event_cap)
+        stats, events = self._buffers(pop, cap)
         self._inverse = None
-        if plan is not None:
-            plans = plan if isinstance(plan, (list, tuple)) else [plan]
-            self._ensure_buffers(pop)
-            self._last_plans = plans
-            for pl in plans:
-                (self._evaluate_tiled if isinstance(pl, TilePlan) else self._evaluate_chunked)(indiv_dev, pl)
-            with torch.cuda.device(self.market.device):
-                _lib.call("b200bt_fitness_reduce", self._stats.data_ptr(), pop, self.market.S, fitness_dev.data_ptr(),
-                          _lib.current_stream())
-            return
+        self._last_plans = [] if plan is None else plan if isinstance(plan, (list, tuple)) else [plan]
+        with torch.cuda.device(m.device):
+            st = _lib.current_stream()
+            data = self._data_args()
+            if plan is None:
+                _lib.call("b200bt_sweep", *data, indiv_dev.data_ptr(), _lib.ptr(order_dev), pop, C.byref(self.cfg),
+                          stats.data_ptr(), _lib.ptr(events), cap, st)
+            for pl in self._last_plans:
+                part = slice(pl.lo, pl.lo + pl.pop)
+                pl.launch(self, data, indiv_dev.data_ptr() + pl.lo * C.sizeof(_lib.Individual), stats[part],
+                          None if events is None else events[part], cap, st)
+            _lib.call("b200bt_fitness_reduce", stats.data_ptr(), pop, m.S, fitness_dev.data_ptr(), st)
+
+    def _data_args(self) -> tuple:
+        """The leading arguments of every sweep entry point: price rows, RSI bank, P, S, N."""
         m = self.market
-        self._last_plans = []
-        if self._stats is None or self._pop != pop:
+        return (m.close.data_ptr(), _lib.ld(m.close), self.bank.data_ptr(), _lib.ld(self.bank), self.bank.shape[1], m.S, m.N)
+
+    def _buffers(self, pop: int, event_cap: int) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
+        """Lane stats [pop][S] and event words [pop][S][event_cap] of an evaluation, kept while pop and event_cap stay."""
+        if self._buffer_key != (pop, event_cap):
+            m = self.market
             self._stats = torch.empty((pop, m.S, _lib.LANE_STATS_WORDS), dtype=torch.float64, device=m.device)
-            self._events = (torch.zeros((pop, m.S, self.event_cap), dtype=torch.int32, device=m.device)
-                            if self.event_cap else None)
-            self._pop = pop
-        with torch.cuda.device(m.device):
-            st = _lib.current_stream()
-            _lib.call("b200bt_sweep", m.close.data_ptr(), _lib.ld(m.close), self.bank.data_ptr(),
-                      _lib.ld(self.bank), self.bank.shape[1], m.S, m.N, indiv_dev.data_ptr(),
-                      _lib.ptr(order_dev), pop, C.byref(self.cfg), self._stats.data_ptr(),
-                      _lib.ptr(self._events), self.event_cap, st)
-            _lib.call("b200bt_fitness_reduce", self._stats.data_ptr(), pop, m.S, fitness_dev.data_ptr(), st)
-
-    def _ensure_buffers(self, pop: int) -> None:
-        m = self.market
-        if self._stats is None or self._pop != pop:
-            self._stats = torch.empty((pop, m.S, _lib.LANE_STATS_WORDS), dtype=torch.float64, device=m.device)
-            self._events = (torch.zeros((pop, m.S, self.event_cap), dtype=torch.int32, device=m.device)
-                            if self.event_cap else None)
-            self._pop = pop
-
-    def _evaluate_chunked(self, indiv_dev, plan: "ChunkPlan") -> None:
-        """One slice [plan.lo, plan.lo + plan.pop) of the population through the chunked kernels; lanes whose
-        chunk boundaries failed verification are re-evaluated by the fused kernel."""
-        m = self.market
-        lo, n = plan.lo, plan.pop
-        stats = self._stats[lo:lo + n]
-        events = self._events[lo:lo + n] if self._events is not None else None
-        with torch.cuda.device(m.device):
-            st = _lib.current_stream()
-            _lib.call("b200bt_sweep_chunked", m.close.data_ptr(), _lib.ld(m.close), self.bank.data_ptr(), _lib.ld(self.bank),
-                      self.bank.shape[1], m.S, m.N, indiv_dev.data_ptr() + lo * C.sizeof(_lib.Individual),
-                      plan.order_dev.data_ptr(), n,
-                      plan.items.data_ptr(), plan.n_seg, plan.seg_base_dev.data_ptr(), plan.n_chunks_dev.data_ptr(),
-                      plan.n_seg, plan.warm, plan.max_repair_rounds, plan.pool_blocks, plan.workspace.data_ptr(), plan.workspace.numel(),
-                      C.byref(self.cfg), stats.data_ptr(), _lib.ptr(events), self.event_cap,
-                      plan.invalid.data_ptr(), plan.overflow.data_ptr(), st)
-
-    def _evaluate_tiled(self, indiv_dev, plan: "TilePlan") -> None:
-        """One slice of the population through the thread-per-lane kernels (same verification / fallback)."""
-        m = self.market
-        lo, n = plan.lo, plan.pop
-        stats = self._stats[lo:lo + n]
-        events = self._events[lo:lo + n] if self._events is not None else None
-        with torch.cuda.device(m.device):
-            st = _lib.current_stream()
-            _lib.call("b200bt_sweep_tiled", m.close.data_ptr(), _lib.ld(m.close), self.bank.data_ptr(), _lib.ld(self.bank),
-                      self.bank.shape[1], m.S, m.N, _lib.ptr(self._zones_if_amortised()),
-                      indiv_dev.data_ptr() + lo * C.sizeof(_lib.Individual),
-                      plan.slots_dev.data_ptr(), len(plan.slots), plan.slots_dev.data_ptr() + 4 * len(plan.slots), n, plan.K, plan.warm,
-                      plan.max_repair_rounds, plan.pool_blocks,
-                      plan.workspace.data_ptr(), plan.workspace.numel(), C.byref(self.cfg), stats.data_ptr(),
-                      _lib.ptr(events), self.event_cap, plan.invalid.data_ptr(), plan.overflow.data_ptr(), st)
+            self._events = torch.zeros((pop, m.S, event_cap), dtype=torch.int32, device=m.device) if event_cap else None
+            self._buffer_key = (pop, event_cap)
+        return self._stats, self._events
 
     # Lanes the time-chunked kernels flagged (a boundary still inconsistent after the repair passes, a full event pool, a warp
     # not packed for the thread-per-lane scan) are re-evaluated by the fused kernel ON THE DEVICE, inside b200bt_sweep_chunked /
-    # b200bt_sweep_tiled: an evaluation reads nothing back.  These two look at the flags of the last evaluation afterwards.
-    def _sync_flags(self):
+    # b200bt_sweep_tiled: an evaluation reads nothing back.  _flags looks at the flags of the last evaluation afterwards.
+    def _flags(self) -> Tuple[np.ndarray, int, float]:
+        """After synchronising the stream: the last evaluation's int[5] flags (_pinned_flags) summed over its plans, the
+        pool blocks they used net of the 2 * n_seg * S floor of _Plan._size_pool, and the blocks their cost model predicted."""
         torch.cuda.current_stream(self.market.device).synchronize()
-        return [pl.overflow for pl in (getattr(self, "_last_plans", None) or [])]
+        flags = np.zeros(5, dtype=np.int64)
+        used, predicted = 0, 0
+        for pl in self._last_plans:
+            f = pl.overflow.numpy()
+            flags += f
+            used += int(f[2]) - 2 * pl.n_seg * self.market.S
+            predicted += pl.pred_blocks
+        return flags, used, predicted
 
     @property
     def last_invalid_lanes(self) -> int:
         """(individual, symbol) lanes of the last evaluation that went through the exact fallback."""
-        return int(sum(int(f[1]) for f in self._sync_flags()))
+        return int(self._flags()[0][1])
 
     @property
     def last_scan_stalls(self) -> int:
         """Tiles of the last thread-per-lane scan whose bulk copy did not complete in time (their chunks were re-scanned by the
         repair pass or their lanes re-run by the exact fallback; 0 in normal operation)."""
-        return int(sum(int(f[3]) for f in self._sync_flags()))
+        return int(self._flags()[0][3])
 
     @property
     def last_peak_chunks(self) -> int:
         """(individual, symbol, chunk) time chunks of the last time-chunked evaluation that set a new equity peak: only those
         take the record-by-record drawdown pass (chunk_peak_kernel); the others' drawdown comes from three per-chunk sums."""
-        return int(sum(int(f[4]) for f in self._sync_flags()))
+        return int(self._flags()[0][4])
 
     @property
     def last_pool_overflow(self) -> bool:
         """The event pool of the last evaluation was too small (its lanes were re-run exactly; the next plan is larger)."""
-        return any(bool(f[0]) for f in self._sync_flags())
+        return bool(self._flags()[0][0])
 
     def set_gap(self, gap_bar: int, gap_minutes: int) -> None:
         """Declare the series as two pieces glued at `gap_bar`, the second one `gap_minutes` later on the calendar
@@ -701,7 +699,7 @@ class PopulationSweep:
 
     def zone_map(self) -> torch.Tensor:
         """(min, max) per 32-bar block of the price rows and of the RSI bank (b200bt_zone_map), built on first use."""
-        if getattr(self, "_zones", None) is None:
+        if self._zones is None:
             m = self.market
             n = int(_lib.load().b200bt_zone_map_floats(self.bank.shape[1], m.S, m.N))
             z = torch.empty(n, dtype=torch.float32, device=m.device)
@@ -716,8 +714,8 @@ class PopulationSweep:
     def _zones_if_amortised(self) -> Optional[torch.Tensor]:
         """The zone map costs about as much as it saves in ONE sweep (0.8 ms against ~0.2 ms at C2): it is built
         when this bank is swept a second time (a GA sweeps it every generation), not for a one-off evaluation."""
-        self._tiled_sweeps = getattr(self, "_tiled_sweeps", 0) + 1
-        if not self.use_zones or (self._tiled_sweeps < 2 and getattr(self, "_zones", None) is None):
+        self._tiled_sweeps += 1
+        if not self.use_zones or (self._tiled_sweeps < 2 and self._zones is None):
             return None
         return self.zone_map()
 
@@ -738,29 +736,33 @@ class PopulationSweep:
         options = dict(self.chunk_options)
         if not tiled and self.mode == "auto":
             options.setdefault("target_events", 8192)
-        # Event-pool sizing learns from the previous sweep of this bank: the cost model behind `pred` is calibrated on random
-        # populations, while the populations a GA evolves write several times more records.  The pool is scaled by the
-        # measured blocks-per-predicted-block ratio (never below the model), and by 4x more whenever it still overflowed.
-        if getattr(self, "_last_plans", None):
-            flags = self._sync_flags()
-            used = sum(int(f[2]) - 2 * pl.n_seg * self.market.S for f, pl in zip(flags, self._last_plans))
-            predicted = sum(pl.pred_blocks for pl in self._last_plans)
-            if any(bool(f[0]) for f in flags):
-                self._pool_factor = 4.0 * max(getattr(self, "_pool_factor", 1.0), 1.0)
-                options.pop("pool_blocks", None)
-            elif predicted > 0:
-                self._pool_factor = max(1.0, 1.2 * used / predicted)
-        if getattr(self, "_pool_factor", 1.0) > 1.0:
-            options["pool_scale"] = getattr(self, "_pool_factor") * options.get("pool_scale", 1.5)
+        self._pool_options(options)
         if tiled and rows is None and len(self.timeframes) > 1:
             rows = decode_population(population, self.period_row, len(self.timeframes))["rsi_row"]
         return self.plan_batches(population, tiled=tiled, pred=pred, rows=rows, **options)
 
+    def _pool_options(self, options: Dict) -> None:
+        """Event-pool sizing learns from the previous sweep of this bank: the cost model behind `pred` is calibrated on random
+        populations, while the populations a GA evolves write several times more records.  The pool is scaled by the
+        measured blocks-per-predicted-block ratio (never below the model), and by 4x more whenever it still overflowed (a
+        fixed `pool_blocks` is then dropped).  Synchronises the stream when there is a previous sweep to learn from."""
+        if self._last_plans:
+            flags, used, predicted = self._flags()
+            if flags[0]:
+                self._pool_factor *= 4.0
+                options.pop("pool_blocks", None)
+            elif predicted > 0:
+                self._pool_factor = max(1.0, 1.2 * used / predicted)
+        if self._pool_factor > 1.0:
+            options["pool_scale"] = self._pool_factor * options.get("pool_scale", 1.5)
+
     def plan_tiles(self, population: List[Dict], **kw) -> "TilePlan":
-        return TilePlan(population, self.market.N, self.market.S, self.market.device, **kw)
+        m = self.market
+        return _allocate_plans([TilePlan(population, m.N, m.S, m.device, **kw)], m.S, m.device)[0]
 
     def plan_chunks(self, population: List[Dict], **kw) -> "ChunkPlan":
-        return ChunkPlan(population, self.market.N, self.market.S, self.market.device, **kw)
+        m = self.market
+        return _allocate_plans([ChunkPlan(population, m.N, m.S, m.device, **kw)], m.S, m.device)[0]
 
     def plan_batches(self, population: List[Dict], max_pool_bytes: int = 8 << 30, tiled: bool = False,
                      pred: Optional[np.ndarray] = None, rows: Optional[np.ndarray] = None, **kw) -> List:
@@ -773,47 +775,49 @@ class PopulationSweep:
         if pred is None:
             pred = predicted_events(population, self.market.N)
         rows_of = (lambda lo, hi: {"rows": None if rows is None else rows[lo:hi]}) if tiled else (lambda lo, hi: {})
-        if kw.get("pool_blocks") is not None:
-            return [cls(population, self.market.N, self.market.S, self.market.device, pred=pred, **rows_of(0, None), **kw)]
-        pool_bytes = pred * (self.market.S * 8 * kw.get("pool_scale", 1.5))
-        if float(pool_bytes.sum()) <= max_pool_bytes:
-            return [cls(population, self.market.N, self.market.S, self.market.device, pred=pred, **rows_of(0, None), **kw)]
-        cuts, acc = [0], 0.0
-        for i, b in enumerate(pool_bytes):
-            if acc + b > max_pool_bytes and i > cuts[-1]:
-                cuts.append(i)
-                acc = 0.0
-            acc += b
-        cuts.append(len(population))
-        plans = [cls(population[lo:hi], self.market.N, self.market.S, self.market.device, lo=lo, workspace=DEFERRED,
-                     pred=pred[lo:hi], **rows_of(lo, hi), **kw) for lo, hi in zip(cuts[:-1], cuts[1:])]
-        shared = torch.empty(max(pl.ws_bytes for pl in plans), dtype=torch.uint8, device=self.market.device)
-        for pl in plans:
-            pl.workspace = shared        # the slices run one after the other on the same stream
-        return sorted(plans, key=lambda pl: pl.lo)
+        pool_bytes = None if kw.get("pool_blocks") is not None else pred * (self.market.S * 8 * kw.get("pool_scale", 1.5))
+        if pool_bytes is None or float(pool_bytes.sum()) <= max_pool_bytes:
+            plans = [cls(population, self.market.N, self.market.S, self.market.device, pred=pred, **rows_of(0, None), **kw)]
+        else:
+            cuts, acc = [0], 0.0
+            for i, b in enumerate(pool_bytes):
+                if acc + b > max_pool_bytes and i > cuts[-1]:
+                    cuts.append(i)
+                    acc = 0.0
+                acc += b
+            cuts.append(len(population))
+            plans = [cls(population[lo:hi], self.market.N, self.market.S, self.market.device, lo=lo, pred=pred[lo:hi],
+                         **rows_of(lo, hi), **kw) for lo, hi in zip(cuts[:-1], cuts[1:])]
+        return _allocate_plans(plans, self.market.S, self.market.device)
 
     # -- host-facing evaluation --------------------------------------------
+    def _unique(self, population: List[Dict]) -> Tuple[np.ndarray, List[Dict], Optional[np.ndarray]]:
+        """Decoded records of the individuals of `population` that decode differently, in population order, their dicts,
+        and the index that expands per-unique results back to `population` (None when all are distinct).  Individuals
+        that decode to the same kernel parameters (the reference rule reads 6 of the 18 genes, and elitism / crossover
+        copy individuals) are evaluated once."""
+        packed = decode_population(population, self.period_row, len(self.timeframes))
+        dup = _duplicate_classes(packed)
+        if dup is None:
+            return packed, population, None
+        first, inverse = dup
+        keep = np.sort(first)
+        rank = np.empty(len(first), dtype=np.int64)
+        rank[np.argsort(first)] = np.arange(len(first))
+        return np.ascontiguousarray(packed[keep]), [population[i] for i in keep], rank[inverse.reshape(-1)]
+
     def evaluate(self, population: List[Dict]) -> np.ndarray:
         """fitness (float64[pop]) of a list of parameter dicts; H2D of the decoded
         population and D2H of the fitness vector happen inside this call."""
         if not population:
             return np.zeros(0, dtype=np.float64)
+        return self._evaluate_unique(*self._unique(population), self.event_cap)
+
+    def _evaluate_unique(self, packed: np.ndarray, population: List[Dict], expand: Optional[np.ndarray],
+                         event_cap: int) -> np.ndarray:
+        """evaluate() on the output of _unique, keeping `event_cap` event words per lane."""
         dev = self.market.device
-        packed = decode_population(population, self.period_row, len(self.timeframes))
-        # individuals that decode to the same kernel parameters (the reference rule reads 6 of the 18 genes,
-        # and elitism / crossover copy individuals) are evaluated once
-        expand = None
-        dup = _duplicate_classes(packed)
-        if dup is not None:
-            first, inverse = dup
-            keep = np.sort(first)                       # unique individuals in population order
-            rank = np.empty(len(first), dtype=np.int64)
-            rank[np.argsort(first)] = np.arange(len(first))
-            expand = rank[inverse.reshape(-1)]
-            packed = np.ascontiguousarray(packed[keep])
-            population = [population[i] for i in keep]
-        self.last_unique = len(population)
-        pop = len(population)
+        self.last_unique = pop = len(population)
         pred = EVENTS_PER_COST_BAR * costs_from_packed(packed, self.periods, self.timeframes) * self.market.N
         plan = self.plan(population, pred=pred, rows=packed["rsi_row"])
         if plan is None:       # the fused kernel dispatches in this order: same RSI period adjacent, most expensive first
@@ -832,7 +836,7 @@ class PopulationSweep:
         indiv_dev = staged[:nbytes]
         order_dev = staged[nbytes:].view(torch.int32) if order.size else None
         fit = torch.empty(pop, dtype=torch.float64, device=dev)
-        self.evaluate_device(indiv_dev, order_dev, pop, fit, plan=plan)
+        self.evaluate_device(indiv_dev, order_dev, pop, fit, plan=plan, event_cap=event_cap)
         self._inverse = expand
         out = self._pinned_out[:pop]
         out.copy_(fit, non_blocking=True)
@@ -840,7 +844,7 @@ class PopulationSweep:
         self.h2d_bytes = nbytes + order.nbytes
         self.d2h_bytes = pop * 8
         res = out.numpy().copy()
-        return res if self._inverse is None else res[self._inverse]
+        return res if expand is None else res[expand]
 
     TRADE_PNL_MAX_BYTES = 4 << 30
 
@@ -857,38 +861,28 @@ class PopulationSweep:
         if not population:
             raise ValueError("trade_pnl needs at least one individual")
         m = self.market
-        packed = decode_population(population, self.period_row, len(self.timeframes))
-        dup = _duplicate_classes(packed)
-        if dup is not None:                                     # evaluate() sweeps these, in this order
-            packed = np.ascontiguousarray(packed[np.sort(dup[0])])
+        packed, unique, expand = self._unique(population)
         U, P, S = len(packed), len(population), m.S
-        saved_cap = self.event_cap
-        try:
-            self.event_cap, self._stats = 0, None
-            self.evaluate(population)
-            cap = int(self._stats[:, :, 0].max().item())           # n_records of the busiest lane (always even)
-            cap = max(2, cap + (cap & 1))
-            T = cap // 2
-            need = U * S * cap * 4 + (U + P) * S * T * 8
-            if need > max_bytes:
-                raise ValueError(f"trade_pnl: {need} bytes of event and trip PnL buffers for {P} individuals x {S} symbols "
-                                 f"(up to {cap} records per lane) exceed the budget of {max_bytes} bytes; pass the top "
-                                 f"of the population, not all of it")
-            self.event_cap, self._stats = cap, None
-            self.evaluate(population)
-            indiv = torch.from_numpy(packed.view(np.uint8)).to(m.device)
-            trip = torch.empty((U, S, T), dtype=torch.float64, device=m.device)
-            n_trips = torch.empty((U, S), dtype=torch.int32, device=m.device)
-            fee = torch.empty((U, S), dtype=torch.float64, device=m.device)
-            with torch.cuda.device(m.device):
-                _lib.call("b200bt_trade_pnl", m.close.data_ptr(), _lib.ld(m.close), S, m.N, indiv.data_ptr(), U,
-                          self._stats.data_ptr(), self._events.data_ptr(), cap, trip.data_ptr(), T, n_trips.data_ptr(),
-                          fee.data_ptr(), _lib.current_stream())
-        finally:
-            self.event_cap = saved_cap
-            self._pop = -1                 # the next evaluation allocates stats / events for its own event_cap
-        if self._inverse is not None:
-            inv = torch.from_numpy(self._inverse).to(m.device)
+        self._evaluate_unique(packed, unique, expand, 0)
+        cap = int(self._stats[:, :, 0].max().item())           # n_records of the busiest lane (always even)
+        cap = max(2, cap + (cap & 1))
+        T = cap // 2
+        need = U * S * cap * 4 + (U + P) * S * T * 8
+        if need > max_bytes:
+            raise ValueError(f"trade_pnl: {need} bytes of event and trip PnL buffers for {P} individuals x {S} symbols "
+                             f"(up to {cap} records per lane) exceed the budget of {max_bytes} bytes; pass the top "
+                             f"of the population, not all of it")
+        self._evaluate_unique(packed, unique, expand, cap)
+        indiv = torch.from_numpy(packed.view(np.uint8)).to(m.device)
+        trip = torch.empty((U, S, T), dtype=torch.float64, device=m.device)
+        n_trips = torch.empty((U, S), dtype=torch.int32, device=m.device)
+        fee = torch.empty((U, S), dtype=torch.float64, device=m.device)
+        with torch.cuda.device(m.device):
+            _lib.call("b200bt_trade_pnl", m.close.data_ptr(), _lib.ld(m.close), S, m.N, indiv.data_ptr(), U,
+                      self._stats.data_ptr(), self._events.data_ptr(), cap, trip.data_ptr(), T, n_trips.data_ptr(),
+                      fee.data_ptr(), _lib.current_stream())
+        if expand is not None:
+            inv = torch.from_numpy(expand).to(m.device)
             trip, n_trips, fee = trip.index_select(0, inv), n_trips.index_select(0, inv), fee.index_select(0, inv)
         if bool((n_trips < 0).any()):
             raise RuntimeError("trade_pnl: a lane wrote more records than its event buffer held")
@@ -897,7 +891,7 @@ class PopulationSweep:
     def lane_stats(self) -> Dict[str, np.ndarray]:
         """Per-lane metrics of the last evaluation: dict field -> [pop][S] array."""
         raw = self._stats.cpu().numpy()
-        if getattr(self, "_inverse", None) is not None:
+        if self._inverse is not None:
             raw = raw[self._inverse]
         out = {name: raw[:, :, i] for i, name in enumerate(_lib.LANE_STATS_FIELDS[:-1])}
         out["trade_hash"] = np.ascontiguousarray(raw[:, :, _lib.LANE_STATS_WORDS - 1]).view(np.uint64)
@@ -926,7 +920,7 @@ class PopulationSweep:
         if self._events is None:
             return None
         ev = self._events.cpu().numpy().view(np.uint32)
-        return ev if getattr(self, "_inverse", None) is None else ev[self._inverse]
+        return ev if self._inverse is None else ev[self._inverse]
 
     @property
     def fitness_function(self):

@@ -274,9 +274,9 @@ int b200bt_sweep(const float* price, int64_t ld_price,
  * max_repair_rounds: 0 = no repair, 1 = one chunk-parallel pass (every wrong chunk re-scanned once, trusting its
  * predecessor's recorded end state), >= 2 = that pass plus a lane-sequential one beside the metrics kernels that finishes
  * the lanes whose re-scans run through chunk after chunk; nothing is read back.
- * A lane that still has a mismatch (or lost events to a full pool) is flagged in lane_invalid[pop][S]
- * (stats of flagged lanes are NOT written: re-evaluate those individuals with b200bt_sweep, passing them
- * as `order`).  One work item per (individual, chunk); `segment` = seg_base[individual] + chunk.
+ * A lane that still has a mismatch (or lost events to a full pool) is flagged in lane_invalid[pop][S] and re-evaluated
+ * exactly inside this call (see below).  One work item per (individual, chunk); `segment` = seg_base[individual] + chunk.
+ *  order      unused (kept for the ABI), may be NULL
  *  items      [n_items] device      seg_base, n_chunks  [pop] device int32      n_seg = sum of n_chunks
  *  pool_blocks  event pool size in blocks of 256 events; a chunk that cannot get a block flags its lane
  *  workspace  b200bt_sweep_chunked_workspace_bytes(pool_blocks, S, n_seg) device bytes
@@ -311,8 +311,8 @@ int b200bt_sweep_chunked(const float* price, int64_t ld_price, const float* rsi,
  * Verification, in-place repair, metrics and the lane_invalid / overflow outputs are those of b200bt_sweep_chunked.
  * slots: device int32[n_slots] (n_slots a multiple of 32): individual run by each thread slot, -1 = empty; 32 consecutive
  *        slots form a warp, which may read at most TWO distinct RSI rows (rsi_row) -- the host packs individuals by row and
- *        similar cost; a warp that breaks the rule is not scanned: its lanes are flagged in lane_invalid and the caller
- *        re-evaluates them with b200bt_sweep (exact).  NULL = identity (thread k runs individual k).
+ *        similar cost; a warp that breaks the rule is not scanned: its lanes are flagged in lane_invalid and re-evaluated
+ *        by the fused kernel inside this call (exact).  NULL = identity (thread k runs individual k).
  * order: device int32[pop], the individuals in dispatch order (by predicted cost), NULL = identity: the order in which the
  *        per-chunk metrics kernels list their work (one thread per chunk: neighbours should hold similar record counts).
  * zones: optional zone map of the same price / RSI arrays (b200bt_zone_map), NULL = none: (min, max) per 32-bar

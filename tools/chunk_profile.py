@@ -15,6 +15,6 @@ indiv = torch.from_numpy(decode_population(pop, sw.period_row).view(np.uint8)).c
 fit = torch.empty(POP, dtype=torch.float64, device="cuda")
 plan = sw.plan_chunks(pop, target_events=target, warm=warm)
 for _ in range(2):
-    sw.evaluate_device(indiv, plan.order_dev, POP, fit, plan=plan)
+    sw.evaluate_device(indiv, None, POP, fit, plan=plan)
 torch.cuda.synchronize()
 print("done", sw.last_invalid_lanes)

@@ -15,11 +15,11 @@ indiv = torch.from_numpy(packed.view(np.uint8)).cuda()
 fit = torch.empty(POP, dtype=torch.float64, device="cuda")
 
 def timed(plan, reps=3):
-    for _ in range(2): sw.evaluate_device(indiv, plan.order_dev if plan else None, POP, fit, plan=plan)
+    for _ in range(2): sw.evaluate_device(indiv, None, POP, fit, plan=plan)
     torch.cuda.synchronize()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
-    for _ in range(reps): sw.evaluate_device(indiv, plan.order_dev if plan else None, POP, fit, plan=plan)
+    for _ in range(reps): sw.evaluate_device(indiv, None, POP, fit, plan=plan)
     e1.record(); torch.cuda.synchronize()
     return e0.elapsed_time(e1) / reps
 

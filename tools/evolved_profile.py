@@ -29,7 +29,7 @@ for _ in range(5):
     sw.evaluate_device(indiv, None, POP, fit, plan=plan)
 e1.record(); torch.cuda.synchronize()
 print("ms per sweep (CUDA events, 5 sweeps)", e0.elapsed_time(e1) / 5, "invalid lanes", sw.last_invalid_lanes, "overflow", sw.last_pool_overflow,
-      "pool blocks", [p.pool_blocks for p in plan], "used", [int(p.overflow[2]) for p in plan], "pool factor", getattr(sw, "_pool_factor", None))
+      "pool blocks", [p.pool_blocks for p in plan], "used", [int(p.overflow[2]) for p in plan], "pool factor", sw._pool_factor)
 import time
 t0 = time.perf_counter()
 for _ in range(5):
