@@ -458,16 +458,20 @@ __global__ void lane_tables_kernel(int pop, int K, const int32_t* __restrict__ o
 }
 
 #ifndef B200BT_LS_MIN_BLOCKS
-#define B200BT_LS_MIN_BLOCKS 3      // 80 registers, 4 / 28 B spilled without / with zones (nvcc 12.9); at 4 CTAs/SM (64) 3 % slower
+#define B200BT_LS_MIN_BLOCKS 3      // 80 registers, 0 / 16 B spilled without / with zones (nvcc 12.9); at 4 CTAs/SM (64) 3 % slower
 #endif
 #ifndef B200BT_LS_STAGES
 #define B200BT_LS_STAGES 2
 #endif
-#ifndef B200BT_LS_UNROLL
-#define B200BT_LS_UNROLL 2
-#endif
+// 4-bar groups per iteration of the scan loop, chosen per launch from the event density the pool was sized for.  The scan
+// is issue-bound and its group body holds four inlined copies of the event step: unrolled twice the kernel has 2704 SASS
+// instructions with zones, not unrolled 2144.  On the H100 the smaller loop scans the random configs[1] population ~7 %
+// faster, while a population with ~7x the events (generation 3 of a GA run) is ~1 % faster unrolled.  (A rolled loop over
+// the four bars -- one step copy, bars read back from the stage -- is ~45 % slower: the group's float4 registers and the
+// straight-line selects are what make the step cheap.)
+constexpr int LS_UNROLL_SPARSE = 1, LS_UNROLL_DENSE = 2;
+constexpr double LS_DENSE_EVENTS = 0.05;      // pool events per machine and bar from which the dense form is launched
 constexpr int LS_STAGES = B200BT_LS_STAGES;   // tiles in flight per warp (ring depth)
-constexpr int LS_UNROLL = B200BT_LS_UNROLL;   // 4-bar groups per iteration of the scan loop
 constexpr int LS_WARPS = LS_THREADS / 32;
 constexpr int LS_RSI_ROWS = 2;                // distinct RSI rows the 32 machines of a warp may read (host packing)
 constexpr int LS_ROWS = 1 + LS_RSI_ROWS;      // staged rows per warp: price + its RSI rows
@@ -493,10 +497,11 @@ __device__ __forceinline__ void lane_scan_give_up(const LaneScanArgs& A, const i
 }
 
 // -> false: a tile of this item did not arrive (see the wait below); the warp must not take another item
-template <bool ZONES>
+template <bool ZONES, int UNROLL>
 __device__ __forceinline__ bool lane_scan_item(const LaneScanArgs& A, const bool vec16, const int wslot, const int sym, const int c,
                                                float* const wtile, float2* const wzone, unsigned long long* const full,
-                                               float (*ls_mul)[LS_THREADS], const void* (*ls_src_w)[3], int& ring_stage, unsigned& ring_parity) {
+                                               float (*ls_mul)[LS_THREADS], double (*ls_tpsl)[LS_THREADS], const void* (*ls_src_w)[3],
+                                               int& ring_stage, unsigned& ring_parity) {
     constexpr int ZB = LS_T / LS_ZONE;                  // zone blocks per tile
     constexpr int FG = LS_T / 4;                        // 4-bar groups per tile
     constexpr int ZR = ZB + FG;                         // float2 per staged row: coarse ranges, then fine ranges
@@ -515,6 +520,10 @@ __device__ __forceinline__ bool lane_scan_item(const LaneScanArgs& A, const bool
         float* m = &ls_mul[0][threadIdx.x];
         m[0 * LS_THREADS] = sc.hiL_c; m[1 * LS_THREADS] = sc.loL_c; m[2 * LS_THREADS] = sc.hiL_d; m[3 * LS_THREADS] = sc.loL_d;
         m[4 * LS_THREADS] = sc.hiS_c; m[5 * LS_THREADS] = sc.loS_c; m[6 * LS_THREADS] = sc.hiS_d; m[7 * LS_THREADS] = sc.loS_d;
+        // take-profit / stop-loss of the float64 exit decision inside the screening band, beside them: read back from
+        // here, the step no longer re-reads A.indiv[ind] (whose address the scan loop otherwise keeps in registers)
+        ls_tpsl[0][threadIdx.x] = iv.take_profit;
+        ls_tpsl[1][threadIdx.x] = iv.stop_loss;
     }
     __syncwarp();
     // The ring's barriers are initialised ONCE per warp (lane_scan_kernel) and their phases roll on from item to item: every
@@ -628,7 +637,7 @@ __device__ __forceinline__ bool lane_scan_item(const LaneScanArgs& A, const bool
             if (!((p >= hd) || (p <= ld))) {
                 const double ed = (double)e_px, pd = (double)p;
                 const double q = lng_open ? __ddiv_rn(__dsub_rn(pd, ed), ed) : __ddiv_rn(__dsub_rn(ed, pd), ed);
-                ev = (q >= A.indiv[ind].take_profit) || (q <= -A.indiv[ind].stop_loss);
+                ev = (q >= ls_tpsl[0][threadIdx.x]) || (q <= -ls_tpsl[1][threadIdx.x]);
             }
         }
         if (!ev) return;
@@ -681,7 +690,7 @@ __device__ __forceinline__ bool lane_scan_item(const LaneScanArgs& A, const bool
                     const float2 rz = zr[zb], pz = zp[zb];
                     if (!__any_sync(amask, (rz.x < rlo) | (rz.y > rhi) | (pz.x <= plo) | (pz.y >= phi))) continue;
                 }
-#pragma unroll LS_UNROLL
+#pragma unroll UNROLL
                 for (int g = zb * (LS_ZONE / 4); g < (zb + 1) * (LS_ZONE / 4); ++g) {
                     bool hit;
                     if (ZONES) {
@@ -726,13 +735,14 @@ __device__ __forceinline__ bool lane_scan_item(const LaneScanArgs& A, const bool
 // most expensive warp-slots first -- from a global counter until none is left, so all warp slots of the GPU stay busy until
 // the queue is empty and the last items to run are the cheapest ones (a static grid left the busiest CTAs running alone
 // at the end while the rest of their SM sat idle).
-template <bool ZONES>
+template <bool ZONES, int UNROLL>
 __global__ void __launch_bounds__(LS_THREADS, B200BT_LS_MIN_BLOCKS)
 lane_scan_kernel(const LaneScanArgs A, const bool vec16) {   // by value, not __grid_constant__ (see sweep.cu)
     // [LS_WARPS][LS_STAGES][LS_ROWS][LS_STRIDE] floats, then (ZONES) per warp and stage [LS_ROWS][LS_T / 32 + LS_T / 4] float2
     extern __shared__ __align__(16) float ls_tile[];
     __shared__ __align__(8) unsigned long long ls_full[LS_WARPS][LS_STAGES];   // "tile landed" (1 arrival + the copies' bytes)
     __shared__ float ls_mul[8][LS_THREADS];
+    __shared__ double ls_tpsl[2][LS_THREADS];
     __shared__ const void* ls_src[LS_WARPS][LS_ROWS][3];
     constexpr int ZR = LS_T / LS_ZONE + LS_T / 4;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -758,7 +768,8 @@ lane_scan_kernel(const LaneScanArgs A, const bool vec16) {   // by value, not __
         const int wslot = item / per_slot, rest = item - wslot * per_slot;
         const int c = rest / A.S, sym = rest - c * A.S;
         if (retired) { lane_scan_give_up(A, wslot, sym, c); continue; }     // (every item is either scanned or marked)
-        retired = !lane_scan_item<ZONES>(A, vec16, wslot, sym, c, wtile, wzone, ls_full[warp], ls_mul, ls_src[warp], ring_stage, ring_parity);
+        retired = !lane_scan_item<ZONES, UNROLL>(A, vec16, wslot, sym, c, wtile, wzone, ls_full[warp], ls_mul, ls_tpsl, ls_src[warp],
+                                            ring_stage, ring_parity);
         __syncwarp();
     }
 }
@@ -1511,7 +1522,9 @@ extern "C" int b200bt_sweep_tiled(const float* price, int64_t ld_price, const fl
     L.indiv = indiv; L.slots = slots; L.n_slots = n_slots; L.pop = pop; L.K = K; L.warm = warm;
     L.work = &w.ctr->scan_work; L.ctr = w.ctr;
     const bool vec16 = vec16_rows(price, ld_price, rsi, ld_rsi);
-    auto kern = zones_or_null ? lane_scan_kernel<true> : lane_scan_kernel<false>;
+    const bool dense = (double)pool_blocks * CK_BLOCK >= LS_DENSE_EVENTS * (double)pop * S * (double)N;
+    auto kern = zones_or_null ? (dense ? lane_scan_kernel<true, LS_UNROLL_DENSE> : lane_scan_kernel<true, LS_UNROLL_SPARSE>)
+                              : (dense ? lane_scan_kernel<false, LS_UNROLL_DENSE> : lane_scan_kernel<false, LS_UNROLL_SPARSE>);
     e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
     if (e != cudaSuccess) return cuda_status(e, "sweep_tiled: cudaFuncSetAttribute");
