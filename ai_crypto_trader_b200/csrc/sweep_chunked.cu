@@ -800,18 +800,26 @@ struct ChunkPartial {
 };
 static_assert(sizeof(ChunkPartial) == 160, "ChunkPartial layout");
 
-// One step of walk_records, per lane: records 2 lane and 2 lane + 1 of the step (a0 / a1: they exist), priced.
-struct RecordPair {
-    int cnt;                             // records in the step (<= 64)
-    bool a0, a1;
-    unsigned w0, w1; float pf0, pf1;     // event words, prices
-    double pnl0, pnl1, s2, eq0, eq1;     // PnL of each record (0 for an entry), pnl0 + pnl1, equity after each record
-    int dur0, dur1;
+// One step of walk_records, per lane: records 4 lane + j (j = 0..3) of the step, priced.  A record that does not exist
+// (a[j] false: the step's last lane may be partial) has PnL 0 and the equity of the record in front of it.
+constexpr int WR_PER_LANE = 4;
+constexpr int WR_STEP = 32 * WR_PER_LANE;     // records per step; CK_BLOCK is a whole number of steps
+static_assert(CK_BLOCK % WR_STEP == 0, "a step never straddles two pool blocks");
+struct RecordQuad {
+    int cnt;                                  // records in the step (<= WR_STEP)
+    bool a[WR_PER_LANE];
+    unsigned w[WR_PER_LANE];                  // event words
+    double pnl[WR_PER_LANE];                  // PnL of each record (0 for an entry)
+    double eq[WR_PER_LANE];                   // equity after each record
+    double sum;                               // the lane's PnL sum
+    int dur[WR_PER_LANE];
 };
 
-// The records of chunk `seg` in time order, 64 per step, two per lane (one 16-byte load): every record is priced against
-// the one before it (the first against the entry the chunk's verified start state holds), the equity runs on from `equity`
-// by an inclusive warp scan, and body(pair, step's PnL sum) consumes the step.  -> the chunk's record count (0: lost).
+// The records of chunk `seg` in time order, WR_STEP per step, four per lane (two 16-byte loads): every record is priced
+// against the one before it (the lane's first by shuffle from the lane in front; lane 0's against the last record of the
+// previous step, or the entry the chunk's verified start state holds), the equity runs on from `equity` by an in-lane
+// prefix over the four PnLs and one inclusive warp scan, and body(quad, step's PnL sum) consumes the step.  -> the
+// chunk's record count (0: lost).
 template <class Body>
 __device__ __forceinline__ unsigned walk_records(const uint2* __restrict__ pool, const int* __restrict__ next, const int pool_blocks,
                                                  const int* __restrict__ seg_first, const unsigned* __restrict__ seg_count,
@@ -831,42 +839,51 @@ __device__ __forceinline__ unsigned walk_records(const uint2* __restrict__ pool,
     int b = left ? seg_first[seg] : -1, off = 0;
     if ((unsigned)b >= (unsigned)pool_blocks) left = 0;
     while (left) {
-        RecordPair r;
-        r.cnt = (int)min(64u, left);
-        r.a0 = 2 * lane < r.cnt; r.a1 = 2 * lane + 1 < r.cnt;
-        uint4 ev = make_uint4(0u, 0u, 0u, 0u);
-        if (r.a0) ev = *reinterpret_cast<const uint4*>(pool + (int64_t)b * CK_BLOCK + off + 2 * lane);
-        r.w0 = ev.x; r.w1 = ev.z;
-        r.pf0 = __uint_as_float(ev.y); r.pf1 = __uint_as_float(ev.w);
-        float p_prev = __shfl_up_sync(FULL, r.pf1, 1);
-        unsigned w_prev = __shfl_up_sync(FULL, r.w1, 1);
+        RecordQuad r;
+        r.cnt = (int)min((unsigned)WR_STEP, left);
+        const int first = WR_PER_LANE * lane;
+#pragma unroll
+        for (int j = 0; j < WR_PER_LANE; ++j) r.a[j] = first + j < r.cnt;
+        const uint4* src = reinterpret_cast<const uint4*>(pool + (int64_t)b * CK_BLOCK + off + first);
+        const uint4 e01 = r.a[0] ? src[0] : make_uint4(0u, 0u, 0u, 0u);
+        const uint4 e23 = r.a[2] ? src[1] : make_uint4(0u, 0u, 0u, 0u);
+        r.w[0] = e01.x; r.w[1] = e01.z; r.w[2] = e23.x; r.w[3] = e23.z;
+        const float pf[WR_PER_LANE] = {__uint_as_float(e01.y), __uint_as_float(e01.w), __uint_as_float(e23.y), __uint_as_float(e23.w)};
+        float p_prev = __shfl_up_sync(FULL, pf[3], 1);
+        unsigned w_prev = __shfl_up_sync(FULL, r.w[3], 1);
         if (lane == 0) { p_prev = p_carry; w_prev = w_carry; }
-        r.pnl0 = record_pnl(r.a0, r.w0, r.pf0, w_prev, p_prev, size, fee1, fee2, r.dur0);
-        r.pnl1 = record_pnl(r.a1, r.w1, r.pf1, r.w0, r.pf0, size, fee1, fee2, r.dur1);
-        r.s2 = r.pnl0 + r.pnl1;
-        double cs = r.s2;
+        double run = 0.0;                         // in-lane prefix of the PnLs
+#pragma unroll
+        for (int j = 0; j < WR_PER_LANE; ++j) {
+            r.pnl[j] = record_pnl(r.a[j], r.w[j], pf[j], j ? r.w[j - 1] : w_prev, j ? pf[j - 1] : p_prev, size, fee1, fee2, r.dur[j]);
+            run = j ? run + r.pnl[j] : r.pnl[j];
+            r.eq[j] = run;
+        }
+        r.sum = run;
+        double cs = run;
 #pragma unroll
         for (int d = 1; d < 32; d <<= 1) {
             const double up = shfl_up_d(cs, d);
             if (lane >= d) cs += up;
         }
-        r.eq0 = equity + (cs - r.s2) + r.pnl0;
-        r.eq1 = equity + cs;
+        const double base = equity + (cs - run);  // equity in front of the lane's first record
+#pragma unroll
+        for (int j = 0; j < WR_PER_LANE; ++j) r.eq[j] = base + r.eq[j];
         const double step_sum = shfl_d(cs, 31);
         equity += step_sum;
         body(r, step_sum);
-        const int last = (r.cnt - 1) >> 1;
-        w_carry = __shfl_sync(FULL, (r.cnt & 1) ? r.w0 : r.w1, last);
-        p_carry = __shfl_sync(FULL, (r.cnt & 1) ? r.pf0 : r.pf1, last);
+        // (only a full step is followed by another one: its last record is lane 31's last)
+        w_carry = __shfl_sync(FULL, r.w[3], 31);
+        p_carry = __shfl_sync(FULL, pf[3], 31);
         left -= r.cnt;
-        off += 64;
+        off += WR_STEP;
         if (off == CK_BLOCK && left) { b = next[b]; off = 0; if ((unsigned)b >= (unsigned)pool_blocks) break; }
     }
     return count;
 }
 
 #ifndef B200BT_M2_MIN_BLOCKS
-#define B200BT_M2_MIN_BLOCKS 5      // 96 registers, no spills (nvcc 12.9, sm_90a); at 6 CTAs/SM (80) it spills 64 B
+#define B200BT_M2_MIN_BLOCKS 5      // 96 registers, 20 B spilled (nvcc 12.9, sm_90a); at 4 CTAs/SM (108, no spill) ~6 % slower
 #endif
 __global__ void __launch_bounds__(128, B200BT_M2_MIN_BLOCKS)
 chunk_partial_kernel(const float* __restrict__ price, int64_t ld_price, const b200bt_individual* __restrict__ indiv,
@@ -895,14 +912,13 @@ chunk_partial_kernel(const float* __restrict__ price, int64_t ld_price, const b2
     // Order-dependent state (equity relative to the chunk's start, calendar day) is warp-uniform and lives in registers;
     // what is a plain sum / max / min / xor over the records is accumulated PER LANE and reduced once at the end of the chunk.
     double equity = 0.0, l_top = -INFINITY, l_bottom = INFINITY;
-    DayAcc da{0.0, 0.0, 0.0, 0u, 0};
+    DayAcc da{0.0, 0.0, 0.0, 0u, 0};   // this lane's share of the chunk's finished days (merged in lane order at the end)
     int day_valid = 0, day_cur = 0, first_done = 0, first_id = 0;
     double day_sum = 0.0, first_sum = 0.0;
     unsigned index = first_index;
     double l_gain = 0.0, l_loss = 0.0, l_maxp = 0.0, l_minl = 0.0;
-    unsigned l_win = 0, l_los = 0;
-    long long l_dur = 0;
-    unsigned long long l_hash = 0ull;
+    unsigned l_win = 0, l_los = 0, l_dur = 0;   // (l_dur: a lane's trades do not overlap, so the chunk's sum is < N < 2^30)
+    unsigned l_hlo = 0u, l_hhi = 0u;
     uint32_t* const ev_out = events ? events + ((int64_t)item.individual * S + sym) * ev_cap : nullptr;
     const unsigned minute0 = (unsigned)cfg.minute0, bar_minutes = (unsigned)cfg.bar_minutes;
     const unsigned gap_bar = cfg.gap_bar > 0 ? (unsigned)cfg.gap_bar : 0xffffffffu, gap_minutes = (unsigned)cfg.gap_minutes;
@@ -910,79 +926,99 @@ chunk_partial_kernel(const float* __restrict__ price, int64_t ld_price, const b2
         const unsigned bar = w & 0x3fffffffu;
         return (int)((minute0 + bar * bar_minutes + (bar >= gap_bar ? gap_minutes : 0u)) / 1440u);
     };
-    auto finish_day = [&](int id, double x) {     // the chunk's first day may continue the previous chunk's last one
-        if (!first_done) { first_done = 1; first_id = id; first_sum = x; }
-        else day_complete(da, x);
-    };
+    constexpr int R = WR_PER_LANE;
 
     // equity relative to the chunk's start
     const unsigned count = walk_records(pool, next, pool_blocks, seg_first, seg_count, seg_in, price + (int64_t)sym * ld_price, seg,
-                                        iv.position_size, equity, [&](const RecordPair& r, const double batch_sum) {
+                                        iv.position_size, equity, [&](const RecordQuad& r, const double batch_sum) {
         const int cnt = r.cnt;
-        const bool a0 = r.a0, a1 = r.a1;
-        const unsigned w0 = r.w0, w1 = r.w1;
-        const double pnl0 = r.pnl0, pnl1 = r.pnl1, s2 = r.s2;
-        if (pnl0 > 0.0) { l_gain += pnl0; ++l_win; l_maxp = fmax(l_maxp, pnl0); }
-        else if (pnl0 < 0.0) { l_loss += pnl0; ++l_los; l_minl = fmin(l_minl, pnl0); }
-        if (pnl1 > 0.0) { l_gain += pnl1; ++l_win; l_maxp = fmax(l_maxp, pnl1); }
-        else if (pnl1 < 0.0) { l_loss += pnl1; ++l_los; l_minl = fmin(l_minl, pnl1); }
-        l_dur += r.dur0 + r.dur1;
-        const unsigned i0 = index + 2 * lane;
-        if (a0) {
-            l_hash ^= event_hash(i0, w0);
-            if (ev_out && (int64_t)i0 < ev_cap) ev_out[i0] = w0;
+        const unsigned i0 = index + R * lane;
+        int d[R];                     // calendar day of each record (a missing record: its predecessor's)
+#pragma unroll
+        for (int j = 0; j < R; ++j) {
+            const double pnl = r.pnl[j];
+            if (pnl > 0.0) { l_gain += pnl; ++l_win; l_maxp = fmax(l_maxp, pnl); }
+            else if (pnl < 0.0) { l_loss += pnl; ++l_los; l_minl = fmin(l_minl, pnl); }
+            l_dur += (unsigned)r.dur[j];
+            if (r.a[j]) {
+                const unsigned long long h = event_hash(i0 + j, r.w[j]);
+                l_hlo ^= (unsigned)h; l_hhi ^= (unsigned)(h >> 32);
+                if (ev_out && (int64_t)i0 + j < ev_cap) ev_out[i0 + j] = r.w[j];
+                l_top = fmax(l_top, r.eq[j]); l_bottom = fmin(l_bottom, r.eq[j]);
+            }
+            d[j] = r.a[j] ? day_of(r.w[j]) : (j ? d[j - 1] : 0);
         }
-        if (a1) {
-            l_hash ^= event_hash(i0 + 1, w1);
-            if (ev_out && (int64_t)i0 + 1 < ev_cap) ev_out[i0 + 1] = w1;
-        }
-        if (a0) { l_top = fmax(l_top, r.eq0); l_bottom = fmin(l_bottom, r.eq0); }
-        if (a1) { l_top = fmax(l_top, r.eq1); l_bottom = fmin(l_bottom, r.eq1); }
 
         // calendar-day buckets
-        const int last_lane = (cnt - 1) >> 1;
-        const int d0 = a0 ? day_of(w0) : 0;
-        const int d1 = a1 ? day_of(w1) : d0;
-        const int first_day = __shfl_sync(FULL, d0, 0);
-        const int last_day = __shfl_sync(FULL, d1, last_lane);
+        const int last_lane = (cnt - 1) / R;
+        const int first_day = __shfl_sync(FULL, d[0], 0);
+        const int last_day = __shfl_sync(FULL, d[R - 1], last_lane);
         if (first_day == last_day && (!day_valid || first_day == day_cur)) {
             day_sum = (day_valid ? day_sum : 0.0) + batch_sum;      // the whole step falls into the open day
         } else {
-            // a record is a HEAD if it opens a day within the step; running day sum = segmented scan by heads.
-            // As a function of the running sum it receives, a lane is either additive (no head) or constant.
+            // a record is a HEAD if it opens a day within the step; running day sum = segmented scan by heads, in-lane
+            // over the four records, then across the warp.  As a function of the running sum it receives, a lane is
+            // either additive (no head) or constant.
             const bool merge_carry = day_valid && (first_day == day_cur);
-            const int d_before = __shfl_up_sync(FULL, d1, 1);
-            const bool head0 = a0 && (lane == 0 ? !merge_carry : d0 != d_before);
-            const bool head1 = a1 && d1 != d0;
-            double sg = head1 ? pnl1 : s2;
-            bool flag = head0 || head1;
+            const int d_before = __shfl_up_sync(FULL, d[R - 1], 1);
+            bool head[R];
+            double part[R];           // running day sum of the lane's own records (from its last head)
+            bool flag = false;
 #pragma unroll
-            for (int d = 1; d < 32; d <<= 1) {
-                const double up = shfl_up_d(sg, d);
-                const int fup = __shfl_up_sync(FULL, (int)flag, d);
-                if (lane >= d && !flag) { sg += up; flag = fup; }
+            for (int j = 0; j < R; ++j) {
+                head[j] = r.a[j] && (j ? d[j] != d[j - 1] : (lane == 0 ? !merge_carry : d[0] != d_before));
+                part[j] = (j == 0 || head[j]) ? r.pnl[j] : part[j - 1] + r.pnl[j];
+                flag = flag || head[j];
+            }
+            double sg = part[R - 1];
+#pragma unroll
+            for (int s = 1; s < 32; s <<= 1) {
+                const double up = shfl_up_d(sg, s);
+                const int fup = __shfl_up_sync(FULL, (int)flag, s);
+                if (lane >= s && !flag) { sg += up; flag = fup; }
             }
             // (the open day carried in is part of lane 0's chain when it continues)
             if (merge_carry && !flag) sg += day_sum;          // lanes whose chain reaches back to the step's start
             double carry_in = shfl_up_d(sg, 1);
             if (lane == 0) carry_in = merge_carry ? day_sum : 0.0;
-            const double run0 = head0 ? pnl0 : carry_in + pnl0;     // running day sum after record 2l
-            const double run1 = sg;                                  // ... after record 2l+1 (== run0 if inactive)
-            // TAIL = last record of its day within the step, except the step's last record (its day stays open)
-            const int d_after = __shfl_down_sync(FULL, d0, 1);
-            const bool tail0 = a0 && (a1 ? head1 : false);
-            const bool tail1 = a1 && lane < last_lane && d_after != d1;
-            // (an unpaired last record 2l is the step's last record: its day stays open)
-            unsigned t0m = __ballot_sync(FULL, tail0), t1m = __ballot_sync(FULL, tail1);
-            if (day_valid && !merge_carry) finish_day(day_cur, day_sum);
-            while (t0m | t1m) {
-                const int j = __ffs(t0m | t1m) - 1;
-                const unsigned bit = 1u << j;
-                if (t0m & bit) finish_day(__shfl_sync(FULL, d0, j), shfl_d(run0, j));
-                if (t1m & bit) finish_day(__shfl_sync(FULL, d1, j), shfl_d(run1, j));
-                t0m &= ~bit; t1m &= ~bit;
+            // running day sum after each record: records behind a head of their own lane have it in part[]
+            double run[R];
+            bool seen = false;
+#pragma unroll
+            for (int j = 0; j < R; ++j) {
+                seen = seen || head[j];
+                run[j] = seen ? part[j] : carry_in + part[j];
             }
-            day_sum = (cnt & 1) ? shfl_d(run0, last_lane) : shfl_d(run1, last_lane);
+            // TAIL = last record of its day within the step, except the step's last record (its day stays open)
+            const int d_after = __shfl_down_sync(FULL, d[0], 1);
+            unsigned tails = 0u;      // bit j: record j is a tail
+#pragma unroll
+            for (int j = 0; j < R - 1; ++j) tails |= (r.a[j] && head[j + 1]) ? 1u << j : 0u;
+            tails |= (r.a[R - 1] && lane < last_lane && d_after != d[R - 1]) ? 1u << (R - 1) : 0u;
+            // Finished days go to the lane that closes them; the chunk's first finished day, which may continue the
+            // previous chunk's last one, is kept aside (first_sum).  A day carried in that ends at the step's start
+            // comes before every tail of the step.
+            if (day_valid && !merge_carry) {
+                if (!first_done) { first_done = 1; first_id = day_cur; first_sum = day_sum; }
+                else if (lane == 0) day_complete(da, day_sum);
+            }
+            if (!first_done) {
+                const unsigned lanes_with = __ballot_sync(FULL, tails != 0u);
+                if (lanes_with) {
+                    const int src = __ffs(lanes_with) - 1;
+                    const int j = __ffs(tails) - 1;   // (this lane's first tail)
+                    const double x = j == 0 ? run[0] : j == 1 ? run[1] : j == 2 ? run[2] : run[3];
+                    const int id = j == 0 ? d[0] : j == 1 ? d[1] : j == 2 ? d[2] : d[3];
+                    first_sum = shfl_d(x, src);
+                    first_id = __shfl_sync(FULL, id, src);
+                    first_done = 1;
+                    if (lane == src) tails &= tails - 1u;
+                }
+            }
+#pragma unroll
+            for (int j = 0; j < R; ++j)
+                if (tails & (1u << j)) day_complete(da, run[j]);
+            day_sum = shfl_d(run[R - 1], last_lane);          // (a missing record repeats its predecessor's run)
         }
         day_cur = last_day;
         day_valid = 1;
@@ -991,14 +1027,33 @@ chunk_partial_kernel(const float* __restrict__ price, int64_t ld_price, const b2
     // per-lane accumulators -> chunk totals
     const double tot_profit = warp_sum_d(l_gain), tot_loss = warp_sum_d(l_loss);
     const double largest_p = warp_max_d(l_maxp), largest_l = warp_min_d(l_minl);
-    const unsigned n_win = __reduce_add_sync(FULL, l_win), n_loss = __reduce_add_sync(FULL, l_los);
-    long long sum_dur = l_dur;
-    unsigned hlo = (unsigned)l_hash, hhi = (unsigned)(l_hash >> 32);
+    unsigned n_win, n_loss;
+    if (count < 0x10000u) {           // both counts fit a 16-bit half: one reduction
+        const unsigned both = __reduce_add_sync(FULL, l_win | (l_los << 16));
+        n_win = both & 0xffffu; n_loss = both >> 16;
+    } else {
+        n_win = __reduce_add_sync(FULL, l_win); n_loss = __reduce_add_sync(FULL, l_los);
+    }
+    const long long sum_dur = (long long)__reduce_add_sync(FULL, l_dur);
+    const unsigned hlo = __reduce_xor_sync(FULL, l_hlo), hhi = __reduce_xor_sync(FULL, l_hhi);
+    double top = l_top, bottom = l_bottom;
 #pragma unroll
-    for (int m = 16; m > 0; m >>= 1) sum_dur += __shfl_xor_sync(FULL, sum_dur, m);
-    hlo = __reduce_xor_sync(FULL, hlo);
-    hhi = __reduce_xor_sync(FULL, hhi);
-    const double top = warp_max_d(l_top), bottom = warp_min_d(l_bottom);
+    for (int m = 16; m > 0; m >>= 1) {
+        top = fmax(top, shfl_xor_d(top, m));
+        bottom = fmin(bottom, shfl_xor_d(bottom, m));
+    }
+    // the lanes' finished days, merged in lane order (lane l takes lane l + s's, which come after its own)
+    if (__any_sync(FULL, da.n_days != 0u)) {
+#pragma unroll
+        for (int s = 1; s < 32; s <<= 1) {
+            DayAcc o;
+            o.pivot = __shfl_down_sync(FULL, da.pivot, s); o.s1 = __shfl_down_sync(FULL, da.s1, s);
+            o.s2 = __shfl_down_sync(FULL, da.s2, s); o.n_days = __shfl_down_sync(FULL, da.n_days, s); o.pivot_set = 1;
+            o.npivot = __shfl_down_sync(FULL, da.npivot, s); o.ns1 = __shfl_down_sync(FULL, da.ns1, s);
+            o.ns2 = __shfl_down_sync(FULL, da.ns2, s); o.n_neg = __shfl_down_sync(FULL, da.n_neg, s);
+            if (lane + s < 32) day_merge(da, o);
+        }
+    }
     if (lane == 0) {
         ChunkPartial q;
         q.tot_profit = tot_profit; q.tot_loss = tot_loss; q.largest_p = largest_p; q.largest_l = largest_l;
@@ -1045,7 +1100,7 @@ chunk_prefix_kernel(int pop, int S, const int32_t* __restrict__ seg_base, const 
 }
 
 // Drawdown of the listed chunks (chunk_prefix_kernel), one warp per chunk over a device-side count: equity from E0, running
-// peak from P0 and the drawdown candidates record by record (the arithmetic of batch_core, two records per lane).
+// peak from P0 and the drawdown candidates record by record (the arithmetic of batch_core, four records per lane).
 __global__ void __launch_bounds__(128)
 chunk_peak_kernel(const float* __restrict__ price, int64_t ld_price, const b200bt_individual* __restrict__ indiv,
                   const uint2* __restrict__ pool, const int* __restrict__ next, const int* __restrict__ seg_first,
@@ -1059,13 +1114,16 @@ chunk_peak_kernel(const float* __restrict__ price, int64_t ld_price, const b200b
         const int seg = pk.x;
         double equity = seg_e0[seg], peak = seg_p0[seg], maxdd = 0.0;
         walk_records(pool, next, pool_blocks, seg_first, seg_count, seg_in, price + (int64_t)pk.z * ld_price, seg,
-                     indiv[pk.y].position_size, equity, [&](const RecordPair& r, double) {
-            const bool a0 = r.a0, a1 = r.a1;
-            const double eq0 = r.eq0, eq1 = r.eq1;
-            const double m2 = fmax(a0 ? eq0 : -INFINITY, a1 ? eq1 : -INFINITY);
-            double pk0 = peak, pk1 = peak;
-            if (__any_sync(FULL, m2 > peak)) {
-                double p = m2;
+                     indiv[pk.y].position_size, equity, [&](const RecordQuad& r, double) {
+            constexpr int R = WR_PER_LANE;
+            double m = -INFINITY;                          // the lane's largest equity
+#pragma unroll
+            for (int j = 0; j < R; ++j) m = fmax(m, r.a[j] ? r.eq[j] : -INFINITY);
+            double pkj[R];
+#pragma unroll
+            for (int j = 0; j < R; ++j) pkj[j] = peak;
+            if (__any_sync(FULL, m > peak)) {
+                double p = m;
 #pragma unroll
                 for (int d = 1; d < 32; d <<= 1) {
                     const double up = shfl_up_d(p, d);
@@ -1073,15 +1131,21 @@ chunk_peak_kernel(const float* __restrict__ price, int64_t ld_price, const b200b
                 }
                 double before = shfl_up_d(p, 1);           // peak over the records of the lanes in front
                 before = fmax(lane == 0 ? peak : before, peak);
-                pk0 = fmax(before, eq0);
-                pk1 = fmax(pk0, eq1);
+#pragma unroll
+                for (int j = 0; j < R; ++j) pkj[j] = fmax(j ? pkj[j - 1] : before, r.eq[j]);
                 peak = fmax(peak, shfl_d(p, 31));
             }
-            const double gap0 = __dsub_rn(pk0, eq0), gap1 = __dsub_rn(pk1, eq1);
             const double lim = maxdd * (1.0 - 1e-12);
-            const bool c0 = a0 && gap0 > 0.0 && gap0 >= lim * pk0, c1 = a1 && gap1 > 0.0 && gap1 >= lim * pk1;
-            if (__any_sync(FULL, c0 || c1))
-                maxdd = fmax(maxdd, warp_max_d(fmax(c0 ? __ddiv_rn(gap0, pk0) : 0.0, c1 ? __ddiv_rn(gap1, pk1) : 0.0)));
+            double cand = 0.0;
+            bool any = false;
+#pragma unroll
+            for (int j = 0; j < R; ++j) {
+                const double gap = __dsub_rn(pkj[j], r.eq[j]);
+                const bool c = r.a[j] && gap > 0.0 && gap >= lim * pkj[j];
+                if (c) cand = fmax(cand, __ddiv_rn(gap, pkj[j]));
+                any = any || c;
+            }
+            if (__any_sync(FULL, any)) maxdd = fmax(maxdd, warp_max_d(cand));
         });
         if (lane == 0) partial[seg].maxdd = maxdd;
     }
@@ -1163,20 +1227,8 @@ __global__ void lane_combine_kernel(const b200bt_individual* __restrict__ indiv,
             if (open_day == q.first_day) x += open_sum; else day_complete(da, open_sum);
         }
         day_complete(da, x);
-        if (q.n_days) {
-            // the chunk's own finished days, accumulated about its pivot: shift to the lane's pivot
-            const double d = q.pivot - da.pivot, n = (double)q.n_days;
-            da.s1 += q.s1 + n * d;
-            da.s2 += q.s2 + 2.0 * d * q.s1 + n * d * d;
-            da.n_days += q.n_days;
-        }
-        if (q.n_neg) {
-            if (da.n_neg == 0) da.npivot = q.npivot;
-            const double d = q.npivot - da.npivot, n = (double)q.n_neg;
-            da.ns1 += q.ns1 + n * d;
-            da.ns2 += q.ns2 + 2.0 * d * q.ns1 + n * d * d;
-            da.n_neg += q.n_neg;
-        }
+        // the chunk's own finished days, accumulated about its pivots: shifted to the lane's
+        day_merge(da, DayAcc{q.pivot, q.s1, q.s2, q.n_days, 1, q.npivot, q.ns1, q.ns2, q.n_neg});
         open = true; open_day = q.day_cur; open_sum = q.day_sum;
     }
     a.pivot = da.pivot; a.s1 = da.s1; a.s2 = da.s2; a.n_days = da.n_days; a.pivot_set = da.pivot_set;

@@ -93,6 +93,25 @@ __device__ __forceinline__ void day_complete(DayAcc& a, double x) {
     }
 }
 
+// Append the days of `b` (which come after those of `a`) to `a`: b's moments are shifted from its pivots to a's (an
+// empty `a` takes b's pivots, shift 0).
+__device__ __forceinline__ void day_merge(DayAcc& a, const DayAcc& b) {
+    if (b.n_days) {
+        if (a.n_days == 0) { a.pivot = b.pivot; a.pivot_set = 1; }
+        const double d = b.pivot - a.pivot, n = (double)b.n_days;
+        a.s1 += b.s1 + n * d;
+        a.s2 += b.s2 + 2.0 * d * b.s1 + n * d * d;
+        a.n_days += b.n_days;
+    }
+    if (b.n_neg) {
+        if (a.n_neg == 0) a.npivot = b.npivot;
+        const double d = b.npivot - a.npivot, n = (double)b.n_neg;
+        a.ns1 += b.ns1 + n * d;
+        a.ns2 += b.ns2 + 2.0 * d * b.ns1 + n * d * d;
+        a.n_neg += b.n_neg;
+    }
+}
+
 // PnL of one trade record (strategy_evaluation.py:798,:819,:836): an entry record costs the entry fee,
 // an exit record realises quantity * move - both fees, with quantity = position_size / entry_price.
 __device__ __forceinline__ double record_pnl(bool active, unsigned w, float pf, unsigned w_prev, float p_prev,
