@@ -181,6 +181,15 @@ __global__ void fitness_reduce_kernel(const b200bt_lane_stats* __restrict__ stat
 using namespace b200bt;
 
 namespace b200bt {
+int check_sweep_clock(const char* who, const b200bt_sweep_config* cfg, int64_t N) {
+    B200BT_REQUIRE(cfg->bar_minutes > 0 && cfg->minute0 >= 0 && cfg->gap_minutes >= 0, B200BT_EINVAL,
+                   "%s: bar_minutes must be > 0, minute0 and gap_minutes >= 0", who);
+    // (minute0 is compared against the rest: no int64 overflow for any minute0)
+    B200BT_REQUIRE(cfg->minute0 < (1ll << 32) - 1440 - N * (int64_t)cfg->bar_minutes - cfg->gap_minutes, B200BT_ELIMIT,
+                   "%s: minute0 + N*bar_minutes + gap_minutes must stay below 2^32 - 1440 minutes", who);
+    return B200BT_OK;
+}
+
 // The fused sweep over the first *pop_dev (<= pop) entries of `order`: the grid covers `pop` entries and warps beyond the
 // device-side count leave at once.  The exact fallback of the time-chunked sweeps: the list of individuals to re-run and its
 // length never leave the device.
@@ -211,13 +220,10 @@ extern "C" int b200bt_sweep(const float* price, int64_t ld_price, const float* r
     B200BT_REQUIRE(S > 0 && N > 0 && P > 0 && pop > 0, B200BT_EINVAL, "sweep: bad sizes");
     B200BT_REQUIRE(ld_price >= N && ld_rsi >= N, B200BT_EINVAL, "sweep: row stride shorter than N");
     B200BT_REQUIRE(N < (1ll << 30), B200BT_ELIMIT, "sweep: N must be < 2^30 bars");
-    B200BT_REQUIRE(cfg_host->bar_minutes > 0, B200BT_EINVAL, "sweep: bar_minutes must be > 0");
-    B200BT_REQUIRE(cfg_host->gap_minutes >= 0, B200BT_EINVAL, "sweep: negative gap_minutes");
-    B200BT_REQUIRE(cfg_host->minute0 >= 0 &&
-                       cfg_host->minute0 + N * (int64_t)cfg_host->bar_minutes + cfg_host->gap_minutes < (1ll << 32) - 1440,
-                   B200BT_ELIMIT, "sweep: minute0 + N*bar_minutes must stay below 2^32 minutes");
+    int rc = check_sweep_clock("sweep", cfg_host, N);
+    if (rc) return rc;
     B200BT_REQUIRE(events == nullptr || event_cap > 0, B200BT_EINVAL, "sweep: event buffer without capacity");
-    int rc = check_device();
+    rc = check_device();
     if (rc) return rc;
     return launch_sweep(price, ld_price, rsi, ld_rsi, P, S, N, indiv, order, pop, nullptr, cfg_host, stats, events, event_cap,
                         (cudaStream_t)stream);

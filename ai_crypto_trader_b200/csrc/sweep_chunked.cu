@@ -1442,9 +1442,8 @@ int check_sweep_args(const char* who, const float* price, int64_t ld_price, cons
     B200BT_REQUIRE(S > 0 && N > 0 && P > 0, B200BT_EINVAL, "%s: bad sizes", who);
     B200BT_REQUIRE(ld_price >= N && ld_rsi >= N, B200BT_EINVAL, "%s: row stride shorter than N", who);
     B200BT_REQUIRE(N < (1ll << 30), B200BT_ELIMIT, "%s: N must be < 2^30 bars", who);
-    B200BT_REQUIRE(cfg_host->bar_minutes > 0 && cfg_host->minute0 >= 0 && cfg_host->gap_minutes >= 0 &&
-                       cfg_host->minute0 + N * (int64_t)cfg_host->bar_minutes + cfg_host->gap_minutes < (1ll << 32) - 1440,
-                   B200BT_ELIMIT, "%s: minute0 + N*bar_minutes must stay below 2^32 minutes", who);
+    const int rc = check_sweep_clock(who, cfg_host, N);
+    if (rc) return rc;
     B200BT_REQUIRE(events == nullptr || event_cap > 0, B200BT_EINVAL, "%s: event buffer without capacity", who);
     return B200BT_OK;
 }

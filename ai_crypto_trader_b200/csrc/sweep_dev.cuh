@@ -13,6 +13,11 @@ int launch_sweep(const float* price, int64_t ld_price, const float* rsi, int64_t
                  const b200bt_sweep_config* cfg_host, b200bt_lane_stats* stats, uint32_t* events, int64_t event_cap,
                  cudaStream_t stream);
 
+// The calendar clock of b200bt_sweep_config, checked on the host by all three sweep entry points (N < 2^30 already checked):
+// a negative field (minute0, gap_minutes) or bar_minutes <= 0 is B200BT_EINVAL; minute0 + N * bar_minutes + gap_minutes
+// >= 2^32 - 1440 is B200BT_ELIMIT, so that every minute the kernels form fits their unsigned 32-bit arithmetic.
+int check_sweep_clock(const char* who, const b200bt_sweep_config* cfg, int64_t N);
+
 constexpr int SW_WARPS = 8;         // warps (lanes of the sweep) per CTA
 #ifndef B200BT_SW_MIN_BLOCKS
 #define B200BT_SW_MIN_BLOCKS 2
@@ -192,7 +197,7 @@ static __device__ __noinline__ void batch_core(WarpAcc* __restrict__ acc, int cn
     const double peak_out = shfl_d(pk, cnt - 1);
 
     // daily buckets: segmented sum by calendar day over the batch, merged with the carry day
-    // calendar day of a record, relative to bar 0's day (32-bit: the host checks N*bar_minutes < 2^31 - 1440)
+    // calendar day of a record (unsigned 32-bit minutes: the host checks minute0 + N*bar_minutes + gap_minutes < 2^32 - 1440)
     const int day = active ? (int)(((unsigned)minute0 + bar * (unsigned)bar_minutes + (bar >= acc->gap_bar ? acc->gap_minutes : 0u)) / 1440u) : 0;
     DayAcc da{acc->pivot, acc->s1, acc->s2, acc->n_days, acc->pivot_set, acc->npivot, acc->ns1, acc->ns2, acc->n_neg};
     const int hold_first = acc->hold_first;

@@ -256,7 +256,8 @@ typedef struct b200bt_sweep_config {
  *  stats   [pop][S] lane stats (device, out)
  *  events  optional [pop][S][event_cap] uint32 (device, out), first event_cap
  *          event words per lane; NULL to skip
- * Limits: N < 2^30.
+ * Limits: N < 2^30 (else B200BT_ELIMIT); bar_minutes > 0, minute0 >= 0 and gap_minutes >= 0 (else B200BT_EINVAL);
+ * minute0 + N*bar_minutes + gap_minutes < 2^32 - 1440 (else B200BT_ELIMIT).  The time-chunked forms below check the same.
  */
 int b200bt_sweep(const float* price, int64_t ld_price,
                  const float* rsi, int64_t ld_rsi, int P,

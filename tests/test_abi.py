@@ -61,3 +61,51 @@ def test_argument_validation(native_lib):
     with pytest.raises(_lib.B200btError) as ei:
         _lib.call("b200bt_rsi_bank", None, 1, 64, 64, (C.c_int * 1)(14), 1, 1, None, None)
     assert ei.value.status == 10001
+
+
+_EINVAL, _ELIMIT = 10001, 10003
+_CLOCK_N, _CLOCK_BAR = 200_000, 7
+_CLOCK_END = (1 << 32) - 1440          # minute0 + N * bar_minutes + gap_minutes must stay below this
+
+
+def _sweep_calls(cfg):
+    """The three sweep entry points with real sizes (P = 26 periods, S = 2 symbols, N = 200 000 7-minute bars, 64
+    individuals) and the host config `cfg`.  The clock in cfg_host is checked before the device is touched; every config
+    passed here is rejected there, so the non-null dummy device pointers are never dereferenced and nothing is launched."""
+    from ai_crypto_trader_b200 import _lib
+    lib = _lib.load()
+    P, S, N, pop, K, n_seg, pool = 26, 2, _CLOCK_N, 64, 8, 64 * 8, 4096
+    dev = 1 << 20                                              # 16-byte aligned, never read
+    ws_c = int(lib.b200bt_sweep_chunked_workspace_bytes(pool, S, n_seg))
+    ws_t = int(lib.b200bt_sweep_tiled_workspace_bytes(pool, S, pop, K))
+    ref = C.byref(cfg)
+    return {
+        "b200bt_sweep": (dev, N, dev, N, P, S, N, dev, None, pop, ref, dev, None, 0, None),
+        "b200bt_sweep_chunked": (dev, N, dev, N, P, S, N, dev, None, pop, dev, n_seg, dev, dev, n_seg, 2048, 8, pool, dev,
+                                 ws_c, ref, dev, None, 0, dev, None, None),
+        "b200bt_sweep_tiled": (dev, N, dev, N, P, S, N, None, dev, dev, pop, None, pop, K, 1536, 2, pool, dev, ws_t, ref,
+                               dev, None, 0, dev, None, None),
+    }
+
+
+@pytest.mark.parametrize("case, minute0, gap_minutes, bar_minutes, status", [
+    ("sum at 2^32 - 1440", _CLOCK_END - _CLOCK_N * _CLOCK_BAR - 1441, 1441, _CLOCK_BAR, _ELIMIT),
+    ("minute0 at 2^32 - 1440", _CLOCK_END, 0, _CLOCK_BAR, _ELIMIT),
+    ("minute0 near 2^62", 1 << 62, 0, _CLOCK_BAR, _ELIMIT),
+    ("negative minute0", -1, 0, _CLOCK_BAR, _EINVAL),
+    ("negative gap_minutes", 0, -1, _CLOCK_BAR, _EINVAL),
+    ("negative gap_minutes, large minute0", _CLOCK_END - _CLOCK_N * _CLOCK_BAR, -1, _CLOCK_BAR, _EINVAL),
+    ("zero bar_minutes", 0, 0, 0, _EINVAL),
+])
+def test_sweep_entry_points_reject_an_out_of_range_calendar(native_lib, case, minute0, gap_minutes, bar_minutes, status):
+    """The kernels form calendar minutes in unsigned 32 bits: the three sweep entry points refuse a clock that leaves that
+    range (ELIMIT) and a negative clock field (EINVAL) alike.  The largest accepted clock, one minute lower than the
+    first case, is swept on the GPU in tests/test_gpu_sweep_calendar.py."""
+    from ai_crypto_trader_b200 import _lib
+    cfg = _lib.SweepConfig(initial_capital=10000.0, minute0=minute0, bar_minutes=bar_minutes, primary=0, secondary_mask=7,
+                           variant=0, gap_bar=_CLOCK_N // 2, gap_minutes=gap_minutes)
+    for name, args in _sweep_calls(cfg).items():
+        with pytest.raises(_lib.B200btError) as ei:
+            _lib.call(name, *args)
+        assert ei.value.status == status, (case, name, str(ei.value))
+        assert "minute0" in str(ei.value) or "bar_minutes" in str(ei.value), (case, name, str(ei.value))
