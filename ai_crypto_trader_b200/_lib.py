@@ -134,6 +134,8 @@ _SIGNATURES = {
     "b200bt_sweep_tiled": (C.c_int, [_vp, _i64, _vp, _i64, _i, _i, _i64, _vp, _vp, _vp, _i, _vp, _i, _i, _i, _i, _i,
                                      _vp, _i64, C.POINTER(SweepConfig), _vp, _vp, _i64, _vp, _vp, _vp]),
     "b200bt_fitness_reduce": (C.c_int, [_vp, _i, _i, _vp, _vp]),
+    "b200bt_book_metrics": (C.c_int, [_vp, _i64, _i, _i64, _vp, _i, C.POINTER(SweepConfig), _vp, _vp, _i64, _vp, _vp,
+                                      _vp]),
     "b200bt_backtest_ref": (C.c_int, [_vp, _i64, _i, _i64, _vp, _vp, _vp, _i64, _vp, _i64, _vp]),
     "b200bt_mc_gbm": (C.c_int, [C.c_double, C.c_double, C.c_double, C.c_double, _i64, _i, C.c_uint64, C.c_uint64,
                                 _vp, _vp, _vp, _vp]),

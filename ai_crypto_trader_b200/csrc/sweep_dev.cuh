@@ -133,26 +133,13 @@ __device__ __forceinline__ double record_pnl(bool active, unsigned w, float pf, 
     return -fee1;
 }
 
-// Consume `cnt` events in time order (lane j holds event j: word w, price pf); an exit record is
-// priced against the entry record that precedes it -- lane j-1, or for lane 0 the last event of
-// the previous batch (w_carry, p_carry).  The trade-record metrics of calculate_metrics
-// (strategy_evaluation.py:97-188) are advanced in `acc` (shared memory, one slot per warp).
-static __device__ __noinline__ void batch_core(WarpAcc* __restrict__ acc, int cnt, unsigned w, float pf, unsigned w_carry,
-                                        float p_carry, long long minute0, int bar_minutes, int64_t ev_cap) {
+// Advance the trade-record metrics of calculate_metrics (strategy_evaluation.py:97-188) in `acc` (shared memory, one slot
+// per warp) by `cnt` records in time order, already priced: lane j holds record j (event word w, pnl, duration dur counted
+// on this record).  `hw` is the word the trade hash mixes (w for a lane; w tagged with its symbol for a book, csrc/book.cu).
+__device__ __forceinline__ void batch_records(WarpAcc* __restrict__ acc, int cnt, bool active, unsigned w, unsigned hw,
+                                              double pnl, int dur, long long minute0, int bar_minutes, int64_t ev_cap) {
     const int lane = threadIdx.x & 31;
-#ifdef B200BT_SW_NOBATCH   // timing experiment only: skip the batch arithmetic
-    if (lane == 0) acc->n_events += cnt;
-    __syncwarp();
-    return;
-#endif
-    const bool active = lane < cnt;
-    float p_prev = __shfl_up_sync(FULL, pf, 1);
-    unsigned w_prev = __shfl_up_sync(FULL, w, 1);
-    if (lane == 0) { p_prev = p_carry; w_prev = w_carry; }
     const unsigned bar = w & 0x3fffffffu;
-
-    int dur;
-    const double pnl = record_pnl(active, w, pf, w_prev, p_prev, acc->size, acc->fee1, acc->fee2, dur);
     // wins / losses
     const bool win = active && pnl > 0.0, loss = active && pnl < 0.0;
     const unsigned n_win = acc->n_win + __popc(__ballot_sync(FULL, win));
@@ -248,7 +235,7 @@ static __device__ __noinline__ void batch_core(WarpAcc* __restrict__ acc, int cn
 
     // trade hash + optional event buffer
     const unsigned n_events = acc->n_events;
-    const unsigned long long h = active ? event_hash(n_events + lane, w) : 0ull;
+    const unsigned long long h = active ? event_hash(n_events + lane, hw) : 0ull;
     const unsigned hlo = __reduce_xor_sync(FULL, (unsigned)h);
     const unsigned hhi = __reduce_xor_sync(FULL, (unsigned)(h >> 32));
     uint32_t* ev_out = acc->ev_out;
@@ -271,6 +258,27 @@ static __device__ __noinline__ void batch_core(WarpAcc* __restrict__ acc, int cn
         acc->n_events = n_events + cnt;
     }
     __syncwarp();
+}
+
+// Consume `cnt` events in time order (lane j holds event j: word w, price pf); an exit record is
+// priced against the entry record that precedes it -- lane j-1, or for lane 0 the last event of
+// the previous batch (w_carry, p_carry).
+static __device__ __noinline__ void batch_core(WarpAcc* __restrict__ acc, int cnt, unsigned w, float pf, unsigned w_carry,
+                                        float p_carry, long long minute0, int bar_minutes, int64_t ev_cap) {
+    const int lane = threadIdx.x & 31;
+#ifdef B200BT_SW_NOBATCH   // timing experiment only: skip the batch arithmetic
+    if (lane == 0) acc->n_events += cnt;
+    __syncwarp();
+    return;
+#endif
+    const bool active = lane < cnt;
+    float p_prev = __shfl_up_sync(FULL, pf, 1);
+    unsigned w_prev = __shfl_up_sync(FULL, w, 1);
+    if (lane == 0) { p_prev = p_carry; w_prev = w_carry; }
+
+    int dur;
+    const double pnl = record_pnl(active, w, pf, w_prev, p_prev, acc->size, acc->fee1, acc->fee2, dur);
+    batch_records(acc, cnt, active, w, w, pnl, dur, minute0, bar_minutes, ev_cap);
 }
 
 // Fused kernel: consume 32 (or the last few) queued events; batches there start on an entry record.

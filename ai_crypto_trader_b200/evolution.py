@@ -26,7 +26,10 @@ logger = logging.getLogger("b200bt.evolution")
 
 class StrategyEvolutionService:
     def __init__(self, market: MarketData, config: Optional[Dict] = None, leverage_trading: Optional[bool] = None,
-                 random_seed: Optional[int] = None):
+                 random_seed: Optional[int] = None, aggregation: Optional[str] = None):
+        """aggregation: the GA fitness of a multi-symbol strategy, "mean" of the per-symbol scores or the score of its
+        "book" (all symbols as one trade list, PopulationSweep); default: config key evolution.fitness_aggregation,
+        else "mean"."""
         self.config = config or {}
         if leverage_trading is None:
             leverage_trading = os.getenv("LEVERAGE_TRADING", "false").lower() == "true"     # :62
@@ -37,7 +40,9 @@ class StrategyEvolutionService:
         goals = self.config.get("evolution", {}).get("optimization_goals") or DEFAULT_GOALS
         self.market = market
         rsi_lo, rsi_hi = self.param_ranges["rsi_period"]
-        self.sweep = PopulationSweep(market, rsi_periods=range(int(rsi_lo), int(rsi_hi) + 1), optimization_goals=goals)
+        self.aggregation = aggregation or self.config.get("evolution", {}).get("fitness_aggregation") or "mean"
+        self.sweep = PopulationSweep(market, rsi_periods=range(int(rsi_lo), int(rsi_hi) + 1), optimization_goals=goals,
+                                     aggregation=self.aggregation)
         self.fitness = ShardedFitness(self.sweep.evaluate, device=market.device)
         self.random_seed = random_seed
         self.evolution_records: List[Dict] = []

@@ -24,6 +24,7 @@ import torch
 
 from . import _lib
 from .sweep import DEFAULT_GOALS, MarketData, PopulationSweep
+from .synth import bar_timestamp
 
 logger = logging.getLogger("b200bt.strategy_evaluation")
 
@@ -415,7 +416,47 @@ class StrategyEvaluationSystem:
 
     # -- batched form -------------------------------------------------------------
     def evaluate_population(self, population: List[Dict], market: MarketData,
-                            sweep: Optional[PopulationSweep] = None) -> np.ndarray:
-        """fitness[i] = mean over symbols of score(metrics(simulate(population[i], symbol)))."""
-        sweep = sweep or PopulationSweep(market, optimization_goals=self.optimization_goals)
+                            sweep: Optional[PopulationSweep] = None, aggregation: str = "mean") -> np.ndarray:
+        """aggregation "mean": fitness[i] = mean over symbols of score(metrics(simulate(population[i], symbol)));
+        "book": fitness[i] = score(metrics(records of population[i] on every symbol, as one trade list)).  A given
+        `sweep` evaluates under its own aggregation."""
+        sweep = sweep or PopulationSweep(market, optimization_goals=self.optimization_goals, aggregation=aggregation)
         return sweep.evaluate(population)
+
+    def evaluate_book(self, strategy_id: str, parameters: Dict, market: MarketData) -> Dict:
+        """evaluate_strategy (:528-577) on the book of one strategy: its records on every symbol of `market`, in symbol
+        order, as ONE trade list.  Returns calculate_metrics + calculate_advanced_metrics of that list (daily / monthly
+        returns, equity curve and symbol dicts included, built on the host from the records, formatted as
+        _simulate_trades formats them) and `score`, the GPU book pass's score on the advanced dict (the composition of
+        evaluate_strategy).  Errors: logged, {} returned (the reference's convention)."""
+        try:
+            sweep = PopulationSweep(market, optimization_goals=self.optimization_goals, aggregation="book",
+                                    score_on_advanced=True)
+            fitness = sweep.evaluate([dict(parameters)])
+            lanes = sweep.lane_stats()["n_records"][0]
+            events = sweep.events()
+            close = market.close.cpu().numpy()
+            size = 10000 * (min(parameters.get("max_position_size", 5), 20) / 100)      # :761-764
+            trades = []
+            for s in range(market.S):
+                entry = 0.0
+                for w in events[0, s, :int(lanes[s])].tolist():
+                    bar, is_exit, sell = w & _lib.EVENT_BAR_MASK, bool(w & _lib.EVENT_EXIT), bool(w & _lib.EVENT_SELL)
+                    px = float(close[s, bar])
+                    if not is_exit:
+                        entry = px
+                        qty, pnl = size / px, -size * 0.001
+                    else:
+                        qty = size / entry
+                        pnl = qty * ((px - entry) if sell else (entry - px)) - size * 0.002
+                    trades.append({"timestamp": bar_timestamp(bar, market.minute0, market.bar_minutes),
+                                   "symbol": market.symbols[s], "side": "sell" if sell else "buy", "price": px,
+                                   "quantity": qty, "fees": size * 0.001, "pnl": pnl})
+            metrics = StrategyPerformanceMetrics.calculate_metrics(trades, sweep.cfg.initial_capital)
+            out = StrategyPerformanceMetrics.calculate_advanced_metrics(metrics)
+            out.update(strategy_id=strategy_id, parameters=parameters, score=float(fitness[0]),
+                       timestamp=datetime.now().isoformat())
+            return out
+        except Exception as e:        # reference convention: log, return an empty result
+            logger.error("Error evaluating the book of strategy %s: %s", strategy_id, e)
+            return {}

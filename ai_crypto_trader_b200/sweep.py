@@ -11,7 +11,9 @@ reference evaluates serially in Python:
 and reduces fitness(individual) = mean over symbols of score.  (The
 composition simulate -> metrics -> score is the reference's own, see
 cross_validate_strategy :682-691; the mean over symbols mirrors its mean over
-folds, :1030-1060.)
+folds, :1030-1060.)  With aggregation="book" the fitness is instead the score of the
+individual's combined multi-symbol trade list (`b200bt_book_metrics`), the list
+evaluate_strategy (:528-577) hands to calculate_metrics.
 
 PyTorch is used for device memory and streams only; all arithmetic happens in
 the hand-written sm_90a kernels behind the C-ABI.
@@ -509,6 +511,13 @@ def evaluation_order(population: List[Dict]) -> np.ndarray:
     return np.lexsort((np.arange(len(population)), -lane_costs(population), period)).astype(np.int32)
 
 
+BOOK_MAX_SYMBOLS = 64                  # b200bt_book_metrics: one 64-bit symbol mask per bar
+# Event buffers of one book slice: 24 GiB holds configs[1] (1024 individuals x 10 symbols) unsliced up to 629 k records in
+# its busiest lane (of 1M bars), beside the sweep's own event pool (plan_batches' 8 GiB), on an 80 GB H100.
+BOOK_MAX_EVENT_BYTES = 24 << 30
+BOOK_CAP_HEADROOM = 4                  # a learnt event cap is the last busiest lane + 1/4
+
+
 class PopulationSweep:
     """Evaluate a GA population against device-resident market data.
 
@@ -520,20 +529,36 @@ class PopulationSweep:
     def __init__(self, market: MarketData, rsi_periods: Iterable[int] = range(5, 31),
                  optimization_goals: Optional[Dict] = None, initial_capital: float = 10000.0,
                  event_cap: int = 0, mode: str = "auto", chunk_options: Optional[Dict] = None,
-                 score_on_advanced: bool = False, timeframes: Sequence[int] = ()):
+                 score_on_advanced: bool = False, timeframes: Sequence[int] = (), aggregation: str = "mean",
+                 max_event_bytes: Optional[int] = None):
         """score_on_advanced: take the strategy score on calculate_advanced_metrics' dict (the composition of
         evaluate_strategy, strategy_evaluation.py:545-557: `expectancy`, `sortino_ratio`, ... exist as keys) instead of the
         plain calculate_metrics dict (cross_validate_strategy :683-691, the default).
         mode: "fused" (one warp per lane, serial in time), "chunked" (expensive lanes split into verified
         time chunks, one warp per chunk), "tiled" (every lane split into the same K verified chunks, one THREAD
-        per chunk; csrc/sweep_chunked.cu) or "auto" (tiled from 131072 bars up, fused below)."""
+        per chunk; csrc/sweep_chunked.cu) or "auto" (tiled from 131072 bars up, fused below).
+        aggregation: how evaluate() turns an individual's symbols into one fitness: "mean" = the mean over symbols of the
+        per-symbol scores, "book" = the score of the book, the individual's records on every symbol in one trade list
+        (evaluate_strategy's composition, strategy_evaluation.py:528-577; see book_stats()).
+        max_event_bytes: budget of the event buffers of a book evaluation (default BOOK_MAX_EVENT_BYTES); a population whose
+        buffers exceed it is swept and booked in slices."""
         self._setup(market, sorted(set(int(p) for p in rsi_periods)), optimization_goals, initial_capital, event_cap, mode,
-                    chunk_options, score_on_advanced, timeframes)
+                    chunk_options, score_on_advanced, timeframes, aggregation=aggregation, max_event_bytes=max_event_bytes)
 
     def _setup(self, market: MarketData, periods: List[int], optimization_goals: Optional[Dict], initial_capital: float,
                event_cap: int, mode: str, chunk_options: Optional[Dict], score_on_advanced: bool, timeframes: Sequence[int],
-               bank: Optional[torch.Tensor] = None) -> None:
+               bank: Optional[torch.Tensor] = None, aggregation: str = "mean", max_event_bytes: Optional[int] = None) -> None:
         """The initialisation of both constructors: `periods` in bank-row order, `bank` = None computes the bank."""
+        if aggregation not in ("mean", "book"):
+            raise ValueError(f"aggregation must be 'mean' or 'book', not {aggregation!r}")
+        if aggregation == "book" and market.S > BOOK_MAX_SYMBOLS:
+            raise ValueError(f"aggregation='book' handles at most {BOOK_MAX_SYMBOLS} symbols ({market.S} given)")
+        self.aggregation = aggregation
+        self.max_event_bytes = int(BOOK_MAX_EVENT_BYTES if max_event_bytes is None else max_event_bytes)
+        self._book_cap = 0                     # event_cap learnt from the previous book evaluation (0: count first)
+        self._book = None                      # book stats [pop][20] float64 of the last book evaluation (host)
+        self.book_resweeps = 0                 # slices of the last book evaluation swept again with the exact cap
+        self.last_event_bytes = 0              # largest event buffer of the last book evaluation
         self.market = market
         self.periods = periods
         self.period_row = {p: i for i, p in enumerate(self.periods)}
@@ -605,14 +630,15 @@ class PopulationSweep:
     @classmethod
     def from_bank(cls, market: MarketData, bank: torch.Tensor, periods, optimization_goals=None,
                   initial_capital: float = 10000.0, event_cap: int = 0, mode: str = "fused",
-                  score_on_advanced: bool = False) -> "PopulationSweep":
+                  score_on_advanced: bool = False, aggregation: str = "mean",
+                  max_event_bytes: Optional[int] = None) -> "PopulationSweep":
         """Sweep over a caller-supplied RSI bank [S][P][N] (e.g. the 'rsi' field of the reference's
         market-data points) instead of one computed from the close prices."""
         periods = [int(p) for p in periods]
         assert bank.is_cuda and bank.dtype == torch.float32 and tuple(bank.shape) == (market.S, len(periods), market.N)
         self = cls.__new__(cls)
         self._setup(market, periods, optimization_goals, initial_capital, event_cap, mode, None, score_on_advanced, (),
-                    bank=bank.contiguous())
+                    bank=bank.contiguous(), aggregation=aggregation, max_event_bytes=max_event_bytes)
         return self
 
     # -- device-side evaluation (inputs already resident) -------------------
@@ -811,7 +837,92 @@ class PopulationSweep:
         population and D2H of the fitness vector happen inside this call."""
         if not population:
             return np.zeros(0, dtype=np.float64)
+        if self.aggregation == "book":
+            return self._evaluate_book(*self._unique(population))
         return self._evaluate_unique(*self._unique(population), self.event_cap)
+
+    def _evaluate_book(self, packed: np.ndarray, population: List[Dict], expand: Optional[np.ndarray]) -> np.ndarray:
+        """evaluate() under aggregation="book": sweep with event buffers, then b200bt_book_metrics.
+
+        The event cap of the first book evaluation is exact: a sweep without events counts every lane's records first.
+        Later evaluations reuse the largest lane of the previous one with BOOK_CAP_HEADROOM; a slice in which some book
+        lost records to a too-small guess is swept again with its exact cap (the lane counts are exact either way), so the
+        results never depend on the guess.  Slices of the population keep their event buffers within max_event_bytes."""
+        m = self.market
+        U, S = len(packed), m.S
+        cap = self._book_cap
+        if cap <= 0:
+            self._evaluate_unique(packed, population, None, 0)
+            cap = self._exact_cap(self._stats)
+        per_row = lambda c: max(1, self.max_event_bytes // (S * c * 4))     # individuals whose event buffers fit the budget
+        lanes = torch.empty((U, S, _lib.LANE_STATS_WORDS), dtype=torch.float64, device=m.device)
+        book = torch.empty((U, _lib.LANE_STATS_WORDS), dtype=torch.float64, device=m.device)
+        fit = torch.empty(U, dtype=torch.float64, device=m.device)
+        indiv = torch.from_numpy(packed.view(np.uint8)).to(m.device).view(U, -1)
+        self.book_resweeps, self.last_event_bytes, busiest = 0, 0, 0
+        rows = per_row(cap)
+        todo = [(lo, min(U, lo + rows), cap, False) for lo in range(0, U, rows)]      # (lo, hi, event cap, cap is exact)
+        while todo:
+            lo, hi, c, exact = todo.pop(0)
+            self._evaluate_unique(packed[lo:hi], population[lo:hi], None, c)
+            self.last_event_bytes = max(self.last_event_bytes, (hi - lo) * S * c * 4)
+            if not exact and int(self._stats[:, :, 0].max().item()) > c:
+                # records were lost to a too-small guess: the slice's lane counts are exact, so it is swept again with its
+                # exact cap, cut again so that every piece keeps within the budget (the guessed buffers are freed first)
+                self.book_resweeps += 1
+                need = self._exact_cap(self._stats)
+                self._stats = self._events = self._buffer_key = None
+                step = per_row(need)
+                todo[:0] = [(a, min(hi, a + step), need, True) for a in range(lo, hi, step)]
+                continue
+            self._book_slice(indiv[lo:hi], book[lo:hi], fit[lo:hi], c)
+            lanes[lo:hi] = self._stats
+            busiest = max(busiest, self._exact_cap(self._stats))
+        self._book_cap = busiest + busiest // BOOK_CAP_HEADROOM + 2
+        if self._stats.shape[0] != U:                  # the event words of the slices were not kept together
+            self._events, self._buffer_key = None, None
+        self._stats, self._inverse = lanes, expand
+        self._book = book.cpu().numpy()
+        if expand is not None:
+            self._book = self._book[expand]
+        res = fit.cpu().numpy()
+        return res if expand is None else res[expand]
+
+    @staticmethod
+    def _exact_cap(stats: torch.Tensor) -> int:
+        """Event cap that holds every record of every lane of `stats` (n_records of the busiest lane, at least 2)."""
+        return max(2, int(stats[:, :, 0].max().item()))
+
+    def _book_slice(self, indiv: torch.Tensor, book: torch.Tensor, fit: torch.Tensor, cap: int) -> None:
+        """b200bt_book_metrics on the lanes and event words of the last sweep (one slice of the population)."""
+        m = self.market
+        with torch.cuda.device(m.device):
+            _lib.call("b200bt_book_metrics", m.close.data_ptr(), _lib.ld(m.close), m.S, m.N, indiv.data_ptr(), indiv.shape[0],
+                      C.byref(self.cfg), self._stats.data_ptr(), self._events.data_ptr(), cap, book.data_ptr(),
+                      fit.data_ptr(), _lib.current_stream())
+
+    def book_stats(self) -> Dict[str, np.ndarray]:
+        """Book metrics of the last aggregation="book" evaluation: the lane_stats() fields as [pop] arrays, computed on each
+        individual's records on every symbol as one trade list (b200bt_book_metrics), plus
+          return_pct          net_profit / initial_capital * 100
+          avg_trade_duration  minutes, over the merged record pairs (2k, 2k+1) (calculate_metrics :166-178, whose pairs may
+                              mix symbols); bars * bar_minutes, so a pair across the seam of a glued series (set_gap)
+                              does not count the gap
+          profitable_symbols  bool [pop][S]: the symbol's records net a profit (symbol_pnl > 0, :190-199); a symbol without
+                              records is in neither of the reference's symbol dicts, so test it with n_records of lane_stats()
+        lane_stats() still describes the per-symbol lanes of the same evaluation."""
+        if self._book is None:
+            raise RuntimeError("book_stats() needs an evaluate() under aggregation='book' first")
+        raw = self._book
+        out = {name: raw[:, i] for i, name in enumerate(_lib.LANE_STATS_FIELDS[:-1])}
+        out["trade_hash"] = np.ascontiguousarray(raw[:, _lib.LANE_STATS_WORDS - 1]).view(np.uint64)
+        out["return_pct"] = out["net_profit"] / self.cfg.initial_capital * 100
+        pairs = np.floor(out["n_records"] / 2)
+        with np.errstate(divide="ignore", invalid="ignore"):
+            out["avg_trade_duration"] = np.where(pairs > 0, out["sum_duration_bars"] * self.market.bar_minutes / pairs, 0.0)
+        lanes = self.lane_stats()
+        out["profitable_symbols"] = (lanes["n_records"] > 0) & (lanes["net_profit"] > 0)
+        return out
 
     def _evaluate_unique(self, packed: np.ndarray, population: List[Dict], expand: Optional[np.ndarray],
                          event_cap: int) -> np.ndarray:

@@ -345,6 +345,29 @@ int b200bt_sweep_scan_wait_cycles(int64_t cycles);
 int b200bt_fitness_reduce(const b200bt_lane_stats* stats, int pop, int S,
                           double* fitness, b200bt_stream_t stream);
 
+/* Book metrics: the score of ONE account trading every symbol.  StrategyEvaluationSystem.evaluate_strategy
+ * (services/strategy_evaluation.py:528-577) passes one trade list to calculate_metrics (:32-228), which sorts it by timestamp
+ * (:67) and walks one equity curve, one drawdown and one set of daily buckets over all of it (:118-188).  The book of
+ * individual i is the concatenation, in symbol order 0..S-1, of its records on every symbol (_simulate_trades :746-878),
+ * sorted stably by timestamp: the order (bar, symbol, record index within the lane).  book_stats[i] holds calculate_metrics'
+ * scalars on that list, with the lane rules of b200bt_lane_stats: Sharpe / Sortino over the calendar days of the whole
+ * book, n_records < 2 gives the short dict of :43-92; and _calculate_strategy_score (:579-633) under cfg's score rule, with
+ * two book-specific fields:
+ *   sum_duration_bars  sum over the merged pairs (2k, 2k+1) of bar(2k+1) - bar(2k): avg_trade_duration pairs neighbouring
+ *                      records of the merged list (:166-178) even when they belong to different symbols (a quirk of the
+ *                      reference, kept for parity)
+ *   trade_hash         xor over merged records r (index r in the book) of event_hash(r, word_r ^ (symbol_r * 0x9E3779B1));
+ *                      with S = 1 it is the lane's trade_hash
+ * Records are priced as b200bt_trade_pnl prices them.  Inputs are a sweep's: lane_stats [pop][S] (n_records), events
+ * [pop][S][event_cap] and price [S][ld_price] (device), indiv [pop] (device), cfg (host; its clock is checked like the
+ * sweeps').  A book with a lane of n_records > event_cap lost records: it gets n_records = -1, score and fitness NaN, and
+ * must be computed again from a sweep with a larger event_cap.  fitness_or_null: optional device float64 [pop] = score.
+ * Limits: S <= 64 (B200BT_ELIMIT above: one 64-bit symbol mask per bar), N < 2^30, S * (N + 1) < 2^32.  No synchronisation. */
+int b200bt_book_metrics(const float* price, int64_t ld_price, int S, int64_t N,
+                        const b200bt_individual* indiv, int pop, const b200bt_sweep_config* cfg,
+                        const b200bt_lane_stats* lane_stats, const uint32_t* events, int64_t event_cap,
+                        b200bt_lane_stats* book_stats, double* fitness_or_null, b200bt_stream_t stream);
+
 /* ------------------------------------------------------------------------
  * The reference's own single-symbol bar loop (BASELINE configs[0]):
  *   StrategyTester.backtest_strategy   backtesting/strategy_tester.py:156-312

@@ -1,0 +1,181 @@
+#!/usr/bin/env python
+"""Cost of the book pass (b200bt_book_metrics) on the configs[1] workload, beside the sweep that feeds it.
+
+    python tools/book_bench.py [--reps 5] [--check 3]
+
+The configs[1] synthetic market of bench.py (10 symbols x 1M 1-minute bars) and two populations of 1024: the random one
+(seed 42) and generation 3 of GeneticAlgorithm(seed 42) started from it (its lanes write several times more records).  For
+each population, in alternating rounds, CUDA events time
+  * the sweep without event buffers (PopulationSweep.evaluate_device, the plan `evaluate` uses);
+  * the same sweep writing every lane's event words (event_cap = the busiest lane);
+  * b200bt_book_metrics on those buffers.
+records/s = the population's trade records / time.  `--check` books of each population (the busiest ones and a random
+sample) are compared with the record-by-record oracle (tests/book_ref.py on the C oracle's lanes).  Prints one JSON line
+with the card's name, power limit, the SM clock sampled while timing and the book kernel's registers / local memory.
+Needs an H100; no fallback.
+"""
+import argparse
+import json
+import re
+import subprocess
+import sys
+import time
+from pathlib import Path
+
+ROOT = Path(__file__).resolve().parents[1]
+sys.path.insert(0, str(ROOT))
+sys.path.insert(0, str(ROOT / "tests"))
+import ctypes as C
+
+import numpy as np
+import torch
+
+
+def _card():
+    out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i",
+                          str(torch.cuda.current_device())], capture_output=True, text=True, timeout=30).stdout
+    name, power = [x.strip() for x in out.strip().splitlines()[0].split(",")]
+    return name, power
+
+
+def _resources():
+    from ai_crypto_trader_b200 import _lib
+    import shutil
+    tool = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
+    try:
+        text = subprocess.run([tool, "-res-usage", str(_lib.LIB_PATH)], capture_output=True, text=True, timeout=120).stdout
+    except OSError:
+        return None
+    fn = None
+    for line in text.splitlines():
+        m = re.search(r"Function (\S+):", line)
+        if m:
+            fn = m.group(1)
+            continue
+        if fn and "book_kernel" in fn:
+            r, loc, sh = re.search(r"REG:(\d+)", line), re.search(r"LOCAL:(\d+)", line), re.search(r"SHARED:(\d+)", line)
+            if r:
+                return {"registers": int(r.group(1)), "local_bytes": int(loc.group(1)) if loc else None,
+                        "shared_bytes": int(sh.group(1)) if sh else None}
+    return None
+
+
+def _check(sweep, population, idx, close, bank):
+    """Largest relative deviation of the GPU books `idx` (of the last book evaluation) from the oracle's."""
+    import book_ref
+    from oracle import sim_oracle
+    got = sweep.book_stats()
+    cfg = sim_oracle.config_of(sweep.market.minute0, sweep.market.bar_minutes)
+    worst, exact = 0.0, True
+    for i in idx:
+        p = population[i]
+        evs, pns = [], []
+        for s in range(close.shape[0]):
+            _, ev, pn = sim_oracle.lane(close[s], bank[s, sweep.period_row[int(p["rsi_period"])]], p, cfg,
+                                        event_cap=close.shape[1] + 2)
+            evs.append(ev)
+            pns.append(pn)
+        want = book_ref.book(evs, pns, cfg)
+        for f in ("n_records", "trade_hash", "n_wins", "n_losses", "n_days", "n_negative_days", "sum_duration_bars"):
+            exact &= bool(got[f][i] == want[f])
+        for f in ("net_profit", "max_drawdown", "sharpe_ratio", "sortino_ratio", "score"):
+            a, b = float(got[f][i]), float(want[f])
+            if not (a == b or (np.isnan(a) and np.isnan(b))):
+                worst = max(worst, abs(a - b) / max(abs(b), 1e-300))
+    return {"books": len(idx), "exact_fields_equal": exact, "max_rel_dev": worst}
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--reps", type=int, default=5)
+    ap.add_argument("--check", type=int, default=3)
+    ap.add_argument("--symbols", type=int, default=10)
+    ap.add_argument("--bars", type=int, default=1_000_000)
+    ap.add_argument("--pop", type=int, default=1024)
+    a = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("book_bench needs a CUDA device (H100); there is no CPU path")
+    from bench import ClockSampler
+    from ai_crypto_trader_b200 import _lib, synth
+    from ai_crypto_trader_b200.genetic_algorithm import GeneticAlgorithm
+    from ai_crypto_trader_b200.sweep import MarketData, PopulationSweep, decode_population
+    torch.cuda.set_device(0)
+    ohlcv = synth.synth_ohlcv(a.symbols, a.bars)
+    market = MarketData(ohlcv)
+    random_pop = synth.random_population(a.pop, seed=42)
+    ga = GeneticAlgorithm(synth.param_ranges(), PopulationSweep(market).fitness_function, population_size=a.pop,
+                          generations=3, random_seed=42)
+    ga.run(seeded_individuals=random_pop)
+    name, power = _card()
+    out = {"workload": f"configs[1]: population {a.pop} x {a.symbols} symbols x {a.bars} 1-minute bars",
+           "card": name, "power_limit": power, "book_kernel": _resources(), "populations": {}}
+    rng = np.random.default_rng(7)
+    for label, population in (("random", random_pop), ("generation_3", list(ga.population))):
+        sweep = PopulationSweep(market, aggregation="book")
+        sweep.evaluate(population)                        # plans, buffers, zone map, learnt cap
+        sweep.evaluate(population)
+        packed = decode_population(population, sweep.period_row)
+        pop = len(population)
+        indiv = torch.from_numpy(packed.view(np.uint8)).to(market.device)
+        plan = sweep.plan(population)
+        lanes = sweep.lane_stats()
+        records = float(lanes["n_records"].sum())
+        cap = max(2, int(lanes["n_records"].max()))
+        fit = torch.empty(pop, dtype=torch.float64, device=market.device)
+        book = torch.empty((pop, _lib.LANE_STATS_WORDS), dtype=torch.float64, device=market.device)
+        st = _lib.current_stream()
+
+        # the sweep without events runs on its own instance: one instance would reallocate (and zero) its event buffer
+        # every time the event cap changes between the timed legs
+        plain = PopulationSweep(market)
+        plain.evaluate(population)
+        plain_plan = plain.plan(population)
+        plain_fit = torch.empty(pop, dtype=torch.float64, device=market.device)
+
+        def sweep_plain():
+            plain.evaluate_device(indiv, None, pop, plain_fit, plan=plain_plan, event_cap=0)
+
+        def sweep_events():
+            sweep.evaluate_device(indiv, None, pop, fit, plan=plan, event_cap=cap)
+
+        def book_pass():
+            _lib.call("b200bt_book_metrics", market.close.data_ptr(), _lib.ld(market.close), market.S, market.N,
+                      indiv.data_ptr(), pop, C.byref(sweep.cfg), sweep._stats.data_ptr(), sweep._events.data_ptr(), cap,
+                      book.data_ptr(), fit.data_ptr(), st)
+
+        legs = {"sweep_no_events": sweep_plain, "sweep_with_events": sweep_events, "book_metrics": book_pass}
+        sweep_plain(); sweep_events(); book_pass(); torch.cuda.synchronize()
+        times = {k: [] for k in legs}
+        clocks = ClockSampler(torch.cuda.current_device())
+        clocks.start()
+        time.sleep(0.3)
+        w0 = time.time()
+        for _ in range(a.reps):
+            for k, fn in legs.items():
+                if k == "book_metrics":
+                    sweep_events()                        # the book reads the buffers this sweep wrote
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record()
+                fn()
+                e1.record()
+                torch.cuda.synchronize()
+                times[k].append(e0.elapsed_time(e1))
+        w1 = time.time()
+        res = {k: {"ms_median": float(np.median(v)), "ms_runs": v, "records_per_s": records / (float(np.median(v)) * 1e-3)}
+               for k, v in times.items()}
+        # the timed book equals the one evaluate() returned
+        mine = book.cpu().numpy()
+        ref = sweep._book if sweep._inverse is None else None
+        same = None if ref is None else bool(np.array_equal(mine[:, 0], ref[:, 0]) and
+                                             np.array_equal(mine[:, -1].view(np.uint64), ref[:, -1].view(np.uint64)))
+        busiest = list(np.argsort(-sweep.book_stats()["n_records"])[:max(1, a.check // 2)])
+        sample = busiest + list(rng.choice(pop, size=max(0, a.check - len(busiest)), replace=False))
+        check = _check(sweep, population, sample, ohlcv[3], sweep.bank.cpu().numpy()) if a.check else None
+        out["populations"][label] = {"records": records, "busiest_lane": cap, "event_buffer_bytes": pop * market.S * cap * 4,
+                                     "legs": res, "sm_clock": clocks.stop(w0, w1), "timed_book_equals_evaluate": same,
+                                     "oracle_check": check}
+    print(json.dumps(out))
+
+
+if __name__ == "__main__":
+    main()
