@@ -11,6 +11,17 @@
 //                         uniform crossover (one coin per gene, :180-186); then per gene with probability
 //                         mutation_rate (:191-223): integer genes +-max(1, int(0.1 (hi - lo))), float genes either
 //                         x U(0.8, 1.2) or + U(-0.1 span, 0.1 span), clamped to the range.
+//
+// The stream is a function of the source alone, so tests/ga_ref.py restates it draw for draw:
+//   words      counter = (slot or pair index, generation, stream id, block index), key = (seed low, seed high); a block's
+//              words are handed out x[3], x[2], x[1], x[0], and one (slot, stream) is one continuous word stream, so a
+//              uniform() after an odd number of words takes its two words from two blocks
+//   uniform()  53 bits: the high 27 from the first word drawn, the low 26 from the second (sequenced statements, not
+//              one expression whose operand order the compiler picks)
+//   arithmetic the three products that are fused are written as fma() -- init lo + (hi - lo) u, the x U(0.8, 1.2)
+//              factor and the + U(-0.1 span, 0.1 span) step -- so the results do not depend on --fmad; every other
+//              float64 operation is rounded on its own
+#include <math.h>
 #include "common.cuh"
 #include "philox.cuh"
 
@@ -24,7 +35,8 @@ struct GaRanges {
     int is_int[GA_MAX_GENES];
 };
 
-// a stream of uniforms for one (generation, slot, stream id): counter = (slot, generation, stream, block index)
+// a stream of words for one (generation, slot, stream id): counter = (slot, generation, stream, block index); words
+// x[3], x[2], x[1], x[0] of block 0, then of block 1, ...
 struct GaRng {
     uint32_t k0, k1, c0, c1, c2, blk, have;
     uint32_t x[4];
@@ -34,7 +46,11 @@ struct GaRng {
         if (have == 0) { philox4x32_10(c0, c1, c2, blk++, k0, k1, x); have = 4; }
         return x[--have];
     }
-    __device__ double uniform() { return ((double)(next() >> 5) * 67108864.0 + (double)(next() >> 6)) * (1.0 / 9007199254740992.0); }  // [0,1), 53 bits
+    __device__ double uniform() {                      // [0,1), 53 bits: high 27 from the first word, low 26 from the second
+        const double hi = (double)(next() >> 5);
+        const double lo = (double)(next() >> 6);
+        return (hi * 67108864.0 + lo) * (1.0 / 9007199254740992.0);
+    }
     __device__ uint32_t below(uint32_t n) { return (uint32_t)(((uint64_t)next() * n) >> 32); }   // uniform integer in [0, n)
 };
 
@@ -93,10 +109,10 @@ __global__ void ga_breed_kernel(const double* __restrict__ params, const int32_t
                     const double step = fmax(1.0, floor((hi - lo) * 0.1));
                     v += (mut.next() & 1u) ? step : -step;
                 } else if (mut.uniform() < 0.5) {
-                    v *= 0.8 + 0.4 * mut.uniform();
+                    v *= fma(mut.uniform(), 0.4, 0.8);
                 } else {
                     const double span = hi - lo;
-                    v += (2.0 * mut.uniform() - 1.0) * 0.1 * span;
+                    v = fma((2.0 * mut.uniform() - 1.0) * 0.1, span, v);
                 }
                 v = fmax(lo, fmin(hi, v));
             }
@@ -116,7 +132,7 @@ __global__ void ga_init_kernel(int pop, int genes, int n_seeded, const GaRanges 
         double v;
         if (j < n_seeded) v = fmax(lo, fmin(hi, params[(int64_t)j * genes + g]));
         else if (R.is_int[g]) v = lo + (double)rng.below((uint32_t)(hi - lo) + 1u);
-        else v = lo + (hi - lo) * rng.uniform();
+        else v = fma(hi - lo, rng.uniform(), lo);
         params[(int64_t)j * genes + g] = v;
     }
 }
@@ -156,13 +172,14 @@ extern "C" int b200bt_ga_next_generation(const double* params, const double* fit
                    "ga_next_generation: null or aliased pointer");
     B200BT_REQUIRE(pop > 0 && tournament >= 1 && tournament <= GA_MAX_TOURNAMENT && tournament <= pop, B200BT_EINVAL,
                    "ga_next_generation: 1 <= tournament <= min(pop, %d)", GA_MAX_TOURNAMENT);
+    B200BT_REQUIRE(isfinite(elitism_pct), B200BT_EINVAL, "ga_next_generation: elitism_pct is not finite");
     GaRanges R;
     int rc = fill_ranges(lo_host, hi_host, is_int_host, genes, R, "ga_next_generation");
     if (rc) return rc;
     if ((rc = check_device())) return rc;
-    int n_elite = (int)(elitism_pct * pop);
-    if (n_elite < 1) n_elite = 1;          // (:142)
-    if (n_elite > pop) n_elite = pop;
+    // min(pop, max(1, int(elitism_pct * pop))) (:142), clamped in double so that no out-of-range value is cast to int
+    const double elite_count = elitism_pct * pop;
+    const int n_elite = elite_count >= (double)pop ? pop : elite_count < 1.0 ? 1 : (int)elite_count;
     cudaStream_t st = (cudaStream_t)stream;
     ga_select_kernel<<<(pop + 127) / 128, 128, 0, st>>>(fitness, ranked, pop, n_elite, tournament, seed, generation, selected_workspace);
     B200BT_LAUNCH_CHECK("ga_select launch");

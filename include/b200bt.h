@@ -539,7 +539,8 @@ int b200bt_correlation(const float* x, int64_t ld, int S, int64_t N, double* out
  * The operators of services/genetic_algorithm.py:83-252 over a device matrix params [pop][genes] float64 (integer
  * genes hold integral values).  Ranges: host arrays lo / hi / is_int of length genes (<= 64).  Randomness is
  * Philox4x32-10 keyed by (seed; generation, slot): parity with the reference's Mersenne-twister stream is
- * DISTRIBUTIONAL (same operators and probabilities), results are a pure function of (seed, generation, inputs). */
+ * DISTRIBUTIONAL (same operators and probabilities), results are a pure function of (seed, generation, inputs),
+ * restated draw for draw by tests/ga_ref.py. */
 
 /* initialize_population (:83-117): rows >= n_seeded are drawn uniformly from the ranges (randint / uniform),
  * rows < n_seeded (already written by the caller) are clamped to the ranges. */
@@ -550,7 +551,10 @@ int b200bt_ga_init(double* params, int pop, int genes, int n_seeded, const doubl
  * ranked: device int32[pop], indices by descending fitness (stable); selected_workspace: device int32[pop].
  * elites = max(1, int(elitism_pct * pop)) best, copied unchanged to the first rows; every other selected slot is the
  * winner of a tournament of `tournament` (<= 8) distinct contenders; offspring pairs come from two uniform draws
- * of the selected list, uniform crossover with probability crossover_rate, per-gene mutation with mutation_rate. */
+ * of the selected list, uniform crossover with probability crossover_rate, per-gene mutation with mutation_rate.
+ * elitism_pct must be finite (EINVAL otherwise, checked before the device); the elite count is clamped in double
+ * precision, so any elitism_pct * pop >= pop gives pop elites (a plain copy of the best individuals) and any value
+ * below 1 gives one. */
 int b200bt_ga_next_generation(const double* params, const double* fitness, const int32_t* ranked, int pop, int genes,
                               const double* lo, const double* hi, const int* is_int, double elitism_pct,
                               int tournament, double crossover_rate, double mutation_rate, uint64_t seed,
