@@ -1,0 +1,444 @@
+// Backtest overfitting of an evolved population (sm_90a): per-day PnL rows of a sweep's records, and the combinatorially
+// symmetric cross-validation (CSCV) of Bailey, Borwein, Lopez de Prado and Zhu (2015) on a matrix of such rows.
+//
+// daily_pnl_kernel  one warp per (individual, symbol) lane walks the lane's event words 32 at a time: coalesced word
+//                   loads, the entry word of an exit by shuffle (records come in (entry, exit) pairs and batches start on
+//                   an even index), record_pnl as trade_pnl_kernel / book_kernel price, a segmented warp sum by calendar
+//                   day, and the open day carried to the next batch.  Each (lane, day) cell is written once by its warp.
+// book_rows_kernel  one thread per (individual, day): the sum over symbols 0..S-1, in that order, of the lane rows.
+// cscv_*            moments (one thread per trial), a trial-tile-major combination pass that stages a tile's block
+//                   statistics in registers once and walks a run of combinations, a reduction to the selected trial,
+//                   and a second tile pass that counts the trials below / tied with the selected one out of sample.
+// Every fp64 operation of the CSCV path is an explicit _rn intrinsic: nothing is contracted into an FMA, so that
+// tests/cscv_ref.py restates the arithmetic bit for bit.
+#include <math.h>
+#include "sweep_dev.cuh"
+
+namespace b200bt {
+
+constexpr int DP_WARPS = 4;                  // lanes per CTA of the row pass
+constexpr unsigned DP_BAR_MASK = 0x3fffffffu;
+constexpr int CS_THREADS = 256;              // trials per tile of the combination passes
+constexpr int CS_WARPS = CS_THREADS / 32;
+constexpr int CS_RUN = 64;                   // combinations per shared-memory run of a tile pass
+constexpr int CS_MAX_BLOCKS = 20;
+
+// ---- per-day PnL rows ----------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(DP_WARPS * 32)
+daily_pnl_kernel(const float* __restrict__ price, int64_t ld_price, int S, const b200bt_individual* __restrict__ indiv,
+                 const b200bt_sweep_config cfg, const b200bt_lane_stats* __restrict__ lane_stats,
+                 const uint32_t* __restrict__ events, int64_t event_cap, double* __restrict__ lane_pnl, int64_t D,
+                 int first_day, int64_t n_lanes) {
+    const int lane = threadIdx.x & 31;
+    const int64_t w = (int64_t)blockIdx.x * DP_WARPS + (threadIdx.x >> 5);
+    if (w >= n_lanes) return;
+    double* row = lane_pnl + w * D;
+    const int64_t n_rec = (int64_t)lane_stats[w].n_records;
+    if (n_rec > event_cap) {                 // the event buffer lost records of this lane: no row
+        for (int64_t d = lane; d < D; d += 32) row[d] = NAN;
+        return;
+    }
+    const int s = (int)(w % S);
+    const double size = indiv[w / S].position_size;
+    const double fee1 = __dmul_rn(size, 0.001), fee2 = __dmul_rn(size, 0.002);
+    const unsigned gap_bar = cfg.gap_bar > 0 ? (unsigned)cfg.gap_bar : 0xffffffffu;
+    const unsigned gap_minutes = (unsigned)cfg.gap_minutes, minute0 = (unsigned)cfg.minute0;
+    const unsigned bar_minutes = (unsigned)cfg.bar_minutes;
+    const uint32_t* ev = events + w * event_cap;
+    const float* prow = price + (int64_t)s * ld_price;
+    int carry_day = -1;                      // open day of the previous batch (-1: none)
+    double carry = 0.0;
+    for (int64_t base = 0; base < n_rec; base += 32) {
+        const int64_t j = base + lane;
+        const bool active = j < n_rec;
+        const int n = (int)min((int64_t)32, n_rec - base);
+        const unsigned wd = active ? __ldg(ev + j) : 0u;
+        const unsigned bar = wd & DP_BAR_MASK;
+        const float pf = active ? __ldg(prow + bar) : 0.f;
+        const unsigned w_prev = __shfl_up_sync(FULL, wd, 1);     // an exit (odd index) follows its entry in this batch
+        const float p_prev = __shfl_up_sync(FULL, pf, 1);
+        int dur;
+        const double pnl = record_pnl(active, wd, pf, w_prev, p_prev, size, fee1, fee2, dur);
+        // calendar day: batch_records' unsigned 32-bit expression
+        const int day = active ? (int)((minute0 + bar * bar_minutes + (bar >= gap_bar ? gap_minutes : 0u)) / 1440u) : 0x7fffffff;
+        const int day_prev = __shfl_up_sync(FULL, day, 1), day_next = __shfl_down_sync(FULL, day, 1);
+        const bool head = lane == 0 || day != day_prev;
+        const bool tail = active && (lane == n - 1 || day != day_next);
+        double seg = pnl;
+        bool flag = head;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const double up = shfl_up_d(seg, d);
+            const int fup = __shfl_up_sync(FULL, (int)flag, d);
+            if (lane >= d && !flag) { seg += up; flag = fup; }
+        }
+        const int batch_first = __shfl_sync(FULL, day, 0);
+        if (carry_day >= 0 && carry_day != batch_first && lane == 0) row[carry_day - first_day] = carry;
+        if (tail && day == carry_day) seg = __dadd_rn(carry, seg);  // only the first segment can continue the open day
+        if (tail && lane != n - 1) row[day - first_day] = seg;
+        carry = shfl_d(seg, n - 1);
+        carry_day = __shfl_sync(FULL, day, n - 1);
+    }
+    if (carry_day >= 0 && lane == 0) row[carry_day - first_day] = carry;
+}
+
+__global__ void book_rows_kernel(const double* __restrict__ lane_pnl, int S, int64_t D, int64_t n, double* __restrict__ book) {
+    const int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= n) return;
+    const int64_t i = k / D, d = k - i * D;
+    const double* p = lane_pnl + i * S * D + d;
+    double acc = p[0];
+    for (int s = 1; s < S; ++s) acc = __dadd_rn(acc, p[(int64_t)s * D]);
+    book[k] = acc;
+}
+
+// ---- CSCV -----------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ int binom(int n, int r) {
+    if (r < 0 || r > n) return 0;
+    int c = 1;
+    for (int i = 1; i <= r; ++i) c = c * (n - r + i) / i;
+    return c;
+}
+
+// Combination c of itertools.combinations(range(B), B / 2) as a mask g: block b is in the set iff bit B-1-b of g is 0.
+// Lexicographic order of the index tuples is decreasing order of their bit-reversed masks, i.e. increasing order of the
+// complements g, which is the order of the combinatorial number system: g = sum over its set bits p_i of C(p_i, i).
+__device__ __forceinline__ unsigned unrank(int c, int B) {
+    unsigned g = 0u;
+    for (int i = B / 2, p = B - 1; i >= 1; --i) {
+        while (binom(p, i) > c) --p;
+        g |= 1u << p;
+        c -= binom(p, i);
+        --p;
+    }
+    return g;
+}
+
+__device__ __forceinline__ unsigned next_mask(unsigned g) {   // next mask with as many bits (Gosper)
+    const unsigned t = g | (g - 1u);
+    return (t + 1u) | (((~t & (0u - ~t)) - 1u) >> __ffs(g));
+}
+
+// Sharpe of a set of blocks: in-sample (the blocks of combination g) or out-of-sample (its complement).
+template <int B>
+__device__ __forceinline__ double set_sharpe(const double (&a)[B], const double (&q)[B], unsigned g, bool in_sample,
+                                             double mu, double n_set) {
+    double A = 0.0, Q = 0.0;
+#pragma unroll
+    for (int b = 0; b < B; ++b) {
+        const bool in = (((g >> (B - 1 - b)) & 1u) == 0u) == in_sample;
+        A = __dadd_rn(A, in ? a[b] : 0.0);          // A starts at +0.0: adding +0.0 leaves it bit-identical
+        Q = __dadd_rn(Q, in ? q[b] : 0.0);
+    }
+    const double m = __ddiv_rn(A, n_set);
+    const double v = __dsub_rn(__ddiv_rn(Q, n_set), __dmul_rn(m, m));
+    return v > 0.0 ? __dmul_rn(__ddiv_rn(__dadd_rn(mu, m), __dsqrt_rn(v)), __dsqrt_rn(252.0)) : 0.0;
+}
+
+__device__ __forceinline__ bool key_better(double s, int n, double bs, int bn) { return s > bs || (s == bs && n < bn); }
+
+__global__ void cscv_moments_kernel(const double* __restrict__ pnl, int64_t ld, int N, int64_t r, int B, int64_t L,
+                                    double* __restrict__ ab, double* __restrict__ qb, double* __restrict__ mu_out,
+                                    double* __restrict__ m2_out, double* __restrict__ m3_out, double* __restrict__ m4_out,
+                                    double* __restrict__ sr_out) {
+    const int n = blockIdx.x * blockDim.x + threadIdx.x;
+    if (n >= N) return;
+    const double* x = pnl + (int64_t)n * ld + r;
+    const int64_t T = (int64_t)B * L;
+    double s = 0.0;
+    for (int64_t t = 0; t < T; ++t) s = __dadd_rn(s, x[t]);
+    const double nt = (double)T;
+    const double mu = __ddiv_rn(s, nt);
+    double m2 = 0.0, m3 = 0.0, m4 = 0.0;
+    for (int b = 0; b < B; ++b) {
+        double a = 0.0, q = 0.0;
+        for (int64_t t = b * L; t < (b + 1) * L; ++t) {
+            const double d = __dsub_rn(x[t], mu), d2 = __dmul_rn(d, d);
+            a = __dadd_rn(a, d);
+            q = __dadd_rn(q, d2);
+            m2 = __dadd_rn(m2, d2);
+            m3 = __dadd_rn(m3, __dmul_rn(d2, d));
+            m4 = __dadd_rn(m4, __dmul_rn(d2, d2));
+        }
+        ab[(int64_t)b * N + n] = a;
+        qb[(int64_t)b * N + n] = q;
+    }
+    m2 = __ddiv_rn(m2, nt);
+    mu_out[n] = mu;
+    m2_out[n] = m2;
+    m3_out[n] = __ddiv_rn(m3, nt);
+    m4_out[n] = __ddiv_rn(m4, nt);
+    sr_out[n] = m2 > 0.0 ? __dmul_rn(__ddiv_rn(mu, __dsqrt_rn(m2)), __dsqrt_rn(252.0)) : 0.0;
+}
+
+template <int B>
+__device__ __forceinline__ void load_trial(const double* __restrict__ ab, const double* __restrict__ qb, int N, int n,
+                                           double (&a)[B], double (&q)[B]) {
+#pragma unroll
+    for (int b = 0; b < B; ++b) {
+        a[b] = n < N ? ab[(int64_t)b * N + n] : 0.0;
+        q[b] = n < N ? qb[(int64_t)b * N + n] : 0.0;
+    }
+}
+
+// Pass 1: per (combination, tile) the in-sample argmax of the tile's trials, key (SR, -n).
+template <int B>
+__global__ void __launch_bounds__(CS_THREADS)
+cscv_select_kernel(const double* __restrict__ ab, const double* __restrict__ qb, const double* __restrict__ mu_in, int N,
+                   double n_set, int C, double* __restrict__ part_sr, int* __restrict__ part_n) {
+    __shared__ double wsr[CS_WARPS][CS_RUN];
+    __shared__ int wn[CS_WARPS][CS_RUN];
+    const int tiles = gridDim.x, tile = blockIdx.x;
+    const int n = tile * CS_THREADS + threadIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const bool valid = n < N;
+    double a[B], q[B];
+    load_trial<B>(ab, qb, N, n, a, q);
+    const double mu = valid ? mu_in[n] : 0.0;
+    const int runs = (C + CS_RUN - 1) / CS_RUN;
+    for (int run = blockIdx.y; run < runs; run += gridDim.y) {
+        const int c0 = run * CS_RUN, cnt = min(CS_RUN, C - c0);
+        unsigned g = unrank(c0, B);
+        for (int k = 0; k < cnt; ++k) {
+            double s = valid ? set_sharpe<B>(a, q, g, true, mu, n_set) : -INFINITY;
+            int id = valid ? n : 0x7fffffff;
+#pragma unroll
+            for (int m = 16; m > 0; m >>= 1) {
+                const double os = shfl_xor_d(s, m);
+                const int on = __shfl_xor_sync(FULL, id, m);
+                if (key_better(os, on, s, id)) { s = os; id = on; }
+            }
+            if (lane == 0) { wsr[warp][k] = s; wn[warp][k] = id; }
+            g = next_mask(g);
+        }
+        __syncthreads();
+        if ((int)threadIdx.x < cnt) {
+            const int k = threadIdx.x;
+            double s = wsr[0][k];
+            int id = wn[0][k];
+            for (int v = 1; v < CS_WARPS; ++v)
+                if (key_better(wsr[v][k], wn[v][k], s, id)) { s = wsr[v][k]; id = wn[v][k]; }
+            part_sr[(int64_t)(c0 + k) * tiles + tile] = s;
+            part_n[(int64_t)(c0 + k) * tiles + tile] = id;
+        }
+        __syncthreads();
+    }
+}
+
+// Pass 2: per combination, the tiles' partials in ascending order (ties stay with the lowest trial), and the selected
+// trial's out-of-sample Sharpe.
+template <int B>
+__global__ void cscv_reduce_kernel(const double* __restrict__ ab, const double* __restrict__ qb, const double* __restrict__ mu_in,
+                                   int N, double n_set, int C, int tiles, const double* __restrict__ part_sr,
+                                   const int* __restrict__ part_n, int32_t* __restrict__ sel, double* __restrict__ is_sr,
+                                   double* __restrict__ oos_sr) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= C) return;
+    double s = part_sr[(int64_t)c * tiles];
+    int id = part_n[(int64_t)c * tiles];
+    for (int t = 1; t < tiles; ++t) {
+        const double ts = part_sr[(int64_t)c * tiles + t];
+        const int tn = part_n[(int64_t)c * tiles + t];
+        if (key_better(ts, tn, s, id)) { s = ts; id = tn; }
+    }
+    double a[B], q[B];
+    load_trial<B>(ab, qb, N, id, a, q);
+    sel[c] = id;
+    is_sr[c] = s;
+    oos_sr[c] = set_sharpe<B>(a, q, unrank(c, B), false, mu_in[id], n_set);
+}
+
+// Pass 3: per combination, trials whose out-of-sample Sharpe is below / equal to the selected trial's (integer counts,
+// added with integer atomics: the totals do not depend on the order).
+template <int B>
+__global__ void __launch_bounds__(CS_THREADS)
+cscv_count_kernel(const double* __restrict__ ab, const double* __restrict__ qb, const double* __restrict__ mu_in, int N,
+                  double n_set, int C, const int32_t* __restrict__ sel, const double* __restrict__ oos_sr,
+                  int32_t* __restrict__ n_below, int32_t* __restrict__ n_tied) {
+    __shared__ double o_sr[CS_RUN];
+    __shared__ int o_sel[CS_RUN], below[CS_RUN], tied[CS_RUN];
+    const int n = blockIdx.x * CS_THREADS + threadIdx.x, lane = threadIdx.x & 31;
+    const bool valid = n < N;
+    double a[B], q[B];
+    load_trial<B>(ab, qb, N, n, a, q);
+    const double mu = valid ? mu_in[n] : 0.0;
+    const int runs = (C + CS_RUN - 1) / CS_RUN;
+    for (int run = blockIdx.y; run < runs; run += gridDim.y) {
+        const int c0 = run * CS_RUN, cnt = min(CS_RUN, C - c0);
+        if ((int)threadIdx.x < cnt) {
+            o_sr[threadIdx.x] = oos_sr[c0 + threadIdx.x];
+            o_sel[threadIdx.x] = sel[c0 + threadIdx.x];
+            below[threadIdx.x] = 0;
+            tied[threadIdx.x] = 0;
+        }
+        __syncthreads();
+        unsigned g = unrank(c0, B);
+        for (int k = 0; k < cnt; ++k) {
+            const double s = valid ? set_sharpe<B>(a, q, g, false, mu, n_set) : 0.0;
+            const unsigned lo = __ballot_sync(FULL, valid && s < o_sr[k]);
+            const unsigned eq = __ballot_sync(FULL, valid && n != o_sel[k] && s == o_sr[k]);
+            if (lane == 0 && (lo | eq)) {
+                atomicAdd(&below[k], __popc(lo));
+                atomicAdd(&tied[k], __popc(eq));
+            }
+            g = next_mask(g);
+        }
+        __syncthreads();
+        if ((int)threadIdx.x < cnt) {
+            if (below[threadIdx.x]) atomicAdd(n_below + c0 + threadIdx.x, below[threadIdx.x]);
+            if (tied[threadIdx.x]) atomicAdd(n_tied + c0 + threadIdx.x, tied[threadIdx.x]);
+        }
+        __syncthreads();
+    }
+}
+
+struct CscvArgs {
+    const double* ab;
+    const double* qb;
+    const double* mu;
+    int N, C, tiles;
+    double n_set;
+    double* part_sr;
+    int* part_n;
+    int32_t *sel, *n_below, *n_tied;
+    double *is_sr, *oos_sr;
+};
+
+template <int B>
+int cscv_passes(const CscvArgs& A, cudaStream_t st) {
+    const int runs = (A.C + CS_RUN - 1) / CS_RUN;
+    const unsigned ny = (unsigned)max(1, min(runs, (4 * device_sm_count() + A.tiles - 1) / A.tiles));
+    cscv_select_kernel<B><<<dim3((unsigned)A.tiles, ny), CS_THREADS, 0, st>>>(A.ab, A.qb, A.mu, A.N, A.n_set, A.C, A.part_sr,
+                                                                               A.part_n);
+    B200BT_LAUNCH_CHECK("cscv select");
+    cscv_reduce_kernel<B><<<(unsigned)((A.C + 127) / 128), 128, 0, st>>>(A.ab, A.qb, A.mu, A.N, A.n_set, A.C, A.tiles,
+                                                                         A.part_sr, A.part_n, A.sel, A.is_sr, A.oos_sr);
+    B200BT_LAUNCH_CHECK("cscv reduce");
+    cscv_count_kernel<B><<<dim3((unsigned)A.tiles, ny), CS_THREADS, 0, st>>>(A.ab, A.qb, A.mu, A.N, A.n_set, A.C, A.sel,
+                                                                              A.oos_sr, A.n_below, A.n_tied);
+    B200BT_LAUNCH_CHECK("cscv count");
+    return B200BT_OK;
+}
+
+int64_t host_binom(int n, int r) {
+    int64_t c = 1;
+    for (int i = 1; i <= r; ++i) c = c * (n - r + i) / i;
+    return c;
+}
+
+// workspace: ab, qb [B][N] float64, then per (combination, tile) the argmax partials (float64 SR, int32 trial)
+int64_t cscv_layout(int N, int B, int64_t* part_off, int64_t* n_part) {
+    const int64_t tiles = (N + CS_THREADS - 1) / CS_THREADS;
+    const int64_t parts = host_binom(B, B / 2) * tiles;
+    const int64_t stats = 2 * (int64_t)B * N * 8;
+    if (part_off) *part_off = stats;
+    if (n_part) *n_part = parts;
+    return stats + parts * 12;
+}
+
+}  // namespace b200bt
+
+using namespace b200bt;
+
+extern "C" int b200bt_daily_pnl(const float* price, int64_t ld_price, int S, int64_t N, const b200bt_individual* indiv,
+                                int pop, const b200bt_sweep_config* cfg, const b200bt_lane_stats* lane_stats,
+                                const uint32_t* events, int64_t event_cap, double* lane_pnl, int64_t D,
+                                double* book_pnl_or_null, b200bt_stream_t stream) {
+    B200BT_REQUIRE(price && indiv && cfg && lane_stats && lane_pnl, B200BT_EINVAL, "daily_pnl: null pointer");
+    B200BT_REQUIRE(S >= 1 && pop >= 1 && N >= 1 && ld_price >= N, B200BT_EINVAL, "daily_pnl: bad sizes");
+    B200BT_REQUIRE(event_cap >= 0 && (events || event_cap == 0), B200BT_EINVAL, "daily_pnl: bad event buffer");
+    B200BT_REQUIRE(N < (1ll << 30), B200BT_ELIMIT, "daily_pnl: N must be < 2^30 bars");
+    int rc = check_sweep_clock("daily_pnl", cfg, N);
+    if (rc) return rc;
+    // calendar days of bar 0 and bar N - 1 (the kernels' unsigned 32-bit expression; the clock check keeps it exact)
+    const int64_t last = N - 1;
+    const int64_t gap = (cfg->gap_bar > 0 && last >= cfg->gap_bar) ? cfg->gap_minutes : 0;
+    const int64_t first_day = cfg->minute0 / 1440;
+    const int64_t span = (cfg->minute0 + last * cfg->bar_minutes + gap) / 1440 - first_day + 1;
+    B200BT_REQUIRE(D >= span, B200BT_EINVAL, "daily_pnl: D = %lld columns do not cover the %lld calendar days of the series",
+                   (long long)D, (long long)span);
+    B200BT_REQUIRE((int64_t)pop * S <= INT64_MAX / D, B200BT_ELIMIT, "daily_pnl: pop * S * D must fit int64");
+    rc = check_device();
+    if (rc) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    const int64_t lanes = (int64_t)pop * S;
+    rc = cuda_status(cudaMemsetAsync(lane_pnl, 0, (size_t)(lanes * D) * sizeof(double), st), "daily_pnl memset");
+    if (rc) return rc;
+    daily_pnl_kernel<<<(unsigned)((lanes + DP_WARPS - 1) / DP_WARPS), DP_WARPS * 32, 0, st>>>(
+        price, ld_price, S, indiv, *cfg, lane_stats, events, event_cap, lane_pnl, D, (int)first_day, lanes);
+    B200BT_LAUNCH_CHECK("daily_pnl");
+    if (book_pnl_or_null) {
+        const int64_t n = (int64_t)pop * D;
+        book_rows_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(lane_pnl, S, D, n, book_pnl_or_null);
+        B200BT_LAUNCH_CHECK("daily_pnl book rows");
+    }
+    return B200BT_OK;
+}
+
+static int cscv_check(int N, int64_t T, int B) {
+    B200BT_REQUIRE(N >= 2, B200BT_EINVAL, "cscv: need at least 2 trials (N = %d)", N);
+    B200BT_REQUIRE(B >= 2 && B % 2 == 0, B200BT_EINVAL, "cscv: the block count must be even and >= 2 (B = %d)", B);
+    B200BT_REQUIRE(B <= CS_MAX_BLOCKS, B200BT_ELIMIT, "cscv: at most %d blocks (B = %d)", CS_MAX_BLOCKS, B);
+    B200BT_REQUIRE(T >= 0 && T / B >= 2, B200BT_EINVAL, "cscv: T = %lld days give blocks of fewer than 2 days at B = %d",
+                   (long long)T, B);
+    return B200BT_OK;
+}
+
+extern "C" int64_t b200bt_cscv_workspace_bytes(int N, int64_t T, int B) {
+    if (N < 2 || B < 2 || B % 2 || B > CS_MAX_BLOCKS || T / B < 2) return 0;
+    return cscv_layout(N, B, nullptr, nullptr);
+}
+
+extern "C" int b200bt_cscv(const double* pnl, int64_t ld, int N, int64_t T, int B, void* workspace, int64_t workspace_bytes,
+                           int32_t* sel, double* is_sr, double* oos_sr, int32_t* n_below, int32_t* n_tied, double* mu,
+                           double* m2, double* m3, double* m4, double* sr, b200bt_stream_t stream) {
+    B200BT_REQUIRE(pnl && workspace && sel && is_sr && oos_sr && n_below && n_tied && mu && m2 && m3 && m4 && sr,
+                   B200BT_EINVAL, "cscv: null pointer");
+    int rc = cscv_check(N, T, B);
+    if (rc) return rc;
+    B200BT_REQUIRE(ld >= T, B200BT_EINVAL, "cscv: row stride %lld below T = %lld", (long long)ld, (long long)T);
+    int64_t part_off = 0, n_part = 0;
+    const int64_t need = cscv_layout(N, B, &part_off, &n_part);
+    B200BT_REQUIRE(workspace_bytes >= need, B200BT_EINVAL, "cscv: workspace too small (%lld < %lld)",
+                   (long long)workspace_bytes, (long long)need);
+    B200BT_REQUIRE(((uintptr_t)workspace & 15) == 0, B200BT_EINVAL, "cscv: workspace must be 16-byte aligned");
+    rc = check_device();
+    if (rc) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    const int64_t L = T / B, r = T - (int64_t)B * L;
+    const int C = (int)host_binom(B, B / 2);
+    char* ws = (char*)workspace;
+    CscvArgs A;
+    A.ab = (const double*)ws;
+    A.qb = (const double*)ws + (int64_t)B * N;
+    A.mu = mu;
+    A.N = N;
+    A.C = C;
+    A.tiles = (N + CS_THREADS - 1) / CS_THREADS;
+    A.n_set = (double)((int64_t)(B / 2) * L);
+    A.part_sr = (double*)(ws + part_off);
+    A.part_n = (int*)(ws + part_off + n_part * 8);
+    A.sel = sel;
+    A.is_sr = is_sr;
+    A.oos_sr = oos_sr;
+    A.n_below = n_below;
+    A.n_tied = n_tied;
+    cscv_moments_kernel<<<(unsigned)((N + 127) / 128), 128, 0, st>>>(pnl, ld, N, r, B, L, (double*)A.ab, (double*)A.qb, mu,
+                                                                     m2, m3, m4, sr);
+    B200BT_LAUNCH_CHECK("cscv moments");
+    rc = cuda_status(cudaMemsetAsync(n_below, 0, (size_t)C * 4, st), "cscv memset");
+    if (rc) return rc;
+    rc = cuda_status(cudaMemsetAsync(n_tied, 0, (size_t)C * 4, st), "cscv memset");
+    if (rc) return rc;
+    switch (B) {
+        case 2: return cscv_passes<2>(A, st);
+        case 4: return cscv_passes<4>(A, st);
+        case 6: return cscv_passes<6>(A, st);
+        case 8: return cscv_passes<8>(A, st);
+        case 10: return cscv_passes<10>(A, st);
+        case 12: return cscv_passes<12>(A, st);
+        case 14: return cscv_passes<14>(A, st);
+        case 16: return cscv_passes<16>(A, st);
+        case 18: return cscv_passes<18>(A, st);
+        default: return cscv_passes<20>(A, st);
+    }
+}

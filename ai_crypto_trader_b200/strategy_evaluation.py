@@ -460,3 +460,33 @@ class StrategyEvaluationSystem:
         except Exception as e:        # reference convention: log, return an empty result
             logger.error("Error evaluating the book of strategy %s: %s", strategy_id, e)
             return {}
+
+    def backtest_overfitting(self, population: List[Dict], market: MarketData, n_blocks: int = 16,
+                             sweep: Optional[PopulationSweep] = None) -> Dict:
+        """How much of the best backtest of `population` is selection bias: CSCV and the Deflated Sharpe Ratio on the
+        per-day PnL of every individual's book (its records on every symbol of `market`, PopulationSweep.daily_pnl).  The
+        trials are the distinct decoded individuals; the rows hold every calendar day of the series, zeros included, and
+        the Sharpe ratios are calculate_metrics' daily rule over all those days (overfitting.cscv).
+
+        Returns pbo, prob_oos_loss, degradation {slope, intercept, r2}, n_trials, n_combinations, n_blocks, block_days,
+        dropped_days, first_day, the per-combination arrays sel (a trial index), is_sr, oos_sr, n_below, n_tied, omega,
+        logit; [pop] arrays sharpe (annualised, all kept days) and deflated_sharpe; and best {index, sharpe,
+        deflated_sharpe}, the individual of highest full-sample Sharpe (the first one on ties).  Errors: logged, {}
+        returned (the reference's convention)."""
+        from .overfitting import cscv, deflated_sharpe
+        try:
+            sweep = sweep or PopulationSweep(market, optimization_goals=self.optimization_goals)
+            _, unique, expand = sweep._unique(population)
+            book, _, first_day = sweep.daily_pnl(unique)
+            res = cscv(book, n_blocks)
+            dsr = deflated_sharpe(res, res["n_trials"])
+            idx = np.arange(len(population)) if expand is None else np.asarray(expand)
+            out = {k: v for k, v in res.items() if k not in ("mu", "m2", "m3", "m4", "sharpe")}
+            out.update(first_day=first_day, sharpe=res["sharpe"][idx], deflated_sharpe=dsr[idx])
+            best = int(np.argmax(out["sharpe"]))
+            out["best"] = {"index": best, "sharpe": float(out["sharpe"][best]),
+                           "deflated_sharpe": float(out["deflated_sharpe"][best])}
+            return out
+        except Exception as e:        # reference convention: log, return an empty result
+            logger.error("Error measuring the backtest overfitting of a population: %s", e)
+            return {}

@@ -854,12 +854,32 @@ class PopulationSweep:
         if cap <= 0:
             self._evaluate_unique(packed, population, None, 0)
             cap = self._exact_cap(self._stats)
-        per_row = lambda c: max(1, self.max_event_bytes // (S * c * 4))     # individuals whose event buffers fit the budget
         lanes = torch.empty((U, S, _lib.LANE_STATS_WORDS), dtype=torch.float64, device=m.device)
         book = torch.empty((U, _lib.LANE_STATS_WORDS), dtype=torch.float64, device=m.device)
         fit = torch.empty(U, dtype=torch.float64, device=m.device)
         indiv = torch.from_numpy(packed.view(np.uint8)).to(m.device).view(U, -1)
-        self.book_resweeps, self.last_event_bytes, busiest = 0, 0, 0
+        busiest = 0
+        for lo, hi, c in self._event_slices(packed, population, cap):
+            self._book_slice(indiv[lo:hi], book[lo:hi], fit[lo:hi], c)
+            lanes[lo:hi] = self._stats
+            busiest = max(busiest, self._exact_cap(self._stats))
+        self._book_cap = busiest + busiest // BOOK_CAP_HEADROOM + 2
+        self._keep_slice_stats(lanes, expand)
+        self._book = book.cpu().numpy()
+        if expand is not None:
+            self._book = self._book[expand]
+        res = fit.cpu().numpy()
+        return res if expand is None else res[expand]
+
+    def _event_slices(self, packed: np.ndarray, population: List[Dict], cap: int):
+        """Sweep the decoded individuals `packed` with event buffers, in slices whose buffers keep within max_event_bytes,
+        and yield (lo, hi, event cap) once the slice [lo, hi) is swept: its lane stats and event words are then
+        self._stats / self._events, every record of every lane held.  `cap` is a guess (a learnt cap) or exact; a slice in
+        which some lane lost records to a too-small guess is swept again with its exact cap (the lane counts are exact
+        either way), cut again so that every piece keeps within the budget."""
+        U, S = len(packed), self.market.S
+        per_row = lambda c: max(1, self.max_event_bytes // (S * c * 4))     # individuals whose event buffers fit the budget
+        self.book_resweeps, self.last_event_bytes = 0, 0
         rows = per_row(cap)
         todo = [(lo, min(U, lo + rows), cap, False) for lo in range(0, U, rows)]      # (lo, hi, event cap, cap is exact)
         while todo:
@@ -867,26 +887,20 @@ class PopulationSweep:
             self._evaluate_unique(packed[lo:hi], population[lo:hi], None, c)
             self.last_event_bytes = max(self.last_event_bytes, (hi - lo) * S * c * 4)
             if not exact and int(self._stats[:, :, 0].max().item()) > c:
-                # records were lost to a too-small guess: the slice's lane counts are exact, so it is swept again with its
-                # exact cap, cut again so that every piece keeps within the budget (the guessed buffers are freed first)
                 self.book_resweeps += 1
                 need = self._exact_cap(self._stats)
-                self._stats = self._events = self._buffer_key = None
+                self._stats = self._events = self._buffer_key = None       # the guessed buffers are freed first
                 step = per_row(need)
                 todo[:0] = [(a, min(hi, a + step), need, True) for a in range(lo, hi, step)]
                 continue
-            self._book_slice(indiv[lo:hi], book[lo:hi], fit[lo:hi], c)
-            lanes[lo:hi] = self._stats
-            busiest = max(busiest, self._exact_cap(self._stats))
-        self._book_cap = busiest + busiest // BOOK_CAP_HEADROOM + 2
-        if self._stats.shape[0] != U:                  # the event words of the slices were not kept together
+            yield lo, hi, c
+
+    def _keep_slice_stats(self, lanes: torch.Tensor, expand: Optional[np.ndarray]) -> None:
+        """After _event_slices: lane_stats() describes every slice (`lanes`, assembled by the caller); the event words are
+        kept only when one slice held the whole population."""
+        if self._stats.shape[0] != lanes.shape[0]:     # the event words of the slices were not kept together
             self._events, self._buffer_key = None, None
         self._stats, self._inverse = lanes, expand
-        self._book = book.cpu().numpy()
-        if expand is not None:
-            self._book = self._book[expand]
-        res = fit.cpu().numpy()
-        return res if expand is None else res[expand]
 
     @staticmethod
     def _exact_cap(stats: torch.Tensor) -> int:
@@ -998,6 +1012,54 @@ class PopulationSweep:
         if bool((n_trips < 0).any()):
             raise RuntimeError("trade_pnl: a lane wrote more records than its event buffer held")
         return trip, n_trips, fee
+
+    DAILY_PNL_MAX_BYTES = 8 << 30
+
+    def calendar_days(self) -> Tuple[int, int]:
+        """(first_day, D): the calendar day of bar 0 (days since 1970-01-01 of the market's minute clock) and the number of
+        days from it to the day of the last bar, the skipped days of a glued series (set_gap) included."""
+        c, last = self.cfg, self.market.N - 1
+        first = c.minute0 // 1440
+        gap = c.gap_minutes if (c.gap_bar > 0 and last >= c.gap_bar) else 0
+        return first, (c.minute0 + last * c.bar_minutes + gap) // 1440 - first + 1
+
+    def daily_pnl(self, population: List[Dict], max_bytes: int = DAILY_PNL_MAX_BYTES):
+        """Per-day PnL of every individual's book and of its lanes, on the device, in the order of `population`:
+        (book float64 [pop][D], lanes float64 [pop][S][D], first_day).  Column d is calendar day first_day + d (days since
+        1970-01-01); lanes[i, s, d] is the sum of the pnl of the records of individual i on symbol s dated on that day,
+        book[i, d] their sum over symbols -- the daily buckets of calculate_metrics (strategy_evaluation.py:141-159) on the
+        book, kept for every calendar day of the series (a day without records is 0.0).  b200bt_daily_pnl.
+
+        A counting sweep gives the exact event cap, then slices of the population whose event buffers keep within
+        max_event_bytes are swept and bucketed.  Individuals that decode alike are swept once.  A ValueError names the
+        bytes when the output rows alone exceed `max_bytes`.  Afterwards lane_stats() describes this population."""
+        if not population:
+            raise ValueError("daily_pnl needs at least one individual")
+        m = self.market
+        packed, unique, expand = self._unique(population)
+        U, P, S = len(packed), len(population), m.S
+        first_day, D = self.calendar_days()
+        need = (U + (P if expand is not None else 0)) * (S + 1) * D * 8
+        if need > max_bytes:
+            raise ValueError(f"daily_pnl: {need} bytes of per-day rows for {P} individuals x {S} symbols x {D} days exceed "
+                             f"the budget of {max_bytes} bytes")
+        self._evaluate_unique(packed, unique, None, 0)
+        cap = self._exact_cap(self._stats)
+        stats = torch.empty((U, S, _lib.LANE_STATS_WORDS), dtype=torch.float64, device=m.device)
+        lanes = torch.empty((U, S, D), dtype=torch.float64, device=m.device)
+        book = torch.empty((U, D), dtype=torch.float64, device=m.device)
+        indiv = torch.from_numpy(packed.view(np.uint8)).to(m.device).view(U, -1)
+        for lo, hi, c in self._event_slices(packed, unique, cap):
+            with torch.cuda.device(m.device):
+                _lib.call("b200bt_daily_pnl", m.close.data_ptr(), _lib.ld(m.close), S, m.N, indiv[lo:hi].data_ptr(), hi - lo,
+                          C.byref(self.cfg), self._stats.data_ptr(), self._events.data_ptr(), c, lanes[lo:hi].data_ptr(),
+                          D, book[lo:hi].data_ptr(), _lib.current_stream())
+            stats[lo:hi] = self._stats
+        self._keep_slice_stats(stats, expand)
+        if expand is not None:
+            inv = torch.from_numpy(expand).to(m.device)
+            book, lanes = book.index_select(0, inv), lanes.index_select(0, inv)
+        return book, lanes, int(first_day)
 
     def lane_stats(self) -> Dict[str, np.ndarray]:
         """Per-lane metrics of the last evaluation: dict field -> [pop][S] array."""

@@ -513,6 +513,51 @@ int b200bt_trade_mc(const double* trip_pnl, int64_t ld_trip, const int32_t* n_tr
                     int64_t n_paths, uint64_t seed, uint64_t path_offset, float* finals, float* maxdd,
                     b200bt_stream_t stream);
 
+/* ---- backtest overfitting of a population (csrc/overfitting.cu) -------------------------------------
+ * The best of many backtests is biased upward by the search that found it.  These entry points give the inputs and
+ * the core of the two standard measures: the Probability of Backtest Overfitting by combinatorially symmetric
+ * cross-validation (CSCV; Bailey, Borwein, Lopez de Prado, Zhu 2015) and the Deflated Sharpe Ratio (Bailey, Lopez de
+ * Prado 2014). */
+
+/* Per-day PnL rows from a sweep's records: the daily buckets of calculate_metrics (services/strategy_evaluation.py
+ * :141-159) kept as an array instead of folded into Sharpe / Sortino moments.  Inputs as b200bt_book_metrics: price
+ * [S][ld_price], indiv [pop], lane_stats [pop][S], events [pop][S][event_cap] (device), cfg (host; clock checked like the
+ * sweeps').  Records are priced with the expression of b200bt_trade_pnl (an entry record is -position_size * 0.001).
+ * The calendar day of a record on bar b is (minute0 + b * bar_minutes + (b >= gap_bar ? gap_minutes : 0)) / 1440 in
+ * unsigned 32 bits (gap_bar <= 0: no gap); first_day = minute0 / 1440 is the day of bar 0.
+ *   lane_pnl [pop][S][D] float64 (device): [i][s][d] = sum of the pnl of lane (i, s)'s records on day first_day + d, in
+ *            record order within each warp batch of 32 records; a day without records holds exactly 0.0 (the skipped
+ *            days of a glued series are zero columns).  A lane with n_records > event_cap lost records: its row is NaN.
+ *   book_pnl_or_null [pop][D] float64 (device, optional): sum over symbols 0..S-1, in that order, of lane_pnl[i][s][d]
+ *            (NaN when any lane of the individual lost records).
+ * D must cover the series: D >= day(N - 1) - first_day + 1 (B200BT_EINVAL otherwise).  Limits: N < 2^30, pop * S * D
+ * fits int64.  Deterministic: every cell is written by one warp in a fixed order, no atomics. */
+int b200bt_daily_pnl(const float* price, int64_t ld_price, int S, int64_t N, const b200bt_individual* indiv, int pop,
+                     const b200bt_sweep_config* cfg, const b200bt_lane_stats* lane_stats, const uint32_t* events,
+                     int64_t event_cap, double* lane_pnl, int64_t D, double* book_pnl_or_null, b200bt_stream_t stream);
+
+/* CSCV of N trials.  pnl: device float64 [N][ld >= T], one row of T per-period returns per trial (the periods must be
+ * the same for every trial: rows of b200bt_daily_pnl's book_pnl hold every calendar day, zeros included); B even,
+ * 2 <= B <= 20 (ELIMIT above 20), L = T / B >= 2, N >= 2.  The earliest r = T - B*L days are dropped; block b holds the
+ * days [r + b*L, r + (b+1)*L).  Arithmetic (correctly rounded float64, no FMA contraction, sums in ascending order from
+ * +0.0), per trial n over the kept days x_t:
+ *   mu = (sum x_t) / (B*L);  d_t = x_t - mu;  a_b = sum over block b of d_t;  q_b = sum over block b of d_t*d_t
+ *   m2 = (sum d_t*d_t) / (B*L), m3 = (sum (d_t*d_t)*d_t) / (B*L), m4 = (sum (d_t*d_t)*(d_t*d_t)) / (B*L)   (day order)
+ *   sr = mu / sqrt(m2) * sqrt(252) if m2 > 0, else 0
+ * Set J of k = B/2 blocks (ascending): A = sum a_b, Q = sum q_b, n = k*L, m = A/n, v = Q/n - m*m,
+ *   SR_J = (mu + m) / sqrt(v) * sqrt(252) if v > 0, else 0
+ * -- calculate_metrics' daily Sharpe rule, mean / std(ddof 0) * sqrt(252), 0 for std 0 (:180-188), but over every
+ * calendar day of J including days without records, so that all trials share the same rows.
+ * Combination c = 0 .. C(B, B/2) - 1 in itertools.combinations(range(B), B // 2) order: J_c in sample, its complement
+ * out of sample.  Outputs (device): sel[c] = argmax over n of SR_IS (ties to the lowest n), is_sr[c] = SR_IS[sel],
+ * oos_sr[c] = SR_OOS[sel], n_below[c] = #{n : SR_OOS_n < oos_sr[c]}, n_tied[c] = #{n != sel : SR_OOS_n == oos_sr[c]}
+ * (int32 [C]); mu, m2, m3, m4, sr float64 [N].  Rows must be finite.  Deterministic.  Workspace: device, 16-byte aligned,
+ * of b200bt_cscv_workspace_bytes(N, T, B) bytes (0 for arguments outside the limits). */
+int64_t b200bt_cscv_workspace_bytes(int N, int64_t T, int B);
+int b200bt_cscv(const double* pnl, int64_t ld, int N, int64_t T, int B, void* workspace, int64_t workspace_bytes,
+                int32_t* sel, double* is_sr, double* oos_sr, int32_t* n_below, int32_t* n_tied, double* mu, double* m2,
+                double* m3, double* m4, double* sr, b200bt_stream_t stream);
+
 /* ---- portfolio risk (SURVEY 8-f4) -------------------------------------------------------------------
  * Replaces the numeric core of services/portfolio_risk_service.py. */
 
