@@ -4,6 +4,13 @@
 // close = last, volume = sum over each clock-aligned k-minute bucket, like an exchange kline /
 // pandas resample), and a higher-timeframe indicator is brought back to the 1-minute clock by
 // "last COMPLETED higher-timeframe bar" (no look-ahead).
+//
+// Buckets are aligned to the Unix epoch: bucket b covers the minutes [b*k, (b+1)*k) counted from 1970-01-01 00:00 UTC,
+// i.e. pandas' resample(f"{k}min", origin="epoch"), not its default origin="start_day" (the two differ for a k that does
+// not divide 1440).  A base bar starting at minute m belongs to the bucket of m; it completes its bucket when the next
+// bar's start, m + bar_minutes, lies in a later bucket.  minute0 must be >= 0 (the entry points refuse a negative clock:
+// the bucket arithmetic is C's truncating division).  Input is expected free of NaN: open / close take the first / last
+// bar of a bucket and volume sums every bar, where pandas' first / last / sum would skip a NaN.
 #include "common.cuh"
 
 namespace b200bt {
@@ -64,7 +71,7 @@ align_kernel(const float* __restrict__ src, int S, int64_t M, int64_t N, int64_t
 using namespace b200bt;
 
 extern "C" int64_t b200bt_resample_bars(int64_t N, int64_t minute0, int bar_minutes, int k) {
-    if (N <= 0 || bar_minutes <= 0 || k <= 0) return 0;
+    if (N <= 0 || minute0 < 0 || bar_minutes <= 0 || k <= 0) return 0;
     return (minute0 + (N - 1) * (int64_t)bar_minutes) / k - minute0 / k + 1;
 }
 
@@ -73,6 +80,7 @@ extern "C" int b200bt_resample(const float* ohlcv, int S, int64_t N, int64_t min
     B200BT_REQUIRE(ohlcv && out, B200BT_EINVAL, "resample: null pointer");
     B200BT_REQUIRE(S > 0 && N > 0 && bar_minutes > 0 && k >= bar_minutes && k % bar_minutes == 0, B200BT_EINVAL,
                    "resample: k must be a positive multiple of bar_minutes");
+    B200BT_REQUIRE(minute0 >= 0, B200BT_EINVAL, "resample: minute0 must be >= 0");
     B200BT_REQUIRE(M == b200bt_resample_bars(N, minute0, bar_minutes, k), B200BT_EINVAL, "resample: M must be b200bt_resample_bars()");
     int rc = check_device();
     if (rc) return rc;
@@ -85,6 +93,7 @@ extern "C" int b200bt_resample(const float* ohlcv, int S, int64_t N, int64_t min
 extern "C" int b200bt_align(const float* src, int S, int64_t M, int64_t N, int64_t minute0, int bar_minutes, int k,
                             float* out, b200bt_stream_t stream) {
     B200BT_REQUIRE(src && out && S > 0 && M > 0 && N > 0 && bar_minutes > 0 && k > 0, B200BT_EINVAL, "align: bad argument");
+    B200BT_REQUIRE(minute0 >= 0, B200BT_EINVAL, "align: minute0 must be >= 0");
     int rc = check_device();
     if (rc) return rc;
     dim3 grid((unsigned)((N + 255) / 256), (unsigned)S);

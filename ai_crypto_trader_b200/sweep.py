@@ -111,8 +111,9 @@ class MarketData:
         return cls(ohlcv, symbols=symbols, minute0=minute0, bar_minutes=bar_minutes, device=close.device)
 
     def materialise(self) -> "MarketData":
-        """Make all five fields device-resident now."""
+        """Make all five fields device-resident now (ordered before later work on the current stream)."""
         self._wait_others()
+        self._join_close()
         return self
 
     def _wait_others(self) -> None:
@@ -126,7 +127,9 @@ class MarketData:
 
     @property
     def ohlcv(self) -> torch.Tensor:
+        # all five rows, close included: a reader of the whole array (resample) must not overtake the close copies
         self._wait_others()
+        self._join_close()
         return self._ohlcv
 
     def _join_close(self) -> None:
@@ -720,7 +723,10 @@ class PopulationSweep:
 
     def set_gap(self, gap_bar: int, gap_minutes: int) -> None:
         """Declare the series as two pieces glued at `gap_bar`, the second one `gap_minutes` later on the calendar
-        (training folds of cross_validate_strategy): only the daily buckets of the metrics see it."""
+        (training folds of cross_validate_strategy): only the daily buckets of the metrics see it.  A gap is refused on a
+        multi-timeframe sweep: its derived clocks were bucketed on the unbroken clock minute0 + t * bar_minutes."""
+        if len(self.timeframes) > 1 and int(gap_minutes) != 0:
+            raise ValueError("set_gap: a multi-timeframe bank is bucketed on the unbroken clock and cannot see a gap")
         self.cfg.gap_bar, self.cfg.gap_minutes = int(gap_bar), int(gap_minutes)
 
     def zone_map(self) -> torch.Tensor:

@@ -129,7 +129,8 @@ int b200bt_vwap(const float* high, const float* low, const float* close, const f
  * each timeframe is its own kline series, :168-171).  b200bt_resample derives clock-aligned k-minute
  * OHLCV [5][S][M] from 1-minute (or bar_minutes) OHLCV [5][S][N]; M = b200bt_resample_bars(...).
  * b200bt_align maps a higher-timeframe series [S][M] back onto the base clock [S][N] using the last
- * COMPLETED higher-timeframe bar (NaN before the first one). */
+ * COMPLETED higher-timeframe bar (NaN before the first one).  Buckets are aligned to the Unix epoch (pandas'
+ * origin="epoch").  minute0 < 0 is refused: EINVAL from both, and b200bt_resample_bars returns 0. */
 int64_t b200bt_resample_bars(int64_t N, int64_t minute0, int bar_minutes, int k);
 int b200bt_resample(const float* ohlcv, int S, int64_t N, int64_t minute0, int bar_minutes, int k,
                     float* out, int64_t M, b200bt_stream_t stream);

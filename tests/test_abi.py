@@ -109,3 +109,21 @@ def test_sweep_entry_points_reject_an_out_of_range_calendar(native_lib, case, mi
             _lib.call(name, *args)
         assert ei.value.status == status, (case, name, str(ei.value))
         assert "minute0" in str(ei.value) or "bar_minutes" in str(ei.value), (case, name, str(ei.value))
+
+
+@pytest.mark.parametrize("minute0", [-1, -1439, -(1 << 40)])
+def test_resample_and_align_reject_a_negative_clock(native_lib, minute0):
+    """The derived clocks bucket minute0 + t * bar_minutes with truncating division, which floors only from 0 up: a negative
+    minute0 would start the first bucket on the wrong minute.  Both entry points refuse it (checked before the device is
+    touched; the dummy pointers are never read) and b200bt_resample_bars reports no bars."""
+    from ai_crypto_trader_b200 import _lib
+    lib = _lib.load()
+    N, bar, k, dev = 1000, 5, 15, 1 << 20
+    assert lib.b200bt_resample_bars(N, minute0, bar, k) == 0
+    assert lib.b200bt_resample_bars(N, 0, bar, k) == (N * bar + k - 1) // k
+    M = int(lib.b200bt_resample_bars(N, 0, bar, k))
+    for name, args in (("b200bt_resample", (dev, 2, N, minute0, bar, k, dev, M, None)),
+                       ("b200bt_align", (dev, 2, M, N, minute0, bar, k, dev, None))):
+        with pytest.raises(_lib.B200btError) as ei:
+            _lib.call(name, *args)
+        assert ei.value.status == _EINVAL and "minute0" in str(ei.value), (name, str(ei.value))
