@@ -65,100 +65,19 @@ sweep_kernel(const float* __restrict__ price, int64_t ld_price,
     const long long minute0 = cfg.minute0;
     const int bar_minutes = cfg.bar_minutes;
 
-    Machine m;
-    m.pos = 0; m.e = 0.f;
-    m.rlo = iv.rsi_lo; m.rhi = iv.rsi_hi; m.plo = -INFINITY; m.phi = INFINITY;
-    m.qhead = 0; m.entry_bar = 0;
-    const ScanConst c = ws->sc;                // warp-uniform constants of the scan, kept in registers
-    unsigned qtail = 0;
-
-    // Streams are staged through a per-warp shared-memory ring filled with cp.async
-    // (16 B per thread = 128 bars per instruction when the rows are 16-byte aligned):
-    // SW_STAGES-1 groups are always in flight, no registers are tied up by prefetch.
-    constexpr int G = SW_GROUP;               // bars per group
-    float* const sp = &ws->ring[0][0][0];
+    // the whole series, group by group through the warp's cp.async ring
     const int n = (int)N;
-    const int n_full = n / G;                 // groups copied without bounds checks
-    const int n_groups = (n + G - 1) / G;
-    // running producer state: next group to issue, its ring slot, its source pointers
-    int issued = 0;
-    float* idst = sp + (VEC16 ? lane * 4 : lane);
-    const float* ip = pr + (VEC16 ? lane * 4 : lane);
-    const float* ir = rr + (VEC16 ? lane * 4 : lane);
-    auto issue = [&]() {
-        if (issued < n_full) {
-            if (VEC16) {
-#pragma unroll
-                for (int i = 0; i < G / 128; ++i) {
-                    cp_async16(idst + i * 128, ip + i * 128);
-                    cp_async16(idst + G + i * 128, ir + i * 128);
-                }
-            } else {
-#pragma unroll
-                for (int i = 0; i < G / 32; ++i) {
-                    cp_async4(idst + i * 32, ip + i * 32);
-                    cp_async4(idst + G + i * 32, ir + i * 32);
-                }
-            }
-        } else if (issued < n_groups) {
-            // ragged last group: guarded loads, NaN beyond the series (NaN never fires an event)
-            const float qnan = __int_as_float(0x7fc00000);
-            float* dst = sp + (issued % SW_STAGES) * (2 * G);
-            for (int i = lane; i < G; i += 32) {
-                const int t = issued * G + i;
-                dst[i] = t < n ? __ldg(pr + t) : qnan;
-                dst[G + i] = t < n ? __ldg(rr + t) : qnan;
-            }
-        }
-        cp_async_commit();  // always commit (possibly empty) so the group accounting stays uniform
-        ++issued;
-        ip += G; ir += G;
-        idst = (issued % SW_STAGES == 0) ? idst - (SW_STAGES - 1) * (2 * G) : idst + 2 * G;
-    };
-#pragma unroll
-    for (int g = 0; g < SW_STAGES - 1; ++g) issue();
-    const float* cur = sp + lane;
-    int cstage = 0;
+    const int n_groups = (n + SW_GROUP - 1) / SW_GROUP;
+    GroupRing<VEC16> ring(ws, pr, rr, n, 0, n_groups);
+    const ScanConst c = ws->sc;                // warp-uniform constants of the scan, kept in registers
+    Machine m = flat_machine(iv);
+    unsigned qtail = 0;
+    auto batch = [&](unsigned at, int cnt) { process_batch(ws, at, cnt, minute0, bar_minutes, ev_cap); };
     for (int g = 0; g < n_groups; ++g) {
-        issue();
-        cp_async_wait<SW_STAGES - 1>();       // group g has landed
-        __syncwarp();
-        const float* w = cur;
-        int t0 = g * G;
-#pragma unroll 1
-        for (int v = 0; v < G / 64; ++v, w += 64, t0 += 64) {
-            // two windows per step: both ballots are issued before either is needed
-            const float p0 = w[0], r0 = w[G];
-            const float p1 = w[32], r1 = w[G + 32];
-            const unsigned h0 = __ballot_sync(FULL, fires(m, p0, r0));
-            const unsigned h1 = __ballot_sync(FULL, fires(m, p1, r1));
-            if (h0 | h1) {
-                if (h0) scan_window(p0, r0, w - lane, t0, ws, c, m);
-                scan_window(p1, r1, w - lane + 32, t0 + 32, ws, c, m);
-                while (m.qhead - qtail >= 32) {
-                    __syncwarp();
-                    process_batch(ws, qtail, 32, minute0, bar_minutes, ev_cap);
-                    qtail += 32;
-                }
-            }
-        }
-        __syncwarp();                         // stage is refilled by the next iteration's issue
-        if (++cstage == SW_STAGES) { cstage = 0; cur -= (SW_STAGES - 1) * (2 * G); } else cur += 2 * G;
+        scan_group(ring.land(), g * SW_GROUP, ws, c, m, qtail, true, batch);
+        ring.release();
     }
-    cp_async_wait<0>();
-    if (m.pos != 0) {
-        // force-close at the last bar (:849-876)
-        const float pl = __ldg(pr + (N - 1));
-        const unsigned word = (unsigned)(N - 1) | B200BT_EVENT_EXIT | (m.pos > 0 ? B200BT_EVENT_SELL : 0u);
-        if (lane == 0) ws->evq[m.qhead & (SW_EVQ - 1)] = make_uint2(word, __float_as_uint(pl));
-        ++m.qhead;
-    }
-    __syncwarp();
-    while (m.qhead != qtail) {
-        const int cnt = min(32u, m.qhead - qtail);
-        process_batch(ws, qtail, cnt, minute0, bar_minutes, ev_cap);
-        qtail += cnt;
-    }
+    finish_scan(ws, m, qtail, pr, N, true, batch);
 
     if (lane == 0) {
         b200bt_lane_stats o;
@@ -190,6 +109,22 @@ int check_sweep_clock(const char* who, const b200bt_sweep_config* cfg, int64_t N
     return B200BT_OK;
 }
 
+int check_sweep_args(const char* who, const float* price, int64_t ld_price, const float* rsi, int64_t ld_rsi, int P, int S,
+                     int64_t N, const b200bt_sweep_config* cfg_host, const uint32_t* events, int64_t event_cap) {
+    B200BT_REQUIRE(price && rsi && cfg_host, B200BT_EINVAL, "%s: null pointer", who);
+    B200BT_REQUIRE(S > 0 && N > 0 && P > 0, B200BT_EINVAL, "%s: bad sizes", who);
+    B200BT_REQUIRE(ld_price >= N && ld_rsi >= N, B200BT_EINVAL, "%s: row stride shorter than N", who);
+    B200BT_REQUIRE(N < (1ll << 30), B200BT_ELIMIT, "%s: N must be < 2^30 bars", who);
+    const int rc = check_sweep_clock(who, cfg_host, N);
+    if (rc) return rc;
+    B200BT_REQUIRE(events == nullptr || event_cap > 0, B200BT_EINVAL, "%s: event buffer without capacity", who);
+    return B200BT_OK;
+}
+
+bool vec16_rows(const float* price, int64_t ld_price, const float* rsi, int64_t ld_rsi) {
+    return (((uintptr_t)price | (uintptr_t)rsi) & 15) == 0 && ld_price % 4 == 0 && ld_rsi % 4 == 0;
+}
+
 // The fused sweep over the first *pop_dev (<= pop) entries of `order`: the grid covers `pop` entries and warps beyond the
 // device-side count leave at once.  The exact fallback of the time-chunked sweeps: the list of individuals to re-run and its
 // length never leave the device.
@@ -199,13 +134,10 @@ int launch_sweep(const float* price, int64_t ld_price, const float* rsi, int64_t
                  cudaStream_t stream) {
     const int64_t blocks = (int64_t)((pop + SW_WARPS - 1) / SW_WARPS) * S;
     B200BT_REQUIRE(blocks < (1ll << 31), B200BT_ELIMIT, "sweep: too many lanes");
-    const size_t smem = sizeof(WarpShared) * SW_WARPS;
-    // 16-byte cp.async needs every (symbol, period) row to start on a 16-byte boundary
-    const bool vec16 = (((uintptr_t)price | (uintptr_t)rsi) & 15) == 0 && ld_price % 4 == 0 && ld_rsi % 4 == 0;
-    auto kern = vec16 ? sweep_kernel<true> : sweep_kernel<false>;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return cuda_status(e, "sweep: cudaFuncSetAttribute");
-    kern<<<(unsigned)blocks, SW_WARPS * 32, smem, stream>>>(
+    auto kern = vec16_rows(price, ld_price, rsi, ld_rsi) ? sweep_kernel<true> : sweep_kernel<false>;
+    const int rc = allow_sw_smem(kern, "sweep: cudaFuncSetAttribute");
+    if (rc) return rc;
+    kern<<<(unsigned)blocks, SW_WARPS * 32, SW_SMEM, stream>>>(
         price, ld_price, rsi, ld_rsi, P, S, N, indiv, order, pop, pop_dev, *cfg_host, stats, events, event_cap);
     B200BT_LAUNCH_CHECK("sweep launch");
     return B200BT_OK;
@@ -216,13 +148,10 @@ extern "C" int b200bt_sweep(const float* price, int64_t ld_price, const float* r
                             int S, int64_t N, const b200bt_individual* indiv, const int32_t* order, int pop,
                             const b200bt_sweep_config* cfg_host, b200bt_lane_stats* stats,
                             uint32_t* events, int64_t event_cap, b200bt_stream_t stream) {
-    B200BT_REQUIRE(price && rsi && indiv && cfg_host && stats, B200BT_EINVAL, "sweep: null pointer");
-    B200BT_REQUIRE(S > 0 && N > 0 && P > 0 && pop > 0, B200BT_EINVAL, "sweep: bad sizes");
-    B200BT_REQUIRE(ld_price >= N && ld_rsi >= N, B200BT_EINVAL, "sweep: row stride shorter than N");
-    B200BT_REQUIRE(N < (1ll << 30), B200BT_ELIMIT, "sweep: N must be < 2^30 bars");
-    int rc = check_sweep_clock("sweep", cfg_host, N);
+    B200BT_REQUIRE(indiv && stats, B200BT_EINVAL, "sweep: null pointer");
+    B200BT_REQUIRE(pop > 0, B200BT_EINVAL, "sweep: bad sizes");
+    int rc = check_sweep_args("sweep", price, ld_price, rsi, ld_rsi, P, S, N, cfg_host, events, event_cap);
     if (rc) return rc;
-    B200BT_REQUIRE(events == nullptr || event_cap > 0, B200BT_EINVAL, "sweep: event buffer without capacity");
     rc = check_device();
     if (rc) return rc;
     return launch_sweep(price, ld_price, rsi, ld_rsi, P, S, N, indiv, order, pop, nullptr, cfg_host, stats, events, event_cap,

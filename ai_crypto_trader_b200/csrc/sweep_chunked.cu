@@ -123,25 +123,12 @@ __device__ __forceinline__ bool chunk_scan_item(const ChunkScanArgs& A, const b2
     s0 &= ~(SW_GROUP - 1);
     const int seg = sym * A.n_seg + item.segment;
 
-    Machine m;
-    m.pos = 0; m.e = 0.f; m.entry_bar = 0;
-    m.rlo = iv.rsi_lo; m.rhi = iv.rsi_hi; m.plo = -INFINITY; m.phi = INFINITY;
-    m.qhead = 0;
+    Machine m = flat_machine(iv);
     unsigned qtail = 0;
     if (REPAIR) {
         // true state at T0 = end state of the preceding chunk (position side, entry bar -> entry price)
         const int2 z = A.seg_out[seg - 1];
-        if (z.x != 0) {
-            const float e = __ldg(pr + z.y);
-            m.pos = z.x; m.e = e; m.entry_bar = z.y;
-            if (z.x > 0) {
-                m.rlo = -INFINITY; m.rhi = c.ob_f;
-                m.phi = e * c.hiL_c; m.plo = e * c.loL_c;
-            } else {
-                m.rlo = c.os_f; m.rhi = INFINITY;
-                m.phi = e * c.hiS_c; m.plo = e * c.loS_c;
-            }
-        }
+        if (z.x != 0) set_open(m, c, z.x > 0, __ldg(pr + z.y), z.y);
     }
 
     // REPAIR: the chain the speculative scan recorded for this chunk and the state it assumed at T0.  Two trajectories that
@@ -161,7 +148,7 @@ __device__ __forceinline__ bool chunk_scan_item(const ChunkScanArgs& A, const b2
 
     // event sink: 32 queued events -> one coalesced 256-byte store into the chunk's current pool block
     int cur_block = -1, fill = CK_BLOCK, dead = 0;
-    auto flush = [&](int cnt) {
+    auto flush = [&](unsigned at, int cnt) {
         if (fill == CK_BLOCK && !dead) {
             int b = cur_block;
             if (lane == 0 && !pool_take_block(A, seg, b)) b = -1;
@@ -169,57 +156,16 @@ __device__ __forceinline__ bool chunk_scan_item(const ChunkScanArgs& A, const b2
             if (b < 0) dead = 1; else { cur_block = b; fill = 0; }
         }
         if (!dead) {
-            if (lane < cnt) A.pool[(int64_t)cur_block * CK_BLOCK + fill + lane] = ws->evq[(qtail + lane) & (SW_EVQ - 1)];
+            if (lane < cnt) A.pool[(int64_t)cur_block * CK_BLOCK + fill + lane] = ws->evq[(at + lane) & (SW_EVQ - 1)];
             fill += 32;   // only the last flush of a chunk is partial
         }
-        qtail += cnt;
     };
 
     constexpr int G = SW_GROUP;
-    float* const sp = &ws->ring[0][0][0];
-    const int n_full = n / G;
     const int g_begin = s0 / G, g_end = (T1 + G - 1) / G;
-    int issued = g_begin;
-    float* idst = sp + (g_begin % SW_STAGES) * (2 * G) + (VEC16 ? lane * 4 : lane);
-    const float* ip = pr + (int64_t)g_begin * G + (VEC16 ? lane * 4 : lane);
-    const float* ir = rr + (int64_t)g_begin * G + (VEC16 ? lane * 4 : lane);
-    auto issue = [&]() {
-        if (issued < n_full && issued < g_end) {
-            if (VEC16) {
-#pragma unroll
-                for (int i = 0; i < G / 128; ++i) {
-                    cp_async16(idst + i * 128, ip + i * 128);
-                    cp_async16(idst + G + i * 128, ir + i * 128);
-                }
-            } else {
-#pragma unroll
-                for (int i = 0; i < G / 32; ++i) {
-                    cp_async4(idst + i * 32, ip + i * 32);
-                    cp_async4(idst + G + i * 32, ir + i * 32);
-                }
-            }
-        } else if (issued < g_end) {
-            const float qnan = __int_as_float(0x7fc00000);   // ragged last group of the series
-            float* dst = sp + (issued % SW_STAGES) * (2 * G);
-            for (int i = lane; i < G; i += 32) {
-                const int t = issued * G + i;
-                dst[i] = t < n ? __ldg(pr + t) : qnan;
-                dst[G + i] = t < n ? __ldg(rr + t) : qnan;
-            }
-        }
-        cp_async_commit();
-        ++issued;
-        ip += G; ir += G;
-        idst = (issued % SW_STAGES == 0) ? idst - (SW_STAGES - 1) * (2 * G) : idst + 2 * G;
-    };
-#pragma unroll
-    for (int g = 0; g < SW_STAGES - 1; ++g) issue();
-    int cstage = g_begin % SW_STAGES;
-    const float* cur = sp + cstage * (2 * G) + lane;
+    GroupRing<VEC16> ring(ws, pr, rr, n, g_begin, g_end);
     for (int g = g_begin; g < g_end; ++g) {
-        issue();
-        cp_async_wait<SW_STAGES - 1>();
-        __syncwarp();
+        const float* w = ring.land();
         const bool emit = g * G >= T0;
         if (g * G == T0 && lane == 0) A.seg_in[seg] = make_int2(m.pos, m.pos != 0 ? m.entry_bar : -1);
         if (REPAIR && old_ok && g > g_begin) {
@@ -248,48 +194,24 @@ __device__ __forceinline__ bool chunk_scan_item(const ChunkScanArgs& A, const b2
                     old_idx += n_here; old_left -= (unsigned)n_here;
                     if (old_idx == CK_BLOCK && old_left) { old_block = A.next[old_block]; old_idx = 0; }
                     __syncwarp();
-                    while (m.qhead - qtail >= 32) flush(32);
+                    // (inline rather than drain_full: the splice synchronises once per copied block, and drain_full's
+                    // __syncwarp per batch makes the repair kernels' code larger)
+                    while (m.qhead - qtail >= 32) { flush(qtail, 32); qtail += 32; }
                     __syncwarp();
                 }
                 spliced = true;
                 break;
             }
         }
-        const float* w = cur;
-        int t0 = g * G;
-#pragma unroll 1
-        for (int v = 0; v < G / 64; ++v, w += 64, t0 += 64) {
-            const float p0 = w[0], r0 = w[G];
-            const float p1 = w[32], r1 = w[G + 32];
-            const unsigned h0 = __ballot_sync(FULL, fires(m, p0, r0));
-            const unsigned h1 = __ballot_sync(FULL, fires(m, p1, r1));
-            if (h0 | h1) {
-                if (h0) scan_window(p0, r0, w - lane, t0, ws, c, m, emit);
-                scan_window(p1, r1, w - lane + 32, t0 + 32, ws, c, m, emit);
-                while (m.qhead - qtail >= 32) {
-                    __syncwarp();
-                    flush(32);
-                }
-            }
-        }
-        __syncwarp();
-        if (++cstage == SW_STAGES) { cstage = 0; cur -= (SW_STAGES - 1) * (2 * G); } else cur += 2 * G;
+        scan_group(w, g * G, ws, c, m, qtail, emit, flush);
+        ring.release();
     }
-    cp_async_wait<0>();
     if (lane == 0 && !spliced) {
         const int2 st = make_int2(m.pos, m.pos != 0 ? m.entry_bar : -1);
         A.seg_out[seg] = st;
         if (T0 >= T1) A.seg_in[seg] = st;   // empty chunk: its assumed state is the state after the warm-up
     }
-    if (!spliced && item.chunk == item.n_chunks - 1 && m.pos != 0) {
-        // force-close at the last bar (:849-876)
-        const float pl = __ldg(pr + (A.N - 1));
-        const unsigned word = (unsigned)(A.N - 1) | B200BT_EVENT_EXIT | (m.pos > 0 ? B200BT_EVENT_SELL : 0u);
-        if (lane == 0) ws->evq[m.qhead & (SW_EVQ - 1)] = make_uint2(word, __float_as_uint(pl));
-        ++m.qhead;
-    }
-    __syncwarp();
-    while (m.qhead != qtail) flush((int)min(32u, m.qhead - qtail));
+    finish_scan(ws, m, qtail, pr, A.N, !spliced && item.chunk == item.n_chunks - 1, flush);
     if (lane == 0) A.seg_count[seg] = dead ? SEG_LOST : m.qhead;
     __syncwarp();
     return spliced;      // REPAIR: the chunk's recorded end state stands
@@ -1299,11 +1221,6 @@ ChunkWorkspace carve(void* workspace, const ChunkLayout& L, int pool_blocks) {
     return w;
 }
 
-// price and RSI rows that allow 16-byte copies
-bool vec16_rows(const float* price, int64_t ld_price, const float* rsi, int64_t ld_rsi) {
-    return (((uintptr_t)price | (uintptr_t)rsi) & 15) == 0 && ld_price % 4 == 0 && ld_rsi % 4 == 0;
-}
-
 // arguments of the warp-per-chunk scan and of the repair and metrics kernels both schedules share
 ChunkScanArgs scan_args(const float* price, int64_t ld_price, const float* rsi, int64_t ld_rsi, int P, int S, int64_t N,
                         const b200bt_individual* indiv, const b200bt_chunk_item* items, int n_items, int n_seg,
@@ -1351,10 +1268,9 @@ int finish_chunks(const ChunkScanArgs& A, const ChunkWorkspace& w, const bool ve
     const b200bt_chunk_item* const items = A.items;
     auto kern_fix = vec16 ? chunk_repair_kernel<true> : chunk_repair_kernel<false>;
     auto kern_walk = vec16 ? lane_repair_kernel<true> : lane_repair_kernel<false>;
-    const size_t smem = sizeof(WarpShared) * SW_WARPS;
-    cudaError_t e = cudaFuncSetAttribute(kern_fix, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(kern_walk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return cuda_status(e, "sweep_chunked: cudaFuncSetAttribute");
+    int rc = allow_sw_smem(kern_fix, "sweep_chunked: cudaFuncSetAttribute");
+    if (!rc) rc = allow_sw_smem(kern_walk, "sweep_chunked: cudaFuncSetAttribute");
+    if (rc) return rc;
     const int64_t lanes = (int64_t)pop * S;
     const int64_t mblocks = (int64_t)((n_items + 3) / 4) * S;
     B200BT_REQUIRE(mblocks < (1ll << 31), B200BT_ELIMIT, "sweep_chunked: too many work items");
@@ -1365,8 +1281,8 @@ int finish_chunks(const ChunkScanArgs& A, const ChunkWorkspace& w, const bool ve
     auto repair_pass = [&](cudaStream_t rs, int pass, unsigned char* redo) -> int {
         ChunkScanArgs R = A;
         R.redo = redo;
-        if (pass == 0) kern_fix<<<repair_grid, SW_WARPS * 32, smem, rs>>>(R, &w.ctr->chunk_repair_work);
-        else kern_walk<<<repair_grid, SW_WARPS * 32, smem, rs>>>(R, pop, seg_base, &w.ctr->lane_repair_work);
+        if (pass == 0) kern_fix<<<repair_grid, SW_WARPS * 32, SW_SMEM, rs>>>(R, &w.ctr->chunk_repair_work);
+        else kern_walk<<<repair_grid, SW_WARPS * 32, SW_SMEM, rs>>>(R, pop, seg_base, &w.ctr->lane_repair_work);
         B200BT_LAUNCH_CHECK("repair launch");
         return B200BT_OK;
     };
@@ -1379,7 +1295,7 @@ int finish_chunks(const ChunkScanArgs& A, const ChunkWorkspace& w, const bool ve
         return B200BT_OK;
     };
 
-    int rc = B200BT_OK;
+    cudaError_t e;
     const bool tail = max_repair_rounds >= 2;
     if (max_repair_rounds >= 1 && (rc = repair_pass(st, 0, nullptr))) return rc;
     SideStream* side = nullptr;
@@ -1436,18 +1352,6 @@ int finish_chunks(const ChunkScanArgs& A, const ChunkWorkspace& w, const bool ve
     return B200BT_OK;
 }
 
-int check_sweep_args(const char* who, const float* price, int64_t ld_price, const float* rsi, int64_t ld_rsi, int P, int S,
-                     int64_t N, const b200bt_sweep_config* cfg_host, const uint32_t* events, int64_t event_cap) {
-    B200BT_REQUIRE(price && rsi && cfg_host, B200BT_EINVAL, "%s: null pointer", who);
-    B200BT_REQUIRE(S > 0 && N > 0 && P > 0, B200BT_EINVAL, "%s: bad sizes", who);
-    B200BT_REQUIRE(ld_price >= N && ld_rsi >= N, B200BT_EINVAL, "%s: row stride shorter than N", who);
-    B200BT_REQUIRE(N < (1ll << 30), B200BT_ELIMIT, "%s: N must be < 2^30 bars", who);
-    const int rc = check_sweep_clock(who, cfg_host, N);
-    if (rc) return rc;
-    B200BT_REQUIRE(events == nullptr || event_cap > 0, B200BT_EINVAL, "%s: event buffer without capacity", who);
-    return B200BT_OK;
-}
-
 }  // namespace
 
 extern "C" int64_t b200bt_sweep_chunked_workspace_bytes(int pool_blocks, int S, int n_seg) {
@@ -1482,12 +1386,10 @@ extern "C" int b200bt_sweep_chunked(const float* price, int64_t ld_price, const 
     const ChunkScanArgs A = scan_args(price, ld_price, rsi, ld_rsi, P, S, N, indiv, items, n_items, n_seg, n_chunks, warm, w);
     const bool vec16 = vec16_rows(price, ld_price, rsi, ld_rsi);
     auto kern = vec16 ? chunk_scan_kernel<true> : chunk_scan_kernel<false>;
-    const size_t smem = sizeof(WarpShared) * SW_WARPS;
-    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return cuda_status(e, "sweep_chunked: cudaFuncSetAttribute");
+    if ((rc = allow_sw_smem(kern, "sweep_chunked: cudaFuncSetAttribute"))) return rc;
     const int64_t blocks = (int64_t)((n_items + SW_WARPS - 1) / SW_WARPS) * S;
     B200BT_REQUIRE(blocks < (1ll << 31), B200BT_ELIMIT, "sweep_chunked: too many work items");
-    kern<<<(unsigned)blocks, SW_WARPS * 32, smem, st>>>(A);
+    kern<<<(unsigned)blocks, SW_WARPS * 32, SW_SMEM, st>>>(A);
     B200BT_LAUNCH_CHECK("chunk_scan launch");
     return finish_chunks(A, w, vec16, seg_base, pop, max_repair_rounds, cfg_host, stats, events, event_cap, lane_invalid,
                          overflow_host_or_null, st);

@@ -1,6 +1,8 @@
-// Device code shared by the fused population sweep (sweep.cu) and the time-chunked sweep
-// (sweep_chunked.cu): per-warp shared-memory working set, the bar scan, the event-batch
-// arithmetic (calculate_metrics) and the score epilogue.
+// Code shared by the fused population sweep (sweep.cu) and the time-chunked sweep
+// (sweep_chunked.cu): the per-warp shared-memory working set; the warp-per-lane bar scan that
+// sweep_kernel and the warp-per-chunk scan / repair kernels run (machine, cp.async group ring,
+// group step, force-close); the event-batch arithmetic (calculate_metrics) and the score epilogue;
+// the host-side argument checks and launch set-up of the warp-per-lane kernels.
 #pragma once
 #include <math.h>
 #include "common.cuh"
@@ -17,6 +19,14 @@ int launch_sweep(const float* price, int64_t ld_price, const float* rsi, int64_t
 // a negative field (minute0, gap_minutes) or bar_minutes <= 0 is B200BT_EINVAL; minute0 + N * bar_minutes + gap_minutes
 // >= 2^32 - 1440 is B200BT_ELIMIT, so that every minute the kernels form fits their unsigned 32-bit arithmetic.
 int check_sweep_clock(const char* who, const b200bt_sweep_config* cfg, int64_t N);
+
+// The arguments all three sweep entry points take alike: price / RSI rows and their strides, P, S, N (< 2^30), the calendar
+// clock (check_sweep_clock) and the optional event buffer.  B200BT_OK, or the first failing check's status.
+int check_sweep_args(const char* who, const float* price, int64_t ld_price, const float* rsi, int64_t ld_rsi, int P, int S,
+                     int64_t N, const b200bt_sweep_config* cfg_host, const uint32_t* events, int64_t event_cap);
+
+// price and RSI rows that allow 16-byte copies: every (symbol, period) row starts on a 16-byte boundary
+bool vec16_rows(const float* price, int64_t ld_price, const float* rsi, int64_t ld_rsi);
 
 constexpr int SW_WARPS = 8;         // warps (lanes of the sweep) per CTA
 #ifndef B200BT_SW_MIN_BLOCKS
@@ -72,6 +82,14 @@ struct __align__(16) WarpShared {
     WarpAcc acc;
     ScanConst sc;
 };
+
+// Dynamic shared memory of a warp-per-lane kernel (sweep_kernel, chunk_scan_kernel, chunk_repair_kernel,
+// lane_repair_kernel): one WarpShared per warp.
+constexpr size_t SW_SMEM = sizeof(WarpShared) * SW_WARPS;
+template <class Kernel>
+int allow_sw_smem(Kernel kern, const char* what) {
+    return cuda_status(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SW_SMEM), what);
+}
 
 struct DayAcc {
     double pivot, s1, s2;
@@ -469,6 +487,34 @@ __device__ __forceinline__ bool fires(const Machine& m, float p, float r) {
     return (r < m.rlo) | (r > m.rhi) | (p <= m.plo) | (p >= m.phi);
 }
 
+// Flat: only an entry signal (RSI below the oversold threshold os or above the overbought one ob) fires.
+__device__ __forceinline__ void set_flat(Machine& m, float os, float ob) {
+    m.pos = 0;
+    m.rlo = os; m.rhi = ob;
+    m.plo = -INFINITY; m.phi = INFINITY;
+}
+
+// The machine at the start of a scan: flat, nothing queued.
+__device__ __forceinline__ Machine flat_machine(const b200bt_individual& iv) {
+    Machine m;
+    set_flat(m, iv.rsi_lo, iv.rsi_hi);
+    m.e = 0.f; m.entry_bar = 0;
+    m.qhead = 0;
+    return m;
+}
+
+// Open a position (strategy_evaluation.py:784-813): long (`lng`) or short, entered at price e on `bar`; the exit
+// thresholds are an RSI reversal and the fp32 candidate bounds of take-profit / stop-loss around e.
+__device__ __forceinline__ void set_open(Machine& m, const ScanConst& c, bool lng, float e, int bar) {
+    m.e = e;
+    m.entry_bar = bar;
+    m.pos = lng ? 1 : -1;
+    m.rlo = lng ? -INFINITY : c.os_f;
+    m.rhi = lng ? c.ob_f : INFINITY;
+    m.phi = e * (lng ? c.hiL_c : c.hiS_c);
+    m.plo = e * (lng ? c.loL_c : c.loS_c);
+}
+
 // Advance the machine through every event of one 32-bar window (lane l holds bar t0+l).
 // `emit` = false runs the machine without recording events (warm-up bars of a time chunk).
 // `win` points at the window's 32 prices in the shared-memory ring (RSI values SW_GROUP floats further):
@@ -488,15 +534,9 @@ __device__ __forceinline__ void scan_window(const float p, const float r, const 
         unsigned word;
         bool ev = true;
         if (m.pos == 0) {
-            // entry (strategy_evaluation.py:784-813): long has priority over short
+            // entry: long has priority over short
             const bool lng = rk < c.os_f;
-            m.e = pk;
-            m.entry_bar = (int)bar;
-            m.pos = lng ? 1 : -1;
-            m.rlo = lng ? -INFINITY : c.os_f;
-            m.rhi = lng ? c.ob_f : INFINITY;
-            m.phi = pk * (lng ? c.hiL_c : c.hiS_c);
-            m.plo = pk * (lng ? c.loL_c : c.loS_c);
+            set_open(m, c, lng, pk, (int)bar);
             word = lng ? bar : (bar | B200BT_EVENT_SELL);
         } else {
             // exit candidate (:815-847); an RSI reversal is always definite, a price trigger inside the
@@ -512,9 +552,7 @@ __device__ __forceinline__ void scan_window(const float p, const float r, const 
             }
             if (ev) {
                 word = bar | B200BT_EVENT_EXIT | (m.pos > 0 ? B200BT_EVENT_SELL : 0u);
-                m.pos = 0;
-                m.rlo = c.os_f; m.rhi = c.ob_f;
-                m.plo = -INFINITY; m.phi = INFINITY;
+                set_flat(m, c.os_f, c.ob_f);
             }
         }
         if (ev) {
@@ -523,6 +561,137 @@ __device__ __forceinline__ void scan_window(const float p, const float r, const 
             ws->evq[m.qhead & (SW_EVQ - 1)] = make_uint2(word, __float_as_uint(pk));
             m.qhead += emit ? 1u : 0u;
         }
+    }
+}
+
+// The per-warp cp.async ring of the bar scan: streams groups [g_begin, g_end) of SW_GROUP bars of one (price, RSI) row
+// pair through WarpShared::ring, SW_STAGES - 1 groups ahead of the scan, with no registers tied up by prefetch.  Full
+// groups are copied 16 B per thread (128 bars per instruction) when the rows start on 16-byte boundaries (VEC16), 4 B per
+// thread otherwise; the ragged last group of the series is loaded with guards and padded with NaN (NaN never fires an
+// event).  land() issues one more group and returns the oldest one in flight once it has landed; release() hands its
+// stage back to be refilled.  Only the producer's running position is kept (the rows themselves are reached through it),
+// which keeps the state that lives across the scan loop small.
+template <bool VEC16>
+struct GroupRing {
+    static constexpr int G = SW_GROUP;
+    float* sp;                           // the warp's ring
+    int n, n_full, g_end;                // bars, groups copied without bounds checks, end of the range
+    int issued;                          // producer: next group to issue, its ring slot and sources (this lane's part)
+    float* idst;
+    const float* ip; const float* ir;
+    int cstage;                          // consumer: stage of the next group to land, this lane's first bar of it
+    const float* cur;
+
+    // pr, rr: the price and RSI rows from bar 0
+    __device__ __forceinline__ GroupRing(WarpShared* ws, const float* pr, const float* rr, int n_, int g_begin, int g_end_)
+        : sp(&ws->ring[0][0][0]), n(n_), n_full(n_ / G), g_end(g_end_), issued(g_begin) {
+        const int lane = threadIdx.x & 31, off = VEC16 ? lane * 4 : lane;
+        idst = sp + (g_begin % SW_STAGES) * (2 * G) + off;
+        ip = pr + (int64_t)g_begin * G + off;
+        ir = rr + (int64_t)g_begin * G + off;
+#pragma unroll
+        for (int g = 0; g < SW_STAGES - 1; ++g) issue();
+        cstage = g_begin % SW_STAGES;
+        cur = sp + cstage * (2 * G) + lane;
+    }
+
+    __device__ __forceinline__ void issue() {
+        if (issued < g_end) {
+            if (issued < n_full) {
+                if (VEC16) {
+#pragma unroll
+                    for (int i = 0; i < G / 128; ++i) {
+                        cp_async16(idst + i * 128, ip + i * 128);
+                        cp_async16(idst + G + i * 128, ir + i * 128);
+                    }
+                } else {
+#pragma unroll
+                    for (int i = 0; i < G / 32; ++i) {
+                        cp_async4(idst + i * 32, ip + i * 32);
+                        cp_async4(idst + G + i * 32, ir + i * 32);
+                    }
+                }
+            } else {
+                const float qnan = __int_as_float(0x7fc00000);
+                const int lane = threadIdx.x & 31, off = VEC16 ? lane * 4 : lane;
+                float* dst = sp + (issued % SW_STAGES) * (2 * G);
+                const float* gp = ip - off; const float* gr = ir - off;   // the group's first bar, issued * G
+                for (int i = lane; i < G; i += 32) {
+                    const int t = issued * G + i;
+                    dst[i] = t < n ? __ldg(gp + i) : qnan;
+                    dst[G + i] = t < n ? __ldg(gr + i) : qnan;
+                }
+            }
+        }
+        cp_async_commit();  // always commit (possibly empty) so the group accounting stays uniform
+        ++issued;
+        ip += G; ir += G;
+        idst = (issued % SW_STAGES == 0) ? idst - (SW_STAGES - 1) * (2 * G) : idst + 2 * G;
+    }
+
+    __device__ __forceinline__ const float* land() {
+        issue();
+        cp_async_wait<SW_STAGES - 1>();
+        __syncwarp();
+        return cur;
+    }
+
+    __device__ __forceinline__ void release() {
+        __syncwarp();                         // the stage is refilled by the next land()
+        if (++cstage == SW_STAGES) { cstage = 0; cur -= (SW_STAGES - 1) * (2 * G); } else cur += 2 * G;
+    }
+};
+
+// Event sinks: sink(at, cnt) consumes the `cnt` queued events from queue position `at` on (lane j: event at + j).
+
+// Hand every full batch of 32 queued events to `sink`.
+template <class Sink>
+__device__ __forceinline__ void drain_full(const Machine& m, unsigned& qtail, Sink& sink) {
+    while (m.qhead - qtail >= 32) {
+        __syncwarp();
+        sink(qtail, 32);
+        qtail += 32;
+    }
+}
+
+// Scan one landed group, bars [t0, t0 + SW_GROUP) (`w`: this lane's first bar of it in the ring), two 32-bar windows
+// per step with both ballots issued before either is needed; full batches of queued events go to `sink`.
+template <class Sink>
+__device__ __forceinline__ void scan_group(const float* w, int t0, WarpShared* ws, const ScanConst& c,
+                                           Machine& m, unsigned& qtail, const bool emit, Sink& sink) {
+    const int lane = threadIdx.x & 31;
+#pragma unroll 1
+    for (int v = 0; v < SW_GROUP / 64; ++v, w += 64, t0 += 64) {
+        const float p0 = w[0], r0 = w[SW_GROUP];
+        const float p1 = w[32], r1 = w[SW_GROUP + 32];
+        const unsigned h0 = __ballot_sync(FULL, fires(m, p0, r0));
+        const unsigned h1 = __ballot_sync(FULL, fires(m, p1, r1));
+        if (h0 | h1) {
+            if (h0) scan_window(p0, r0, w - lane, t0, ws, c, m, emit);
+            scan_window(p1, r1, w - lane + 32, t0 + 32, ws, c, m, emit);
+            drain_full(m, qtail, sink);
+        }
+    }
+}
+
+// End of a scan: wait for the ring's last (empty) copy groups; with `close`, force-close an open position at the last
+// bar N - 1 (strategy_evaluation.py:849-876) by queueing its exit event; then hand every queued event to `sink`, the
+// last batch partial.
+template <class Sink>
+__device__ __forceinline__ void finish_scan(WarpShared* ws, Machine& m, unsigned& qtail, const float* pr,
+                                            int64_t N, const bool close, Sink& sink) {
+    cp_async_wait<0>();
+    if (close && m.pos != 0) {
+        const float pl = __ldg(pr + (N - 1));
+        const unsigned word = (unsigned)(N - 1) | B200BT_EVENT_EXIT | (m.pos > 0 ? B200BT_EVENT_SELL : 0u);
+        if ((threadIdx.x & 31) == 0) ws->evq[m.qhead & (SW_EVQ - 1)] = make_uint2(word, __float_as_uint(pl));
+        ++m.qhead;
+    }
+    __syncwarp();
+    while (m.qhead != qtail) {
+        const int cnt = (int)min(32u, m.qhead - qtail);
+        sink(qtail, cnt);
+        qtail += cnt;
     }
 }
 
