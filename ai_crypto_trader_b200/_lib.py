@@ -157,6 +157,9 @@ _SIGNATURES = {
     "b200bt_ga_next_generation": (C.c_int, [_vp, _vp, _vp, _i, _i, C.POINTER(C.c_double), C.POINTER(C.c_double),
                                             C.POINTER(C.c_int), C.c_double, _i, C.c_double, C.c_double, C.c_uint64,
                                             C.c_uint32, _vp, _vp, _vp]),
+    "b200bt_objective_matrix": (C.c_int, [_vp, _i, _i, C.POINTER(C.c_int), _i, _vp, _i64, _vp]),
+    "b200bt_pareto_workspace_bytes": (C.c_int64, [_i, _i]),
+    "b200bt_pareto_rank": (C.c_int, [_vp, _i64, _i, _i, C.POINTER(C.c_int), _vp, _i64, _vp, _vp, _vp, _vp, _vp]),
     "b200bt_daily_pnl": (C.c_int, [_vp, _i64, _i, _i64, _vp, _i, C.POINTER(SweepConfig), _vp, _vp, _i64, _vp, _i64, _vp,
                                    _vp]),
     "b200bt_cscv_workspace_bytes": (C.c_int64, [_i, _i64, _i]),

@@ -17,7 +17,8 @@ from datetime import datetime
 from typing import Dict, List, Optional
 
 from .dist import ShardedFitness, broadcast_seed
-from .genetic_algorithm import GeneticAlgorithm
+from .genetic_algorithm import GeneticAlgorithm, ParetoGeneticAlgorithm
+from .pareto import objectives_from_goals
 from .sweep import DEFAULT_GOALS, MarketData, PopulationSweep
 from .synth import param_ranges
 
@@ -38,6 +39,7 @@ class StrategyEvolutionService:
         self.ga_generations = int(os.getenv("GA_GENERATIONS", 10))                          # :79
         self.param_ranges = param_ranges(leverage_trading)
         goals = self.config.get("evolution", {}).get("optimization_goals") or DEFAULT_GOALS
+        self.goals = goals
         self.market = market
         rsi_lo, rsi_hi = self.param_ranges["rsi_period"]
         self.aggregation = aggregation or self.config.get("evolution", {}).get("fitness_aggregation") or "mean"
@@ -73,4 +75,37 @@ class StrategyEvolutionService:
             return optimized
         except Exception as e:        # reference convention (:692-694): log, return None
             logger.error("Error in genetic algorithm optimization: %s", e)
+            return None
+
+    async def optimize_pareto(self, current_params: Dict) -> Optional[List[Dict]]:
+        """NSGA-II over the optimisation goals (ParetoGeneticAlgorithm): the objectives are the goals' primary and secondary
+        metrics, each in its own direction (pareto.objectives_from_goals), instead of their product.  Returns the final
+        Pareto front, [{"parameters": dict, "objectives": {name: value}}], and appends an evolution record whose new_params
+        is the front's member with the best primary metric.  Single process: the objective matrix is not gathered over
+        ranks, so under a torch.distributed world of more than one process this logs an error and returns None."""
+        try:
+            import torch.distributed as dist
+            if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+                logger.error("optimize_pareto runs in a single process (world size %d)", dist.get_world_size())
+                return None
+            objectives = objectives_from_goals(self.goals)
+            sweep = self.sweep
+            ga = ParetoGeneticAlgorithm(param_ranges=self.param_ranges,
+                                        objective_function=lambda pop: sweep.evaluate_objectives_device(pop, objectives),
+                                        objectives=objectives, population_size=self.ga_population_size,
+                                        generations=self.ga_generations, mutation_rate=0.2, crossover_rate=0.8,
+                                        random_seed=self.random_seed, device=self.market.device)
+            seeds = [dict(current_params)] if current_params else None
+            front = ga.run(seeded_individuals=seeds)
+            history = ga.generation_history
+            self.evolution_records.append({
+                "id": str(uuid.uuid4()), "algorithm": "nsga2", "timestamp": datetime.now().isoformat(),
+                "objectives": [{"name": n, "maximize": m} for n, m in objectives],
+                "initial_best": history[0]["best_objectives"], "final_best": history[-1]["best_objectives"],
+                "front_size": len(front), "generations": len(history), "population_size": self.ga_population_size,
+                "old_params": current_params, "new_params": ga.best_individual})
+            self.last_pareto = ga
+            return front
+        except Exception as e:        # reference convention (:692-694): log, return None
+            logger.error("Error in Pareto optimization: %s", e)
             return None

@@ -300,3 +300,135 @@ class DeviceGeneticAlgorithm:
 
     def get_best_individual(self) -> Dict:
         return dict(self.best_individual)
+
+
+class ParetoGeneticAlgorithm(DeviceGeneticAlgorithm):
+    """NSGA-II (Deb, Pratap, Agarwal, Meyarivan 2002) on the device: the GA searches for the Pareto front of several
+    objectives instead of the maximum of one product of them.
+
+    objective_function: List[Dict] -> [len][M] objective values in each metric's own sense (a device float64 tensor, or
+    anything torch.as_tensor takes), e.g. `lambda pop: sweep.evaluate_objectives_device(pop, objectives)`.
+    objectives: [(name, maximize)] (pareto.objectives_from_goals).
+
+    Generation 0: b200bt_ga_init (seeded rows as DeviceGeneticAlgorithm), evaluated and ranked (b200bt_pareto_rank); the
+    population P is kept in crowded order, so row r has tournament key -r.  Generation t: the offspring Q come from
+    b200bt_ga_next_generation(P, fitness = -arange(N), ranked = arange(N), one elite, `tournament_size` contenders), so
+    each tournament is NSGA-II's crowded comparison; Q[0] is the kernel's copy of P[0] and is dropped, so N - 1 new
+    individuals are evaluated.  R = [P; Q[1:]] with the objectives of P kept (never re-evaluated) is ranked, and the next
+    P is R[order[:N]] with its objective rows, gathered on the device.
+
+    After run(): `pareto_front` (front 0 of the final population as [{"parameters", "objectives"}], in crowded order),
+    `objective_values` [N][M], `front`, `crowding` (numpy, in population order), `population` (dicts),
+    `generation_history` (per generation: number of fronts, size of front 0, best value per objective) and
+    `best_individual`: the front-0 member first in crowded order among those with the best first objective."""
+
+    MAX_POPULATION = 32768           # R has 2N - 1 <= 65535 rows, within b200bt_pareto_rank's limit
+
+    def __init__(self, param_ranges: Dict[str, Tuple], objective_function: Callable[[List[Dict]], object],
+                 objectives: Sequence[Tuple[str, bool]], population_size: int = 20, generations: int = 10,
+                 mutation_rate: float = 0.2, crossover_rate: float = 0.8, tournament_size: int = 2,
+                 random_seed: Optional[int] = None, device=None):
+        if not 2 <= int(population_size) <= self.MAX_POPULATION:
+            raise ValueError(f"population_size must be in 2..{self.MAX_POPULATION} ({population_size} given)")
+        if not 1 <= int(tournament_size) <= min(8, int(population_size)):
+            raise ValueError("tournament_size must be in 1..min(8, population_size)")
+        super().__init__(param_ranges, objective_function, population_size=population_size, generations=generations,
+                         mutation_rate=mutation_rate, crossover_rate=crossover_rate, elitism_pct=0.0,
+                         tournament_size=tournament_size, random_seed=random_seed, device=device)
+        from .pareto import ParetoRanker
+        self.objective_function = objective_function
+        self.objectives = [(str(n), bool(m)) for n, m in objectives]
+        if not 1 <= len(self.objectives) <= 8:
+            raise ValueError("1..8 objectives")
+        self.maximize = [m for _, m in self.objectives]
+        self._ranker = ParetoRanker()
+        torch = self._torch
+        N = self.population_size
+        self._key = -torch.arange(N, dtype=torch.float64, device=self.device)      # row r of P has key -r
+        self._ranked = torch.arange(N, dtype=torch.int32, device=self.device)
+        self._obj = None                  # objectives of P [N][M] (device), row for row
+        self._front = self._crowding = None
+        self.last_offspring = None        # Q of the last generation [N][G] (device; Q[0] is the copy of P[0])
+        self.last_objectives_R = None     # objectives of R = [P; Q[1:]] of the last generation [2N - 1][M] (device)
+        self.pareto_front: List[Dict] = []
+        self.objective_values = self.front = self.crowding = None
+
+    def _evaluate_rows(self, rows):
+        torch = self._torch
+        dicts = self._to_dicts(rows.cpu().numpy())
+        out = self.objective_function(dicts)
+        out = torch.as_tensor(out, dtype=torch.float64).to(self.device)
+        if tuple(out.shape) != (len(dicts), len(self.objectives)):
+            raise ValueError("objective function returned shape %s for %d individuals x %d objectives"
+                             % (tuple(out.shape), len(dicts), len(self.objectives)))
+        return out
+
+    def _survive(self, rows, obj) -> None:
+        """P, its objectives, fronts and crowding = the first N rows of rows' crowded order."""
+        front, crowding, order, _ = self._ranker.rank(obj, self.maximize)
+        keep = order[:self.population_size].long()
+        self.params = rows.index_select(0, keep)          # a new tensor: self._next never aliases it
+        self._obj = obj.index_select(0, keep)
+        self._front, self._crowding = front.index_select(0, keep), crowding.index_select(0, keep)
+
+    def evaluate_population(self) -> None:
+        """Generation 0: evaluate the initial population and put it in crowded order."""
+        self._survive(self.params, self._evaluate_rows(self.params))
+
+    def evolve_generation(self, generation: int) -> None:
+        torch, lib = self._torch, self._lib
+        with torch.cuda.device(self.device):
+            lib.call("b200bt_ga_next_generation", self.params.data_ptr(), self._key.data_ptr(), self._ranked.data_ptr(),
+                     self.population_size, len(self.names), self._lo, self._hi, self._is_int, 0.0, self.tournament_size,
+                     self.crossover_rate, self.mutation_rate, self.seed, int(generation), self._sel.data_ptr(),
+                     self._next.data_ptr(), lib.current_stream())
+        offspring = self._next
+        self.last_offspring = offspring
+        rows = torch.cat([self.params, offspring[1:]])
+        obj = torch.cat([self._obj, self._evaluate_rows(offspring[1:])])
+        self.last_objectives_R = obj
+        self._survive(rows, obj)
+
+    def _host_state(self) -> None:
+        self.objective_values = self._obj.cpu().numpy()
+        self.front = self._front.cpu().numpy()
+        self.crowding = self._crowding.cpu().numpy()
+        self.population = self._to_dicts(self.params.cpu().numpy())
+
+    def _oriented(self) -> np.ndarray:
+        """Objective values with larger = better, NaN -> -inf (the ranking's view)."""
+        v = np.where(np.array(self.maximize)[None, :], self.objective_values, -self.objective_values)
+        return np.where(np.isnan(v), -np.inf, v)
+
+    def record_generation(self, generation: int) -> None:
+        self._host_state()
+        v = self._oriented()
+        best = {}
+        for j, (name, maximize) in enumerate(self.objectives):
+            top = float(v[:, j].max())
+            best[name] = top if maximize else -top
+        self.generation_history.append({
+            "generation": generation, "timestamp": datetime.now().isoformat(),
+            "n_fronts": int(self.front.max()) + 1, "front0_size": int((self.front == 0).sum()),
+            "best_objectives": best, "diversity": self.calculate_diversity()})
+
+    def _finish(self) -> None:
+        names = [n for n, _ in self.objectives]
+        rows = np.flatnonzero(self.front == 0)            # P is in crowded order: front 0 comes first
+        self.pareto_front = [{"parameters": dict(self.population[i]),
+                              "objectives": {n: float(self.objective_values[i, j]) for j, n in enumerate(names)}}
+                             for i in rows]
+        first = self._oriented()[rows, 0]
+        pick = rows[int(np.argmax(first == first.max()))]
+        self.best_individual = dict(self.population[pick])
+        self.best_fitness = float(self.objective_values[pick, 0])
+
+    def run(self, seeded_individuals: Optional[List[Dict]] = None) -> List[Dict]:
+        self.initialize_population(seeded_individuals)
+        self.evaluate_population()
+        self.record_generation(0)
+        for generation in range(1, self.generations + 1):
+            self.evolve_generation(generation)
+            self.record_generation(generation)
+        self._finish()
+        return self.pareto_front

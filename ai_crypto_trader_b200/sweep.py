@@ -560,6 +560,7 @@ class PopulationSweep:
         self.max_event_bytes = int(BOOK_MAX_EVENT_BYTES if max_event_bytes is None else max_event_bytes)
         self._book_cap = 0                     # event_cap learnt from the previous book evaluation (0: count first)
         self._book = None                      # book stats [pop][20] float64 of the last book evaluation (host)
+        self._book_dev = None                  # the same stats of its unique individuals, on the device
         self.book_resweeps = 0                 # slices of the last book evaluation swept again with the exact cap
         self.last_event_bytes = 0              # largest event buffer of the last book evaluation
         self.market = market
@@ -847,6 +848,28 @@ class PopulationSweep:
             return self._evaluate_book(*self._unique(population))
         return self._evaluate_unique(*self._unique(population), self.event_cap)
 
+    def evaluate_objectives_device(self, population: List[Dict], objectives) -> torch.Tensor:
+        """Objective matrix float64 [pop][M] on the device: one evaluate() (same deduplication, schedules and book slicing),
+        then b200bt_objective_matrix on its stats -- the lane stats averaged over the symbols under aggregation="mean", the
+        book stats under "book".  objectives: [(lane-stat field, maximize)] (pareto.objectives_from_goals); the values are
+        in the metric's own sense, so ("score", True) under "mean" gives evaluate()'s fitness bit for bit."""
+        from . import pareto
+        objectives = list(objectives)
+        for name, _ in objectives:
+            pareto._field(name)
+        if not population:
+            return torch.zeros((0, len(objectives)), dtype=torch.float64, device=self.market.device)
+        self.evaluate(population)
+        stats = self._book_dev if self.aggregation == "book" else self._stats
+        out = pareto.objective_matrix(stats, objectives)
+        if self._inverse is not None:
+            out = out.index_select(0, torch.from_numpy(self._inverse).to(out.device))
+        return out
+
+    def evaluate_objectives(self, population: List[Dict], objectives) -> np.ndarray:
+        """evaluate_objectives_device on the host: float64 [pop][M]."""
+        return self.evaluate_objectives_device(population, objectives).cpu().numpy()
+
     def _evaluate_book(self, packed: np.ndarray, population: List[Dict], expand: Optional[np.ndarray]) -> np.ndarray:
         """evaluate() under aggregation="book": sweep with event buffers, then b200bt_book_metrics.
 
@@ -871,6 +894,7 @@ class PopulationSweep:
             busiest = max(busiest, self._exact_cap(self._stats))
         self._book_cap = busiest + busiest // BOOK_CAP_HEADROOM + 2
         self._keep_slice_stats(lanes, expand)
+        self._book_dev = book
         self._book = book.cpu().numpy()
         if expand is not None:
             self._book = self._book[expand]

@@ -607,6 +607,41 @@ int b200bt_ga_next_generation(const double* params, const double* fitness, const
                               uint32_t generation, int32_t* selected_workspace, double* params_out,
                               b200bt_stream_t stream);
 
+/* ---- multi-objective ranking (NSGA-II; Deb, Pratap, Agarwal, Meyarivan 2002) ---------------------------------------
+ * csrc/pareto.cu; restated by tests/pareto_ref.py. */
+
+/* Objective matrix of a population: out[i][j] = (sum over s = 0..S-1, ascending, from +0.0, of stats[i][s].<field j>) / S
+ * -- b200bt_fitness_reduce's expression, so field 12 (score) gives its fitness bit for bit.  stats: device [pop][S] (a
+ * book's [pop] stats with S = 1); fields_host: host int[M], indices 0..18 of the fields of b200bt_lane_stats, trade_hash
+ * is not one (EINVAL); out: device float64 [pop][ld_out].  1 <= M <= 8 (ELIMIT above), M <= ld_out (EINVAL).  Values are copied as
+ * they are (NaN and +-inf included, no sign change). */
+int b200bt_objective_matrix(const b200bt_lane_stats* stats, int pop, int S, const int* fields_host, int M, double* out,
+                            int64_t ld_out, b200bt_stream_t stream);
+
+/* Non-dominated fronts, crowding distance and crowded order of n points with M objectives.
+ *   obj: device float64 [n][ld]; maximize_host: host int[M] (non-zero: larger is better).
+ *   v[p][j] = maximize_j ? obj[p][j] : -obj[p][j], a NaN becomes -inf; larger v is better.
+ *   p dominates q iff v[p][j] >= v[q][j] for every j and v[p][j] > v[q][j] for some j (identical vectors do not dominate
+ *   each other; -inf == -inf).
+ *   front (device int32 [n]): 0 for the non-dominated points; front k + 1 = the non-dominated points once fronts 0..k are
+ *   removed.
+ *   crowding (device float64 [n]): per front F and objective j, F's members ordered by (v[.][j], index) ascending; the
+ *   first and the last get +inf; with r = v_max - v_min over F, an interior member adds (v_next - v_prev) / r unless r is
+ *   0 or not finite.  Summed over j ascending from +0.0, correctly rounded (__dsub_rn, __ddiv_rn, __dadd_rn).  A front of
+ *   one or two members is all +inf; crowding is never NaN.
+ *   order (device int32 [n]): the indices sorted by (front asc, crowding desc, index asc).
+ *   key_or_null (device float64 [n], optional): key[p] = -(position of p in order), +0.0 for the first -- the fitness
+ *   with which b200bt_ga_next_generation's "first maximum wins" tournament is NSGA-II's crowded-comparison tournament.
+ * Limits: 1 <= n <= 65536 (ELIMIT above), 1 <= M <= 8 (ELIMIT above), ld >= M.  Workspace: device, 256-byte aligned, of
+ * b200bt_pareto_workspace_bytes(n, M) bytes (n^2 / 8 bytes of dominance bits and O(n M) more; 0 outside the limits).
+ * No host synchronisation; deterministic (integer atomics only, and no output depends on their order).  Cost: the
+ * dominance pass is O(n^2 M); the fronts take one grid-wide barrier each, so a chain of n fronts (M = 1, or perfectly
+ * correlated objectives) is the worst case; crowding and order are O(sum over fronts of |F|^2 M). */
+int64_t b200bt_pareto_workspace_bytes(int n, int M);
+int b200bt_pareto_rank(const double* obj, int64_t ld, int n, int M, const int* maximize_host, void* workspace,
+                       int64_t workspace_bytes, int32_t* front, double* crowding, int32_t* order, double* key_or_null,
+                       b200bt_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

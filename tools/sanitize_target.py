@@ -19,7 +19,7 @@ from ai_crypto_trader_b200.monte_carlo import PathEngine, risk_statistics
 from ai_crypto_trader_b200.sweep import MarketData, PopulationSweep
 from oracle import indicators_ref, sim_oracle
 
-legs = sys.argv[1:] or ["sweep", "mc", "joint", "indicators"]
+legs = sys.argv[1:] or ["sweep", "mc", "joint", "indicators", "pareto"]
 torch.cuda.set_device(0)
 
 if "sweep" in legs:
@@ -77,5 +77,16 @@ if "indicators" in legs:
     ta = ind.TechnicalAnalyzer(m)
     ind.multi_timeframe_indicators(m, 0)
     print("indicators ok", ta.get_all_indicators(0)["rsi"], flush=True)
+if "pareto" in legs:
+    # multi-objective ranking: the cooperative peel (grid barriers, rotating counters, appended member slots) and the
+    # dominance tile in opted-in dynamic shared memory, on heavy ties and duplicate rows; checked against the host form
+    sys.path.insert(0, str(Path(__file__).resolve().parents[1] / "tests"))
+    import pareto_ref
+    from ai_crypto_trader_b200.pareto import pareto_rank
+    obj, mx = pareto_ref.make_input("ties", 4101, 3)
+    got = [t.cpu().numpy() for t in pareto_rank(torch.from_numpy(obj).cuda(), mx, with_key=True)]
+    want = pareto_ref.pareto_numpy(obj, mx)
+    assert all(a.tobytes() == b.tobytes() for a, b in zip(got, want))
+    print("pareto ok:", int(got[0].max()) + 1, "fronts of 4101 points, bit-identical to pareto_numpy", flush=True)
 torch.cuda.synchronize()
 print("sanitize target done")
