@@ -54,6 +54,22 @@ class SweepConfig(C.Structure):
     ]
 
 
+class RegimeParams(C.Structure):
+    """b200bt_regime_params: the point clock and the thresholds of detect_regime_from_data
+    (services/market_regime_service.py:100-118, at their defaults)."""
+    _fields_ = [
+        ("sample_minutes", C.c_int32), ("reserved", C.c_int32),
+        ("volatile_volatility", C.c_double), ("bull_price_change", C.c_double), ("bull_trend_strength", C.c_double),
+        ("bear_price_change", C.c_double), ("bear_trend_strength", C.c_double), ("ranging_price_range", C.c_double),
+        ("ranging_trend_strength", C.c_double),
+    ]
+
+
+REGIMES = ("bull", "bear", "ranging", "volatile", "unknown")          # B200BT_REGIME_* = index
+REGIME_WINDOW_DTYPE = [("start_minute", "<i8"), ("n_points", "<i4"), ("label", "<i4"), ("volatility", "<f8"),
+                       ("change_pct", "<f8"), ("mean_strength", "<f8"), ("up_frac", "<f8"), ("down_frac", "<f8"),
+                       ("sideways_frac", "<f8")]                      # b200bt_regime_window, 64 bytes
+
 LANE_STATS_FIELDS = (
     "n_records", "n_wins", "n_losses", "total_profit", "total_loss", "net_profit",
     "max_drawdown", "sharpe_ratio", "n_days", "largest_profit", "largest_loss",
@@ -164,6 +180,11 @@ _SIGNATURES = {
                                    _vp]),
     "b200bt_cscv_workspace_bytes": (C.c_int64, [_i, _i64, _i]),
     "b200bt_cscv": (C.c_int, [_vp, _i64, _i, _i64, _i, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "b200bt_regime_max_windows": (C.c_int64, [_i64, _i]),
+    "b200bt_regime_labels": (C.c_int, [_vp, _vp, _vp, _vp, _i, _i64, _i64, _i64, _i, C.POINTER(RegimeParams), _vp, _i64,
+                                       _vp, _i64, _vp]),
+    "b200bt_class_stats": (C.c_int, [_vp, _i64, _i, _i64, _vp, _i, C.POINTER(SweepConfig), _vp, _vp, _i64, _vp, _i64, _i,
+                                     _vp, _vp]),
     "b200bt_pct_change": (C.c_int, [_vp, _i64, _i, _i64, _vp, _i64, _vp]),
     "b200bt_tail_stats_workspace_bytes": (C.c_int64, [_i64]),
     "b200bt_tail_stats": (C.c_int, [_vp, _i64, C.c_double, _vp, _vp, _i64, _vp]),

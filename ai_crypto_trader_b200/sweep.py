@@ -1091,6 +1091,54 @@ class PopulationSweep:
             book, lanes = book.index_select(0, inv), lanes.index_select(0, inv)
         return book, lanes, int(first_day)
 
+    def class_stats(self, population: List[Dict], labels: torch.Tensor, n_classes: int):
+        """Trade metrics of every lane split by the label of each record's bar (b200bt_class_stats), in the order of
+        `population`: (stats float64 [R][pop][S][20] on the device, [R dicts field -> [pop][S] array]).  Block r holds
+        calculate_metrics and the score on the records of lane (i, s) whose bar carries label r; labels >= R belong to no
+        class.  labels: device uint8 [S][N]; [1][N] (or a row expanded to [S][N]) is one row shared by every symbol.
+
+        A counting sweep gives the exact event cap, then slices of the population whose event buffers keep within
+        max_event_bytes are swept and split.  Individuals that decode alike are swept once.  Afterwards lane_stats()
+        describes this population."""
+        if not population:
+            raise ValueError("class_stats needs at least one individual")
+        m = self.market
+        R = int(n_classes)
+        if not 1 <= R <= 8:
+            raise ValueError(f"class_stats: n_classes must be 1..8, not {R}")
+        if not (labels.is_cuda and labels.dtype == torch.uint8 and labels.dim() == 2 and labels.shape[0] in (1, m.S)
+                and labels.shape[1] == m.N):
+            raise ValueError(f"class_stats: labels must be a device uint8 tensor [{m.S} or 1][{m.N}]")
+        shared = labels.shape[0] == 1 or labels.stride(0) == 0
+        labels = labels[:1].contiguous() if shared else labels.contiguous()
+        ld_labels = 0 if shared else m.N
+        packed, unique, expand = self._unique(population)
+        U, S = len(packed), m.S
+        self._evaluate_unique(packed, unique, None, 0)
+        cap = self._exact_cap(self._stats)
+        stats = torch.empty((U, S, _lib.LANE_STATS_WORDS), dtype=torch.float64, device=m.device)
+        out = torch.empty((R, U, S, _lib.LANE_STATS_WORDS), dtype=torch.float64, device=m.device)
+        part = torch.empty_like(out)
+        indiv = torch.from_numpy(packed.view(np.uint8)).to(m.device).view(U, -1)
+        for lo, hi, c in self._event_slices(packed, unique, cap):
+            piece = part.view(-1)[:R * (hi - lo) * S * _lib.LANE_STATS_WORDS].view(R, hi - lo, S, -1)   # [R][slice][S]
+            with torch.cuda.device(m.device):
+                _lib.call("b200bt_class_stats", m.close.data_ptr(), _lib.ld(m.close), S, m.N, indiv[lo:hi].data_ptr(),
+                          hi - lo, C.byref(self.cfg), self._stats.data_ptr(), self._events.data_ptr(), c,
+                          labels.data_ptr(), ld_labels, R, piece.data_ptr(), _lib.current_stream())
+            out[:, lo:hi] = piece
+            stats[lo:hi] = self._stats
+        self._keep_slice_stats(stats, expand)
+        if expand is not None:
+            out = out.index_select(1, torch.from_numpy(expand).to(m.device))
+        raw = out.cpu().numpy()
+        views = []
+        for r in range(R):
+            d = {name: raw[r, :, :, i] for i, name in enumerate(_lib.LANE_STATS_FIELDS[:-1])}
+            d["trade_hash"] = np.ascontiguousarray(raw[r, :, :, _lib.LANE_STATS_WORDS - 1]).view(np.uint64)
+            views.append(d)
+        return out, views
+
     def lane_stats(self) -> Dict[str, np.ndarray]:
         """Per-lane metrics of the last evaluation: dict field -> [pop][S] array."""
         raw = self._stats.cpu().numpy()

@@ -642,6 +642,80 @@ int b200bt_pareto_rank(const double* obj, int64_t ld, int n, int M, const int* m
                        int64_t workspace_bytes, int32_t* front, double* crowding, int32_t* order, double* key_or_null,
                        b200bt_stream_t stream);
 
+/* ---- market regimes (csrc/regime.cu) -----------------------------------------------------------------------------
+ * services/market_regime_service.py labels the market bull / bear / ranging / volatile (detect_regime_from_data
+ * :503-603) in 24-hour windows (update_strategy_performance_by_regime :844-889) and scores strategies per regime.  These
+ * entry points give the labels of a market's own bars and the trade metrics of a sweep's records per label. */
+#define B200BT_REGIME_BULL 0
+#define B200BT_REGIME_BEAR 1
+#define B200BT_REGIME_RANGING 2
+#define B200BT_REGIME_VOLATILE 3
+#define B200BT_REGIME_UNKNOWN 4
+
+typedef struct b200bt_regime_params {
+    int32_t sample_minutes;          /* minutes per point; a positive multiple of 5 and of bar_minutes (60: hourly)     */
+    int32_t reserved;
+    double volatile_volatility;      /* 1.5   VOLATILE_THRESHOLD                                                       */
+    double bull_price_change;        /* 5.0   BULL_PRICE_CHANGE (percent)                                              */
+    double bull_trend_strength;      /* 0.6   BULL_TREND_STRENGTH (compared with the fraction of uptrend points)        */
+    double bear_price_change;        /* -5.0  BEAR_PRICE_CHANGE                                                        */
+    double bear_trend_strength;      /* 0.6   BEAR_TREND_STRENGTH (fraction of downtrend points)                        */
+    double ranging_price_range;      /* 3.0   RANGING_PRICE_RANGE (|change| in percent)                                 */
+    double ranging_trend_strength;   /* 0.3   RANGING_TREND_STRENGTH (mean trend_strength)                              */
+} b200bt_regime_params; /* 64 bytes */
+
+typedef struct b200bt_regime_window {
+    int64_t start_minute;            /* t0 + 1440 k; -1 for rows past the symbol's last window                          */
+    int32_t n_points;                /* 0: the window is skipped (the reference never forms it)                         */
+    int32_t label;                   /* B200BT_REGIME_*                                                                 */
+    double volatility;               /* std (ddof 1) of the returns * sqrt(24); NaN with fewer than 2 returns           */
+    double change_pct;               /* (last - first) / first * 100                                                    */
+    double mean_strength;            /* mean trend_strength                                                             */
+    double up_frac, down_frac, sideways_frac;
+} b200bt_regime_window; /* 64 bytes */
+
+/* Regime labels of every bar.  close, sma20, sma50, sma20_5m_aligned: device float32 [S][ld], ld >= N (SMA20 / SMA50 of
+ * the closes and SMA20 of the 5-minute closes brought to this clock by b200bt_align: the last COMPLETED 5-minute bar; NaN
+ * where undefined).  Bar t starts at minute m_t = minute0 + t * bar_minutes (minute0 >= 0: the unbroken clock, no glued
+ * series).
+ *   Points: one per epoch-aligned sample_minutes bucket, at its last bar t (the next bar starts in a later bucket; a
+ *   bucket cut by the end of the series has none), from the first such bar where all three averages are defined.  The
+ *   point's price is close[t]; with s1 = (c - sma20) / sma20 * 100 and s5 = (c - sma20_5m) / sma20_5m * 100 its
+ *   trend_strength is |s1 * 0.6 + s5 * 0.4| and its trend up if c > sma20 > sma50, down if c < sma20 < sma50, else
+ *   sideways (market_monitor_service.py:263-280; float64, correctly rounded, no FMA contraction).
+ *   Windows: k = 0, 1, ... cover the minutes [t0 + 1440 k, t0 + 1440 (k + 1)), t0 = the first point's minute, while their
+ *   start < the last point's minute.  Per window over its points p_0..p_{n-1} in time order: returns p_i / p_{i-1} - 1,
+ *   volatility = their sample std * sqrt(24) (NaN below 2 returns, and NaN is never volatile), change = (p_{n-1} - p_0) /
+ *   p_0 * 100, the mean trend_strength and the up / down / sideways fractions.  Fewer than 2 points: UNKNOWN.  Otherwise,
+ *   in order: VOLATILE if volatility > volatile_volatility; BULL if change > bull_price_change and up >
+ *   bull_trend_strength; BEAR if change < bear_price_change and down > bear_trend_strength; RANGING if |change| <
+ *   ranging_price_range and mean strength < ranging_trend_strength; else BULL if up > down and up > sideways, BEAR if
+ *   down > up and down > sideways, else RANGING.
+ *   labels: device uint8 [S][ld_labels] (ld_labels >= N unless S == 1): the label of the window holding m_t; UNKNOWN
+ *   before t0, after the last window and in skipped or unknown windows.
+ *   window_stats_or_null: device [S][max_windows] rows, row k = window k; max_windows >= b200bt_regime_max_windows(N,
+ *   bar_minutes) (EINVAL otherwise).
+ * Checked before the device: null pointers, sizes, minute0 < 0, sample_minutes not a positive multiple of 5 and of
+ * bar_minutes (all EINVAL), N >= 2^30 (ELIMIT).  No atomics on outputs; deterministic. */
+int64_t b200bt_regime_max_windows(int64_t N, int bar_minutes);
+int b200bt_regime_labels(const float* close, const float* sma20, const float* sma50, const float* sma20_5m_aligned, int S,
+                         int64_t N, int64_t ld, int64_t minute0, int bar_minutes, const b200bt_regime_params* params,
+                         uint8_t* labels, int64_t ld_labels, b200bt_regime_window* window_stats_or_null,
+                         int64_t max_windows, b200bt_stream_t stream);
+
+/* Trade metrics per bar label.  Inputs as b200bt_daily_pnl, plus labels: device uint8 [S][ld_labels] (ld_labels >= N),
+ * or ld_labels = 0 for one row shared by every symbol.  class_stats: device [R][pop][S], 1 <= R <= 8 (ELIMIT above):
+ * block r holds, for lane (i, s), calculate_metrics and the cfg's score on the sub-list of the lane's records whose own
+ * bar carries label r (an entry and its exit may fall into different classes; labels >= R belong to no class).  Inside a
+ * class everything is as b200bt_book_metrics on a mixed list: equity from initial_capital, the calendar days of the
+ * class's records (the cfg's gap applies), sum_duration_bars over the pairs (2k, 2k + 1) of the class list, trade_hash =
+ * xor of event_hash(index in the class list, word).  With R = 1 and every label 0, counts and hash equal the lane's.  A
+ * lane with n_records > event_cap gives n_records = -1, score NaN and zeros in every class.  Deterministic. */
+int b200bt_class_stats(const float* price, int64_t ld_price, int S, int64_t N, const b200bt_individual* indiv, int pop,
+                       const b200bt_sweep_config* cfg, const b200bt_lane_stats* lane_stats, const uint32_t* events,
+                       int64_t event_cap, const uint8_t* labels, int64_t ld_labels, int R,
+                       b200bt_lane_stats* class_stats, b200bt_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

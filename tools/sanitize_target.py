@@ -19,7 +19,7 @@ from ai_crypto_trader_b200.monte_carlo import PathEngine, risk_statistics
 from ai_crypto_trader_b200.sweep import MarketData, PopulationSweep
 from oracle import indicators_ref, sim_oracle
 
-legs = sys.argv[1:] or ["sweep", "mc", "joint", "indicators", "pareto"]
+legs = sys.argv[1:] or ["sweep", "mc", "joint", "indicators", "pareto", "regime"]
 torch.cuda.set_device(0)
 
 if "sweep" in legs:
@@ -88,5 +88,33 @@ if "pareto" in legs:
     want = pareto_ref.pareto_numpy(obj, mx)
     assert all(a.tobytes() == b.tobytes() for a, b in zip(got, want))
     print("pareto ok:", int(got[0].max()) + 1, "fronts of 4101 points, bit-identical to pareto_numpy", flush=True)
+if "regime" in legs:
+    # market regimes: the labelling pass (block-wide head search, one warp per window) and the class pass (per-class
+    # shared-memory staging, R WarpAccs per warp), on a market with a NaN head and labels >= R; checked against the oracle
+    sys.path.insert(0, str(Path(__file__).resolve().parents[1] / "tests"))
+    import regime_ref
+    from ai_crypto_trader_b200 import regime
+    S, N, POP = 2, 6_000, 12
+    ohlcv = synth.synth_ohlcv(S, N, first_symbol=2)
+    market = MarketData(ohlcv)
+    labels, _ = regime.regime_labels(market, 15)
+    rows = regime.trend_rows(market).cpu().numpy()
+    for s in range(S):
+        assert np.array_equal(labels[s].cpu().numpy(), regime_ref.symbol_labels(*rows[:, s], market.minute0, 1, 15)[0])
+    sweep = PopulationSweep(market, rsi_periods=range(5, 31))
+    population = synth.random_population(POP, seed=2)
+    mixed = torch.from_numpy(np.random.default_rng(0).integers(0, 7, (S, N)).astype(np.uint8)).cuda()
+    _, views = sweep.class_stats(population, mixed, 5)
+    cfg = sim_oracle.config_of(market.minute0, 1)
+    lab = mixed.cpu().numpy()
+    for s in range(S):
+        bank = sweep.bank[s].cpu().numpy()
+        for i, p in enumerate(population):
+            _, ev, pn = sim_oracle.lane(ohlcv[3, s], bank[sweep.period_row[p["rsi_period"]]], p, cfg, event_cap=N + 2)
+            want = regime_ref.class_stats(ev, pn, lab[s], 5, cfg)
+            for r in range(5):
+                assert views[r]["n_records"][i, s] == want[r]["n_records"]
+                assert int(views[r]["trade_hash"][i, s]) == int(want[r]["trade_hash"])
+    print("regime ok: labels equal the restatement,", S * POP, "lanes x 5 classes match the oracle", flush=True)
 torch.cuda.synchronize()
 print("sanitize target done")
