@@ -65,6 +65,29 @@ class RegimeParams(C.Structure):
     ]
 
 
+class GridIndividual(C.Structure):
+    """b200bt_grid_individual: one grid parameter set, decoded by the host (grid.py)."""
+    _fields_ = [
+        ("num_grids", C.c_int32), ("grid_type", C.c_int32), ("rebalance_ticks", C.c_int32), ("adjust_ticks", C.c_int32),
+        ("flags", C.c_int32), ("reserved", C.c_int32), ("lower_pct", C.c_double), ("upper_pct", C.c_double),
+    ]
+
+
+class GridRegimeRule(C.Structure):
+    """b200bt_grid_regime_rule: what the adjustment's regime rule sets for one label."""
+    _fields_ = [("apply", C.c_int32), ("num_grids", C.c_int32), ("lower_pct", C.c_double), ("upper_pct", C.c_double)]
+
+
+GRID_STATS_FIELDS = (
+    "total_profit", "total_trades", "profitable_trades", "win_rate", "profit_per_day", "up_crossings", "down_crossings",
+    "n_regenerations", "num_grids", "lower", "upper", "cash", "position", "mark_to_market", "max_position",
+    "min_position", "n_rebalance_checks", "n_adjustments", "n_ticks", "near_ties",
+)                                                                     # b200bt_grid_stats, 160 bytes
+GRID_ADAPT_REGIME = 1
+GRID_AUTO_BOUNDARIES = 2
+GRID_MAX_GRIDS = 127
+GRID_TYPES = ("arithmetic", "geometric")                              # B200BT_GRID_* = index
+
 REGIMES = ("bull", "bear", "ranging", "volatile", "unknown")          # B200BT_REGIME_* = index
 REGIME_WINDOW_DTYPE = [("start_minute", "<i8"), ("n_points", "<i4"), ("label", "<i4"), ("volatility", "<f8"),
                        ("change_pct", "<f8"), ("mean_strength", "<f8"), ("up_frac", "<f8"), ("down_frac", "<f8"),
@@ -185,6 +208,8 @@ _SIGNATURES = {
                                        _vp, _i64, _vp]),
     "b200bt_class_stats": (C.c_int, [_vp, _i64, _i, _i64, _vp, _i, C.POINTER(SweepConfig), _vp, _vp, _i64, _vp, _i64, _i,
                                      _vp, _vp]),
+    "b200bt_grid_sweep": (C.c_int, [_vp, _i64, _i, _i64, _i64, _i, _i64, _vp, _i, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _i64,
+                                    _vp]),
     "b200bt_pct_change": (C.c_int, [_vp, _i64, _i, _i64, _vp, _i64, _vp]),
     "b200bt_tail_stats_workspace_bytes": (C.c_int64, [_i64]),
     "b200bt_tail_stats": (C.c_int, [_vp, _i64, C.c_double, _vp, _vp, _i64, _vp]),

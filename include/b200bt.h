@@ -716,6 +716,111 @@ int b200bt_class_stats(const float* price, int64_t ld_price, int S, int64_t N, c
                        int64_t event_cap, const uint8_t* labels, int64_t ld_labels, int R,
                        b200bt_lane_stats* class_stats, b200bt_stream_t stream);
 
+/* ---- grid trading (csrc/grid.cu) ----------------------------------------------------------------------------------
+ * A backtest of services/grid_trading_strategy.py's GridTradingStrategy, whose only evaluation is "simulation mode": the
+ * live loop of run() (:122-233) against the exchange ticker.  Here every (individual, symbol) lane is ONE symbol's service
+ * instance run over a market's bars (the reference keeps num_grids and the pcts service-wide, so a multi-symbol service
+ * couples its symbols at each adjustment; that coupled form is not modelled).
+ *
+ * Clock: tick k = 0 .. T - 1 is bar start_bar + k (T = N - start_bar); its price is the bar's close widened to float64.
+ * __init__ / _initialize_grid (:245-345) run at tick 0: start_time, last_rebalance and last_adjustment are t0.  On every tick,
+ * tick 0 included, the loop body runs, in order:
+ *   _process_grid_simulation (:679-779) with last = the previous tick's price (tick 0: last == cur, nothing happens).
+ *     Up move (cur > last): every level with last <= L_i <= cur is a trade with profit (L_i - L_{i-1}) * qty (0 for i = 0),
+ *     profitable when the profit is > 0.  Down move: every level with cur <= L_i <= last is a trade with no profit.  Equal
+ *     prices do nothing; a level equal to the last price is counted again.  qty = qty[s] (symbol_settings' quantity_per_grid,
+ *     else the global one, :387-400).
+ *   The rebalance check (:178-186): (now - last_rebalance) > rebalance_frequency with a strict >, and last_rebalance is reset
+ *     whenever the check runs, so it runs on the ticks k = m * rebalance_ticks (m >= 1), rebalance_ticks =
+ *     floor(frequency / bar_seconds) + 1 (61 at 1-minute bars and 3600 s).  _rebalance_grid (:781-838): when cur <
+ *     lower * 1.05 or cur > upper * 0.95 the grid is regenerated around cur with the CURRENT pcts and num_grids:
+ *     lower = cur * (1 - lower_pct / 100), upper = cur * (1 + upper_pct / 100).  Quirks kept: with 5 % boundaries the two
+ *     thresholds overlap, so nearly every check regenerates; symbol_settings' boundary pcts are never read.
+ *   The adjustment check (:189-196), same timing with adjust_ticks from auto_adjust_period (1441 at 1-minute bars and one
+ *     day), _adjust_grid_parameters (:840-905):
+ *     regime rule (:847-883), only with B200BT_GRID_ADAPT_REGIME and a regime source (labels and table; none = the
+ *       reference without market_regime_history in Redis): the label of the adjust tick's bar selects table[label]; an
+ *       entry with apply != 0 sets num_grids and both pcts (ranging_* / volatile_* of the config; b200bt_regime_labels
+ *       emits no "trending" label, so the trending_* branch never fires).
+ *     win-rate rule (:886-905): when total_trades > 10, profitable / total < 0.4 gives num_grids = max(5, n - 2), > 0.7
+ *       gives min(20, n + 2).  grid_spread feeds no level and is not simulated.
+ *     Both take effect at the next regeneration.
+ * Levels (_generate_grid_levels :347-385), i = 0 .. n: arithmetic lower + i * step, step = (upper - lower) / n, exact IEEE
+ * float64 (no FMA contraction); geometric lower * pow(ratio, i), ratio = pow(upper / lower, 1 / n) with CUDA's pow, which
+ * may differ from the C library's by a few ulps.  near_ties counts the ticks on which a price compared with a geometric
+ * level lies within |L| * 2^-50 (<= 4 ulps) of it: only those ticks can decide a compare differently from the reference.
+ * Levels must be non-decreasing in i (true for finite lower <= upper); "volatility_based" draws random numbers and is not
+ * a grid type here.
+ *
+ * init_bounds (device float64 [pop][S][2]): the initial (lower, upper) of each lane, computed by the caller from the
+ * individual's boundary rule (fixed pcts or auto_boundaries' volatility of the daily closes, :266-289).  qty: device float64
+ * [S].  labels_or_null: device uint8 [S][ld_labels] bar labels (ld_labels = 0: one row for every symbol; B200BT_REGIME_*),
+ * regime_table_host_or_null: host [B200BT_GRID_REGIME_RULES] rules indexed by label (labels >= 5 change nothing).
+ * stats: device [pop][S].  day_profit_or_null: device float64 [pop][D]: row i, column d = the realised profit of
+ * individual i on calendar day first_day + d summed over its symbols 0..S-1 in that order (first_day = minute0 / 1440, the
+ * day of bar 0; a day is (minute0 + bar * bar_minutes) / 1440), b200bt_cscv's row shape; D >= day(N - 1) - first_day + 1.
+ * With day_profit the symbols of an individual run one after another in one warp; stats are the same either way.
+ * An individual outside the limits (num_grids 1 .. B200BT_GRID_MAX_GRIDS, grid_type 0 / 1, periods >= 1) gets NaN stats.
+ * Checked before the device: null pointers, sizes, start_bar in [0, N - 1], bar_minutes > 0, minute0 >= 0, ld_labels, D,
+ * the table's num_grids (all EINVAL); N >= 2^30 (ELIMIT).  Deterministic: no atomics. */
+#define B200BT_GRID_ARITHMETIC 0
+#define B200BT_GRID_GEOMETRIC 1
+#define B200BT_GRID_ADAPT_REGIME 1       /* adapt_to_market_regime                                          */
+#define B200BT_GRID_AUTO_BOUNDARIES 2    /* auto_boundaries: read by the host that makes init_bounds only   */
+#define B200BT_GRID_MAX_GRIDS 127
+#define B200BT_GRID_REGIME_RULES 5
+
+typedef struct b200bt_grid_individual {
+    int32_t num_grids;        /* service-wide num_grids at t0                                                     */
+    int32_t grid_type;        /* B200BT_GRID_ARITHMETIC / _GEOMETRIC                                              */
+    int32_t rebalance_ticks;  /* floor(rebalance_frequency / bar_seconds) + 1                                     */
+    int32_t adjust_ticks;     /* floor(auto_adjust_period / bar_seconds) + 1                                      */
+    int32_t flags;            /* B200BT_GRID_ADAPT_REGIME | B200BT_GRID_AUTO_BOUNDARIES                           */
+    int32_t reserved;
+    double lower_pct;         /* lower_boundary_pct: regenerations (and the initial grid without auto_boundaries)  */
+    double upper_pct;         /* upper_boundary_pct                                                               */
+} b200bt_grid_individual;     /* 40 bytes */
+
+typedef struct b200bt_grid_regime_rule {
+    int32_t apply;            /* 0: the label changes nothing                                                     */
+    int32_t num_grids;
+    double lower_pct;
+    double upper_pct;
+} b200bt_grid_regime_rule;    /* 24 bytes */
+
+/* Per-lane result: 20 float64 fields (160 bytes, the size of b200bt_lane_stats), so b200bt_objective_matrix averages any
+ * field 0..18 over the symbols unchanged. */
+typedef struct b200bt_grid_stats {
+    double total_profit;       /* grid_profits[symbol]['total_profit'] (order of float64 additions may differ)          */
+    double total_trades;       /* up_crossings + down_crossings                                                         */
+    double profitable_trades;
+    double win_rate;           /* profitable / total, 0 without trades (_update_performance_metrics :941-958)           */
+    double profit_per_day;     /* total_profit / ((t_last - t0) in days), 0 when T = 1 (:951)                           */
+    double up_crossings;
+    double down_crossings;
+    double n_regenerations;    /* rebalance checks that regenerated the grid                                            */
+    double num_grids;          /* the service's num_grids at the end                                                    */
+    double lower;              /* the active grid's boundaries at the end                                               */
+    double upper;
+    /* beyond the reference: the simulated fills marked to market.  A down-crossing buys qty at the level, an up-crossing
+     * sells qty at the level; the reference's profit ignores the inventory this accumulates and never goes negative. */
+    double cash;               /* sum of +-level * qty                                                                  */
+    double position;           /* (down - up crossings) * qty                                                           */
+    double mark_to_market;     /* cash + position * last close                                                          */
+    double max_position;       /* largest and smallest position after any tick (0 at t0)                                */
+    double min_position;
+    double n_rebalance_checks;
+    double n_adjustments;
+    double n_ticks;            /* T                                                                                     */
+    double near_ties;          /* see above; 0 on arithmetic grids                                                      */
+} b200bt_grid_stats;           /* 160 bytes */
+
+int b200bt_grid_sweep(const float* price, int64_t ld_price, int S, int64_t N, int64_t start_bar, int bar_minutes,
+                      int64_t minute0, const b200bt_grid_individual* indiv, int pop, const double* qty,
+                      const double* init_bounds, const uint8_t* labels_or_null, int64_t ld_labels,
+                      const b200bt_grid_regime_rule* regime_table_host_or_null, b200bt_grid_stats* stats,
+                      double* day_profit_or_null, int64_t D, b200bt_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
