@@ -78,6 +78,26 @@ class GridRegimeRule(C.Structure):
     _fields_ = [("apply", C.c_int32), ("num_grids", C.c_int32), ("lower_pct", C.c_double), ("upper_pct", C.c_double)]
 
 
+class DcaIndividual(C.Structure):
+    """b200bt_dca_individual: one DCA parameter set as the host's lookup tables (dca.py)."""
+    _fields_ = [
+        ("later_us", (C.c_int64 * 2) * 5 * 2), ("order", (C.c_double * 2) * 2 * 2), ("dip_threshold_pct", C.c_double),
+        ("max_deviation_pct", C.c_double), ("dip_cooldown_minutes", C.c_int64), ("rebalance_first", C.c_int64),
+        ("rebalance_period", C.c_int64), ("flags", C.c_int32), ("reserved", C.c_int32),
+    ]
+
+
+DCA_STATS_FIELDS = (
+    "total_invested", "total_quantity", "average_price", "current_value", "profit_loss", "profit_loss_pct",
+    "n_scheduled", "n_dip", "n_rebalance", "order_usdc", "last_purchase_price", "last_purchase_tick",
+    "next_scheduled_us", "last_dip_tick", "n_zero_quantity", "n_rebalance_checks", "min_day_profit_loss",
+    "purchase_hash", "n_ticks", "reserved",
+)                                                                     # b200bt_dca_stats, 160 bytes
+DCA_SERVICE_FIELDS = ("total_purchases", "total_invested", "total_value", "total_profit", "total_profit_pct")
+DCA_DIP = 1
+DCA_REBALANCE = 2
+DCA_MAX_COUPLED = 32
+
 GRID_STATS_FIELDS = (
     "total_profit", "total_trades", "profitable_trades", "win_rate", "profit_per_day", "up_crossings", "down_crossings",
     "n_regenerations", "num_grids", "lower", "upper", "cash", "position", "mark_to_market", "max_position",
@@ -210,6 +230,10 @@ _SIGNATURES = {
                                      _vp, _vp]),
     "b200bt_grid_sweep": (C.c_int, [_vp, _i64, _i, _i64, _i64, _i, _i64, _vp, _i, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _i64,
                                     _vp]),
+    "b200bt_dca_dip_pct": (C.c_int, [_vp, _vp, _i64, _i, _i64, _i64, _i, _vp, _i64, _vp]),
+    "b200bt_dca_workspace_bytes": (C.c_int64, [_i, _i64]),
+    "b200bt_dca_sweep": (C.c_int, [_vp, _i64, _vp, _i64, _i, _i64, _i64, _i, _i64, _vp, _i64, _vp, _vp, _i, _i, _vp, _vp,
+                                   _vp, _i64, C.c_double, _vp, _vp, _vp, _i64, _vp]),
     "b200bt_pct_change": (C.c_int, [_vp, _i64, _i, _i64, _vp, _i64, _vp]),
     "b200bt_tail_stats_workspace_bytes": (C.c_int64, [_i64]),
     "b200bt_tail_stats": (C.c_int, [_vp, _i64, C.c_double, _vp, _vp, _i64, _vp]),

@@ -821,6 +821,125 @@ int b200bt_grid_sweep(const float* price, int64_t ld_price, int S, int64_t N, in
                       const b200bt_grid_regime_rule* regime_table_host_or_null, b200bt_grid_stats* stats,
                       double* day_profit_or_null, int64_t D, b200bt_stream_t stream);
 
+/* ---- dollar-cost averaging (csrc/dca.cu) --------------------------------------------------------------------------
+ * A backtest of services/dca_strategy.py's DCAStrategy, whose only evaluation is "simulation mode": the live loop of run()
+ * (:140-239) against the exchange ticker.  Here one individual is ONE service instance trading all S symbols of a market
+ * (the rebalance couples them), run over the market's bars.  Every float64 operation of the reference happens in a fixed
+ * order within an individual, and the kernel performs the same operations in the same order with explicit _rn
+ * intrinsics (no FMA contraction): every output field is bit-exact.
+ *
+ * Clock: tick k = 0 .. T - 1 is bar start_bar + k (T = N - start_bar); its time is the bar's start minute m, its price the
+ * bar's close widened to float64, its weekday that of its UTC day ((m / 1440 + 3) % 7, Monday = 0; the reference reads the
+ * naive local clock).  One tick per bar stands in for update_interval.  __init__ and _initialize_dca_strategy (:241-320)
+ * run at tick 0: last_rebalance = t0 - rebalance_interval_days (:124), and each symbol's first next_scheduled_buy is
+ * _calculate_next_purchase_time at t0.  On every tick, tick 0 included, in this order:
+ *   1. _process_dca (:452-501) for each symbol in order: a scheduled purchase when now >= next_scheduled_buy, then
+ *      next_scheduled_buy = now + interval (_calculate_next_purchase_time :347-450).  _check_market_conditions always
+ *      proceeds (nothing in the reference writes market_volatility or market_sentiment to Redis).  The interval:
+ *        with adaptive_scheduling and a non-empty market_regime_based dict, the tick's label picks bull_ / bear_ /
+ *        volatile_interval_hours (crab_ never fires: b200bt_regime_labels emits ranging, not crab; ranging, unknown,
+ *        labels >= 5 and no label source leave it unchanged);
+ *        with adaptive_scheduling and weighted_scheduling, it is multiplied by 1 + 0.2 * day_of_week_weight on Saturday
+ *        and Sunday and clamped to [0.5, 1.5] x itself; the volatility and sentiment factors stay 1 (no data source);
+ *        timedelta(hours=x) rounds it to microseconds; the purchase fires on the first later tick whose time is >= next.
+ *   2. The rebalance check (:191-200): (now - last_rebalance).days >= R, with last_rebalance = now whenever it runs: tick 0,
+ *      then every ceil(R * 1440 / bar_minutes) ticks (every tick for R <= 0).  _rebalance_portfolio, simulation branch
+ *      (:864-1021): v_s = Q_s * p_s after step 1, total = (v_0 + ... + v_{S-1}) + usdc_balance, alloc_s = v_s / total
+ *      (0 when total <= 0); symbol s buys total * target_s - v_s USDC when |(alloc_s - target_s) / target_s| * 100 >
+ *      max_deviation_pct (0 when target_s <= 0) and v_s < total * target_s.  All decisions precede the buys, which go
+ *      through _update_position_after_purchase with no clamp and no effect on last_purchases or the dip state.
+ *   3. _check_for_dips (:817-862) for each symbol in order, with price_dip_detection: skipped while (now - last
+ *      dip).days < max_dip_frequency_days; otherwise a dip purchase when dip_pct[s][bar] >= dip_threshold_pct (NaN never).
+ * A purchase (_execute_dca_purchase :548-649, _calculate_adjusted_order_size :651-740, _update_position_after_purchase
+ * :742-802): order = base, * (1 + additional_dip_allocation) for a dip, * bear_market_adjustment when
+ * increase_in_bear_market and the tick's label is bear, clamped to [min_order, max_order] (the host's table);
+ * q = floor(order / p * 10^prec) / 10^prec; invested += p * q; quantity += q; average = invested / quantity.  The service's
+ * own total_invested adds the order, not p * q (the stats' order_usdc).
+ * Mirrored quirks (the host's tables carry them): _get_symbol_specific_settings (:322-345) REPLACES symbols_config per
+ * symbol, so after initialisation only the LAST symbol keeps its symbol_settings: each symbol's first interval uses its own
+ * interval_hours, later intervals, base orders and rebalance targets use the global values (1 / S) for every symbol but
+ * the last.  _get_quantity_precision (:1094-1100) counts the decimals of str(float(stepSize)): a step of 1e-05 prints in
+ * scientific notation and gives precision 0.  The service never sells; take_profit_*, stop_loss_*, schedule_type,
+ * weekly / monthly_dca_day, total_allocation, auto_adjust_order_size and value_averaging are read and never used.  The USDC
+ * balance (get_account) is constant: simulation mode places no orders.
+ *
+ * b200bt_dca_dip_pct: dip_pct [S][ld_dip] float64, the market-only series of step 3: at bar b (minute m) the klines are
+ * the UTC days whose start is >= m - 7 days and that hold a bar with start <= m, each day's high the max high of those bars
+ * (the current day is partial); with fewer than 2 klines, or a recent high of 0 (ZeroDivisionError, caught), NaN; else
+ * ((H - close) / H) * 100 with H the max of the day highs.  Per-day prefix maxima plus the previous whole days: O(N).
+ * b200bt_dca_sweep: workspace >= b200bt_dca_workspace_bytes(S, N) bytes of device memory (block maxima of dip_pct over 32,
+ * 1 024 and 32 768 bars, rebuilt on every call: a lane skips every block below its threshold).  indiv: device [pop];
+ * first_us: device int64 [pop][S][5][2], each symbol's first interval indexed [label][weekend]; target, pow10: device
+ * float64 [S], the rebalance targets and 10^precision.  labels_or_null as b200bt_grid_sweep.  rebalance_any: nonzero when
+ * some individual has B200BT_DCA_REBALANCE (an individual with it gets NaN stats otherwise).  stats: device [pop][S];
+ * service_or_null: device [pop]; day_or_null: device float64 [pop][D]: row d = the change of sum_s (Q_s * c_s - I_s)
+ * between the last ticks of calendar days first_day + d - 1 and first_day + d, the symbols' changes added in order (the
+ * value before tick 0 is 0; days before the start tick's day are 0), b200bt_cscv's row shape; D as b200bt_grid_sweep.
+ * One CTA per individual and one warp per symbol; the warps meet at rebalance ticks (and day ends with day rows) only.
+ * Checked before the device: null pointers, sizes, ld, start_bar in [0, N - 1], bar_minutes > 0, minute0 >= 0 and the
+ * clock in microseconds < 2^62, ld_labels, D, the workspace size (EINVAL); N >= 2^30, and S > 32 with rebalance_any or
+ * day rows (ELIMIT).  Deterministic: no atomics. */
+#define B200BT_DCA_DIP 1                 /* price_dip_detection                                              */
+#define B200BT_DCA_REBALANCE 2           /* periodic_rebalancing.enabled                                     */
+#define B200BT_DCA_MAX_COUPLED 32        /* symbols of one individual that meet at a rebalance / day end     */
+
+typedef struct b200bt_dca_individual {
+    int64_t later_us[2][5][2];    /* interval after a scheduled purchase, us: [last symbol?][label][weekend]            */
+    double order[2][2][2];        /* clamped order size, USDC: [last symbol?][dip?][bear?]                              */
+    double dip_threshold_pct;
+    double max_deviation_pct;     /* periodic_rebalancing.max_deviation_pct                                             */
+    int64_t dip_cooldown_minutes; /* ceil(max_dip_frequency_days) * 1440, 0 = none                                      */
+    int64_t rebalance_first;      /* tick of the first rebalance (0)                                                    */
+    int64_t rebalance_period;     /* ticks between rebalances, >= 1                                                     */
+    int32_t flags;                /* B200BT_DCA_DIP | B200BT_DCA_REBALANCE                                              */
+    int32_t reserved;
+} b200bt_dca_individual;          /* 272 bytes */
+
+/* Per-lane result: 20 float64 fields (160 bytes), so b200bt_objective_matrix averages any field unchanged. */
+typedef struct b200bt_dca_stats {
+    double total_invested;        /* dca_positions[symbol] at the last tick (:253-264)                                  */
+    double total_quantity;
+    double average_price;
+    double current_value;         /* Q * last close                                                                     */
+    double profit_loss;
+    double profit_loss_pct;
+    double n_scheduled;           /* purchases by kind                                                                  */
+    double n_dip;
+    double n_rebalance;
+    double order_usdc;            /* sum of the clamped orders of the scheduled and dip purchases, in time order        */
+    double last_purchase_price;   /* 0 without a purchase                                                               */
+    double last_purchase_tick;    /* of any kind; -1 without                                                            */
+    double next_scheduled_us;     /* next_scheduled_buy - t0 in microseconds                                            */
+    double last_dip_tick;         /* -1 without                                                                         */
+    /* beyond the reference */
+    double n_zero_quantity;       /* purchases whose quantity rounded to 0                                              */
+    double n_rebalance_checks;
+    double min_day_profit_loss;   /* lowest Q * c - I at the last tick of a day                                         */
+    double purchase_hash;         /* xor over the purchases of fmix32(4 * tick + kind) (MurmurHash3's finaliser, 32-bit), kind
+                                   * 0 scheduled, 1 dip, 2 rebalance                                                    */
+    double n_ticks;               /* T                                                                                  */
+    double reserved;
+} b200bt_dca_stats;               /* 160 bytes */
+
+/* _update_performance_metrics (:1023-1092) at the last tick, the symbols summed in order. */
+typedef struct b200bt_dca_service {
+    double total_purchases;       /* scheduled + dip purchases (rebalance buys do not count, :640-642)                  */
+    double total_invested;
+    double total_value;
+    double total_profit;
+    double total_profit_pct;
+} b200bt_dca_service;             /* 40 bytes */
+
+int b200bt_dca_dip_pct(const float* high, const float* close, int64_t ld, int S, int64_t N, int64_t minute0,
+                       int bar_minutes, double* dip_pct, int64_t ld_dip, b200bt_stream_t stream);
+int64_t b200bt_dca_workspace_bytes(int S, int64_t N);
+int b200bt_dca_sweep(const float* close, int64_t ld_close, const double* dip_pct, int64_t ld_dip, int S, int64_t N,
+                     int64_t start_bar, int bar_minutes, int64_t minute0, void* workspace, int64_t workspace_bytes,
+                     const b200bt_dca_individual* indiv, const int64_t* first_us, int pop, int rebalance_any,
+                     const double* target, const double* pow10, const uint8_t* labels_or_null, int64_t ld_labels,
+                     double usdc_balance, b200bt_dca_stats* stats, b200bt_dca_service* service_or_null,
+                     double* day_or_null, int64_t D, b200bt_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

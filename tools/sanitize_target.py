@@ -19,7 +19,7 @@ from ai_crypto_trader_b200.monte_carlo import PathEngine, risk_statistics
 from ai_crypto_trader_b200.sweep import MarketData, PopulationSweep
 from oracle import indicators_ref, sim_oracle
 
-legs = sys.argv[1:] or ["sweep", "mc", "joint", "indicators", "pareto", "regime"]
+legs = sys.argv[1:] or ["sweep", "mc", "joint", "indicators", "pareto", "regime", "dca"]
 torch.cuda.set_device(0)
 
 if "sweep" in legs:
@@ -116,5 +116,31 @@ if "regime" in legs:
                 assert views[r]["n_records"][i, s] == want[r]["n_records"]
                 assert int(views[r]["trade_hash"][i, s]) == int(want[r]["trade_hash"])
     print("regime ok: labels equal the restatement,", S * POP, "lanes x 5 classes match the oracle", flush=True)
+if "dca" in legs:
+    # DCA: the drop series, the pyramid search, the rebalance and day-end barriers (S = 3) and the grouped CTA (S = 33)
+    import random as _random
+    sys.path.insert(0, str(Path(__file__).resolve().parents[1] / "tests"))
+    import dca_ref
+    from ai_crypto_trader_b200.dca import DCASweep, dca_param_ranges, decode_individual
+    rng = _random.Random(5)
+    pop = [{k: (rng.randint(lo, hi) if isinstance(lo, int) else rng.uniform(lo, hi))
+            for k, (lo, hi) in dca_param_ranges().items()} for _ in range(12)]
+    for S, N, reb in ((3, 12 * 1440, 1), (33, 3 * 288, 0)):
+        ohlcv = synth.synth_ohlcv(S, N)
+        ohlcv[1] = np.maximum(ohlcv[1], ohlcv[3])
+        m = MarketData(ohlcv, bar_minutes=1 if S == 3 else 5)
+        p = [dict(x, periodic_rebalancing=reb, rebalance_interval_days=1) for x in pop]
+        sw = DCASweep(m, start_bar=N // 8, usdc_balance=900.0)
+        st = sw.dca_stats(p)
+        if reb:
+            sw.day_pnl(p)
+        for i in range(0, len(p), 5):
+            want = dca_ref.simulate(m.close.cpu().numpy().astype(np.float64), sw.dip.cpu().numpy(), m.minute0,
+                                    m.bar_minutes, sw.start_bar, decode_individual(p[i], {}, m.symbols, m.bar_minutes),
+                                    usdc_balance=900.0)
+            for s in range(S):
+                assert st["purchase_hash"][i, s] == want["stats"][s]["purchase_hash"], (S, i, s)
+        print("dca ok: S =", S, flush=True)
+
 torch.cuda.synchronize()
 print("sanitize target done")
