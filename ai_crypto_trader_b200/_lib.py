@@ -103,6 +103,10 @@ GRID_STATS_FIELDS = (
     "n_regenerations", "num_grids", "lower", "upper", "cash", "position", "mark_to_market", "max_position",
     "min_position", "n_rebalance_checks", "n_adjustments", "n_ticks", "near_ties",
 )                                                                     # b200bt_grid_stats, 160 bytes
+GRID_SERVICE_FIELDS = (
+    "total_profit", "total_trades", "profitable_trades", "win_rate", "profit_per_day", "num_grids", "lower_pct",
+    "upper_pct", "n_adjustments", "n_num_grids_changes", "min_num_grids", "max_num_grids",
+)                                                                     # b200bt_grid_service_stats, 96 bytes
 GRID_ADAPT_REGIME = 1
 GRID_AUTO_BOUNDARIES = 2
 GRID_MAX_GRIDS = 127
@@ -230,6 +234,8 @@ _SIGNATURES = {
                                      _vp, _vp]),
     "b200bt_grid_sweep": (C.c_int, [_vp, _i64, _i, _i64, _i64, _i, _i64, _vp, _i, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _i64,
                                     _vp]),
+    "b200bt_grid_service_sweep": (C.c_int, [_vp, _i64, _i, _i64, _i64, _i, _i64, _vp, _i, _vp, _vp, _vp, _i64, _vp, _vp,
+                                            _vp, _vp, _i64, _vp]),
     "b200bt_dca_dip_pct": (C.c_int, [_vp, _vp, _i64, _i, _i64, _i64, _i, _vp, _i64, _vp]),
     "b200bt_dca_workspace_bytes": (C.c_int64, [_i, _i64]),
     "b200bt_dca_sweep": (C.c_int, [_vp, _i64, _vp, _i64, _i, _i64, _i64, _i, _i64, _vp, _i64, _vp, _vp, _i, _i, _vp, _vp,

@@ -4,7 +4,10 @@ Reference: services/grid_trading_strategy.py (GridTradingStrategy).  The referen
 "simulation mode": its live loop run() (:122-233) against the exchange ticker, once per update_interval, for as long as
 one waits.  Here one (individual, symbol) lane is one symbol's service instance run over history by b200bt_grid_sweep
 (csrc/grid.cu; the rule restated in include/b200bt.h and DESIGN.md section 3.13): a tick per bar, the bar's close as the
-ticker price, the rebalance and adjustment checks on the ticks the reference's clock arithmetic gives them.
+ticker price, the rebalance and adjustment checks on the ticks the reference's clock arithmetic gives them.  With
+service=True one individual is instead ONE service instance trading all of the market's symbols, as the reference runs
+one instance for its configured symbols (b200bt_grid_service_sweep): num_grids and the pcts are the instance's, and every
+symbol's adjustment mutates them in symbol order.
 
     grid_param_ranges()      genes of the config keys the service reads (grid type as an index, booleans as 0 / 1)
     GridSweep                population fitness / stats / objectives / per-day profit rows on the device
@@ -21,6 +24,7 @@ from __future__ import annotations
 import ctypes as C
 import logging
 import math
+import os
 from datetime import datetime, timedelta, timezone
 from typing import Dict, List, Optional, Sequence, Tuple, Union
 
@@ -34,6 +38,7 @@ logger = logging.getLogger("b200bt.grid")
 FIELDS = _lib.GRID_STATS_FIELDS
 WORDS = len(FIELDS)
 OBJECTIVE_FIELDS = FIELDS[:-1]          # near_ties describes the arithmetic, not the strategy
+SERVICE_FIELDS = _lib.GRID_SERVICE_FIELDS
 GRID_TYPES = _lib.GRID_TYPES
 MAX_TICKS = (1 << 31) - 1
 
@@ -178,12 +183,17 @@ class GridSweep:
     config      config.json dict or its grid_trading block: defaults of the keys an individual does not set, the
                 per-regime keys and the quantities
     objective   the stats field evaluate() averages over the symbols (default total_profit)
+    service     False: one service per (individual, symbol) lane (b200bt_grid_sweep).  True: one service instance per
+                individual trading all symbols, num_grids and pcts coupled across them (b200bt_grid_service_sweep); the
+                regime source is then one label row: regime=True labels the market by PRIMARY_TRADING_SYMBOL (environment,
+                default BTCUSDC), which must be one of the market's symbols, and per-symbol label rows are refused.
 
     Individuals that decode alike (same kernel fields and initial boundaries) are evaluated once."""
 
     def __init__(self, market, quantity: Union[None, float, Sequence[float]] = None, start_bar: Optional[int] = None,
-                 regime=None, config: Optional[Dict] = None, objective: str = "total_profit"):
+                 regime=None, config: Optional[Dict] = None, objective: str = "total_profit", service: bool = False):
         self.market = market
+        self.service = bool(service)
         self.block = grid_block(config)
         self.defaults = {k: self.block.get(k, v) for k, v in DEFAULTS.items()}
         S, N = market.S, market.N
@@ -204,13 +214,22 @@ class GridSweep:
         self.start_bar = int(start_bar)
         if regime is True:
             from .regime import regime_labels
-            regime = regime_labels(market)[0]
+            if self.service:
+                primary = os.getenv("PRIMARY_TRADING_SYMBOL", "BTCUSDC")
+                if primary not in market.symbols:
+                    raise ValueError(f"regime=True in service mode labels the market by PRIMARY_TRADING_SYMBOL = "
+                                     f"{primary!r}, which is not one of the market's symbols {market.symbols}")
+                regime = regime_labels(market, primary=primary)[0]
+            else:
+                regime = regime_labels(market)[0]
         self.labels, self.ld_labels = None, 0
         if regime is not None:
             if not (isinstance(regime, torch.Tensor) and regime.is_cuda and regime.dtype == torch.uint8 and
                     regime.dim() == 2 and regime.shape[0] in (1, S) and regime.shape[1] == N):
                 raise ValueError(f"regime labels must be a device uint8 tensor [{S} or 1][{N}]")
             shared = regime.shape[0] == 1 or regime.stride(0) == 0
+            if self.service and not shared:
+                raise ValueError("service mode reads one regime label row (market_regime_history): pass [1][N] labels")
             self.labels = regime[:1].contiguous() if shared else regime.contiguous()
             self.ld_labels = 0 if shared else N
         self.table = regime_table(self.block)
@@ -219,6 +238,7 @@ class GridSweep:
         self._closes = None                      # host closes up to the start bar (auto boundaries)
         self._vol_cache: Dict[Tuple[int, int], List[float]] = {}
         self._stats = None
+        self._service = None
         self._inverse = None
 
     @staticmethod
@@ -279,11 +299,20 @@ class GridSweep:
         first_day, D = self.calendar_days()
         rows = torch.empty((U, D), dtype=torch.float64, device=m.device) if day else None
         close = m.close
+        table = self.table if self.labels is not None else None
         with torch.cuda.device(m.device):
-            _lib.call("b200bt_grid_sweep", close.data_ptr(), _lib.ld(close), m.S, m.N, self.start_bar, m.bar_minutes,
-                      m.minute0, indiv.data_ptr(), U, self._qty.data_ptr(), bnd.data_ptr(), _lib.ptr(self.labels),
-                      self.ld_labels, self.table if self.labels is not None else None, stats.data_ptr(),
-                      _lib.ptr(rows), D if day else 0, _lib.current_stream())
+            if self.service:
+                service = torch.empty((U, len(SERVICE_FIELDS)), dtype=torch.float64, device=m.device)
+                _lib.call("b200bt_grid_service_sweep", close.data_ptr(), _lib.ld(close), m.S, m.N, self.start_bar,
+                          m.bar_minutes, m.minute0, indiv.data_ptr(), U, self._qty.data_ptr(), bnd.data_ptr(),
+                          _lib.ptr(self.labels), self.ld_labels, table, stats.data_ptr(), service.data_ptr(),
+                          _lib.ptr(rows), D if day else 0, _lib.current_stream())
+                self._service = service
+            else:
+                _lib.call("b200bt_grid_sweep", close.data_ptr(), _lib.ld(close), m.S, m.N, self.start_bar, m.bar_minutes,
+                          m.minute0, indiv.data_ptr(), U, self._qty.data_ptr(), bnd.data_ptr(), _lib.ptr(self.labels),
+                          self.ld_labels, table, stats.data_ptr(), _lib.ptr(rows), D if day else 0,
+                          _lib.current_stream())
         self._stats = stats
         self._inverse = None if U == len(population) else inverse
         return stats, rows
@@ -332,6 +361,18 @@ class GridSweep:
             raise RuntimeError("nothing evaluated yet")
         raw = self._expand(self._stats).cpu().numpy()
         return {name: raw[:, :, f] for f, name in enumerate(FIELDS)}
+
+    def service_stats(self, population: Optional[List[Dict]] = None) -> Dict[str, np.ndarray]:
+        """Service mode: dict field -> [pop] float64 of b200bt_grid_service_stats (the reference's grid_performance plus
+        the service's final num_grids / pcts and its adjustment counts) of `population` or of the last evaluation."""
+        if not self.service:
+            raise RuntimeError("service_stats() needs GridSweep(..., service=True)")
+        if population is not None:
+            self._run(population)
+        if self._service is None:
+            raise RuntimeError("nothing evaluated yet")
+        raw = self._expand(self._service).cpu().numpy()
+        return {name: raw[:, f] for f, name in enumerate(SERVICE_FIELDS)}
 
     def stats_device(self) -> torch.Tensor:
         """The last evaluation's stats float64 [pop][S][20] on the device, in population order."""
@@ -393,4 +434,40 @@ class GridTradingStrategy:
             }
         except Exception as e:
             logger.error("Error backtesting grid for %s: %s", symbol, e)
+            return None
+
+    def backtest_service(self, market, params: Optional[Dict] = None, start_bar: Optional[int] = None,
+                         regime=None) -> Optional[Dict]:
+        """Run ONE service instance on all of the market's symbols (the reference's multi-symbol service, num_grids and
+        pcts shared) with `params` over the market's bars from start_bar.  Returns {"grid_profits": {symbol: the
+        reference's grid_profits[symbol] without last_trade_profit}, "performance": grid_performance (:941-958) at the
+        last tick, "service": the final num_grids / pcts and the adjustment counts, "grid": {symbol: the final grid},
+        "stats": {symbol: every b200bt_grid_stats field}}.  Errors are logged and give None."""
+        try:
+            sweep = GridSweep(market, start_bar=start_bar, regime=regime, config=self.grid_config, service=True)
+            st = sweep.grid_stats([dict(params or {})])
+            sv = {k: float(a[0]) for k, a in sweep.service_stats().items()}
+            t0 = market.minute0 + sweep.start_bar * market.bar_minutes
+            t1 = market.minute0 + (market.N - 1) * market.bar_minutes
+            lanes = {sym: {k: float(a[0, s]) for k, a in st.items()} for s, sym in enumerate(market.symbols)}
+            return {
+                "grid_profits": {sym: {"total_profit": v["total_profit"], "total_trades": int(v["total_trades"]),
+                                       "profitable_trades": int(v["profitable_trades"]), "start_time": _iso(t0)}
+                                 for sym, v in lanes.items()},
+                "performance": {"timestamp": _iso(t1), "start_time": _iso(t0), "running_time_hours": (t1 - t0) * 60 / 3600,
+                                "total_trades": int(sv["total_trades"]), "profitable_trades": int(sv["profitable_trades"]),
+                                "win_rate": sv["win_rate"], "total_profit": sv["total_profit"],
+                                "profit_per_day": sv["profit_per_day"], "symbols": list(market.symbols),
+                                "simulation_mode": True,
+                                "symbol_profits": {sym: v["total_profit"] for sym, v in lanes.items()}},
+                "service": {"num_grids": int(sv["num_grids"]), "lower_boundary_pct": sv["lower_pct"],
+                            "upper_boundary_pct": sv["upper_pct"], "n_adjustments": int(sv["n_adjustments"]),
+                            "n_num_grids_changes": int(sv["n_num_grids_changes"]),
+                            "min_num_grids": int(sv["min_num_grids"]), "max_num_grids": int(sv["max_num_grids"])},
+                "grid": {sym: {"num_grids": int(v["num_grids"]), "lower_boundary": v["lower"],
+                               "upper_boundary": v["upper"]} for sym, v in lanes.items()},
+                "stats": lanes,
+            }
+        except Exception as e:
+            logger.error("Error backtesting the grid service: %s", e)
             return None

@@ -720,7 +720,7 @@ int b200bt_class_stats(const float* price, int64_t ld_price, int S, int64_t N, c
  * A backtest of services/grid_trading_strategy.py's GridTradingStrategy, whose only evaluation is "simulation mode": the
  * live loop of run() (:122-233) against the exchange ticker.  Here every (individual, symbol) lane is ONE symbol's service
  * instance run over a market's bars (the reference keeps num_grids and the pcts service-wide, so a multi-symbol service
- * couples its symbols at each adjustment; that coupled form is not modelled).
+ * couples its symbols at each adjustment; that coupled form is b200bt_grid_service_sweep below).
  *
  * Clock: tick k = 0 .. T - 1 is bar start_bar + k (T = N - start_bar); its price is the bar's close widened to float64.
  * __init__ / _initialize_grid (:245-345) run at tick 0: start_time, last_rebalance and last_adjustment are t0.  On every tick,
@@ -820,6 +820,51 @@ int b200bt_grid_sweep(const float* price, int64_t ld_price, int S, int64_t N, in
                       const double* init_bounds, const uint8_t* labels_or_null, int64_t ld_labels,
                       const b200bt_grid_regime_rule* regime_table_host_or_null, b200bt_grid_stats* stats,
                       double* day_profit_or_null, int64_t D, b200bt_stream_t stream);
+
+/* The coupled multi-symbol service: one individual is ONE service instance trading all S symbols of the market, as run()
+ * (:160-206) runs one instance for every configured symbol (config.json's grid_trading.symbols).  num_grids,
+ * lower_boundary_pct and upper_boundary_pct are fields of the instance (:72-78), so they are per individual, not per lane.
+ * The rule is b200bt_grid_sweep's with these differences:
+ *   Every symbol initialises at tick 0, so all lanes of an individual share the check ticks.  On an adjust tick the loop
+ *   body runs (:166-198): the crossings of every symbol, then every symbol's rebalance check (a regeneration uses the
+ *   service's values before this tick's adjustment, :809-816), then _adjust_grid_parameters(symbol) (:840-905) for
+ *   symbols 0 .. S-1 in order, each MUTATING the shared fields: the regime rule of the tick's label (absolute values),
+ *   then the win-rate rule on that symbol's own grid_profits counts (total_trades > 10; < 0.4 gives max(5, n - 2),
+ *   > 0.7 gives min(20, n + 2)).  So when the regime rule fires, only the last symbol's win rate survives it; without
+ *   it, the +-2 steps of all symbols add up.
+ *   Labels: the reference reads ONE key (market_regime_history), so labels_or_null is one row shared by every symbol
+ *   (ld_labels = 0); per-symbol rows are EINVAL.  Labels >= 5 change nothing, as before.
+ * stats: device [pop][S] in b200bt_grid_stats' layout (b200bt_objective_matrix reads it unchanged); num_grids, lower and
+ * upper are the lane's final grid, n_adjustments the service's.  service_or_null: device [pop].  day_profit_or_null as
+ * b200bt_grid_sweep (symbols 0 .. S-1 added in that order).  Counts, regeneration ticks, final grids and the service's
+ * num_grids are exact on lanes without geometric near ties; profit sums differ from the reference only by the order of
+ * float64 additions (a lane's sums are reduced over its warp at every adjust tick).  With S = 1, or with adjust_ticks >= T,
+ * the lanes are b200bt_grid_sweep's lanes (bit-equal when adjust_ticks >= T).
+ * Schedule: one CTA per individual, min(S, 16) warps, warp w running symbols w, w + W, ... between two adjust ticks, where
+ * the warps meet and thread 0 applies the S rule pairs in order; with day rows one warp runs every symbol in order.
+ * An individual outside the limits gets NaN stats and a NaN service record.  Checked before the device: as
+ * b200bt_grid_sweep, plus labels_or_null with ld_labels != 0 (EINVAL).  Deterministic: no atomics. */
+typedef struct b200bt_grid_service_stats {
+    double total_profit;        /* grid_performance (:941-958): the lanes' total_profit summed in symbol order          */
+    double total_trades;
+    double profitable_trades;
+    double win_rate;            /* profitable / total, 0 without trades                                                  */
+    double profit_per_day;      /* total_profit / ((t_last - t0) in days), 0 when T = 1                                  */
+    double num_grids;           /* the service's num_grids, lower_boundary_pct and upper_boundary_pct at the end          */
+    double lower_pct;
+    double upper_pct;
+    double n_adjustments;       /* adjust ticks                                                                          */
+    double n_num_grids_changes; /* adjust ticks after which num_grids differs from its value before them                 */
+    double min_num_grids;       /* smallest and largest value num_grids took (t0 and after every rule, within a tick too)  */
+    double max_num_grids;
+} b200bt_grid_service_stats;    /* 96 bytes */
+
+int b200bt_grid_service_sweep(const float* price, int64_t ld_price, int S, int64_t N, int64_t start_bar, int bar_minutes,
+                              int64_t minute0, const b200bt_grid_individual* indiv, int pop, const double* qty,
+                              const double* init_bounds, const uint8_t* labels_or_null, int64_t ld_labels,
+                              const b200bt_grid_regime_rule* regime_table_host_or_null, b200bt_grid_stats* stats,
+                              b200bt_grid_service_stats* service_or_null, double* day_profit_or_null, int64_t D,
+                              b200bt_stream_t stream);
 
 /* ---- dollar-cost averaging (csrc/dca.cu) --------------------------------------------------------------------------
  * A backtest of services/dca_strategy.py's DCAStrategy, whose only evaluation is "simulation mode": the live loop of run()

@@ -19,7 +19,7 @@ from ai_crypto_trader_b200.monte_carlo import PathEngine, risk_statistics
 from ai_crypto_trader_b200.sweep import MarketData, PopulationSweep
 from oracle import indicators_ref, sim_oracle
 
-legs = sys.argv[1:] or ["sweep", "mc", "joint", "indicators", "pareto", "regime", "dca"]
+legs = sys.argv[1:] or ["sweep", "mc", "joint", "indicators", "pareto", "regime", "dca", "grid_service"]
 torch.cuda.set_device(0)
 
 if "sweep" in legs:
@@ -141,6 +141,31 @@ if "dca" in legs:
             for s in range(S):
                 assert st["purchase_hash"][i, s] == want["stats"][s]["purchase_hash"], (S, i, s)
         print("dca ok: S =", S, flush=True)
+if "grid_service" in legs:
+    # the coupled grid service: adjust-tick barriers, lane state kept in the stats records, symbol rounds (S = 17), day rows
+    import random as _random
+    sys.path.insert(0, str(Path(__file__).resolve().parents[1] / "tests"))
+    import grid_service_ref
+    from ai_crypto_trader_b200.grid import GridSweep, decode_individual
+    rng = _random.Random(6)
+    pop = [{"num_grids": rng.randint(3, 30), "grid_type": 0, "auto_boundaries": 0, "lower_boundary_pct": rng.uniform(0.5, 3),
+            "upper_boundary_pct": rng.uniform(0.5, 3), "rebalance_frequency": rng.randint(60, 3600),
+            "auto_adjust_period": rng.randint(300, 7200), "adapt_to_market_regime": 0} for _ in range(6)]
+    for S in (3, 17):
+        m = MarketData(synth.synth_ohlcv(S, 2 * 1440))
+        sw = GridSweep(m, quantity=0.01, start_bar=100, service=True)
+        st = sw.grid_stats(pop)
+        sw.day_profit(pop)
+        for i in range(0, len(pop), 3):
+            d = decode_individual(pop[i], sw.defaults, 1)
+            _, bounds = sw.decode([pop[i]])
+            want = grid_service_ref.simulate_service(
+                m.close.cpu().numpy().astype(np.float64)[:, 100:], [tuple(bounds[0, s]) for s in range(S)],
+                d["num_grids"], 0, list(sw.quantity), d["lower_pct"], d["upper_pct"], d["rebalance_ticks"],
+                d["adjust_ticks"])
+            for s in range(S):
+                assert st["total_trades"][i, s] == want["lanes"][s]["total_trades"], (S, i, s)
+        print("grid_service ok: S =", S, flush=True)
 
 torch.cuda.synchronize()
 print("sanitize target done")
