@@ -112,6 +112,23 @@ GRID_AUTO_BOUNDARIES = 2
 GRID_MAX_GRIDS = 127
 GRID_TYPES = ("arithmetic", "geometric")                              # B200BT_GRID_* = index
 
+class RlAgent(C.Structure):
+    """b200bt_rl_agent: one agent's seed, symbol and hyperparameters."""
+    _fields_ = [
+        ("seed", C.c_uint64), ("symbol", C.c_int32), ("batch_size", C.c_int32), ("memory_size", C.c_int32),
+        ("update_target_every", C.c_int32), ("learning_rate", C.c_double), ("gamma", C.c_double),
+        ("epsilon_start", C.c_double), ("epsilon_end", C.c_double), ("epsilon_decay", C.c_double),
+    ]
+
+
+RL_STATE_DTYPE = [("initialized", "<i8"), ("n_transitions", "<i8"), ("replays", "<i8"), ("epsilon", "<f8"),
+                  ("act_words", "<u8"), ("sample_words", "<u8"), ("mean_q", "<f8"), ("reserved", "<i8")]
+                                                                      # b200bt_rl_agent_state, 64 bytes
+RL_FEATURES = 16
+RL_PARAMS = 1083
+RL_MAX_BATCH = 128
+RL_MAX_MEMORY = 1 << 20
+
 REGIMES = ("bull", "bear", "ranging", "volatile", "unknown")          # B200BT_REGIME_* = index
 REGIME_WINDOW_DTYPE = [("start_minute", "<i8"), ("n_points", "<i4"), ("label", "<i4"), ("volatility", "<f8"),
                        ("change_pct", "<f8"), ("mean_strength", "<f8"), ("up_frac", "<f8"), ("down_frac", "<f8"),
@@ -240,6 +257,9 @@ _SIGNATURES = {
     "b200bt_dca_workspace_bytes": (C.c_int64, [_i, _i64]),
     "b200bt_dca_sweep": (C.c_int, [_vp, _i64, _vp, _i64, _i, _i64, _i64, _i, _i64, _vp, _i64, _vp, _vp, _i, _i, _vp, _vp,
                                    _vp, _i64, C.c_double, _vp, _vp, _vp, _i64, _vp]),
+    "b200bt_rl_states": (C.c_int, [_vp, _vp, _vp, _i64, _i, _i64, _i, _vp, _vp]),
+    "b200bt_rl_workspace_bytes": (C.c_int64, [_i, _i]),
+    "b200bt_rl_train": (C.c_int, [_vp, _i, _i64, _vp, _i, _i64, _i, _vp, _i64, _vp, _i, _i, _vp, _vp, _vp, _vp, _i64, _vp]),
     "b200bt_pct_change": (C.c_int, [_vp, _i64, _i, _i64, _vp, _i64, _vp]),
     "b200bt_tail_stats_workspace_bytes": (C.c_int64, [_i64]),
     "b200bt_tail_stats": (C.c_int, [_vp, _i64, C.c_double, _vp, _vp, _i64, _vp]),

@@ -1,4 +1,5 @@
-// Philox4x32-10 counter-based RNG (Salmon et al., SC'11), shared by the Monte-Carlo kernels and the GA operators.
+// Philox4x32-10 counter-based RNG (Salmon et al., SC'11), shared by the Monte-Carlo kernels, the GA operators and the
+// reinforcement-learning agents.
 #pragma once
 #include <stdint.h>
 
@@ -56,6 +57,25 @@ struct BlockBootstrap {
         --left;
         return idx;
     }
+};
+
+// a stream of words for one (generation, slot, stream id): counter = (slot, generation, stream, block index); words
+// x[3], x[2], x[1], x[0] of block 0, then of block 1, ...
+struct GaRng {
+    uint32_t k0, k1, c0, c1, c2, blk, have;
+    uint32_t x[4];
+    __device__ GaRng(uint64_t seed, uint32_t generation, uint32_t slot, uint32_t stream)
+        : k0((uint32_t)seed), k1((uint32_t)(seed >> 32)), c0(slot), c1(generation), c2(stream), blk(0), have(0) {}
+    __device__ uint32_t next() {
+        if (have == 0) { philox4x32_10(c0, c1, c2, blk++, k0, k1, x); have = 4; }
+        return x[--have];
+    }
+    __device__ double uniform() {                      // [0,1), 53 bits: high 27 from the first word, low 26 from the second
+        const double hi = (double)(next() >> 5);
+        const double lo = (double)(next() >> 6);
+        return (hi * 67108864.0 + lo) * (1.0 / 9007199254740992.0);
+    }
+    __device__ uint32_t below(uint32_t n) { return (uint32_t)(((uint64_t)next() * n) >> 32); }   // uniform integer in [0, n)
 };
 
 }  // namespace b200bt

@@ -3,15 +3,17 @@
 Reference: services/strategy_evolution_service.py.
   param_ranges                       :98-117  (synth.param_ranges)
   optimize_with_genetic_algorithm    :525-694 (GA construction :644-655)
+  optimize_with_reinforcement_learning :696-791 (rl.py: the agent on the device, trained on the market's bars)
 The reference's fitness closure (:542-641) is a data-free placeholder that raises
 NameError (SURVEY.md 0); the fitness wired in here is the reference's own
 simulate -> metrics -> score composition (strategy_evaluation.py:682-691) evaluated for
-the whole population by the sweep kernel.  LLM / Redis / regime / RL plumbing is out of scope.
+the whole population by the sweep kernel.  LLM / Redis / regime plumbing is out of scope.
 """
 from __future__ import annotations
 
 import logging
 import os
+import secrets
 import uuid
 from datetime import datetime
 from typing import Dict, List, Optional
@@ -19,6 +21,7 @@ from typing import Dict, List, Optional
 from .dist import ShardedFitness, broadcast_seed
 from .genetic_algorithm import GeneticAlgorithm, ParetoGeneticAlgorithm
 from .pareto import objectives_from_goals
+from .rl import ACTIONS, SERVICE_AGENT, RLPopulation, adjust_params_from_q_values, rl_states
 from .sweep import DEFAULT_GOALS, MarketData, PopulationSweep
 from .synth import param_ranges
 
@@ -48,6 +51,8 @@ class StrategyEvolutionService:
         self.fitness = ShardedFitness(self.sweep.evaluate, device=market.device)
         self.random_seed = random_seed
         self.evolution_records: List[Dict] = []
+        self._rl_states = None
+        self.rl_agents: Dict[int, RLPopulation] = {}      # the persistent agent of each symbol trained so far
 
     async def optimize_with_genetic_algorithm(self, current_params: Dict, performance_data: Optional[Dict] = None,
                                               historical_trades: Optional[List[Dict]] = None) -> Optional[Dict]:
@@ -108,4 +113,54 @@ class StrategyEvolutionService:
             return front
         except Exception as e:        # reference convention (:692-694): log, return None
             logger.error("Error in Pareto optimization: %s", e)
+            return None
+
+    def _states(self):
+        if self._rl_states is None:
+            self._rl_states = rl_states(self.market)
+        return self._rl_states
+
+    async def optimize_with_reinforcement_learning(self, current_params: Dict, end_bar: int,
+                                                   symbol: int = 0) -> Optional[Dict]:
+        """One RL optimisation call (strategy_evolution_service.py:696-791) on the 20 bars of `symbol` ending at end_bar:
+        the persistent agent (the service's hyperparameters, :213-224; one agent per symbol, created on first use) acts,
+        remembers and replays on the device, and the Q-values of the last bar adjust the parameters (:901-975).  Appends
+        the reference's evolution record; on error logs and returns None, as the reference does."""
+        try:
+            agent = self.rl_agents.get(symbol)
+            if agent is None:
+                seed = self.random_seed if self.random_seed is not None else secrets.randbits(63)
+                agent = RLPopulation(self._states(), [dict(SERVICE_AGENT, seed=seed, symbol=symbol)])
+                self.rl_agents[symbol] = agent
+            agent.train([int(end_bar)], points_per_call=20)
+            q = agent.q_values[0, -1]
+            q_values = {a: float(q[i]) for i, a in enumerate(ACTIONS)}
+            adjusted = adjust_params_from_q_values(current_params, q_values, self.param_ranges)
+            self.evolution_records.append({                       # the reference stores this record in Redis (:770-785)
+                "id": str(uuid.uuid4()), "algorithm": "reinforcement_learning", "timestamp": datetime.now().isoformat(),
+                "avg_reward": float(agent.avg_reward[0, -1]), "q_values": q_values, "old_params": current_params,
+                "new_params": adjusted, "epsilon": float(agent.epsilon[0])})
+            return adjusted
+        except Exception as e:        # reference convention (:789-791): log, return None
+            logger.error("Error in reinforcement learning optimization: %s", e)
+            return None
+
+    def optimize_rl_population(self, current_params: Dict, call_end_bars, agents: List[Dict],
+                               points_per_call: int = 20) -> Optional[List[Dict]]:
+        """Train a fresh population of agents (dicts of seed, symbol and any of the reference constructor's
+        hyperparameters; SERVICE_AGENT fills the rest) over the calls ending at call_end_bars, all at once on the device.
+        Returns per agent {"agent", "new_params", "avg_reward", "q_values", "epsilon"} from its last call; the population
+        stays in `last_rl_population`.  On error logs and returns None."""
+        try:
+            pop = RLPopulation(self._states(), agents).train(call_end_bars, points_per_call=points_per_call)
+            self.last_rl_population = pop
+            eps = pop.epsilon
+            out = []
+            for i, a in enumerate(pop.agents):
+                q_values = {name: float(pop.q_values[i, -1, k]) for k, name in enumerate(ACTIONS)}
+                out.append({"agent": a, "new_params": adjust_params_from_q_values(current_params, q_values, self.param_ranges),
+                            "avg_reward": float(pop.avg_reward[i, -1]), "q_values": q_values, "epsilon": float(eps[i])})
+            return out
+        except Exception as e:
+            logger.error("Error in reinforcement learning population optimization: %s", e)
             return None

@@ -985,6 +985,103 @@ int b200bt_dca_sweep(const float* close, int64_t ld_close, const double* dip_pct
                      double usdc_balance, b200bt_dca_stats* stats, b200bt_dca_service* service_or_null,
                      double* day_or_null, int64_t D, b200bt_stream_t stream);
 
+/* ---- reinforcement-learning agents (csrc/rl.cu) -------------------------------------------------------------------
+ * services/reinforcement_learning.py's TradingRLAgent on its NumPy path, trained the way the strategy-evolution service's
+ * `rl` method trains it (optimize_with_reinforcement_learning, strategy_evolution_service.py:696-791), for a population of
+ * agents at once.  The reference trains on `historical_market_data` that nothing writes; the points here are OUR wiring
+ * (the reference never defines them, as with the GA fitness, SURVEY 0): point t of a symbol is bar t of the market on the
+ * caller's clock with price = close, rsi = RSI(14), macd / macd_signal = MACD(12, 26, 9), bb_* = BB(20, 2), ema_short /
+ * ema_long = EMA 12 / 26, atr = ATR(14) (b200bt_analyzer's columns, NaN policy applied), volume = the bar volume,
+ * price_change_1h / _24h = 100 (c_t - c_{t-h}) / c_{t-h} over h = 60 and 1 440 minutes of the clock (0 where t < h, the
+ * reference's .get(..., 0)), trend = TechnicalAnalyzer.get_trend's rule (binance_ml_strategy.py:184-203) per bar on close,
+ * SMA20 and SMA50.
+ *
+ * b200bt_rl_states: states [S][N][B200BT_RL_FEATURES] float64, _convert_market_data_to_state (:793-847) per point, in the
+ * feature order of _initialize_rl_agent (:203-207): rsi / 100, (macd + 1) / 2, (macd_signal + 1) / 2, then with price p > 0
+ * bb_upper = (upper - p) / range, bb_lower = (p - lower) / range (0.5 each when range = upper - lower <= 0), bb_middle =
+ * (p - middle) / p, ema_short / p, ema_long / p, atr / p (p <= 0: 0.5, 0.5, 0.5, 1, 1, 0); min(volume / 10^6, 1);
+ * (pc_1h + 10) / 20; (pc_24h + 30) / 60; the social features at their defaults 50, 0, 0 (no social data): 0.5, 0, 0;
+ * market_trend 0.8 uptrend, 0.2 downtrend, else 0.5.  cols: b200bt_analyzer's output for the same S and N; close, volume:
+ * [S][ld] fp32.  bar_minutes must divide 60.  Every value is formed with explicitly rounded float64 operations.
+ *
+ * b200bt_rl_train: A agents, one warp each, over a schedule of n_calls calls shared by all agents.  Call c covers the points
+ * [max(0, end_c - points_per_call + 1), end_c] of the agent's symbol; per point i (:718-754): state s_i, action = act(s_i),
+ * next state s_{i+1} (the LAST point uses itself, :739-741), reward r = _calculate_reward(action, s_i, next) (:849-899), done
+ * only on the last point (:747), remember, and replay when the memory holds >= batch_size transitions.  After the points:
+ * the online Q-values of the last point and the call's avg_reward = (r_0 + ... + r_{n-1}) / n (:758-779).  The agent
+ * persists across calls and launches: memory and epsilon carry over.
+ *   network (:132-155)   W1 [16][24], b1 [24], W2 [24][24], b2 [24], W3 [24][3], b3 [3] (B200BT_RL_PARAMS doubles in that
+ *                        order, row-major); forward (:157-184) ReLU, ReLU, linear; actions BUY, HOLD, SELL = 0, 1, 2
+ *   act (:292-318)       u = uniform (ACT stream); u < epsilon: below(3); else the argmax of the online Q-values (first
+ *                        maximum); the uniform is drawn for every point
+ *   remember (:320-333)  a deque(maxlen=memory_size): a ring of one word per transition (point, action, done); the state,
+ *                        next state and reward are re-derived from the state table
+ *   replay (:335-419)    1. batch_size distinct positions of the deque, j = the j-th oldest transition, drawn as below(fill)
+ *                        with repeats rejected (SAMPLE stream), used in draw order; 2. current_q with the online, next_q
+ *                        with the target weights, before any update; 3. target = current_q with target[a] = r if done else
+ *                        r + gamma * max(next_q); 4. _numpy_train (:186-241): one SGD step per sample in minibatch order,
+ *                        all six gradients from that sample's pre-update weights, ReLU mask where hidden <= 0, w -= alpha *
+ *                        d (original_outputs has no effect); 5. loss = mean squared error of the post-update outputs (only
+ *                        computed with a history); 6. step += 1, target = online every update_target_every replays; 7.
+ *                        epsilon *= epsilon_decay while epsilon > epsilon_end (per replay); 8. mean_q = mean of max(current_q)
+ *   init (:142-155)      randn * 0.1 for W1, W2, W3 in that order (Box-Muller of the INIT stream: normal pair p from block p,
+ *                        r = sqrt(-2 log(1 - u1)), r cos(2 pi u2), r sin(2 pi u2)), biases 0, target = online; or the
+ *                        caller's init_weights_or_null (device [A][B200BT_RL_PARAMS])
+ * RNG: Philox4x32-10 with counter (global agent index agent_offset + a as two words, stream, block) and key = seed; streams
+ * INIT 0, ACT 1, SAMPLE 2; words handed out as the GA operators' (uniform: 53 bits from two words; below(n): (word * n) >>
+ * 32).  Parity with the reference's Mersenne-twister draws is DISTRIBUTIONAL, as for the GA operators.  An agent's results
+ * do not depend on the launch geometry, the other agents or how the calls are split over launches.
+ * Arithmetic: every float64 operation is rounded on its own (no contraction, no DMMA); every sum runs in index order from
+ * its first term (dot products over the input index, then + bias; the loss over samples, then outputs; mean_q over
+ * samples), so tests/rl_ref.py restates the kernel bit for bit.  The reference's BLAS order differs in the last bits.
+ * Quirks mirrored: bb_upper / bb_middle's forms above; volume capped at 1; the sentiment bonus of _calculate_reward never
+ * fires (sentiment is 0.5); HOLD scores 0.05 when |pc| < 0.01, else 0.05 when rsi in [0.4, 0.6], else -0.05, with pc =
+ * (next.price_change_1h - 0.5) * 2; no replay until the memory holds a batch, possibly several calls later.
+ * agent_state: b200bt_rl_workspace_bytes(A, memory_max) bytes of device memory, zero-filled before the first launch; agent a
+ * at a * (that / A): a b200bt_rl_agent_state, the online then the target weights (B200BT_RL_PARAMS doubles each, canonical
+ * layout), then memory_max ring words.  agents_host: host [A]; call_end_host: host [n_calls].  Outputs (device):
+ * avg_reward [A][n_calls], q_values [A][n_calls][3], history_or_null [A][history_rows][4] = (loss, mean_q, epsilon, step)
+ * per replay of this launch, in order (rows past an agent's replays are not written; null skips the loss pass).
+ * Checked before the device: null pointers, sizes, symbol in [0, S), batch_size in [1, B200BT_RL_MAX_BATCH], memory_size
+ * in [batch_size, memory_max], memory_max <= B200BT_RL_MAX_MEMORY, update_target_every >= 1, every call end in [0, N),
+ * points_per_call >= 1, history_rows >= the launch's points, and the agent-state size (EINVAL). */
+#define B200BT_RL_FEATURES 16
+#define B200BT_RL_PARAMS 1083
+#define B200BT_RL_MAX_BATCH 128
+#define B200BT_RL_MAX_MEMORY (1 << 20)
+
+typedef struct b200bt_rl_agent {
+    uint64_t seed;
+    int32_t symbol;
+    int32_t batch_size;
+    int32_t memory_size;
+    int32_t update_target_every;
+    double learning_rate;
+    double gamma;
+    double epsilon_start;
+    double epsilon_end;
+    double epsilon_decay;
+} b200bt_rl_agent;                /* 64 bytes */
+
+typedef struct b200bt_rl_agent_state {
+    int64_t initialized;          /* 0 before the first launch (weights drawn or copied then)                           */
+    int64_t n_transitions;        /* transitions remembered so far (the deque holds the last min(this, memory_size))    */
+    int64_t replays;              /* step_counter                                                                       */
+    double epsilon;
+    uint64_t act_words;           /* words taken from the ACT and SAMPLE streams                                        */
+    uint64_t sample_words;
+    double mean_q;                /* of the last replay; NaN before the first                                           */
+    int64_t reserved;
+} b200bt_rl_agent_state;          /* 64 bytes */
+
+int b200bt_rl_states(const float* cols, const float* close, const float* volume, int64_t ld, int S, int64_t N,
+                     int bar_minutes, double* states, b200bt_stream_t stream);
+int64_t b200bt_rl_workspace_bytes(int A, int memory_max);
+int b200bt_rl_train(const double* states, int S, int64_t N, const b200bt_rl_agent* agents_host, int A, int64_t agent_offset,
+                    int memory_max, void* agent_state, int64_t agent_state_bytes, const int64_t* call_end_host, int n_calls,
+                    int points_per_call, const double* init_weights_or_null, double* avg_reward, double* q_values,
+                    double* history_or_null, int64_t history_rows, b200bt_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -19,7 +19,7 @@ from ai_crypto_trader_b200.monte_carlo import PathEngine, risk_statistics
 from ai_crypto_trader_b200.sweep import MarketData, PopulationSweep
 from oracle import indicators_ref, sim_oracle
 
-legs = sys.argv[1:] or ["sweep", "mc", "joint", "indicators", "pareto", "regime", "dca", "grid_service"]
+legs = sys.argv[1:] or ["sweep", "mc", "joint", "indicators", "pareto", "regime", "dca", "grid_service", "rl"]
 torch.cuda.set_device(0)
 
 if "sweep" in legs:
@@ -169,3 +169,23 @@ if "grid_service" in legs:
 
 torch.cuda.synchronize()
 print("sanitize target done")
+if "rl" in legs:
+    # RL agents: the state table, replay-memory wraparound, batch 1 and 128, the target copy, the loss pass, two launches
+    sys.path.insert(0, str(Path(__file__).resolve().parents[1] / "tests"))
+    import rl_ref
+    from ai_crypto_trader_b200.rl import SERVICE_AGENT, RLPopulation, rl_states
+    m = MarketData(synth.synth_ohlcv(2, 400), bar_minutes=60)
+    states = rl_states(m)
+    agents = [dict(seed=1, symbol=0, batch_size=1, memory_size=1, update_target_every=2),
+              dict(seed=2, symbol=1, batch_size=128, memory_size=130, update_target_every=3)]
+    w0 = np.stack([rl_ref.init_weights(a["seed"], i) for i, a in enumerate(agents)])
+    pop = RLPopulation(states, agents, init_weights=w0)
+    ends = [150, 151, 300, 399, 20, 250, 260, 270]
+    pop.train(ends[:3], history=True)
+    pop.train(ends[3:], history=True)
+    X = states.cpu().numpy()
+    for i, a in enumerate(agents):
+        ag = rl_ref.Agent(gid=i, weights=w0[i], **dict(SERVICE_AGENT, **a))
+        rl_ref.train(ag, X[a["symbol"]], ends, 20, history=True)
+        assert np.array_equal(pop.weight_vector(i), ag.weights) and pop.replays[i] == ag.replays, i
+    print("rl ok:", int(pop.replays.sum()), "replays equal the restatement", flush=True)
