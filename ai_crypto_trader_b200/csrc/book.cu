@@ -24,7 +24,6 @@ constexpr int BK_WARPS = 2;            // individuals per CTA
 constexpr int BK_CAP = 512;            // records per window (staged and merged)
 constexpr int BK_BARS = 1024;          // bars per window (per-bar symbol masks)
 constexpr int BK_MAX_SYMBOLS = 64;     // one 64-bit symbol mask per bar
-constexpr unsigned BK_BAR_MASK = 0x3fffffffu;
 constexpr unsigned BK_NO_RECORD = 0x3fffffffu;   // staged word past a lane's last record: its bar is beyond any N < 2^30
 constexpr unsigned BK_SYMBOL_TAG = 0x9E3779B1u;  // trade_hash word of a book record: word ^ (symbol * BK_SYMBOL_TAG)
 
@@ -62,11 +61,7 @@ book_kernel(const float* __restrict__ price, int64_t ld_price, int S, int64_t N,
     }
     if (__any_sync(FULL, lost)) {       // the event buffer did not hold every record of some lane: no book
         if (lane == 0) {
-            b200bt_lane_stats o;
-            memset(&o, 0, sizeof(o));
-            o.n_records = -1.0;
-            o.score = NAN;
-            book[ind] = o;
+            book[ind] = lost_lane_stats();
             if (fitness) fitness[ind] = NAN;
         }
         return;
@@ -93,8 +88,8 @@ book_kernel(const float* __restrict__ price, int64_t ld_price, int S, int64_t N,
         // window [b0, B)
         unsigned b0 = BK_NO_RECORD, B = BK_NO_RECORD;
         for (int s = lane; s < S; s += 32) {
-            b0 = min(b0, w.stage[s * K] & BK_BAR_MASK);
-            B = min(B, w.stage[s * K + K - 1] & BK_BAR_MASK);   // K >= 3 records never share one bar: B > b0
+            b0 = min(b0, w.stage[s * K] & B200BT_EVENT_BAR_MASK);
+            B = min(B, w.stage[s * K + K - 1] & B200BT_EVENT_BAR_MASK);   // K >= 3 records never share one bar: B > b0
         }
         b0 = __reduce_min_sync(FULL, b0);
         if (b0 >= (unsigned)N) break;
@@ -105,13 +100,13 @@ book_kernel(const float* __restrict__ price, int64_t ld_price, int S, int64_t N,
         // symbol masks: first records of a (bar, symbol) in mask[], the last bar's second records in `second`
         unsigned long long second = 0ull;
         for (int f = lane; f < staged; f += 32) {
-            const unsigned x = w.stage[f] & BK_BAR_MASK;
+            const unsigned x = w.stage[f] & B200BT_EVENT_BAR_MASK;
             if (x >= B) continue;
             const int s = f / K, j = f - s * K;
-            const bool dup = j > 0 && (w.stage[f - 1] & BK_BAR_MASK) == x;
+            const bool dup = j > 0 && (w.stage[f - 1] & B200BT_EVENT_BAR_MASK) == x;
             if (dup) second |= 1ull << s;
             else atomicOr(&w.mask[x - b0], 1ull << s);
-            if (j == K - 1 || (w.stage[f + 1] & BK_BAR_MASK) >= B) w.take[s] = j + 1;
+            if (j == K - 1 || (w.stage[f + 1] & B200BT_EVENT_BAR_MASK) >= B) w.take[s] = j + 1;
         }
         second = __reduce_or_sync(FULL, (unsigned)second) | ((unsigned long long)__reduce_or_sync(FULL, (unsigned)(second >> 32)) << 32);
         __syncwarp();
@@ -136,11 +131,11 @@ book_kernel(const float* __restrict__ price, int64_t ld_price, int S, int64_t N,
         // price every record of the window and put it at its rank
         for (int f = lane; f < staged; f += 32) {
             const unsigned wd = w.stage[f];
-            const unsigned x = wd & BK_BAR_MASK;
+            const unsigned x = wd & B200BT_EVENT_BAR_MASK;
             if (x >= B) continue;
             const int s = f / K, j = f - s * K;
             const unsigned long long below = (1ull << s) - 1ull;
-            const bool dup = j > 0 && (w.stage[f - 1] & BK_BAR_MASK) == x;
+            const bool dup = j > 0 && (w.stage[f - 1] & B200BT_EVENT_BAR_MASK) == x;
             int rank = w.base[x - b0] + __popcll(w.mask[x - b0] & below);
             if (x == last_bar) rank += __popcll(second & below) + (dup ? 1 : 0);   // a force-close follows its entry
             const float* row = price + (int64_t)s * ld_price;
@@ -149,7 +144,7 @@ book_kernel(const float* __restrict__ price, int64_t ld_price, int S, int64_t N,
                 // the entry record precedes the exit in the same lane: staged, or the symbol's last record before the window
                 const unsigned we = j > 0 ? w.stage[f - 1] : __ldg(ev_ind + (int64_t)s * event_cap + w.cur[s] - 1);
                 int dur;
-                pnl = record_pnl(true, wd, __ldg(row + x), we, __ldg(row + (we & BK_BAR_MASK)), size, fee1, fee2, dur);
+                pnl = record_pnl(true, wd, __ldg(row + x), we, __ldg(row + (we & B200BT_EVENT_BAR_MASK)), size, fee1, fee2, dur);
             }
             w.word[rank] = wd;
             w.sym[rank] = (unsigned char)s;
@@ -164,14 +159,7 @@ book_kernel(const float* __restrict__ price, int64_t ld_price, int S, int64_t N,
             const unsigned wd = active ? w.word[r] : 0u;
             const unsigned s = active ? w.sym[r] : 0u;
             const double pnl = active ? w.pnl[r] : 0.0;
-            const unsigned x = wd & BK_BAR_MASK;
-            unsigned x_prev = __shfl_up_sync(FULL, x, 1);
-            if (lane == 0) x_prev = bar_carry;
-            // avg_trade_duration pairs records (2k, 2k+1) of the merged list (:166-178), whatever their symbols
-            const unsigned g = acc->n_events + (unsigned)lane;
-            const int dur = (active && (g & 1u)) ? (int)(x - x_prev) : 0;
-            bar_carry = __shfl_sync(FULL, x, n - 1);
-            batch_records(acc, n, active, wd, wd ^ (s * BK_SYMBOL_TAG), pnl, dur, cfg.minute0, cfg.bar_minutes, 0);
+            bar_carry = merged_records(acc, n, active, wd, wd ^ (s * BK_SYMBOL_TAG), pnl, bar_carry, cfg);
         }
         __syncwarp();
     }
@@ -191,14 +179,11 @@ extern "C" int b200bt_book_metrics(const float* price, int64_t ld_price, int S, 
                                    int pop, const b200bt_sweep_config* cfg, const b200bt_lane_stats* lane_stats,
                                    const uint32_t* events, int64_t event_cap, b200bt_lane_stats* book_stats,
                                    double* fitness_or_null, b200bt_stream_t stream) {
-    B200BT_REQUIRE(price && indiv && cfg && lane_stats && book_stats, B200BT_EINVAL, "book_metrics: null pointer");
-    B200BT_REQUIRE(S >= 1 && pop >= 1 && N >= 1 && ld_price >= N, B200BT_EINVAL, "book_metrics: bad sizes");
-    B200BT_REQUIRE(event_cap >= 0 && (events || event_cap == 0), B200BT_EINVAL, "book_metrics: bad event buffer");
-    B200BT_REQUIRE(S <= BK_MAX_SYMBOLS, B200BT_ELIMIT, "book_metrics: at most %d symbols (S = %d)", BK_MAX_SYMBOLS, S);
-    B200BT_REQUIRE(N < (1ll << 30), B200BT_ELIMIT, "book_metrics: N must be < 2^30 bars");
-    B200BT_REQUIRE((int64_t)S * (N + 1) < (1ll << 32), B200BT_ELIMIT, "book_metrics: S * (N + 1) records must stay below 2^32");
-    int rc = check_sweep_clock("book_metrics", cfg, N);
+    B200BT_REQUIRE(cfg && book_stats, B200BT_EINVAL, "book_metrics: null pointer");
+    int rc = check_record_args("book_metrics", price, ld_price, S, N, indiv, pop, cfg, lane_stats, events, event_cap);
     if (rc) return rc;
+    B200BT_REQUIRE(S <= BK_MAX_SYMBOLS, B200BT_ELIMIT, "book_metrics: at most %d symbols (S = %d)", BK_MAX_SYMBOLS, S);
+    B200BT_REQUIRE((int64_t)S * (N + 1) < (1ll << 32), B200BT_ELIMIT, "book_metrics: S * (N + 1) records must stay below 2^32");
     rc = check_device();
     if (rc) return rc;
     book_kernel<<<(unsigned)((pop + BK_WARPS - 1) / BK_WARPS), BK_WARPS * 32, 0, (cudaStream_t)stream>>>(

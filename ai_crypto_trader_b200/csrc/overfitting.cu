@@ -2,9 +2,9 @@
 // symmetric cross-validation (CSCV) of Bailey, Borwein, Lopez de Prado and Zhu (2015) on a matrix of such rows.
 //
 // daily_pnl_kernel  one warp per (individual, symbol) lane walks the lane's event words 32 at a time: coalesced word
-//                   loads, the entry word of an exit by shuffle (records come in (entry, exit) pairs and batches start on
-//                   an even index), record_pnl as trade_pnl_kernel / book_kernel price, a segmented warp sum by calendar
-//                   day, and the open day carried to the next batch.  Each (lane, day) cell is written once by its warp.
+//                   loads and the entry word of an exit by shuffle (record_batch), record_pnl as trade_pnl_kernel /
+//                   book_kernel price, batch_records' segmented warp sum by calendar day (day_segments), and the open day
+//                   carried to the next batch.  Each (lane, day) cell is written once by its warp.
 // book_rows_kernel  one thread per (individual, day): the sum over symbols 0..S-1, in that order, of the lane rows.
 // cscv_*            moments (one thread per trial), a trial-tile-major combination pass that stages a tile's block
 //                   statistics in registers once and walks a run of combinations, a reduction to the selected trial,
@@ -17,7 +17,6 @@
 namespace b200bt {
 
 constexpr int DP_WARPS = 4;                  // lanes per CTA of the row pass
-constexpr unsigned DP_BAR_MASK = 0x3fffffffu;
 constexpr int CS_THREADS = 256;              // trials per tile of the combination passes
 constexpr int CS_WARPS = CS_THREADS / 32;
 constexpr int CS_RUN = 64;                   // combinations per shared-memory run of a tile pass
@@ -33,51 +32,27 @@ daily_pnl_kernel(const float* __restrict__ price, int64_t ld_price, int S, const
     const int64_t w = (int64_t)blockIdx.x * DP_WARPS + (threadIdx.x >> 5);
     if (w >= n_lanes) return;
     double* row = lane_pnl + w * D;
-    const int64_t n_rec = (int64_t)lane_stats[w].n_records;
-    if (n_rec > event_cap) {                 // the event buffer lost records of this lane: no row
+    LaneRecords r;
+    if (!read_lane(r, w, S, price, ld_price, indiv, lane_stats, events, event_cap)) {   // lost records: no row
         for (int64_t d = lane; d < D; d += 32) row[d] = NAN;
         return;
     }
-    const int s = (int)(w % S);
-    const double size = indiv[w / S].position_size;
-    const double fee1 = __dmul_rn(size, 0.001), fee2 = __dmul_rn(size, 0.002);
     const unsigned gap_bar = cfg.gap_bar > 0 ? (unsigned)cfg.gap_bar : 0xffffffffu;
     const unsigned gap_minutes = (unsigned)cfg.gap_minutes, minute0 = (unsigned)cfg.minute0;
     const unsigned bar_minutes = (unsigned)cfg.bar_minutes;
-    const uint32_t* ev = events + w * event_cap;
-    const float* prow = price + (int64_t)s * ld_price;
     int carry_day = -1;                      // open day of the previous batch (-1: none)
     double carry = 0.0;
-    for (int64_t base = 0; base < n_rec; base += 32) {
-        const int64_t j = base + lane;
-        const bool active = j < n_rec;
-        const int n = (int)min((int64_t)32, n_rec - base);
-        const unsigned wd = active ? __ldg(ev + j) : 0u;
-        const unsigned bar = wd & DP_BAR_MASK;
-        const float pf = active ? __ldg(prow + bar) : 0.f;
-        const unsigned w_prev = __shfl_up_sync(FULL, wd, 1);     // an exit (odd index) follows its entry in this batch
-        const float p_prev = __shfl_up_sync(FULL, pf, 1);
-        int dur;
-        const double pnl = record_pnl(active, wd, pf, w_prev, p_prev, size, fee1, fee2, dur);
-        // calendar day: batch_records' unsigned 32-bit expression
-        const int day = active ? (int)((minute0 + bar * bar_minutes + (bar >= gap_bar ? gap_minutes : 0u)) / 1440u) : 0x7fffffff;
-        const int day_prev = __shfl_up_sync(FULL, day, 1), day_next = __shfl_down_sync(FULL, day, 1);
-        const bool head = lane == 0 || day != day_prev;
-        const bool tail = active && (lane == n - 1 || day != day_next);
-        double seg = pnl;
-        bool flag = head;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-            const double up = shfl_up_d(seg, d);
-            const int fup = __shfl_up_sync(FULL, (int)flag, d);
-            if (lane >= d && !flag) { seg += up; flag = fup; }
-        }
+    for (int64_t base = 0; base < r.n; base += 32) {
+        const RecordBatch b = record_batch(r, base);
+        const int day = b.active ? (int)record_day(minute0, b.bar, bar_minutes, gap_bar, gap_minutes) : 0x7fffffff;
+        bool tail;
+        double seg = day_segments(b.pnl, day, b.active, b.n, tail);
         const int batch_first = __shfl_sync(FULL, day, 0);
         if (carry_day >= 0 && carry_day != batch_first && lane == 0) row[carry_day - first_day] = carry;
         if (tail && day == carry_day) seg = __dadd_rn(carry, seg);  // only the first segment can continue the open day
-        if (tail && lane != n - 1) row[day - first_day] = seg;
-        carry = shfl_d(seg, n - 1);
-        carry_day = __shfl_sync(FULL, day, n - 1);
+        if (tail && lane != b.n - 1) row[day - first_day] = seg;
+        carry = shfl_d(seg, b.n - 1);
+        carry_day = __shfl_sync(FULL, day, b.n - 1);
     }
     if (carry_day >= 0 && lane == 0) row[carry_day - first_day] = carry;
 }
@@ -343,11 +318,8 @@ extern "C" int b200bt_daily_pnl(const float* price, int64_t ld_price, int S, int
                                 int pop, const b200bt_sweep_config* cfg, const b200bt_lane_stats* lane_stats,
                                 const uint32_t* events, int64_t event_cap, double* lane_pnl, int64_t D,
                                 double* book_pnl_or_null, b200bt_stream_t stream) {
-    B200BT_REQUIRE(price && indiv && cfg && lane_stats && lane_pnl, B200BT_EINVAL, "daily_pnl: null pointer");
-    B200BT_REQUIRE(S >= 1 && pop >= 1 && N >= 1 && ld_price >= N, B200BT_EINVAL, "daily_pnl: bad sizes");
-    B200BT_REQUIRE(event_cap >= 0 && (events || event_cap == 0), B200BT_EINVAL, "daily_pnl: bad event buffer");
-    B200BT_REQUIRE(N < (1ll << 30), B200BT_ELIMIT, "daily_pnl: N must be < 2^30 bars");
-    int rc = check_sweep_clock("daily_pnl", cfg, N);
+    B200BT_REQUIRE(cfg && lane_pnl, B200BT_EINVAL, "daily_pnl: null pointer");
+    int rc = check_record_args("daily_pnl", price, ld_price, S, N, indiv, pop, cfg, lane_stats, events, event_cap);
     if (rc) return rc;
     // calendar days of bar 0 and bar N - 1 (the kernels' unsigned 32-bit expression; the clock check keeps it exact)
     const int64_t last = N - 1;

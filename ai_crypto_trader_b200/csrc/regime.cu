@@ -11,8 +11,8 @@
 //                       deviations of the returns) and the warp writes the window's label on the window's bars.  The
 //                       work is O(points) per symbol: a few points per window, one window per 1440 minutes.
 // class_stats_kernel    one warp per (individual, symbol) lane walks the lane's records once, 32 at a time, as
-//                       daily_pnl_kernel does: a coalesced word load, record_pnl with the entry by shuffle, one label byte
-//                       per record.  For each class present in the batch (ballot) its records are compacted into that
+//                       daily_pnl_kernel does (record_batch: a coalesced word load, record_pnl with the entry by shuffle),
+//                       one label byte per record.  For each class present in the batch (ballot) its records are compacted into that
 //                       class's shared-memory staging (<= 63 entries); each full 32 goes through batch_records with the
 //                       class's own WarpAcc, the rest is flushed at the end, and finalize_lane gives every class's stats.
 #include <math.h>
@@ -24,7 +24,6 @@ constexpr int RG_WARPS = 8;                  // windows per CTA of the labelling
 constexpr int CL_WARPS = 4;                  // lanes per CTA of the class pass
 constexpr int CL_MAX = 8;                    // classes per call
 constexpr int CL_STAGE = 64;                 // staged records per class: < 32 left over + 32 new
-constexpr unsigned CL_BAR_MASK = 0x3fffffffu;
 
 // ---- regime windows and bar labels ---------------------------------------------------------------------------------
 struct RegimeClock {
@@ -165,20 +164,13 @@ struct ClassWarp {
     int fill[CL_MAX];                // staged records of the class
 };
 
-// Run `n` (<= 32) staged records of class `cls` through the metrics step; avg_trade_duration pairs the records (2k, 2k+1)
-// of the class list (calculate_metrics :166-178), whatever their kinds, as book_kernel pairs a merged list.
+// Run `n` (<= 32) staged records of class `cls` through the metrics step as one merged list, as book_kernel runs a book.
 __device__ __forceinline__ void flush_class(ClassWarp& cw, int cls, int n, const b200bt_sweep_config& cfg) {
     const int lane = threadIdx.x & 31;
     const bool act = lane < n;
     const unsigned wd = act ? cw.word[cls][lane] : 0u;
     const double pnl = act ? cw.pnl[cls][lane] : 0.0;
-    const unsigned x = wd & CL_BAR_MASK;
-    unsigned x_prev = __shfl_up_sync(FULL, x, 1);
-    if (lane == 0) x_prev = cw.carry_bar[cls];
-    const unsigned g = cw.acc[cls].n_events + (unsigned)lane;
-    const int dur = (act && (g & 1u)) ? (int)(x - x_prev) : 0;
-    const unsigned carry = __shfl_sync(FULL, x, n - 1);
-    batch_records(&cw.acc[cls], n, act, wd, wd, pnl, dur, cfg.minute0, cfg.bar_minutes, 0);
+    const unsigned carry = merged_records(&cw.acc[cls], n, act, wd, wd, pnl, cw.carry_bar[cls], cfg);
     if (lane == 0) cw.carry_bar[cls] = carry;
     __syncwarp();
 }
@@ -193,42 +185,23 @@ class_stats_kernel(const float* __restrict__ price, int64_t ld_price, int S, con
     const int64_t w = (int64_t)blockIdx.x * CL_WARPS + (threadIdx.x >> 5);
     if (w >= n_lanes) return;
     ClassWarp& cw = shared[threadIdx.x >> 5];
-    const int64_t n_rec = (int64_t)lane_stats[w].n_records;
-    if (n_rec > event_cap) {                 // the event buffer lost records of this lane: no class stats
-        if (lane < R) {
-            b200bt_lane_stats o;
-            memset(&o, 0, sizeof(o));
-            o.n_records = -1.0;
-            o.score = NAN;
-            out[lane * n_lanes + w] = o;
-        }
+    LaneRecords r;
+    if (!read_lane(r, w, S, price, ld_price, indiv, lane_stats, events, event_cap)) {   // lost records: no class stats
+        if (lane < R) out[lane * n_lanes + w] = lost_lane_stats();
         return;
     }
     const int s = (int)(w % S);
-    const b200bt_individual iv = indiv[w / S];
     if (lane < R) {
-        init_acc(cw.acc[lane], iv, cfg, nullptr);
+        init_acc(cw.acc[lane], indiv[w / S], cfg, nullptr);
         cw.carry_bar[lane] = 0u;
         cw.fill[lane] = 0;
     }
     __syncwarp();
-    const double size = iv.position_size;
-    const double fee1 = __dmul_rn(size, 0.001), fee2 = __dmul_rn(size, 0.002);
-    const uint32_t* ev = events + w * event_cap;
-    const float* prow = price + (int64_t)s * ld_price;
     const uint8_t* lab = labels + (int64_t)s * ld_labels;
     const unsigned below = (1u << lane) - 1u;
-    for (int64_t base = 0; base < n_rec; base += 32) {
-        const int64_t j = base + lane;
-        const bool active = j < n_rec;
-        const unsigned wd = active ? __ldg(ev + j) : 0u;
-        const unsigned bar = wd & CL_BAR_MASK;
-        const float pf = active ? __ldg(prow + bar) : 0.f;
-        const unsigned w_prev = __shfl_up_sync(FULL, wd, 1);     // an exit (odd index) follows its entry in this batch
-        const float p_prev = __shfl_up_sync(FULL, pf, 1);
-        int dur;
-        const double pnl = record_pnl(active, wd, pf, w_prev, p_prev, size, fee1, fee2, dur);
-        const int cls = active ? (int)__ldg(lab + bar) : 0xff;
+    for (int64_t base = 0; base < r.n; base += 32) {
+        const RecordBatch b = record_batch(r, base);
+        const int cls = b.active ? (int)__ldg(lab + b.bar) : 0xff;
         unsigned todo = __ballot_sync(FULL, cls < R);
         while (todo) {
             const int c = __shfl_sync(FULL, cls, __ffs(todo) - 1);
@@ -237,8 +210,8 @@ class_stats_kernel(const float* __restrict__ price, int64_t ld_price, int S, con
             int f = cw.fill[c];
             if (cls == c) {
                 const int pos = f + __popc(mask & below);
-                cw.word[c][pos] = wd;
-                cw.pnl[c][pos] = pnl;
+                cw.word[c][pos] = b.w;
+                cw.pnl[c][pos] = b.pnl;
             }
             f += __popc(mask);
             __syncwarp();
@@ -323,16 +296,13 @@ extern "C" int b200bt_class_stats(const float* price, int64_t ld_price, int S, i
                                   int pop, const b200bt_sweep_config* cfg, const b200bt_lane_stats* lane_stats,
                                   const uint32_t* events, int64_t event_cap, const uint8_t* labels, int64_t ld_labels, int R,
                                   b200bt_lane_stats* class_stats, b200bt_stream_t stream) {
-    B200BT_REQUIRE(price && indiv && cfg && lane_stats && labels && class_stats, B200BT_EINVAL, "class_stats: null pointer");
-    B200BT_REQUIRE(S >= 1 && pop >= 1 && N >= 1 && ld_price >= N, B200BT_EINVAL, "class_stats: bad sizes");
-    B200BT_REQUIRE(event_cap >= 0 && (events || event_cap == 0), B200BT_EINVAL, "class_stats: bad event buffer");
+    B200BT_REQUIRE(cfg && labels && class_stats, B200BT_EINVAL, "class_stats: null pointer");
+    int rc = check_record_args("class_stats", price, ld_price, S, N, indiv, pop, cfg, lane_stats, events, event_cap);
+    if (rc) return rc;
     B200BT_REQUIRE(ld_labels == 0 || ld_labels >= N, B200BT_EINVAL,
                    "class_stats: ld_labels must be 0 (one shared row) or >= N");
     B200BT_REQUIRE(R >= 1, B200BT_EINVAL, "class_stats: R = %d classes, need at least 1", R);
     B200BT_REQUIRE(R <= CL_MAX, B200BT_ELIMIT, "class_stats: at most %d classes (R = %d)", CL_MAX, R);
-    B200BT_REQUIRE(N < (1ll << 30), B200BT_ELIMIT, "class_stats: N must be < 2^30 bars");
-    int rc = check_sweep_clock("class_stats", cfg, N);
-    if (rc) return rc;
     rc = check_device();
     if (rc) return rc;
     const int64_t lanes = (int64_t)pop * S;

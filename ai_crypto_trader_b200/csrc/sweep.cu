@@ -121,6 +121,16 @@ int check_sweep_args(const char* who, const float* price, int64_t ld_price, cons
     return B200BT_OK;
 }
 
+int check_record_args(const char* who, const float* price, int64_t ld_price, int S, int64_t N,
+                      const b200bt_individual* indiv, int pop, const b200bt_sweep_config* cfg,
+                      const b200bt_lane_stats* lane_stats, const uint32_t* events, int64_t event_cap) {
+    B200BT_REQUIRE(price && indiv && lane_stats, B200BT_EINVAL, "%s: null pointer", who);
+    B200BT_REQUIRE(S >= 1 && pop >= 1 && N >= 1 && ld_price >= N, B200BT_EINVAL, "%s: bad sizes", who);
+    B200BT_REQUIRE(event_cap >= 0 && (events || event_cap == 0), B200BT_EINVAL, "%s: bad event buffer", who);
+    B200BT_REQUIRE(N < (1ll << 30), B200BT_ELIMIT, "%s: N must be < 2^30 bars", who);
+    return cfg ? check_sweep_clock(who, cfg, N) : B200BT_OK;
+}
+
 bool vec16_rows(const float* price, int64_t ld_price, const float* rsi, int64_t ld_rsi) {
     return (((uintptr_t)price | (uintptr_t)rsi) & 15) == 0 && ld_price % 4 == 0 && ld_rsi % 4 == 0;
 }

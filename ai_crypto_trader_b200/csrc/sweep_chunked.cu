@@ -29,7 +29,6 @@
 namespace b200bt {
 
 constexpr int CK_BLOCK = 256;   // events per pool block
-constexpr unsigned EVENT_BAR_MASK = ~(B200BT_EVENT_EXIT | B200BT_EVENT_SELL);   // event word = bar | flags
 constexpr unsigned SEG_LOST = 0xffffffffu;   // seg_count of a chunk whose events were lost (full pool, tile given up, unpacked warp)
 
 // Device-side counters of one sweep (a workspace section, zeroed at the start of the sweep); the first five are the flags
@@ -174,11 +173,11 @@ __device__ __forceinline__ bool chunk_scan_item(const ChunkScanArgs& A, const b2
             while (old_left) {
                 const int n_here = (int)min(min(32u, old_left), (unsigned)(CK_BLOCK - old_idx));
                 const unsigned word = lane < n_here ? A.pool[(int64_t)old_block * CK_BLOCK + old_idx + lane].x : 0xffffffffu;
-                const int k = __popc(__ballot_sync(FULL, lane < n_here && (word & EVENT_BAR_MASK) < tb));    // (bars ascend: a prefix)
+                const int k = __popc(__ballot_sync(FULL, lane < n_here && (word & B200BT_EVENT_BAR_MASK) < tb));    // (bars ascend: a prefix)
                 if (k) {
                     const unsigned last = __shfl_sync(FULL, word, k - 1);
                     old_pos = (last & B200BT_EVENT_EXIT) ? 0 : ((last & B200BT_EVENT_SELL) ? -1 : 1);
-                    old_ebar = (last & B200BT_EVENT_EXIT) ? -1 : (int)(last & EVENT_BAR_MASK);
+                    old_ebar = (last & B200BT_EVENT_EXIT) ? -1 : (int)(last & B200BT_EVENT_BAR_MASK);
                     old_idx += k; old_left -= (unsigned)k;
                     if (old_idx == CK_BLOCK && old_left) { old_block = A.next[old_block]; old_idx = 0; }
                 }
@@ -845,7 +844,7 @@ chunk_partial_kernel(const float* __restrict__ price, int64_t ld_price, const b2
     const unsigned minute0 = (unsigned)cfg.minute0, bar_minutes = (unsigned)cfg.bar_minutes;
     const unsigned gap_bar = cfg.gap_bar > 0 ? (unsigned)cfg.gap_bar : 0xffffffffu, gap_minutes = (unsigned)cfg.gap_minutes;
     auto day_of = [&](unsigned w) {   // calendar day of a record (a glued series jumps gap_minutes at gap_bar)
-        const unsigned bar = w & 0x3fffffffu;
+        const unsigned bar = w & B200BT_EVENT_BAR_MASK;
         return (int)((minute0 + bar * bar_minutes + (bar >= gap_bar ? gap_minutes : 0u)) / 1440u);
     };
     constexpr int R = WR_PER_LANE;

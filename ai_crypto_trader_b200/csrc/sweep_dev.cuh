@@ -25,6 +25,11 @@ int check_sweep_clock(const char* who, const b200bt_sweep_config* cfg, int64_t N
 int check_sweep_args(const char* who, const float* price, int64_t ld_price, const float* rsi, int64_t ld_rsi, int P, int S,
                      int64_t N, const b200bt_sweep_config* cfg_host, const uint32_t* events, int64_t event_cap);
 
+// The checks the passes over a sweep's records share; the clock (check_sweep_clock) only with a `cfg` (trade_pnl has none).
+int check_record_args(const char* who, const float* price, int64_t ld_price, int S, int64_t N,
+                      const b200bt_individual* indiv, int pop, const b200bt_sweep_config* cfg,
+                      const b200bt_lane_stats* lane_stats, const uint32_t* events, int64_t event_cap);
+
 // price and RSI rows that allow 16-byte copies: every (symbol, period) row starts on a 16-byte boundary
 bool vec16_rows(const float* price, int64_t ld_price, const float* rsi, int64_t ld_rsi);
 
@@ -145,10 +150,83 @@ __device__ __forceinline__ double record_pnl(bool active, unsigned w, float pf, 
         const double e = (double)p_prev, px = (double)pf;
         const double qty = __ddiv_rn(size, e);
         const double diff = (w_prev & B200BT_EVENT_SELL) ? __dsub_rn(e, px) : __dsub_rn(px, e);
-        dur = (int)((w & 0x3fffffffu) - (w_prev & 0x3fffffffu));
+        dur = (int)((w & B200BT_EVENT_BAR_MASK) - (w_prev & B200BT_EVENT_BAR_MASK));
         return __dsub_rn(__dmul_rn(qty, diff), fee2);
     }
     return -fee1;
+}
+
+// One (individual, symbol) lane's records in a sweep's event buffer, as the passes over them read it (lane w = i * S + s).
+struct LaneRecords {
+    const uint32_t* ev;          // event words
+    const float* price;          // close prices of the lane's symbol
+    int64_t n;                   // records
+    double size, fee1, fee2;     // position size, entry fee, the exit's fees (init_acc's)
+};
+
+// Fill `r` for lane w.  False when the event buffer lost records of the lane (n_records > event_cap): only r.n is set then.
+__device__ __forceinline__ bool read_lane(LaneRecords& r, int64_t w, int S, const float* __restrict__ price,
+                                          int64_t ld_price, const b200bt_individual* __restrict__ indiv,
+                                          const b200bt_lane_stats* __restrict__ lane_stats,
+                                          const uint32_t* __restrict__ events, int64_t event_cap) {
+    r.n = (int64_t)lane_stats[w].n_records;
+    if (r.n > event_cap) return false;
+    r.size = indiv[w / S].position_size;
+    r.fee1 = __dmul_rn(r.size, 0.001);
+    r.fee2 = __dmul_rn(r.size, 0.002);
+    r.ev = events + w * event_cap;
+    r.price = price + (int64_t)(int)(w % S) * ld_price;
+    return true;
+}
+
+// Records [base, base + 32) of a lane, base even, lane j holding record base + j: an exit is priced against the entry before it.
+struct RecordBatch { bool active; int n; unsigned w, bar; double pnl; };
+
+__device__ __forceinline__ RecordBatch record_batch(const LaneRecords& r, int64_t base) {
+    RecordBatch b;
+    const int64_t j = base + (threadIdx.x & 31);
+    b.active = j < r.n;
+    b.n = (int)min((int64_t)32, r.n - base);
+    b.w = b.active ? __ldg(r.ev + j) : 0u;
+    b.bar = b.w & B200BT_EVENT_BAR_MASK;
+    const float pf = b.active ? __ldg(r.price + b.bar) : 0.f;
+    const unsigned w_prev = __shfl_up_sync(FULL, b.w, 1);
+    const float p_prev = __shfl_up_sync(FULL, pf, 1);
+    int dur;
+    b.pnl = record_pnl(b.active, b.w, pf, w_prev, p_prev, r.size, r.fee1, r.fee2, dur);
+    return b;
+}
+
+// Stats of a lane or book some of whose records the event buffer lost: n_records = -1, score = NaN, the rest zero.
+__device__ __forceinline__ b200bt_lane_stats lost_lane_stats() {
+    b200bt_lane_stats o = {};
+    o.n_records = -1.0;
+    o.score = NAN;
+    return o;
+}
+
+// Calendar day of bar `bar` in unsigned 32-bit minutes (exact: check_sweep_clock); gap_bar = ~0u: no gap.  The gap goes by
+// reference so that batch_records reads its WarpAcc's gap_minutes only for a bar past the gap, as it always has.
+__device__ __forceinline__ unsigned record_day(unsigned minute0, unsigned bar, unsigned bar_minutes, const unsigned& gap_bar,
+                                               const unsigned& gap_minutes) {
+    return (minute0 + bar * bar_minutes + (bar >= gap_bar ? gap_minutes : 0u)) / 1440u;
+}
+
+// Inclusive warp sum of `x` over each calendar day of records [0, cnt) in time order; `tail`: the day's last record.
+__device__ __forceinline__ double day_segments(double x, int day, bool active, int cnt, bool& tail) {
+    const int lane = threadIdx.x & 31;
+    const int day_prev = __shfl_up_sync(FULL, day, 1);
+    const int day_next = __shfl_down_sync(FULL, day, 1);
+    tail = active && (lane == cnt - 1 || day != day_next);
+    double seg = x;
+    bool flag = active && (lane == 0 || day != day_prev);      // the day's first record
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        double up = shfl_up_d(seg, d);
+        int fup = __shfl_up_sync(FULL, (int)flag, d);
+        if (lane >= d && !flag) { seg += up; flag = fup; }
+    }
+    return seg;
 }
 
 // Advance the trade-record metrics of calculate_metrics (strategy_evaluation.py:97-188) in `acc` (shared memory, one slot
@@ -157,7 +235,7 @@ __device__ __forceinline__ double record_pnl(bool active, unsigned w, float pf, 
 __device__ __forceinline__ void batch_records(WarpAcc* __restrict__ acc, int cnt, bool active, unsigned w, unsigned hw,
                                               double pnl, int dur, long long minute0, int bar_minutes, int64_t ev_cap) {
     const int lane = threadIdx.x & 31;
-    const unsigned bar = w & 0x3fffffffu;
+    const unsigned bar = w & B200BT_EVENT_BAR_MASK;
     // wins / losses
     const bool win = active && pnl > 0.0, loss = active && pnl < 0.0;
     const unsigned n_win = acc->n_win + __popc(__ballot_sync(FULL, win));
@@ -202,8 +280,7 @@ __device__ __forceinline__ void batch_records(WarpAcc* __restrict__ acc, int cnt
     const double peak_out = shfl_d(pk, cnt - 1);
 
     // daily buckets: segmented sum by calendar day over the batch, merged with the carry day
-    // calendar day of a record (unsigned 32-bit minutes: the host checks minute0 + N*bar_minutes + gap_minutes < 2^32 - 1440)
-    const int day = active ? (int)(((unsigned)minute0 + bar * (unsigned)bar_minutes + (bar >= acc->gap_bar ? acc->gap_minutes : 0u)) / 1440u) : 0;
+    const int day = active ? (int)record_day((unsigned)minute0, bar, (unsigned)bar_minutes, acc->gap_bar, acc->gap_minutes) : 0;
     DayAcc da{acc->pivot, acc->s1, acc->s2, acc->n_days, acc->pivot_set, acc->npivot, acc->ns1, acc->ns2, acc->n_neg};
     const int hold_first = acc->hold_first;
     int first_done = acc->first_done, first_id = acc->first_day;
@@ -221,18 +298,8 @@ __device__ __forceinline__ void batch_records(WarpAcc* __restrict__ acc, int cnt
         // common case: the whole batch falls into the open day
         day_sum = (day_valid ? day_sum : 0.0) + batch_sum;
     } else {
-        const int day_prev = __shfl_up_sync(FULL, day, 1);
-        const int day_next = __shfl_down_sync(FULL, day, 1);
-        const bool head = active && (lane == 0 || day != day_prev);
-        const bool tail = active && (lane == cnt - 1 || day != day_next);
-        double seg = pnl;
-        bool flag = head;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-            double up = shfl_up_d(seg, d);
-            int fup = __shfl_up_sync(FULL, (int)flag, d);
-            if (lane >= d && !flag) { seg += up; flag = fup; }
-        }
+        bool tail;
+        double seg = day_segments(pnl, day, active, cnt, tail);
         const bool merge_carry = day_valid && (first_day == day_cur);
         // a tail in the first segment (its day == first_day) absorbs the carry
         if (tail && merge_carry && day == first_day) seg += day_sum;
@@ -276,6 +343,21 @@ __device__ __forceinline__ void batch_records(WarpAcc* __restrict__ acc, int cnt
         acc->n_events = n_events + cnt;
     }
     __syncwarp();
+}
+
+// Run n <= 32 priced records of a merged list through batch_records, pairing durations on the list index (2k, 2k+1)
+// (calculate_metrics :166-178) whatever their symbols; takes and returns the bar of the list's previous record.
+__device__ __forceinline__ unsigned merged_records(WarpAcc* __restrict__ acc, int n, bool active, unsigned wd, unsigned hw,
+                                                   double pnl, unsigned bar_carry, const b200bt_sweep_config& cfg) {
+    const int lane = threadIdx.x & 31;
+    const unsigned x = wd & B200BT_EVENT_BAR_MASK;
+    unsigned x_prev = __shfl_up_sync(FULL, x, 1);
+    if (lane == 0) x_prev = bar_carry;
+    const unsigned g = acc->n_events + (unsigned)lane;
+    const int dur = (active && (g & 1u)) ? (int)(x - x_prev) : 0;
+    const unsigned carry = __shfl_sync(FULL, x, n - 1);
+    batch_records(acc, n, active, wd, hw, pnl, dur, cfg.minute0, cfg.bar_minutes, 0);
+    return carry;
 }
 
 // Consume `cnt` events in time order (lane j holds event j: word w, price pf); an exit record is

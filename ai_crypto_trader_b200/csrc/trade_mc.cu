@@ -7,8 +7,8 @@
 // Resampling rule: services/monte_carlo_service.py:277-298 (iid bootstrap) applied to round trips.
 //
 // Two kernels:
-//   trade_pnl_kernel  a sweep's event words -> per lane (n_trips, fee, trip_pnl[]), one CTA per lane, the exact float64
-//                     expressions of _simulate_trades (explicit _rn intrinsics: nothing is contracted into an FMA).
+//   trade_pnl_kernel  a sweep's event words -> per lane (n_trips, fee, trip_pnl[]), one CTA per lane: each exit priced by
+//                     record_pnl, the sweep's exact float64 expression of _simulate_trades (explicit _rn intrinsics).
 //   trade_mc_kernel   one CTA = TMC_THREADS paths of ONE lane, one thread per path.  The lane's trip PnL is staged in
 //                     shared memory when it fits (TMC_SMEM_TRIPS) and read through L2 otherwise.  Each path draws T trip
 //                     indices (bootstrap, block bootstrap or a keyed permutation) and walks the equity in float64 in the
@@ -21,12 +21,11 @@
 #include <algorithm>
 #include <numeric>
 #include <vector>
-#include "common.cuh"
 #include "philox.cuh"
+#include "sweep_dev.cuh"
 
 namespace b200bt {
 
-constexpr uint32_t TRADE_BAR_MASK = ~(B200BT_EVENT_EXIT | B200BT_EVENT_SELL);
 constexpr int PNL_THREADS = 128;
 
 // ---- round-trip PnL from the sweep's event words ------------------------------------------------------------------
@@ -50,14 +49,11 @@ trade_pnl_kernel(const float* __restrict__ price, int64_t ld, int S, const b200b
     const float* row = price + (int64_t)s * ld;
     const uint32_t* ev = events + lane * event_cap;
     double* out = trip_pnl + lane * ld_trip;
-    const double cost = __dmul_rn(size, 0.002);
+    const double fee2 = __dmul_rn(size, 0.002);
     for (int64_t j = threadIdx.x; j < n_rec / 2; j += blockDim.x) {
-        const uint32_t a = ev[2 * j], b = ev[2 * j + 1];
-        const double entry = (double)row[a & TRADE_BAR_MASK];
-        const double px = (double)row[b & TRADE_BAR_MASK];
-        const double qty = __ddiv_rn(size, entry);
-        const double move = (a & B200BT_EVENT_SELL) ? __dsub_rn(entry, px) : __dsub_rn(px, entry);
-        out[j] = __dsub_rn(__dmul_rn(qty, move), cost);
+        const uint32_t a = ev[2 * j], b = ev[2 * j + 1];     // entry, exit: record_pnl charges an exit no entry fee
+        int dur;
+        out[j] = record_pnl(true, b, row[b & B200BT_EVENT_BAR_MASK], a, row[a & B200BT_EVENT_BAR_MASK], size, 0.0, fee2, dur);
     }
 }
 
@@ -198,14 +194,13 @@ extern "C" int b200bt_trade_pnl(const float* price, int64_t ld, int S, int64_t N
                                 const b200bt_lane_stats* stats, const uint32_t* events, int64_t event_cap,
                                 double* trip_pnl, int64_t ld_trip, int32_t* n_trips, double* fee,
                                 b200bt_stream_t stream) {
-    B200BT_REQUIRE(price && indiv && stats && trip_pnl && n_trips && fee, B200BT_EINVAL, "trade_pnl: null pointer");
-    B200BT_REQUIRE(S >= 1 && pop >= 1 && N >= 1 && ld >= N, B200BT_EINVAL, "trade_pnl: bad sizes");
-    B200BT_REQUIRE(event_cap >= 0 && (events || event_cap == 0), B200BT_EINVAL, "trade_pnl: bad event buffer");
+    B200BT_REQUIRE(trip_pnl && n_trips && fee, B200BT_EINVAL, "trade_pnl: null pointer");
+    int rc = check_record_args("trade_pnl", price, ld, S, N, indiv, pop, nullptr, stats, events, event_cap);
+    if (rc) return rc;
     B200BT_REQUIRE(ld_trip >= 1 && 2 * ld_trip >= event_cap, B200BT_EINVAL,
                    "trade_pnl: ld_trip (%lld) must hold event_cap / 2 trips", (long long)ld_trip);
     B200BT_REQUIRE((int64_t)pop * S <= 0x7fffffff, B200BT_ELIMIT, "trade_pnl: at most 2^31 - 1 lanes");
-    B200BT_REQUIRE(N < ((int64_t)1 << 30), B200BT_ELIMIT, "trade_pnl: N < 2^30");
-    int rc = check_device();
+    rc = check_device();
     if (rc) return rc;
     trade_pnl_kernel<<<(unsigned)((int64_t)pop * S), PNL_THREADS, 0, (cudaStream_t)stream>>>(
         price, ld, S, indiv, stats, events, event_cap, trip_pnl, ld_trip, n_trips, fee);

@@ -269,17 +269,12 @@ class DCASweep:
         self.precision = prec
         self._pow10 = torch.tensor([float(10 ** p) for p in prec], dtype=torch.float64, device=market.device)
         self.usdc_balance = float(usdc_balance)
+        from .regime import label_rows, regime_labels
         if regime is True:
-            from .regime import regime_labels
             regime = regime_labels(market)[0]
         self.labels, self.ld_labels = None, 0
         if regime is not None:
-            if not (isinstance(regime, torch.Tensor) and regime.is_cuda and regime.dtype == torch.uint8 and
-                    regime.dim() == 2 and regime.shape[0] in (1, S) and regime.shape[1] == N):
-                raise ValueError(f"regime labels must be a device uint8 tensor [{S} or 1][{N}]")
-            shared = regime.shape[0] == 1 or regime.stride(0) == 0
-            self.labels = regime[:1].contiguous() if shared else regime.contiguous()
-            self.ld_labels = 0 if shared else N
+            self.labels, self.ld_labels = label_rows(regime, S, N)
         self.objective = objective
         self._column(objective)
         self.dip = dip_pct(market)

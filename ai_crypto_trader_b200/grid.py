@@ -212,8 +212,8 @@ class GridSweep:
         if not 0 <= int(start_bar) < N:
             raise ValueError(f"start_bar = {start_bar} outside [0, {N})")
         self.start_bar = int(start_bar)
+        from .regime import label_rows, regime_labels
         if regime is True:
-            from .regime import regime_labels
             if self.service:
                 primary = os.getenv("PRIMARY_TRADING_SYMBOL", "BTCUSDC")
                 if primary not in market.symbols:
@@ -224,14 +224,9 @@ class GridSweep:
                 regime = regime_labels(market)[0]
         self.labels, self.ld_labels = None, 0
         if regime is not None:
-            if not (isinstance(regime, torch.Tensor) and regime.is_cuda and regime.dtype == torch.uint8 and
-                    regime.dim() == 2 and regime.shape[0] in (1, S) and regime.shape[1] == N):
-                raise ValueError(f"regime labels must be a device uint8 tensor [{S} or 1][{N}]")
-            shared = regime.shape[0] == 1 or regime.stride(0) == 0
-            if self.service and not shared:
+            self.labels, self.ld_labels = label_rows(regime, S, N)
+            if self.service and self.ld_labels:
                 raise ValueError("service mode reads one regime label row (market_regime_history): pass [1][N] labels")
-            self.labels = regime[:1].contiguous() if shared else regime.contiguous()
-            self.ld_labels = 0 if shared else N
         self.table = regime_table(self.block)
         self.objective = objective
         self._field(objective)

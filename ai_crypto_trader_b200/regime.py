@@ -77,6 +77,18 @@ def trend_rows(market: MarketData) -> torch.Tensor:
     return torch.stack([market.close, sma[:, 0], sma[:, 1], sma5])
 
 
+def label_rows(labels: torch.Tensor, S: int, N: int, what: str = "regime labels") -> Tuple[torch.Tensor, int]:
+    """Per-bar labels as the kernels read them: (labels, ld_labels) from a device uint8 tensor [S or 1][N].  One row shared by
+    every symbol ([1][N], or a row expanded to [S][N]) comes back as a contiguous [1][N] with ld_labels = 0, per-symbol
+    rows as a contiguous [S][N] with ld_labels = N.  `what` names the argument in the ValueError of any other tensor."""
+    if not (isinstance(labels, torch.Tensor) and labels.is_cuda and labels.dtype == torch.uint8 and labels.dim() == 2
+            and labels.shape[0] in (1, S) and labels.shape[1] == N):
+        raise ValueError(f"{what} must be a device uint8 tensor [{S} or 1][{N}]")
+    if labels.shape[0] == 1 or labels.stride(0) == 0:
+        return labels[:1].contiguous(), 0
+    return labels.contiguous(), N
+
+
 def regime_labels(market: MarketData, sample_minutes: int = 60, thresholds: Optional[Dict] = None,
                   primary: Optional[Union[int, str]] = None) -> Tuple[torch.Tensor, List[np.ndarray]]:
     """(labels uint8 [S][N] on the device, windows): the regime (an index into REGIMES) of every bar, and per symbol the

@@ -23,7 +23,7 @@ from __future__ import annotations
 import ctypes as C
 import inspect
 import os
-from typing import Dict, Iterable, List, Optional, Sequence, Tuple
+from typing import Callable, Dict, Iterable, List, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -521,6 +521,13 @@ BOOK_MAX_EVENT_BYTES = 24 << 30
 BOOK_CAP_HEADROOM = 4                  # a learnt event cap is the last busiest lane + 1/4
 
 
+def _stats_fields(raw: np.ndarray) -> Dict[str, np.ndarray]:
+    """Stats records float64 [...][LANE_STATS_WORDS] (b200bt_lane_stats) as dict field -> [...] array, trade_hash as uint64."""
+    out = {name: raw[..., i] for i, name in enumerate(_lib.LANE_STATS_FIELDS[:-1])}
+    out["trade_hash"] = np.ascontiguousarray(raw[..., _lib.LANE_STATS_WORDS - 1]).view(np.uint64)
+    return out
+
+
 class PopulationSweep:
     """Evaluate a GA population against device-resident market data.
 
@@ -878,28 +885,44 @@ class PopulationSweep:
         lost records to a too-small guess is swept again with its exact cap (the lane counts are exact either way), so the
         results never depend on the guess.  Slices of the population keep their event buffers within max_event_bytes."""
         m = self.market
-        U, S = len(packed), m.S
-        cap = self._book_cap
-        if cap <= 0:
-            self._evaluate_unique(packed, population, None, 0)
-            cap = self._exact_cap(self._stats)
-        lanes = torch.empty((U, S, _lib.LANE_STATS_WORDS), dtype=torch.float64, device=m.device)
+        U = len(packed)
         book = torch.empty((U, _lib.LANE_STATS_WORDS), dtype=torch.float64, device=m.device)
         fit = torch.empty(U, dtype=torch.float64, device=m.device)
-        indiv = torch.from_numpy(packed.view(np.uint8)).to(m.device).view(U, -1)
-        busiest = 0
-        for lo, hi, c in self._event_slices(packed, population, cap):
-            self._book_slice(indiv[lo:hi], book[lo:hi], fit[lo:hi], c)
-            lanes[lo:hi] = self._stats
-            busiest = max(busiest, self._exact_cap(self._stats))
+
+        def launch(indiv: torch.Tensor, lo: int, hi: int, cap: int) -> None:
+            _lib.call("b200bt_book_metrics", m.close.data_ptr(), _lib.ld(m.close), m.S, m.N, indiv.data_ptr(), hi - lo,
+                      C.byref(self.cfg), self._stats.data_ptr(), self._events.data_ptr(), cap, book[lo:hi].data_ptr(),
+                      fit[lo:hi].data_ptr(), _lib.current_stream())
+
+        self._record_pass(packed, population, expand, self._book_cap, launch)
+        busiest = self._exact_cap(self._stats)
         self._book_cap = busiest + busiest // BOOK_CAP_HEADROOM + 2
-        self._keep_slice_stats(lanes, expand)
         self._book_dev = book
         self._book = book.cpu().numpy()
         if expand is not None:
             self._book = self._book[expand]
         res = fit.cpu().numpy()
         return res if expand is None else res[expand]
+
+    def _record_pass(self, packed: np.ndarray, population: List[Dict], expand: Optional[np.ndarray], cap: int,
+                     launch: Callable[[torch.Tensor, int, int, int], None]) -> None:
+        """Run a pass over the records of the decoded individuals `packed` (their dicts `population`, the output of _unique):
+        with cap <= 0 a sweep without events counts every lane's records first and gives the exact cap; then _event_slices
+        sweeps slices of the population with event buffers and launch(indiv[lo:hi], lo, hi, event cap) runs the pass on
+        each slice's lane stats and event words (self._stats / self._events), on the current stream of the market's device.
+        Afterwards lane_stats() describes every slice (_keep_slice_stats)."""
+        m = self.market
+        U = len(packed)
+        if cap <= 0:
+            self._evaluate_unique(packed, population, None, 0)
+            cap = self._exact_cap(self._stats)
+        stats = torch.empty((U, m.S, _lib.LANE_STATS_WORDS), dtype=torch.float64, device=m.device)
+        indiv = torch.from_numpy(packed.view(np.uint8)).to(m.device).view(U, -1)
+        for lo, hi, c in self._event_slices(packed, population, cap):
+            with torch.cuda.device(m.device):
+                launch(indiv[lo:hi], lo, hi, c)
+            stats[lo:hi] = self._stats
+        self._keep_slice_stats(stats, expand)
 
     def _event_slices(self, packed: np.ndarray, population: List[Dict], cap: int):
         """Sweep the decoded individuals `packed` with event buffers, in slices whose buffers keep within max_event_bytes,
@@ -937,14 +960,6 @@ class PopulationSweep:
         """Event cap that holds every record of every lane of `stats` (n_records of the busiest lane, at least 2)."""
         return max(2, int(stats[:, :, 0].max().item()))
 
-    def _book_slice(self, indiv: torch.Tensor, book: torch.Tensor, fit: torch.Tensor, cap: int) -> None:
-        """b200bt_book_metrics on the lanes and event words of the last sweep (one slice of the population)."""
-        m = self.market
-        with torch.cuda.device(m.device):
-            _lib.call("b200bt_book_metrics", m.close.data_ptr(), _lib.ld(m.close), m.S, m.N, indiv.data_ptr(), indiv.shape[0],
-                      C.byref(self.cfg), self._stats.data_ptr(), self._events.data_ptr(), cap, book.data_ptr(),
-                      fit.data_ptr(), _lib.current_stream())
-
     def book_stats(self) -> Dict[str, np.ndarray]:
         """Book metrics of the last aggregation="book" evaluation: the lane_stats() fields as [pop] arrays, computed on each
         individual's records on every symbol as one trade list (b200bt_book_metrics), plus
@@ -957,9 +972,7 @@ class PopulationSweep:
         lane_stats() still describes the per-symbol lanes of the same evaluation."""
         if self._book is None:
             raise RuntimeError("book_stats() needs an evaluate() under aggregation='book' first")
-        raw = self._book
-        out = {name: raw[:, i] for i, name in enumerate(_lib.LANE_STATS_FIELDS[:-1])}
-        out["trade_hash"] = np.ascontiguousarray(raw[:, _lib.LANE_STATS_WORDS - 1]).view(np.uint64)
+        out = _stats_fields(self._book)
         out["return_pct"] = out["net_profit"] / self.cfg.initial_capital * 100
         pairs = np.floor(out["n_records"] / 2)
         with np.errstate(divide="ignore", invalid="ignore"):
@@ -1073,19 +1086,15 @@ class PopulationSweep:
         if need > max_bytes:
             raise ValueError(f"daily_pnl: {need} bytes of per-day rows for {P} individuals x {S} symbols x {D} days exceed "
                              f"the budget of {max_bytes} bytes")
-        self._evaluate_unique(packed, unique, None, 0)
-        cap = self._exact_cap(self._stats)
-        stats = torch.empty((U, S, _lib.LANE_STATS_WORDS), dtype=torch.float64, device=m.device)
         lanes = torch.empty((U, S, D), dtype=torch.float64, device=m.device)
         book = torch.empty((U, D), dtype=torch.float64, device=m.device)
-        indiv = torch.from_numpy(packed.view(np.uint8)).to(m.device).view(U, -1)
-        for lo, hi, c in self._event_slices(packed, unique, cap):
-            with torch.cuda.device(m.device):
-                _lib.call("b200bt_daily_pnl", m.close.data_ptr(), _lib.ld(m.close), S, m.N, indiv[lo:hi].data_ptr(), hi - lo,
-                          C.byref(self.cfg), self._stats.data_ptr(), self._events.data_ptr(), c, lanes[lo:hi].data_ptr(),
-                          D, book[lo:hi].data_ptr(), _lib.current_stream())
-            stats[lo:hi] = self._stats
-        self._keep_slice_stats(stats, expand)
+
+        def launch(indiv: torch.Tensor, lo: int, hi: int, cap: int) -> None:
+            _lib.call("b200bt_daily_pnl", m.close.data_ptr(), _lib.ld(m.close), S, m.N, indiv.data_ptr(), hi - lo,
+                      C.byref(self.cfg), self._stats.data_ptr(), self._events.data_ptr(), cap, lanes[lo:hi].data_ptr(), D,
+                      book[lo:hi].data_ptr(), _lib.current_stream())
+
+        self._record_pass(packed, unique, expand, 0, launch)
         if expand is not None:
             inv = torch.from_numpy(expand).to(m.device)
             book, lanes = book.index_select(0, inv), lanes.index_select(0, inv)
@@ -1106,47 +1115,32 @@ class PopulationSweep:
         R = int(n_classes)
         if not 1 <= R <= 8:
             raise ValueError(f"class_stats: n_classes must be 1..8, not {R}")
-        if not (labels.is_cuda and labels.dtype == torch.uint8 and labels.dim() == 2 and labels.shape[0] in (1, m.S)
-                and labels.shape[1] == m.N):
-            raise ValueError(f"class_stats: labels must be a device uint8 tensor [{m.S} or 1][{m.N}]")
-        shared = labels.shape[0] == 1 or labels.stride(0) == 0
-        labels = labels[:1].contiguous() if shared else labels.contiguous()
-        ld_labels = 0 if shared else m.N
+        from .regime import label_rows
+        labels, ld_labels = label_rows(labels, m.S, m.N, "class_stats: labels")
         packed, unique, expand = self._unique(population)
         U, S = len(packed), m.S
-        self._evaluate_unique(packed, unique, None, 0)
-        cap = self._exact_cap(self._stats)
-        stats = torch.empty((U, S, _lib.LANE_STATS_WORDS), dtype=torch.float64, device=m.device)
         out = torch.empty((R, U, S, _lib.LANE_STATS_WORDS), dtype=torch.float64, device=m.device)
         part = torch.empty_like(out)
-        indiv = torch.from_numpy(packed.view(np.uint8)).to(m.device).view(U, -1)
-        for lo, hi, c in self._event_slices(packed, unique, cap):
+
+        def launch(indiv: torch.Tensor, lo: int, hi: int, cap: int) -> None:
             piece = part.view(-1)[:R * (hi - lo) * S * _lib.LANE_STATS_WORDS].view(R, hi - lo, S, -1)   # [R][slice][S]
-            with torch.cuda.device(m.device):
-                _lib.call("b200bt_class_stats", m.close.data_ptr(), _lib.ld(m.close), S, m.N, indiv[lo:hi].data_ptr(),
-                          hi - lo, C.byref(self.cfg), self._stats.data_ptr(), self._events.data_ptr(), c,
-                          labels.data_ptr(), ld_labels, R, piece.data_ptr(), _lib.current_stream())
+            _lib.call("b200bt_class_stats", m.close.data_ptr(), _lib.ld(m.close), S, m.N, indiv.data_ptr(), hi - lo,
+                      C.byref(self.cfg), self._stats.data_ptr(), self._events.data_ptr(), cap, labels.data_ptr(),
+                      ld_labels, R, piece.data_ptr(), _lib.current_stream())
             out[:, lo:hi] = piece
-            stats[lo:hi] = self._stats
-        self._keep_slice_stats(stats, expand)
+
+        self._record_pass(packed, unique, expand, 0, launch)
         if expand is not None:
             out = out.index_select(1, torch.from_numpy(expand).to(m.device))
         raw = out.cpu().numpy()
-        views = []
-        for r in range(R):
-            d = {name: raw[r, :, :, i] for i, name in enumerate(_lib.LANE_STATS_FIELDS[:-1])}
-            d["trade_hash"] = np.ascontiguousarray(raw[r, :, :, _lib.LANE_STATS_WORDS - 1]).view(np.uint64)
-            views.append(d)
-        return out, views
+        return out, [_stats_fields(raw[r]) for r in range(R)]
 
     def lane_stats(self) -> Dict[str, np.ndarray]:
         """Per-lane metrics of the last evaluation: dict field -> [pop][S] array."""
         raw = self._stats.cpu().numpy()
         if self._inverse is not None:
             raw = raw[self._inverse]
-        out = {name: raw[:, :, i] for i, name in enumerate(_lib.LANE_STATS_FIELDS[:-1])}
-        out["trade_hash"] = np.ascontiguousarray(raw[:, :, _lib.LANE_STATS_WORDS - 1]).view(np.uint64)
-        return out
+        return _stats_fields(raw)
 
     def advanced_stats(self) -> Dict[str, np.ndarray]:
         """calculate_advanced_metrics (strategy_evaluation.py:231-319) for every lane of the last evaluation,

@@ -246,6 +246,7 @@ typedef struct b200bt_sweep_config {
  * (short entry / long exit).  */
 #define B200BT_EVENT_EXIT 0x40000000u
 #define B200BT_EVENT_SELL 0x80000000u
+#define B200BT_EVENT_BAR_MASK 0x3fffffffu
 
 /* Run the population sweep.
  *  price   [S][N] fp32 (row stride ld_price)       close prices

@@ -33,6 +33,13 @@ def test_library_holds_sm90a_code_only(native_lib):
     assert set(re.findall(r"\.(sm_\w+)\.cubin", out)) == {"sm_90a"}, out
 
 
+def test_event_word_constants_match_header():
+    header = (ROOT / "include" / "b200bt.h").read_text()
+    defined = {k: int(v, 16) for k, v in re.findall(r"#define B200BT_EVENT_(\w+)\s+(0x[0-9a-fA-F]+)u", header)}
+    from ai_crypto_trader_b200 import _lib
+    assert defined == {"EXIT": _lib.EVENT_EXIT, "SELL": _lib.EVENT_SELL, "BAR_MASK": _lib.EVENT_BAR_MASK}
+
+
 def test_struct_layouts_match_header(native_lib):
     from ai_crypto_trader_b200 import _lib
     assert C.sizeof(_lib.Individual) == 40
