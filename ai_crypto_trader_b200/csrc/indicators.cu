@@ -35,18 +35,23 @@ struct RsiBankParams {
 // rows of P_all + 1 entries per symbol with row 0 = price): the bank's (min, max) ranges are produced from the values in
 // registers while they are written -- a lane's four bars ARE one 4-bar group, eight lanes one 32-bar block -- and the price
 // row's from the staged closes, so the first sweep of a fresh bank already skips quiet blocks.
+// kGlobalHalo: the bank's warm-up halo is too long for shared memory (windows above ~1100 bars); only the tile is staged and
+// the halo bars are read from global memory.
 #ifndef B200BT_RSI_MIN_BLOCKS
 #define B200BT_RSI_MIN_BLOCKS 3
 #endif
+template <bool kGlobalHalo>
 __global__ void __launch_bounds__(256, B200BT_RSI_MIN_BLOCKS)
 rsi_bank_kernel(const float* __restrict__ close, int64_t N, int64_t ld,
                 const __grid_constant__ RsiBankParams prm, int P, int fill, int halo_max,
                 float* __restrict__ out, int vec_ok, float2* __restrict__ zc, float2* __restrict__ zf, int P_all, int p0) {
-    extern __shared__ float s_close[];  // [halo_max + RSI_TILE + 1], s_close[i] = close[s0 - 1 + i]
+    extern __shared__ float s_close[];  // [tile_start - s0 + RSI_TILE + 1], s_close[i] = close[s0 - 1 + i]
     const int sym = blockIdx.y;
     const int64_t tile_start = (int64_t)blockIdx.x * RSI_TILE;
     const int64_t tile_end = min(tile_start + (int64_t)RSI_TILE, N);
-    const int64_t s0 = max((int64_t)0, tile_start - halo_max);  // first bar staged (multiple of 4)
+    // first bar staged (multiple of 4); bars before it are read from global memory (kGlobalHalo) or not needed
+    const int64_t s0 = kGlobalHalo ? tile_start : max((int64_t)0, tile_start - halo_max);
+    const int64_t first_bar = kGlobalHalo ? 0 : s0;
     const float* row = close + (int64_t)sym * ld;
     const int n_stage = (int)(tile_start + RSI_TILE - s0) + 1;
     for (int i = threadIdx.x; i < n_stage; i += blockDim.x) {
@@ -103,7 +108,7 @@ rsi_bank_kernel(const float* __restrict__ close, int64_t N, int64_t ld,
             }
         }
         int64_t start = tile_start - prm.halo[pi];
-        start = start < s0 ? s0 : start;
+        start = start < first_bar ? first_bar : start;
         start &= ~(int64_t)3;
         double carryU = 0.0, carryD = 0.0;
         for (int64_t base = start; base < tile_end; base += RSI_STEP) {
@@ -111,7 +116,9 @@ rsi_bank_kernel(const float* __restrict__ close, int64_t N, int64_t ld,
             const int si = (int)(t - s0);  // s_close[si] = close[t-1]
             double x[RSI_K + 1];
 #pragma unroll
-            for (int j = 0; j <= RSI_K; ++j) x[j] = (double)s_close[min(si + j, n_stage - 1)];
+            for (int j = 0; j <= RSI_K; ++j)
+                x[j] = (kGlobalHalo && si + j < 0) ? (double)__ldg(row + max(t - 1 + j, (int64_t)0))   // bar -1: diff = 0, as staged
+                                                   : (double)s_close[min(si + j, n_stage - 1)];
             double u[RSI_K], d[RSI_K];
 #pragma unroll
             for (int j = 0; j < RSI_K; ++j) {
@@ -248,16 +255,18 @@ static int rsi_bank_impl(const float* close, int S, int64_t N, int64_t ld, const
             prm.halo[i] = (w == 1) ? 4 : halo_for_alpha(1.0 / w);
             if (prm.halo[i] > halo_max) halo_max = prm.halo[i];
         }
-        const size_t smem = (size_t)(halo_max + RSI_TILE + 4) * sizeof(float);
-        B200BT_REQUIRE(smem <= 200 * 1024, B200BT_ELIMIT, "rsi_bank: window too long for the shared-memory tile");
-        cudaError_t e = cudaFuncSetAttribute(rsi_bank_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        // the halo is staged with the tile while both fit in shared memory (windows up to ~1100 bars), else read from global
+        const bool global_halo = (size_t)(halo_max + RSI_TILE + 4) * sizeof(float) > 200 * 1024;
+        const size_t smem = (size_t)((global_halo ? 0 : halo_max) + RSI_TILE + 4) * sizeof(float);
+        auto kernel = global_halo ? rsi_bank_kernel<true> : rsi_bank_kernel<false>;
+        cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return cuda_status(e, "rsi_bank: cudaFuncSetAttribute");
         dim3 grid((unsigned)((N + RSI_TILE - 1) / RSI_TILE), (unsigned)S);
         // the launch writes rows [p0, p0+pc) of every symbol: pass the full-P row pitch via (P, pi offset)
         float2* zc = zones ? (float2*)zones + (int64_t)sym0 * (P + 1) * zone_row_stride(N) : nullptr;
         float2* zf = zones ? (float2*)zones + (int64_t)S_total * (P + 1) * zone_row_stride(N) + (int64_t)sym0 * (P + 1) * zone_fine_stride(N) : nullptr;
-        rsi_bank_kernel<<<grid, 256, smem, st>>>(close, N, ld, prm, pc, fill, halo_max,
-                                                  out + (int64_t)p0 * N, vec_ok ? 1 : 0, zc, zf, P, p0);
+        kernel<<<grid, 256, smem, st>>>(close, N, ld, prm, pc, fill, halo_max,
+                                        out + (int64_t)p0 * N, vec_ok ? 1 : 0, zc, zf, P, p0);
         B200BT_LAUNCH_CHECK("rsi_bank launch");
     }
     return B200BT_OK;

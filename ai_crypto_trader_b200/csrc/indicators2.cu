@@ -330,14 +330,18 @@ bollinger_kernel(const float* __restrict__ x, int64_t N, int64_t ld, int w, doub
             continue;
         }
         const int i = (int)(t - s0);
-        const double m1 = (p1[i + 1] - p1[i + 1 - w]) / (double)w;   // mean of d
-        const double m2 = (p2[i + 1] - p2[i + 1 - w]) / (double)w;   // mean of d^2
-        double var = m2 - m1 * m1;
-        if (var < 0.0) var = 0.0;
-        const double sd = sqrt(var), mid = m1 + c;
+        const double close = (double)__ldg(row + t);
+        double mid = close, sd = 0.0;     // one bar is its own mean and has no deviation (the prefix differences leave a residue)
+        if (w > 1) {
+            const double m1 = (p1[i + 1] - p1[i + 1 - w]) / (double)w;   // mean of d
+            const double m2 = (p2[i + 1] - p2[i + 1 - w]) / (double)w;   // mean of d^2
+            double var = m2 - m1 * m1;
+            if (var < 0.0) var = 0.0;
+            sd = sqrt(var);
+            mid = m1 + c;
+        }
         const double hi = mid + kdev * sd, lo = mid - kdev * sd;
         const double rng = hi - lo;
-        const double close = (double)__ldg(row + t);
         o_high[o] = (float)hi;
         o_mid[o] = (float)mid;
         o_low[o] = (float)lo;

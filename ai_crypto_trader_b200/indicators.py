@@ -17,11 +17,16 @@ from . import _lib
 from .sweep import rsi_bank  # noqa: F401  (re-export: RSI lives with the sweep that consumes it)
 
 
-def _check(*ts):
+def _rows(*ts):
+    """-> (S, N, ld, inputs): fp32 CUDA [S][N] inputs with unit time stride, and the one row stride `ld` every kernel reads
+    all of a call's inputs with.  Inputs whose row strides differ (a slice of a padded buffer next to a dense tensor) are
+    copied to contiguous rows first."""
     S, N = ts[0].shape
     for t in ts:
         assert t.is_cuda and t.dtype == torch.float32 and t.dim() == 2 and tuple(t.shape) == (S, N) and t.stride(1) == 1
-    return S, N
+    if len({_lib.ld(t) for t in ts}) > 1:
+        ts = tuple(t.contiguous() for t in ts)
+    return S, N, _lib.ld(ts[0]), ts
 
 
 def _ints(v: Sequence[int]):
@@ -40,10 +45,10 @@ def nanfill_(x: torch.Tensor) -> torch.Tensor:
 
 
 def _bank(fn: str, x: torch.Tensor, windows: Sequence[int], fill: bool, extra=()):
-    S, N = _check(x)
+    S, N, ld, (x,) = _rows(x)
     out = torch.empty((S, len(windows), N), dtype=torch.float32, device=x.device)
     with torch.cuda.device(x.device):
-        _lib.call(fn, *extra, x.data_ptr(), S, N, _lib.ld(x), _ints(windows), len(windows), out.data_ptr(),
+        _lib.call(fn, *extra, x.data_ptr(), S, N, ld, _ints(windows), len(windows), out.data_ptr(),
                   _lib.current_stream())
     return nanfill_(out) if fill else out
 
@@ -57,10 +62,10 @@ def sma_bank(close: torch.Tensor, windows: Sequence[int], fill: bool = True) -> 
 
 
 def atr_bank(high, low, close, windows: Sequence[int]) -> torch.Tensor:
-    S, N = _check(high, low, close)
+    S, N, ld, (high, low, close) = _rows(high, low, close)
     out = torch.empty((S, len(windows), N), dtype=torch.float32, device=close.device)
     with torch.cuda.device(close.device):
-        _lib.call("b200bt_atr_bank", high.data_ptr(), low.data_ptr(), close.data_ptr(), S, N, _lib.ld(close),
+        _lib.call("b200bt_atr_bank", high.data_ptr(), low.data_ptr(), close.data_ptr(), S, N, ld,
                   _ints(windows), len(windows), out.data_ptr(), _lib.current_stream())
     return out
 
@@ -77,57 +82,57 @@ def _maybe_fill(ts, fill):
 
 
 def macd(close, fast: int = 12, slow: int = 26, sign: int = 9, fill: bool = True):
-    S, N = _check(close)
+    S, N, ld, (close,) = _rows(close)
     line, signal, diff = _outs(3, close.contiguous())
     with torch.cuda.device(close.device):
-        _lib.call("b200bt_macd", close.data_ptr(), S, N, _lib.ld(close), fast, slow, sign, line.data_ptr(),
+        _lib.call("b200bt_macd", close.data_ptr(), S, N, ld, fast, slow, sign, line.data_ptr(),
                   signal.data_ptr(), diff.data_ptr(), _lib.current_stream())
     return tuple(_maybe_fill([line, signal, diff], fill))
 
 
 def bollinger(close, window: int = 20, dev: float = 2.0, fill: bool = True):
     """-> (high, mid, low, width, position)."""
-    S, N = _check(close)
+    S, N, ld, (close,) = _rows(close)
     outs = _outs(5, close.contiguous())
     with torch.cuda.device(close.device):
-        _lib.call("b200bt_bollinger", close.data_ptr(), S, N, _lib.ld(close), window, float(dev),
+        _lib.call("b200bt_bollinger", close.data_ptr(), S, N, ld, window, float(dev),
                   *[o.data_ptr() for o in outs], _lib.current_stream())
     return tuple(_maybe_fill(outs, fill))
 
 
 def stochastic(high, low, close, window: int = 14, smooth: int = 3, fill: bool = True):
-    S, N = _check(high, low, close)
+    S, N, ld, (high, low, close) = _rows(high, low, close)
     k, d = _outs(2, close.contiguous())
     with torch.cuda.device(close.device):
-        _lib.call("b200bt_stochastic", high.data_ptr(), low.data_ptr(), close.data_ptr(), S, N, _lib.ld(close),
+        _lib.call("b200bt_stochastic", high.data_ptr(), low.data_ptr(), close.data_ptr(), S, N, ld,
                   window, smooth, k.data_ptr(), d.data_ptr(), _lib.current_stream())
     return tuple(_maybe_fill([k, d], fill))
 
 
 def williams_r(high, low, close, lbp: int = 14, fill: bool = True):
-    S, N = _check(high, low, close)
+    S, N, ld, (high, low, close) = _rows(high, low, close)
     (out,) = _outs(1, close.contiguous())
     with torch.cuda.device(close.device):
-        _lib.call("b200bt_williams_r", high.data_ptr(), low.data_ptr(), close.data_ptr(), S, N, _lib.ld(close), lbp,
+        _lib.call("b200bt_williams_r", high.data_ptr(), low.data_ptr(), close.data_ptr(), S, N, ld, lbp,
                   out.data_ptr(), _lib.current_stream())
     return _maybe_fill([out], fill)[0]
 
 
 def ichimoku(high, low, w1: int = 9, w2: int = 26, w3: int = 52, fill: bool = True):
-    S, N = _check(high, low)
+    S, N, ld, (high, low) = _rows(high, low)
     a, b = _outs(2, high.contiguous())
     with torch.cuda.device(high.device):
-        _lib.call("b200bt_ichimoku", high.data_ptr(), low.data_ptr(), S, N, _lib.ld(high), w1, w2, w3, a.data_ptr(),
+        _lib.call("b200bt_ichimoku", high.data_ptr(), low.data_ptr(), S, N, ld, w1, w2, w3, a.data_ptr(),
                   b.data_ptr(), _lib.current_stream())
     return tuple(_maybe_fill([a, b], fill))
 
 
 def vwap(high, low, close, volume, window: int = 14, fill: bool = True):
-    S, N = _check(high, low, close, volume)
+    S, N, ld, (high, low, close, volume) = _rows(high, low, close, volume)
     (out,) = _outs(1, close.contiguous())
     with torch.cuda.device(close.device):
         _lib.call("b200bt_vwap", high.data_ptr(), low.data_ptr(), close.data_ptr(), volume.data_ptr(), S, N,
-                  _lib.ld(close), window, out.data_ptr(), _lib.current_stream())
+                  ld, window, out.data_ptr(), _lib.current_stream())
     return _maybe_fill([out], fill)[0]
 
 
@@ -144,14 +149,14 @@ class TechnicalAnalyzer:
         assert isinstance(market, MarketData)
         self.market = market
         o, h, l, c, v = market.open, market.high, market.low, market.close, market.volume
-        S, N = _check(h, l, c, v)
+        S, N, ld, (h, l, c, v) = _rows(h, l, c, v)
         # all 21 columns of _calculate_all_indicators (:40-182) + _handle_nan_values in three fused launches and one batched
         # NaN-policy call (b200bt_analyzer): one [21][S][N] allocation, self.data[name] = its [S][N] block
         lib = _lib.load()
         cols = torch.empty((len(_lib.ANALYZER_COLUMNS), S, N), dtype=torch.float32, device=c.device)
         ws = torch.empty(int(lib.b200bt_analyzer_workspace_floats(S, N)), dtype=torch.float32, device=c.device)
         with torch.cuda.device(c.device):
-            _lib.call("b200bt_analyzer", h.data_ptr(), l.data_ptr(), c.data_ptr(), v.data_ptr(), S, N, _lib.ld(c), cols.data_ptr(),
+            _lib.call("b200bt_analyzer", h.data_ptr(), l.data_ptr(), c.data_ptr(), v.data_ptr(), S, N, ld, cols.data_ptr(),
                       ws.data_ptr(), _lib.current_stream())
         d: Dict[str, torch.Tensor] = {name: cols[i] for i, name in enumerate(_lib.ANALYZER_COLUMNS)}
         self.data = d

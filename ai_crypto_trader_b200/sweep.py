@@ -180,12 +180,16 @@ def rsi_bank(close: torch.Tensor, periods: Sequence[int], fill: bool = True,
     ta.momentum.RSIIndicator semantics as used at binance_ml_strategy.py:112.
     `zones`: a sweep zone map (zone_map_floats(P, zones_symbols, N) floats) whose rows of the symbols
     [first_symbol, first_symbol + S) are written in the same pass (b200bt_rsi_bank_zones; needs fill=True).
+    A `close` whose bars are not consecutive in memory (a time-strided view) is copied to contiguous rows first.
     """
     assert close.is_cuda and close.dtype == torch.float32 and close.dim() == 2
+    if close.stride(-1) != 1:
+        close = close.contiguous()
     S, N = close.shape
     P = len(periods)
     if out is None:
         out = torch.empty((S, P, N), dtype=torch.float32, device=close.device)
+    assert out.device == close.device and out.dtype == torch.float32 and tuple(out.shape) == (S, P, N) and out.is_contiguous()
     arr = (C.c_int * P)(*[int(p) for p in periods])
     with torch.cuda.device(close.device):
         if zones is not None:

@@ -49,13 +49,16 @@ int64_t b200bt_launch_count(void);
  * NaN policy follows TechnicalAnalyzer._handle_nan_values
  * (binance_ml_strategy.py:28-38): leading undefined values are back-filled
  * with the first defined value (`fill=1`) or written as NaN (`fill=0`).
+ * Limits (B200BT_ELIMIT outside): windows in [1, 1024] and 1..64 windows per bank call,
+ * MACD spans in [1, 512]; the RSI and ATR banks state their own below.
  * ------------------------------------------------------------------------ */
 
 /* RSI bank.  Replaces ta.momentum.RSIIndicator(close, window=w).rsi() as called
  * at binance_ml_strategy.py:112 (and services/market_monitor_service.py:228),
  * for every window in periods_host[0..P).  Wilder smoothing
  * ewm(alpha=1/w, adjust=False) of up/down moves; rsi = 100 where the smoothed
- * down move is 0. */
+ * down move is 0.  1 <= P <= 128 (P = 0: B200BT_EINVAL, above: B200BT_ELIMIT), every window in
+ * [1, 4096] (B200BT_ELIMIT outside). */
 int b200bt_rsi_bank(const float* close, int S, int64_t N, int64_t ld,
                     const int* periods_host, int P, int fill,
                     float* out, b200bt_stream_t stream);
@@ -117,7 +120,8 @@ int b200bt_ichimoku(const float* high, const float* low, int S, int64_t N, int64
                     int w3, float* a, float* b, b200bt_stream_t stream);
 
 /* ATR bank: ta.volatility.AverageTrueRange(high, low, close, window=w) (:164); zeros before
- * bar w-1 (ta writes 0, not NaN).  out [S][P][N]. */
+ * bar w-1 (ta writes 0, not NaN).  out [S][P][N].  1 <= P <= 64 and every window in [1, 541]
+ * (B200BT_ELIMIT otherwise: the warm-up halo of the longest window is staged in shared memory). */
 int b200bt_atr_bank(const float* high, const float* low, const float* close, int S, int64_t N,
                     int64_t ld, const int* windows_host, int P, float* out, b200bt_stream_t stream);
 
