@@ -134,6 +134,33 @@ REGIME_WINDOW_DTYPE = [("start_minute", "<i8"), ("n_points", "<i4"), ("label", "
                        ("change_pct", "<f8"), ("mean_strength", "<f8"), ("up_frac", "<f8"), ("down_frac", "<f8"),
                        ("sideways_frac", "<f8")]                      # b200bt_regime_window, 64 bytes
 
+class VpParams(C.Structure):
+    """b200bt_vp_params: bins, frame length and the anomaly pass of VolumeProfileAnalyzer."""
+    _fields_ = [("num_bins", C.c_int32), ("frame_bars", C.c_int32), ("anomaly_window", C.c_int32),
+                ("reserved", C.c_int32), ("value_area_pct", C.c_double), ("std_threshold", C.c_double)]
+
+
+VP_ROW_DTYPE = [(n, "<i4") for n in (
+    "n_bars", "valid", "signal", "poc_code", "value_area_code", "at_low_volume_node", "at_high_volume_node", "poc_bin",
+    "value_area_low_bin", "value_area_high_bin", "hvn_count", "lvn_count", "closest_lvn_bin", "pressure",
+    "recent_pressure", "divergence", "has_momentum", "anomaly_status", "total_anomalies", "strongest_offset",
+    "n_recent")] + [("recent_offset", "<i4", (5,)), ("reserved", "<i4", (4,))] + [(n, "<f8") for n in (
+    "price_min", "price_max", "close", "poc", "value_area_low", "value_area_high", "total_volume", "max_volume")] + [
+    ("hvn_price", "<f8", (3,))] + [(n, "<f8") for n in (
+    "closest_lvn", "cumulative_delta", "net_period_delta", "buying_volume", "selling_volume", "buy_sell_ratio",
+    "recent_delta", "delta_momentum", "recent_anomaly_pct", "strongest_significance", "strongest_volume",
+    "strongest_ma")] + [("recent_ma", "<f8", (5,)), ("recent_significance", "<f8", (5,))]   # b200bt_vp_row, 384 bytes
+VP_MAX_BINS = 64
+VP_NO_LABEL = 255
+VP_SIGNALS = ("potential_resistance", "potential_support", "potential_breakout_zone", "overbought", "oversold",
+              "neutral")                                              # row signal / labels = index
+VP_POC_CODES = ("approaching_poc_from_below", "approaching_poc_from_above", "below_poc", "above_poc")
+VP_VALUE_AREA_CODES = ("at_value_area_high", "above_value_area", "at_value_area_low", "below_value_area",
+                       "inside_value_area_lower", "inside_value_area_upper", "inside_value_area_middle")
+VP_PRESSURES = ("strong_buying", "moderate_buying", "strong_selling", "moderate_selling", "neutral")
+VP_RECENT_PRESSURES = ("recent_buying", "recent_selling")
+VP_DIVERGENCES = ("bearish_divergence", "bullish_divergence", "no_divergence")
+
 LANE_STATS_FIELDS = (
     "n_records", "n_wins", "n_losses", "total_profit", "total_loss", "net_profit",
     "max_drawdown", "sharpe_ratio", "n_days", "largest_profit", "largest_loss",
@@ -260,6 +287,7 @@ _SIGNATURES = {
     "b200bt_rl_states": (C.c_int, [_vp, _vp, _vp, _i64, _i, _i64, _i, _vp, _vp]),
     "b200bt_rl_workspace_bytes": (C.c_int64, [_i, _i]),
     "b200bt_rl_train": (C.c_int, [_vp, _i, _i64, _vp, _i, _i64, _i, _vp, _i64, _vp, _i, _i, _vp, _vp, _vp, _vp, _i64, _vp]),
+    "b200bt_volume_profile": (C.c_int, [_vp, _i64, _i, _i64, C.POINTER(VpParams), _vp, _vp, _vp, _i64, _vp]),
     "b200bt_pct_change": (C.c_int, [_vp, _i64, _i, _i64, _vp, _i64, _vp]),
     "b200bt_tail_stats_workspace_bytes": (C.c_int64, [_i64]),
     "b200bt_tail_stats": (C.c_int, [_vp, _i64, C.c_double, _vp, _vp, _i64, _vp]),

@@ -1087,6 +1087,87 @@ int b200bt_rl_train(const double* states, int S, int64_t N, const b200bt_rl_agen
                     int points_per_call, const double* init_weights_or_null, double* avg_reward, double* q_values,
                     double* history_or_null, int64_t history_rows, b200bt_stream_t stream);
 
+/* ---- volume profile (csrc/volume_profile.cu) ---------------------------------------------------------------------
+ * services/utils/volume_profile_analyzer.py, as services/market_monitor_service.py runs it on its df_5m frame (:328-359):
+ * analyze_volume_profile (:43-84; _calculate_volume_profile :86-173, _generate_signals :232-316, the inputs of
+ * _create_summary :318-394), analyze_volume_delta (:564-684) and detect_volume_anomalies (:487-562), for every frame of W
+ * consecutive bars of a market.  The frame ending at bar t is bars t - W + 1 .. t; there is one for every t >= W - 1.
+ * Codes index the name tuples of ai_crypto_trader_b200/_lib.py. */
+#define B200BT_VP_MAX_BINS 64
+#define B200BT_VP_NO_LABEL 255          /* label of a bar without a frame, or of a flat frame (no profile) */
+#define B200BT_VP_RECENT 5              /* recent_anomalies: the last five */
+
+typedef struct b200bt_vp_params {
+    int32_t num_bins;                /* B, 1 <= B <= B200BT_VP_MAX_BINS (20 in the analyzer)                            */
+    int32_t frame_bars;              /* W >= 1 (the monitor's 100 five-minute klines, :170)                               */
+    int32_t anomaly_window;          /* rolling window of the anomaly pass, >= 2 (20)                                     */
+    int32_t reserved;
+    double value_area_pct;           /* 0.7                                                                               */
+    double std_threshold;            /* 2.0                                                                               */
+} b200bt_vp_params; /* 32 bytes */
+
+typedef struct b200bt_vp_row {
+    int32_t n_bars;                  /* W for a frame, 0 for a bar without one (t < W - 1)                                */
+    int32_t valid;                   /* 1: price_max > price_min (else the reference fails on int(NaN) and the monitor
+                                        publishes no profile; every profile field below is NaN / -1 / 0)                */
+    int32_t signal;                  /* overall signal (SIGNALS), B200BT_VP_NO_LABEL without a profile                   */
+    int32_t poc_code;                /* POC_CODES                                                                         */
+    int32_t value_area_code;         /* VALUE_AREA_CODES                                                                  */
+    int32_t at_low_volume_node;      /* a low-volume node within 0.3 % of the close                                       */
+    int32_t at_high_volume_node;
+    int32_t poc_bin;                 /* np.argmax: the first maximum                                                      */
+    int32_t value_area_low_bin, value_area_high_bin;
+    int32_t hvn_count, lvn_count;    /* bins >= 0.7 max / <= 0.3 max                                                      */
+    int32_t closest_lvn_bin;         /* the low-volume node nearest the close (the first on ties), -1 without one         */
+    int32_t pressure;                /* PRESSURES                                                                         */
+    int32_t recent_pressure;         /* 0 recent_buying (recent_delta > 0), 1 recent_selling                              */
+    int32_t divergence;              /* DIVERGENCES                                                                       */
+    int32_t has_momentum;            /* W >= 40                                                                           */
+    int32_t anomaly_status;          /* 1: computed; 0: W < anomaly_window (the reference's error dict)                   */
+    int32_t total_anomalies;
+    int32_t strongest_offset;        /* frame offset (0 .. W-1) of the strongest anomaly (the first on ties), -1: none    */
+    int32_t n_recent;                /* min(5, total_anomalies)                                                           */
+    int32_t recent_offset[B200BT_VP_RECENT];   /* frame offsets of the last n_recent anomalies, oldest first              */
+    int32_t reserved[4];
+    double price_min, price_max, close;
+    double poc, value_area_low, value_area_high;   /* price levels of those bins                                          */
+    double total_volume, max_volume;               /* np.sum of the bins (pairwise); the largest bin                       */
+    double hvn_price[3];                           /* the first three high-volume nodes, NaN past hvn_count                */
+    double closest_lvn;                            /* NaN without one                                                      */
+    double cumulative_delta;                       /* sequential cumsum's last value                                       */
+    double net_period_delta, buying_volume, selling_volume;   /* pairwise sums of all / the positive / the negative deltas */
+    double buy_sell_ratio;                         /* +inf without selling                                                 */
+    double recent_delta;                           /* sum of the last min(20, W) deltas                                    */
+    double delta_momentum;                         /* last 20 - the 20 before; NaN when W < 40                             */
+    double recent_anomaly_pct;                     /* anomalies among the last min(20, W) bars, in percent                 */
+    double strongest_significance, strongest_volume, strongest_ma;
+    double recent_ma[B200BT_VP_RECENT], recent_significance[B200BT_VP_RECENT];
+} b200bt_vp_row; /* 384 bytes */
+
+/* Volume profile of every frame.  ohlcv: device float32 [5][S][ld] (MarketData's layout), ld >= N; values are widened to
+ * float64 and must be finite.  Per frame, in float64 with every operation rounded on its own (no FMA contraction):
+ *   profile   min / max of low / high; bin_size = (max - min) / B; candle c covers bins max(0, int((low - min) /
+ *             bin_size)) .. min(B - 1, int((high - min) / bin_size)), and volume / bins covered is added to each, in bar
+ *             order; edges i * bin_size + min (np.linspace), the last exactly max; level = (edge_i + edge_i+1) / 2.  POC =
+ *             the first maximum; value area: bins in descending volume, EQUAL VOLUMES IN DESCENDING BIN INDEX
+ *             (np.argsort(v, kind="stable")[::-1]; the reference's unstable argsort leaves this order to the platform),
+ *             summed until >= total * value_area_pct.
+ *   signals   poc_distance = |c - poc| / c * 100 etc. in the reference's expressions and priority order (:248-314); a
+ *             single-bin value area at the close gives 0 / 0 = NaN: inside_value_area_middle.
+ *   delta     +volume if close >= open else -volume; sums in numpy's pairwise order (np.sum / Series.sum), the cumulative
+ *             delta sequential; divergence from close[-1] - close[-min(20, W)].
+ *   anomalies rolling mean (sequential sum / w) and std (two-pass, ddof 1) over w = anomaly_window bars, a bar with frame
+ *             offset >= w - 1 is an anomaly if volume > ma + std_threshold * std, significance (volume - ma) / std.
+ *             pandas' rolling algorithm differs from this fixed order in the last bits of ma and std.
+ * rows_or_null [S][ld_rows] (row t: the frame ending at bar t), bins_or_null [S][ld_rows][B] (the bin volumes; 0 without a
+ * profile), labels_or_null uint8 [S][ld_rows] (the overall signal, B200BT_VP_NO_LABEL without a profile); at least one.
+ * Checked before the device: null ohlcv / params / all outputs, S < 1, N < 1, ld < N, ld_rows < N, frame_bars < 1,
+ * num_bins < 1, anomaly_window < 2, a non-finite value_area_pct or std_threshold (EINVAL); num_bins > B200BT_VP_MAX_BINS,
+ * N >= 2^30, S > 65535 (ELIMIT).  One warp per frame; no atomics; deterministic. */
+int b200bt_volume_profile(const float* ohlcv, int64_t ld, int S, int64_t N, const b200bt_vp_params* params,
+                          b200bt_vp_row* rows_or_null, double* bins_or_null, uint8_t* labels_or_null, int64_t ld_rows,
+                          b200bt_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -19,7 +19,8 @@ from ai_crypto_trader_b200.monte_carlo import PathEngine, risk_statistics
 from ai_crypto_trader_b200.sweep import MarketData, PopulationSweep
 from oracle import indicators_ref, sim_oracle
 
-legs = sys.argv[1:] or ["sweep", "mc", "joint", "indicators", "pareto", "regime", "dca", "grid_service", "rl"]
+legs = sys.argv[1:] or ["sweep", "mc", "joint", "indicators", "pareto", "regime", "dca", "grid_service", "rl",
+                        "volume_profile"]
 torch.cuda.set_device(0)
 
 if "sweep" in legs:
@@ -189,3 +190,22 @@ if "rl" in legs:
         rl_ref.train(ag, X[a["symbol"]], ends, 20, history=True)
         assert np.array_equal(pop.weight_vector(i), ag.weights) and pop.replays[i] == ag.replays, i
     print("rl ok:", int(pop.replays.sum()), "replays equal the restatement", flush=True)
+if "volume_profile" in legs:
+    # volume profile: frames shorter and longer than a 32-candle chunk and than the pairwise leaf (W = 300 > 128), 1 and
+    # 64 bins (lanes owning two bins), bars without a frame, rows, bins and labels; checked against the restatement
+    sys.path.insert(0, str(Path(__file__).resolve().parents[1] / "tests"))
+    import volume_profile_ref
+    from ai_crypto_trader_b200 import volume_profile as vp
+    m = MarketData(synth.synth_ohlcv(2, 700, first_symbol=4))
+    host = m.ohlcv.cpu().numpy()
+    for W, B in ((1, 1), (37, 64), (300, 20)):
+        rows, bins, labels = vp._run(m.ohlcv, vp.vp_params(W, B), True, True, m.device)
+        table, bins, labels = vp.rows_table(rows), bins.cpu().numpy(), labels.cpu().numpy()
+        picks = [(s, t) for s in range(2) for t in (0, W - 2, W - 1, W, 350, 699) if t >= 0]
+        want, wb, wl = volume_profile_ref.frames_at(host, picks, W, B)
+        for k, (s, t) in enumerate(picks):
+            for name in table.dtype.names:
+                g, w = table[s, t][name], want[k][name]
+                assert np.array_equal(g, w, equal_nan=g.dtype.kind == "f"), (W, B, s, t, name)
+            assert np.array_equal(bins[s, t], wb[k]) and labels[s, t] == wl[k], (W, B, s, t)
+    print("volume_profile ok: rows, bins and labels equal the restatement", flush=True)
