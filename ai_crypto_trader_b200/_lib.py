@@ -161,6 +161,54 @@ VP_PRESSURES = ("strong_buying", "moderate_buying", "strong_selling", "moderate_
 VP_RECENT_PRESSURES = ("recent_buying", "recent_selling")
 VP_DIVERGENCES = ("bearish_divergence", "bullish_divergence", "no_divergence")
 
+class MonitorParams(C.Structure):
+    """b200bt_monitor_params: frame length, label field and the monitor's trading-opportunity thresholds."""
+    _fields_ = [("frame_bars", C.c_int32), ("label_field", C.c_int32), ("min_price_change_pct", C.c_double),
+                ("min_volume_usdc", C.c_double)]
+
+
+MM_SNAPSHOT_FIELDS = ("current_price", "avg_volume", "rsi", "rsi_3m", "rsi_5m", "stoch_k", "macd", "macd_3m", "macd_5m",
+                      "williams_r", "bb_position", "trend_strength", "price_change_1m", "price_change_3m",
+                      "price_change_5m", "price_change_15m")              # market_update's numeric fields, in its order
+MM_OPTIONAL_FIELDS = ("volume", "ema_12", "ema_26")
+MM_CODE_FIELDS = ("tma_state", "osc_signal", "drsi_signal", "vpc_confirmation", "tsi_direction", "regime",
+                  "breakout_status", "divergence")
+MM_COMBINED_FIELDS = ("trend_confirmation", "momentum_trend_alignment", "tma_score", "volatility_adjusted_momentum",
+                      "volatility_trend_score", "osc_strength", "osc_agreement", "stoch_rsi", "drsi_divergence", "vwpm",
+                      "vpc_strength", "tsi_strength", "tsi_confidence", "regime_confidence", "reversal_probability",
+                      "breakout_confirmation", "divergence_strength")
+MONITOR_ROW_DTYPE = [(n, "<i4") for n in ("valid", "trend", "present", "opportunity")] + [
+    (n, "<f8") for n in MM_SNAPSHOT_FIELDS + MM_OPTIONAL_FIELDS] + [
+    (n, "<i4") for n in ("computed",) + MM_CODE_FIELDS + ("breakout_direction", "reversal_signals", "reserved")] + [
+    (n, "<f8") for n in MM_COMBINED_FIELDS]                          # b200bt_monitor_row, 352 bytes
+MM_NO_LABEL = 255
+MM_HAS = dict(volume=1, ema_12=2, ema_26=4, rsi_3m=8, rsi_5m=16, price_change_3m=32, avg_volume=64)   # present bits
+MM_COMBINATIONS = ("trend_confirmation", "momentum_trend_alignment", "triple_moving_average",
+                   "volatility_adjusted_momentum", "volatility_trend_score", "oscillator_consensus", "stoch_rsi",
+                   "double_rsi", "volume_weighted_price_momentum", "volume_price_confirmation", "trend_strength_index",
+                   "market_regime_indicator", "reversal_probability", "breakout_confirmation",
+                   "divergence_detector")                            # computed bit = index
+MM_TRENDS = ("uptrend", "downtrend", "sideways")
+MM_TMA_STATES = ("bullish", "bearish", "neutral")
+MM_OSC_SIGNALS = ("overbought", "oversold", "neutral")
+MM_DRSI_SIGNALS = ("strong_oversold", "oversold", "strong_overbought", "overbought", "bullish", "bearish", "neutral")
+MM_VPC_CONFIRMATIONS = ("strong_bullish", "weak_bullish", "strong_bearish", "weak_bearish", "neutral")
+MM_TSI_DIRECTIONS = (-1, 0, 1)
+MM_REGIMES = ("trending", "volatile", "ranging")
+MM_BREAKOUT_STATUSES = ("none", "strong_bullish", "strong_bearish", "confirmed_bullish", "confirmed_bearish",
+                        "potential_bullish", "potential_bearish")
+MM_DIVERGENCES = ("none", "bearish_rsi", "bullish_rsi", "bearish_macd", "bullish_macd")
+MM_REVERSAL_SIGNALS = ("rsi_overbought", "rsi_oversold", "williams_overbought", "williams_oversold",
+                       "price_near_upper_band", "price_near_lower_band", "potential_bearish_divergence",
+                       "potential_bullish_divergence")                # reversal_signals bit = index
+# label fields (b200bt_monitor_params.label_field = index): (row field, names of its codes)
+MM_LABEL_FIELDS = (("trend", MM_TRENDS), ("triple_moving_average.state", MM_TMA_STATES),
+                   ("oscillator_consensus.signal", MM_OSC_SIGNALS), ("double_rsi.signal", MM_DRSI_SIGNALS),
+                   ("volume_price_confirmation.confirmation", MM_VPC_CONFIRMATIONS),
+                   ("trend_strength_index.direction", MM_TSI_DIRECTIONS), ("market_regime_indicator.regime", MM_REGIMES),
+                   ("breakout_confirmation.status", MM_BREAKOUT_STATUSES), ("divergence_detector.divergence",
+                                                                            MM_DIVERGENCES))
+
 LANE_STATS_FIELDS = (
     "n_records", "n_wins", "n_losses", "total_profit", "total_loss", "net_profit",
     "max_drawdown", "sharpe_ratio", "n_days", "largest_profit", "largest_loss",
@@ -288,6 +336,9 @@ _SIGNATURES = {
     "b200bt_rl_workspace_bytes": (C.c_int64, [_i, _i]),
     "b200bt_rl_train": (C.c_int, [_vp, _i, _i64, _vp, _i, _i64, _i, _vp, _i64, _vp, _i, _i, _vp, _vp, _vp, _vp, _i64, _vp]),
     "b200bt_volume_profile": (C.c_int, [_vp, _i64, _i, _i64, C.POINTER(VpParams), _vp, _vp, _vp, _i64, _vp]),
+    "b200bt_market_monitor": (C.c_int, [_vp, _i, _i64, _i64, _i, _vp, _i64, _vp, _i64, _vp, _i64, C.POINTER(MonitorParams),
+                                         _vp, _vp, _vp]),
+    "b200bt_indicator_combinations": (C.c_int, [_vp, _i64, _vp]),
     "b200bt_pct_change": (C.c_int, [_vp, _i64, _i, _i64, _vp, _i64, _vp]),
     "b200bt_tail_stats_workspace_bytes": (C.c_int64, [_i64]),
     "b200bt_tail_stats": (C.c_int, [_vp, _i64, C.c_double, _vp, _vp, _i64, _vp]),

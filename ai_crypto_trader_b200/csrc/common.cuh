@@ -68,6 +68,15 @@ __device__ __forceinline__ float rsi_value(double U, double D) {
     return (float)((100.0 * U) * __drcp_rn(S));
 }
 
+// Index of the last k-minute bar COMPLETED by the close of base bar t (bar_minutes long, the series starting at Unix minute
+// minute0 >= 0): buckets are epoch-aligned, and bar t completes its bucket when the next bar starts in a later one.  -1
+// before the first completed bar.  b200bt_align and b200bt_market_monitor share this rule.
+__host__ __device__ __forceinline__ int64_t completed_bucket(int64_t t, int64_t minute0, int bar_minutes, int k) {
+    const int64_t m = minute0 + t * bar_minutes;
+    const int64_t b = m / k - minute0 / k;
+    return (m + bar_minutes) / k != m / k ? b : b - 1;
+}
+
 __device__ __forceinline__ double shfl_up_d(double v, int d) {
     return __shfl_up_sync(FULL, v, d);
 }

@@ -59,10 +59,7 @@ align_kernel(const float* __restrict__ src, int S, int64_t M, int64_t N, int64_t
     const int sym = blockIdx.y;
     const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= N) return;
-    const int64_t m = minute0 + t * bar_minutes;
-    const int64_t b = m / k - minute0 / k;
-    const bool closes_here = (m + bar_minutes) / k != m / k;   // bar t is the last 1-minute bar of its bucket
-    const int64_t j = closes_here ? b : b - 1;
+    const int64_t j = completed_bucket(t, minute0, bar_minutes, k);
     out[(int64_t)sym * N + t] = (j >= 0 && j < M) ? src[(int64_t)sym * M + j] : __int_as_float(0x7fc00000);
 }
 

@@ -1168,6 +1168,91 @@ int b200bt_volume_profile(const float* ohlcv, int64_t ld, int S, int64_t N, cons
                           b200bt_vp_row* rows_or_null, double* bins_or_null, uint8_t* labels_or_null, int64_t ld_rows,
                           b200bt_stream_t stream);
 
+/* ---- market monitor (csrc/market_monitor.cu) ---------------------------------------------------------------------
+ * services/market_monitor_service.py's market_update (:445-465) for every 1-minute bar of a market's history: the
+ * technical snapshot of calculate_technical_indicators (:219-301) on the frames of the 1-, 3-, 5- and 15-minute clocks
+ * (the monitor's 100 klines each, :168-171), the ticker fields current_price / avg_volume (:432-433), the trading-
+ * opportunity test (:561-562), and the fifteen combinations of services/utils/indicator_combinations.py (:96-679) that
+ * the monitor adds as combined_indicators (:474-485).  Codes index the name tuples of ai_crypto_trader_b200/_lib.py. */
+#define B200BT_MM_NO_LABEL 255          /* label of a row that is not valid, or whose combination is None */
+#define B200BT_MM_COMBINATIONS 15
+#define B200BT_MM_LABEL_FIELDS 9        /* trend, tma_state, osc_signal, drsi_signal, vpc_confirmation, tsi_direction,
+                                           regime, breakout_status, divergence (label_field 0 .. 8)                   */
+/* present bits: the keys a market_update dict may lack (volume, ema_12, ema_26 are never set by the monitor) */
+#define B200BT_MM_HAS_VOLUME 1
+#define B200BT_MM_HAS_EMA_12 2
+#define B200BT_MM_HAS_EMA_26 4
+#define B200BT_MM_HAS_RSI_3M 8
+#define B200BT_MM_HAS_RSI_5M 16
+#define B200BT_MM_HAS_PRICE_CHANGE_3M 32
+#define B200BT_MM_HAS_AVG_VOLUME 64
+
+typedef struct b200bt_monitor_params {
+    int32_t frame_bars;              /* W >= 1: klines per frame on every clock (the monitor's 100)                       */
+    int32_t label_field;             /* 0 .. B200BT_MM_LABEL_FIELDS - 1: the categorical field written as the label       */
+    double min_price_change_pct;     /* trading_params.min_price_change_pct (0.5)                                         */
+    double min_volume_usdc;          /* trading_params.min_volume_usdc                                                    */
+} b200bt_monitor_params; /* 24 bytes */
+
+typedef struct b200bt_monitor_row {
+    /* snapshot half: market_update's fields */
+    int32_t valid;                   /* 1: the 1-, 3- and 5-minute frames are full and a 15-minute kline exists          */
+    int32_t trend;                   /* 0 uptrend, 1 downtrend, 2 sideways (any other string in a caller's dict)          */
+    int32_t present;                 /* B200BT_MM_HAS_* bits; the history sets rsi_3m, rsi_5m, price_change_3m, avg_volume */
+    int32_t opportunity;             /* |price_change_1m| >= min_price_change_pct and avg_volume >= min_volume_usdc      */
+    double current_price, avg_volume, rsi, rsi_3m, rsi_5m, stoch_k, macd, macd_3m, macd_5m, williams_r, bb_position,
+           trend_strength, price_change_1m, price_change_3m, price_change_5m, price_change_15m;
+    double volume, ema_12, ema_26;   /* read only where present                                                           */
+    /* combination half: combined_indicators */
+    int32_t computed;                /* bit c: combination c (dict order) computed; clear: the reference's None entry    */
+    int32_t tma_state;               /* triple_moving_average.state                                                      */
+    int32_t osc_signal;              /* oscillator_consensus.signal                                                      */
+    int32_t drsi_signal;             /* double_rsi.signal                                                                */
+    int32_t vpc_confirmation;        /* volume_price_confirmation.confirmation (neutral: strength is the int 0)          */
+    int32_t tsi_direction;           /* trend_strength_index.direction + 1                                               */
+    int32_t regime;                  /* market_regime_indicator.regime                                                   */
+    int32_t breakout_status;         /* breakout_confirmation.status                                                     */
+    int32_t divergence;              /* divergence_detector.divergence                                                   */
+    int32_t breakout_direction;      /* breakout_confirmation.direction: -1, 0, 1                                        */
+    int32_t reversal_signals;        /* reversal_probability.signals: bit i = name i, appended in bit order              */
+    int32_t reserved;
+    double trend_confirmation, momentum_trend_alignment, tma_score, volatility_adjusted_momentum, volatility_trend_score,
+           osc_strength, osc_agreement, stoch_rsi, drsi_divergence, vwpm, vpc_strength, tsi_strength, tsi_confidence,
+           regime_confidence, reversal_probability, breakout_confirmation, divergence_strength;
+} b200bt_monitor_row; /* 352 bytes */
+
+/* Market updates of every 1-minute bar.  ohlcv: device float32 [5][S][N] on a 1-minute clock starting at minute0 (Unix
+ * minutes, >= 0); ohlcv_3m / _5m / _15m: [5][S][M_k] made from it by b200bt_resample (M_k = b200bt_resample_bars).
+ * Row t is the update published at the close of bar t.  Frames: on each clock k the W klines ending at j_k(t), the last
+ * kline COMPLETED by the close of t (b200bt_align's rule; j_1(t) = t), so a partial last bucket never enters a frame.
+ * In float64 from the widened inputs, every operation rounded on its own (no FMA contraction):
+ *   EMAs       pandas' ewm(adjust=False) loop: w = x_0; w = ((1-a) w + a x) / ((1-a) + a) unless w == x; a = 1 / (1 + com)
+ *              with com = (1-alpha)/alpha (RSI, alpha = 1/14) or (span-1)/2 (MACD spans 12, 26); outputs before the
+ *              window's length are NaN.  RSI's first up / down moves are 0 (diff.where turns the leading NaN into 0).
+ *   windows    stochastic %K and Williams %R over 14, Bollinger (20, ddof 0, 2 std), SMA 20 / 50 and the 5-minute SMA 20:
+ *              min / max exact; means the sequential sum (oldest first) / w; the variance the two-pass sum of squared
+ *              deviations (oldest first) / w.
+ *   trend      :262-280; trend_strength = |((c - s20) / s20 * 100) * 0.6 + ((c - s20_5m) / s20_5m * 100) * 0.4|.
+ *   ticker     current_price = close[t]; avg_volume = (sequential sum of the volumes of bars max(0, t - 1439) .. t) *
+ *              close[t] (the 24-hour ticker's v * c, cut at the series start).
+ * A row that is not valid has valid = 0, NaN numeric fields, codes B200BT_MM_NO_LABEL and label B200BT_MM_NO_LABEL.
+ * rows_or_null [S][N], labels_or_null uint8 [S][N] (the code of params->label_field); at least one.
+ * Checked before the device: null ohlcv / resampled inputs / params / both outputs, S < 1, N < 1, bar_minutes != 1,
+ * minute0 < 0, M_k != b200bt_resample_bars(N, minute0, 1, k), frame_bars < 1, label_field outside 0 .. 8 (EINVAL);
+ * N >= 2^30, S > 65535 (ELIMIT).  One thread per row; no atomics; deterministic. */
+int b200bt_market_monitor(const float* ohlcv, int S, int64_t N, int64_t minute0, int bar_minutes,
+                          const float* ohlcv_3m, int64_t M3, const float* ohlcv_5m, int64_t M5, const float* ohlcv_15m,
+                          int64_t M15, const b200bt_monitor_params* params, b200bt_monitor_row* rows_or_null,
+                          uint8_t* labels_or_null, b200bt_stream_t stream);
+
+/* The combination half of n rows whose snapshot half (valid, trend, present and the numeric fields) the caller filled:
+ * calculate_combined_indicators (:56-92) on each row read as a dict of Python floats, through the same device step as
+ * b200bt_market_monitor.  round(x, 4) is numpy's rint(x * 1e4) / 1e4 where the reference's value is a numpy float64
+ * (np.tanh / np.sign in the expression), else Python's correctly rounded decimal rounding; min / max / comparisons follow
+ * Python's NaN behaviour; np.tanh is CUDA's tanh.  Rows with valid == 0 are left as they are.  rows: device; n >= 1
+ * (EINVAL), n < 2^31 (ELIMIT). */
+int b200bt_indicator_combinations(b200bt_monitor_row* rows, int64_t n, b200bt_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -20,7 +20,7 @@ from ai_crypto_trader_b200.sweep import MarketData, PopulationSweep
 from oracle import indicators_ref, sim_oracle
 
 legs = sys.argv[1:] or ["sweep", "mc", "joint", "indicators", "pareto", "regime", "dca", "grid_service", "rl",
-                        "volume_profile"]
+                        "volume_profile", "market_monitor"]
 torch.cuda.set_device(0)
 
 if "sweep" in legs:
@@ -209,3 +209,17 @@ if "volume_profile" in legs:
                 assert np.array_equal(g, w, equal_nan=g.dtype.kind == "f"), (W, B, s, t, name)
             assert np.array_equal(bins[s, t], wb[k]) and labels[s, t] == wl[k], (W, B, s, t)
     print("volume_profile ok: rows, bins and labels equal the restatement", flush=True)
+if "market_monitor" in legs:
+    # market monitor: 1- and 100-kline frames off the 15-minute grid, rows and labels in one launch, rows before the first
+    # full frames and in the partial last buckets; validity and labels checked against the restatement
+    sys.path.insert(0, str(Path(__file__).resolve().parents[1] / "tests"))
+    import market_monitor_ref
+    from ai_crypto_trader_b200 import market_monitor as mm
+    m = MarketData(synth.synth_ohlcv(2, 1211, first_symbol=4), minute0=28_401_127)
+    for W in (1, 100):
+        rows, labels = mm._run(m, mm.monitor_params(W, 3), True, True)
+        table = mm.rows_table(rows)
+        want = [market_monitor_ref.row_at(m.ohlcv.cpu().numpy(), m.minute0, 0, t, W)["valid"] for t in range(1211)]
+        assert np.array_equal(table["valid"][0], want), W
+        assert np.array_equal(labels.cpu().numpy(), np.where(table["valid"] == 1, table["drsi_signal"], 255)), W
+    print("market_monitor ok: rows and labels equal the restatement", flush=True)
