@@ -348,6 +348,10 @@ static int mc_launch(int mode, double s0, double drift, double vol, const float*
     B200BT_REQUIRE(finals && maxdd, B200BT_EINVAL, "mc: null output");
     B200BT_REQUIRE(n_paths > 0 && steps >= 0, B200BT_EINVAL, "mc: bad sizes");
     B200BT_REQUIRE(s0 > 0.0, B200BT_EINVAL, "mc: initial price must be positive");
+    if (mode == 1) {
+        B200BT_REQUIRE(returns && R > 0 && block_len > 0, B200BT_EINVAL, "mc_bootstrap: bad return sample");
+        B200BT_REQUIRE((size_t)R * 4 <= 48 * 1024, B200BT_ELIMIT, "mc_bootstrap: at most 12288 returns");
+    }
     int rc = check_device();
     if (rc) return rc;
     const unsigned blocks = (unsigned)((n_paths + MC_THREADS - 1) / MC_THREADS);
@@ -356,8 +360,6 @@ static int mc_launch(int mode, double s0, double drift, double vol, const float*
         mc_paths_kernel<0><<<blocks, MC_THREADS, 0, st>>>(s0, drift, vol, nullptr, 0, 1, 1, n_paths, steps, seed,
                                                            path_offset, finals, maxdd, paths);
     } else {
-        B200BT_REQUIRE(returns && R > 0 && block_len > 0, B200BT_EINVAL, "mc_bootstrap: bad return sample");
-        B200BT_REQUIRE((size_t)R * 4 <= 48 * 1024, B200BT_ELIMIT, "mc_bootstrap: at most 12288 returns");
         mc_paths_kernel<1><<<blocks, MC_THREADS, (size_t)R * 4, st>>>(s0, 0.0, 0.0, returns, R, block_len, log_returns,
                                                                        n_paths, steps, seed, path_offset, finals, maxdd, paths);
     }

@@ -5,7 +5,7 @@
 //   returns            df['close'].pct_change()                                   :208
 //   calculate_var      np.percentile(returns.dropna(), 100 (1 - c))               :217-246
 //   calculate_cvar     mean(returns[returns <= percentile])                       :248-284
-//   asset correlation  pd.DataFrame(returns).corr()  (pairwise complete, Pearson) :286-326
+//   asset correlation  pd.DataFrame(returns).corr()  (pairwise complete over finite values, Pearson) :286-326
 // The percentile itself is b200bt_select (montecarlo.cu) + np.percentile's interpolation on the host.
 #include "common.cuh"
 
@@ -57,25 +57,9 @@ __global__ void tail_final_kernel(const double* __restrict__ partial, int blocks
 }
 
 // ---- correlation ------------------------------------------------------------------------------------
-// Row means over each row's own valid entries: the shift that keeps the raw-moment sums below well conditioned.
-__global__ void __launch_bounds__(256)
-row_mean_kernel(const float* __restrict__ x, int64_t ld, int64_t N, double* __restrict__ mean) {
-    const float* __restrict__ r = x + (int64_t)blockIdx.x * ld;
-    double s = 0.0, c = 0.0;
-    for (int64_t t = threadIdx.x; t < N; t += blockDim.x) {
-        const double v = (double)r[t];
-        if (v == v) { s += v; c += 1.0; }
-    }
-    __shared__ double sm[2][8];
-    s = warp_sum_d(s); c = warp_sum_d(c);
-    if ((threadIdx.x & 31) == 0) { sm[0][threadIdx.x >> 5] = s; sm[1][threadIdx.x >> 5] = c; }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double a = 0.0, b = 0.0;
-        for (int i = 0; i < 8; ++i) { a += sm[0][i]; b += sm[1][i]; }
-        mean[blockIdx.x] = b > 0.0 ? a / b : 0.0;
-    }
-}
+// An entry is an observation when it is finite: pandas' nancorr masks with np.isfinite, so a ±inf return (after a zero
+// close) is missing data like NaN.
+__device__ __forceinline__ bool observed(float v) { return isfinite(v); }
 
 __device__ __forceinline__ void pair_of(int p, int S, int& i, int& j) {
     // p-th pair (i <= j) in row-major order of the upper triangle
@@ -85,20 +69,23 @@ __device__ __forceinline__ void pair_of(int p, int S, int& i, int& j) {
 }
 
 constexpr int CORR_THREADS = 256;
+constexpr int CORR_PARTIAL = 8;   // n, kx, ky, Su, Sv, Suu, Svv, Suv
 
-// grid (time splits, pair blocks): each thread owns one (i, j) pair and accumulates, over the CTA's share of
-// the time axis and over the bars where BOTH series are valid, n, Sx, Sy, Sxx, Syy, Sxy of the mean-shifted values.
+// grid (time splits, pair blocks): each thread owns one (i, j) pair and accumulates, over the CTA's share of the time
+// axis and over the bars where BOTH series are observed, n and the sums Su, Sv, Suu, Svv, Suv of u = x - kx, v = y - ky,
+// shifted by the split's first joint observation (kx, ky).  The shift is exact in float64, so a series that is constant
+// over the pair's joint observations gives u = 0 and a variance of exactly 0, and the cancellation in Suu - Su^2/n is
+// bounded by the pair's own spread over the split, not by the row's level elsewhere.
 // A tile of all S rows is staged through shared memory (row stride T+1 words: conflict-free column reads).
 __global__ void __launch_bounds__(CORR_THREADS)
-corr_partial_kernel(const float* __restrict__ x, int64_t ld, int S, int64_t N, int T, const double* __restrict__ mean,
-                    double* __restrict__ partial) {
+corr_partial_kernel(const float* __restrict__ x, int64_t ld, int S, int64_t N, int T, double* __restrict__ partial) {
     extern __shared__ float tile[];
     const int n_pairs = S * (S + 1) / 2;
     const int p = blockIdx.y * CORR_THREADS + threadIdx.x;
     int i = 0, j = 0;
     if (p < n_pairs) pair_of(p, S, i, j);
-    const double mi = mean[i], mj = mean[j];
-    double n = 0.0, sx = 0.0, sy = 0.0, sxx = 0.0, syy = 0.0, sxy = 0.0;
+    int64_t n = 0;   // an integer count keeps the FP64 pipe for the sums
+    double kx = 0.0, ky = 0.0, su = 0.0, sv = 0.0, suu = 0.0, svv = 0.0, suv = 0.0;
     const int64_t tiles = (N + T - 1) / T;
     for (int64_t tl = blockIdx.x; tl < tiles; tl += gridDim.x) {
         const int64_t t0 = tl * T;
@@ -112,36 +99,59 @@ corr_partial_kernel(const float* __restrict__ x, int64_t ld, int S, int64_t N, i
         if (p < n_pairs) {
             const float* __restrict__ a = tile + i * (T + 1);
             const float* __restrict__ b = tile + j * (T + 1);
-            for (int c = 0; c < len; ++c) {
+            int c = 0;
+            if (n == 0) {   // until the split's first joint observation, which sets the shift
+                for (; c < len; ++c) {
+                    if (observed(a[c]) && observed(b[c])) { kx = (double)a[c]; ky = (double)b[c]; break; }
+                }
+            }
+            for (; c < len; ++c) {
                 const float fa = a[c], fb = b[c];
-                if (fa == fa && fb == fb) {
-                    const double u = (double)fa - mi, v = (double)fb - mj;
-                    n += 1.0; sx += u; sy += v;
-                    sxx = fma(u, u, sxx); syy = fma(v, v, syy); sxy = fma(u, v, sxy);
+                if (observed(fa) && observed(fb)) {
+                    const double u = (double)fa - kx, v = (double)fb - ky;
+                    ++n; su += u; sv += v;
+                    suu = fma(u, u, suu); svv = fma(v, v, svv); suv = fma(u, v, suv);
                 }
             }
         }
     }
     if (p < n_pairs) {
-        double* o = partial + ((int64_t)blockIdx.x * n_pairs + p) * 6;
-        o[0] = n; o[1] = sx; o[2] = sy; o[3] = sxx; o[4] = syy; o[5] = sxy;
+        double* o = partial + ((int64_t)blockIdx.x * n_pairs + p) * CORR_PARTIAL;
+        o[0] = (double)n; o[1] = kx; o[2] = ky; o[3] = su; o[4] = sv; o[5] = suu; o[6] = svv; o[7] = suv;
     }
 }
 
+// Folds the time splits in order with the pairwise update of mean, M2 and co-moment (Chan, Golub & LeVeque): a split's
+// moments about its own mean, then merged by the difference of the means.  A constant run keeps M2 = 0 exactly.
 __global__ void corr_final_kernel(const double* __restrict__ partial, int splits, int S, double* __restrict__ out) {
     const int n_pairs = S * (S + 1) / 2;
     const int p = blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= n_pairs) return;
     int i, j;
     pair_of(p, S, i, j);
-    double a[6] = {0, 0, 0, 0, 0, 0};
-    for (int s = 0; s < splits; ++s)
-        for (int k = 0; k < 6; ++k) a[k] += partial[((int64_t)s * n_pairs + p) * 6 + k];
-    const double n = a[0];
+    double n = 0.0, mx = 0.0, my = 0.0, m2x = 0.0, m2y = 0.0, cxy = 0.0;
+    for (int s = 0; s < splits; ++s) {
+        const double* q = partial + ((int64_t)s * n_pairs + p) * CORR_PARTIAL;
+        const double nb = q[0];
+        if (nb == 0.0) continue;
+        const double du = q[3] / nb, dv = q[4] / nb;
+        const double bmx = q[1] + du, bmy = q[2] + dv;
+        const double bm2x = q[5] - q[3] * du, bm2y = q[6] - q[4] * dv, bcxy = q[7] - q[3] * dv;
+        if (n == 0.0) {
+            n = nb; mx = bmx; my = bmy; m2x = bm2x; m2y = bm2y; cxy = bcxy;
+            continue;
+        }
+        const double nt = n + nb, ex = bmx - mx, ey = bmy - my, f = n * nb / nt;
+        m2x += bm2x + ex * ex * f;
+        m2y += bm2y + ey * ey * f;
+        cxy += bcxy + ex * ey * f;
+        mx += ex * (nb / nt);
+        my += ey * (nb / nt);
+        n = nt;
+    }
     double r = __longlong_as_double(0x7ff8000000000000ll);
     if (n >= 1.0) {
-        const double vx = a[3] - a[1] * a[1] / n, vy = a[4] - a[2] * a[2] / n, cxy = a[5] - a[1] * a[2] / n;
-        const double den = sqrt(vx * vy);
+        const double den = sqrt(m2x * m2y);
         if (den > 0.0) r = fmin(1.0, fmax(-1.0, cxy / den));
     }
     out[(int64_t)i * S + j] = r;
@@ -156,6 +166,7 @@ extern "C" int b200bt_pct_change(const float* close, int64_t ld, int S, int64_t 
                                  b200bt_stream_t stream) {
     B200BT_REQUIRE(close && out, B200BT_EINVAL, "pct_change: null pointer");
     B200BT_REQUIRE(S > 0 && N > 0 && ld >= N && ld_out >= N, B200BT_EINVAL, "pct_change: bad sizes");
+    B200BT_REQUIRE(S <= 65535, B200BT_ELIMIT, "pct_change: at most 65535 rows (S = %d)", S);
     int rc = check_device();
     if (rc) return rc;
     const unsigned bx = (unsigned)min((int64_t)1184, (N + 255) / 256);
@@ -199,7 +210,7 @@ static int corr_splits(int S, int64_t N) {
 
 extern "C" int64_t b200bt_correlation_workspace_bytes(int S, int64_t N) {
     if (S <= 0 || S > 512 || N <= 0) return 0;
-    return ((int64_t)corr_splits(S, N) * (S * (S + 1) / 2) * 6 + S) * 8;
+    return (int64_t)corr_splits(S, N) * (S * (S + 1) / 2) * CORR_PARTIAL * 8;
 }
 
 extern "C" int b200bt_correlation(const float* x, int64_t ld, int S, int64_t N, double* out, void* workspace,
@@ -210,16 +221,13 @@ extern "C" int b200bt_correlation(const float* x, int64_t ld, int S, int64_t N, 
     int rc = check_device();
     if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    double* mean = (double*)workspace;
-    double* partial = mean + S;
+    double* partial = (double*)workspace;
     const int T = corr_tile(S), splits = corr_splits(S, N);
     const int n_pairs = S * (S + 1) / 2, pair_blocks = (n_pairs + CORR_THREADS - 1) / CORR_THREADS;
     const size_t smem = (size_t)S * (T + 1) * 4;
     cudaError_t e = cudaFuncSetAttribute(corr_partial_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return cuda_status(e, "correlation: cudaFuncSetAttribute");
-    row_mean_kernel<<<S, 256, 0, st>>>(x, ld, N, mean);
-    B200BT_LAUNCH_CHECK("row_mean launch");
-    corr_partial_kernel<<<dim3((unsigned)splits, (unsigned)pair_blocks), CORR_THREADS, smem, st>>>(x, ld, S, N, T, mean, partial);
+    corr_partial_kernel<<<dim3((unsigned)splits, (unsigned)pair_blocks), CORR_THREADS, smem, st>>>(x, ld, S, N, T, partial);
     B200BT_LAUNCH_CHECK("corr_partial launch");
     corr_final_kernel<<<(n_pairs + 127) / 128, 128, 0, st>>>(partial, splits, S, out);
     B200BT_LAUNCH_CHECK("corr_final launch");

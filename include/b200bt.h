@@ -424,13 +424,13 @@ int b200bt_mc_gbm(double s0, double mu, double sigma, double dt, int64_t n_paths
 /* 'historical' simulation (:277-298): bootstrap of the return sample with
  * replacement.  block_len = 1 reproduces the reference (iid); block_len > 1 is a
  * circular block bootstrap.  log_returns != 0: P_t = P_{t-1} exp(r); else
- * P_t = P_{t-1} (1 + r).  `returns` is a device array of R <= 12288 fp32 values. */
+ * P_t = P_{t-1} (1 + r).  `returns` is a device array of R <= 12288 fp32 values (B200BT_ELIMIT above). */
 int b200bt_mc_bootstrap(const float* returns, int R, int block_len, int log_returns, double s0,
                         int64_t n_paths, int steps, uint64_t seed, uint64_t path_offset,
                         float* finals, float* maxdd, float* paths_or_null, b200bt_stream_t stream);
 
 /* Exact order statistics: out[r] = ranks[r]-th smallest (0-based) of x[0..n).
- * ranks_dev: device int64[n_ranks], ASCENDING, n_ranks <= 64.  Two-level radix
+ * ranks_dev: device int64[n_ranks] in any order, repeats allowed, 1 <= n_ranks <= 64.  Two-level radix
  * select; workspace of b200bt_select_workspace_bytes(n_ranks) device bytes.
  * Feeds np.percentile's linear interpolation (:308-317) on the host side. */
 int64_t b200bt_select_workspace_bytes(int n_ranks);
@@ -568,11 +568,12 @@ int b200bt_cscv(const double* pnl, int64_t ld, int N, int64_t T, int B, void* wo
  * Replaces the numeric core of services/portfolio_risk_service.py. */
 
 /* Simple returns, df['close'].pct_change() (portfolio_risk_service.py:208): out[s][0] = NaN,
- * out[s][t] = close[s][t]/close[s][t-1] - 1 in float64, stored fp32.  close, out: device [S][ld]. */
+ * out[s][t] = close[s][t]/close[s][t-1] - 1 in float64, stored fp32 (after a zero close +-inf, or NaN for 0/0, as
+ * pandas gives).  close, out: device [S][ld]; S <= 65535 (B200BT_ELIMIT above). */
 int b200bt_pct_change(const float* close, int64_t ld, int S, int64_t N, float* out, int64_t ld_out,
                       b200bt_stream_t stream);
 
-/* Tail sums for historical CVaR (calculate_conditional_var :248-284), NaN entries skipped (dropna):
+/* Tail sums for historical CVaR (calculate_conditional_var :248-284), NaN entries skipped (dropna; +-inf are kept):
  * out4 (device, float64) = [ sum x[x <= threshold], #(x <= threshold), #(non-NaN), sum non-NaN ].
  * Deterministic (fixed-order fold of per-CTA partials). */
 int64_t b200bt_tail_stats_workspace_bytes(int64_t n);
@@ -580,8 +581,11 @@ int b200bt_tail_stats(const float* x, int64_t n, double threshold, double* out4,
                       int64_t workspace_bytes, b200bt_stream_t stream);
 
 /* Pearson correlation matrix of S return rows (calculate_asset_correlation :286-326, pandas
- * DataFrame.corr(): pairwise-complete observations, NaN = missing; NaN out for <1 joint observation or zero
- * variance).  x: device [S][ld] fp32, out: device float64 [S][S], S <= 512. */
+ * DataFrame.corr(): pairwise-complete observations).  An entry is observed when it is finite: NaN and +-inf are both
+ * missing, as pandas' np.isfinite mask makes them.  NaN out for no joint observation or zero variance over the pair's
+ * joint observations; a series that is constant over them (a stale feed) gives exactly zero variance, hence NaN.
+ * Deterministic (fixed-order fold of per-split partials, no atomics).  x: device [S][ld] fp32, out: device float64
+ * [S][S], S <= 512. */
 int64_t b200bt_correlation_workspace_bytes(int S, int64_t N);
 int b200bt_correlation(const float* x, int64_t ld, int S, int64_t N, double* out, void* workspace,
                        int64_t workspace_bytes, b200bt_stream_t stream);

@@ -1,5 +1,6 @@
-"""Status codes of the joint (portfolio) Monte-Carlo entry points: argument checks come before the device check, so
-EINVAL and ELIMIT are exercised with or without a GPU; ENODEVICE without one."""
+"""Status codes of the risk entry points (joint Monte-Carlo, bootstrap paths, order statistics, returns, tail sums and
+correlation): argument checks come before the device check, so EINVAL and ELIMIT are exercised with or without a GPU;
+ENODEVICE without one."""
 import ctypes as C
 
 import pytest
@@ -62,3 +63,28 @@ def test_portfolio_entry_points_limits(native_lib):
     assert _status(_gbm(S=33)) == ELIMIT
     assert _status(_boot(S=33)) == ELIMIT
     assert _status(_boot(S=4, R=3073)) == ELIMIT                      # R x S > 12288 table entries
+
+
+_BUF = (C.c_float * 64)()
+_P = C.addressof(_BUF)           # any non-null pointer: the arguments are refused before anything is read
+
+
+def test_risk_entry_points_validate_arguments(native_lib):
+    lib = native_lib
+    ws = int(lib.b200bt_correlation_workspace_bytes(4, 100))
+    assert _status(("b200bt_correlation", _P, 100, 513, 100, _P, _P, 1 << 40, None)) == EINVAL      # S > 512
+    assert _status(("b200bt_correlation", _P, 99, 4, 100, _P, _P, ws, None)) == EINVAL              # ld < N
+    assert _status(("b200bt_correlation", _P, 100, 4, 100, _P, _P, ws - 8, None)) == EINVAL         # workspace
+    need = int(lib.b200bt_select_workspace_bytes(3))
+    assert _status(("b200bt_select", _P, 10, _P, 0, _P, _P, 1 << 40, None)) == EINVAL               # no rank
+    assert _status(("b200bt_select", _P, 10, _P, 65, _P, _P, 1 << 40, None)) == EINVAL              # > 64 ranks
+    assert _status(("b200bt_select", _P, 10, _P, 3, _P, _P, need - 1, None)) == EINVAL              # workspace
+    assert _status(("b200bt_tail_stats", _P, 0, 0.0, _P, _P, 1 << 20, None)) == EINVAL              # empty input
+    assert _status(("b200bt_pct_change", _P, 99, 2, 100, _P, 100, None)) == EINVAL                  # ld < N
+
+
+def test_risk_entry_points_limits(native_lib):
+    def boot(R):
+        return ("b200bt_mc_bootstrap", _P, R, 1, 1, 100.0, 8, 4, 1, 0, _P, _P, None, None)
+    assert _status(boot(12289)) == ELIMIT                                # more than 48 KB of table
+    assert _status(("b200bt_pct_change", _P, 10, 65536, 10, _P, 10, None)) == ELIMIT   # S rides on gridDim.y

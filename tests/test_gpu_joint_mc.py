@@ -59,7 +59,7 @@ def test_bootstrap_assets_bit_equal_single_asset_bootstrap(engine, log_returns, 
 
 @pytest.mark.parametrize("n_paths", [1, 129])
 @pytest.mark.parametrize("steps", [0, 1, 3, 29, 1001])
-@pytest.mark.parametrize("S", [1, 3, 8, 32])
+@pytest.mark.parametrize("S", [1, 3, 4, 5, 8, 9, 17, 32])
 def test_joint_gbm_matches_oracle(engine, S, steps, n_paths):
     s0, qty, mu, sigma, L = _params(S, 100 + S)
     f, d, af = engine.portfolio_gbm(s0, qty, mu, sigma, DT, L, n_paths, steps, 99, path_offset=3, asset_finals=True)

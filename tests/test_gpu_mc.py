@@ -18,7 +18,8 @@ def engine(native_lib):
     return PathEngine()
 
 
-@pytest.mark.parametrize("n_paths,steps", [(1, 1), (7, 3), (1000, 29), (4096, 250), (333, 1001)])
+@pytest.mark.parametrize("n_paths,steps", [(1, 1), (7, 3), (1000, 29), (4096, 250), (333, 1001)] +
+                         [(n, s) for n in (255, 256, 257) for s in (0, 2, 4, 5, 8)])
 def test_gbm_matches_philox_oracle(engine, n_paths, steps):
     from oracle import mc_ref
     mu, sigma, dt, s0, seed = 0.126, 0.3175, 1 / 252, 100.0, 2024
