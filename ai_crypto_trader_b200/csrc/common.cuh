@@ -115,4 +115,15 @@ __host__ __device__ __forceinline__ uint64_t event_hash(uint32_t index, uint32_t
     return ((uint64_t)b << 32) | a;
 }
 
+// The bar clock the strategy entry points accept: N bars of bar_minutes > 0 from Unix minute minute0 >= 0, every bar's
+// minute below 2^62.
+inline bool bar_clock_ok(int64_t minute0, int64_t N, int bar_minutes) {
+    return bar_minutes > 0 && minute0 >= 0 && minute0 + N * (int64_t)bar_minutes < (1ll << 62);
+}
+
+// Calendar days from the day of bar 0 (day minute0 / 1440) to the day of bar N - 1: the length of a per-day row.
+inline int64_t series_days(int64_t minute0, int64_t N, int bar_minutes) {
+    return (minute0 + (N - 1) * (int64_t)bar_minutes) / 1440 - minute0 / 1440 + 1;
+}
+
 }  // namespace b200bt

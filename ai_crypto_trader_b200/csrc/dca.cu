@@ -405,12 +405,12 @@ extern "C" int b200bt_dca_dip_pct(const float* high, const float* close, int64_t
     B200BT_REQUIRE(high && close && dip_pct, B200BT_EINVAL, "dca_dip_pct: null pointer");
     B200BT_REQUIRE(S >= 1 && N >= 1 && ld >= N && ld_dip >= N, B200BT_EINVAL, "dca_dip_pct: bad sizes");
     B200BT_REQUIRE(N < (1ll << 30), B200BT_ELIMIT, "dca_dip_pct: N must be < 2^30 bars");
-    B200BT_REQUIRE(bar_minutes > 0 && minute0 >= 0 && minute0 + N * (int64_t)bar_minutes < (1ll << 62), B200BT_EINVAL,
+    B200BT_REQUIRE(bar_clock_ok(minute0, N, bar_minutes), B200BT_EINVAL,
                    "dca_dip_pct: bad bar clock (bar_minutes > 0, minute0 >= 0)");
     int rc = check_device();
     if (rc) return rc;
     const int64_t first_day = minute0 / 1440;
-    const int64_t n_days = (minute0 + (N - 1) * (int64_t)bar_minutes) / 1440 - first_day + 1;
+    const int64_t n_days = series_days(minute0, N, bar_minutes);
     const int64_t warps = (n_days + DIP_RUN - 1) / DIP_RUN * S;
     dca_dip_kernel<<<(unsigned)((warps + 7) / 8), 256, 0, (cudaStream_t)stream>>>(high, close, ld, S, N, minute0, bar_minutes,
                                                                                  dip_pct, ld_dip, first_day, n_days);
@@ -438,16 +438,14 @@ extern "C" int b200bt_dca_sweep(const float* close, int64_t ld_close, const doub
     B200BT_REQUIRE(N < (1ll << 30), B200BT_ELIMIT, "dca_sweep: N must be < 2^30 bars");
     B200BT_REQUIRE(start_bar >= 0 && start_bar < N, B200BT_EINVAL, "dca_sweep: start_bar = %lld outside [0, N = %lld)",
                    (long long)start_bar, (long long)N);
-    B200BT_REQUIRE(bar_minutes > 0 && minute0 >= 0 && minute0 + N * (int64_t)bar_minutes < (1ll << 62) &&
-                       N * (int64_t)bar_minutes < (1ll << 62) / 60000000ll,
+    B200BT_REQUIRE(bar_clock_ok(minute0, N, bar_minutes) && N * (int64_t)bar_minutes < (1ll << 62) / 60000000ll,
                    B200BT_EINVAL, "dca_sweep: bad bar clock (bar_minutes > 0, minute0 >= 0, N * bar_minutes us < 2^62)");
     B200BT_REQUIRE(!labels_or_null || ld_labels == 0 || ld_labels >= N, B200BT_EINVAL,
                    "dca_sweep: ld_labels must be 0 (one shared row) or >= N");
     B200BT_REQUIRE(workspace_bytes >= b200bt_dca_workspace_bytes(S, N), B200BT_EINVAL,
                    "dca_sweep: workspace of %lld bytes, %lld needed", (long long)workspace_bytes,
                    (long long)b200bt_dca_workspace_bytes(S, N));
-    const int64_t first_day = minute0 / 1440;
-    const int64_t need_days = (minute0 + (N - 1) * (int64_t)bar_minutes) / 1440 - first_day + 1;
+    const int64_t need_days = series_days(minute0, N, bar_minutes);
     B200BT_REQUIRE(!day_or_null || D >= need_days, B200BT_EINVAL, "dca_sweep: D = %lld days, the series spans %lld",
                    (long long)D, (long long)need_days);
     B200BT_REQUIRE(!(rebalance_any || day_or_null) || S <= B200BT_DCA_MAX_COUPLED, B200BT_ELIMIT,
@@ -478,7 +476,7 @@ extern "C" int b200bt_dca_sweep(const float* close, int64_t ld_close, const doub
     a.minute0 = minute0;
     a.ld_labels = ld_labels;
     a.D = D;
-    a.first_day = first_day;
+    a.first_day = minute0 / 1440;
     a.tick_us = (int64_t)bar_minutes * 60000000ll;
     a.S = S;
     a.pop = pop;

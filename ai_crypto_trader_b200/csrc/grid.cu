@@ -527,35 +527,35 @@ grid_service_kernel(const GridArgs a, b200bt_grid_service_stats* service) {
 
 using namespace b200bt;
 
-extern "C" int b200bt_grid_sweep(const float* price, int64_t ld_price, int S, int64_t N, int64_t start_bar, int bar_minutes,
-                                 int64_t minute0, const b200bt_grid_individual* indiv, int pop, const double* qty,
-                                 const double* init_bounds, const uint8_t* labels_or_null, int64_t ld_labels,
-                                 const b200bt_grid_regime_rule* regime_table_host_or_null, b200bt_grid_stats* stats,
-                                 double* day_profit_or_null, int64_t D, b200bt_stream_t stream) {
-    B200BT_REQUIRE(price && indiv && qty && init_bounds && stats, B200BT_EINVAL, "grid_sweep: null pointer");
-    B200BT_REQUIRE(S >= 1 && pop >= 1 && N >= 1 && ld_price >= N, B200BT_EINVAL, "grid_sweep: bad sizes");
-    B200BT_REQUIRE(N < (1ll << 30), B200BT_ELIMIT, "grid_sweep: N must be < 2^30 bars");
-    B200BT_REQUIRE(start_bar >= 0 && start_bar < N, B200BT_EINVAL, "grid_sweep: start_bar = %lld outside [0, N = %lld)",
+// The argument checks of both grid entry points (messages prefixed by `what`) and their GridArgs.  The lane sweep reads a
+// label row per symbol or one shared row; the service reads one row.
+static int grid_args(const char* what, bool service, const float* price, int64_t ld_price, int S, int64_t N,
+                     int64_t start_bar, int bar_minutes, int64_t minute0, const b200bt_grid_individual* indiv, int pop,
+                     const double* qty, const double* init_bounds, const uint8_t* labels_or_null, int64_t ld_labels,
+                     const b200bt_grid_regime_rule* regime_table_host_or_null, b200bt_grid_stats* stats,
+                     double* day_profit_or_null, int64_t D, GridArgs& a) {
+    B200BT_REQUIRE(price && indiv && qty && init_bounds && stats, B200BT_EINVAL, "%s: null pointer", what);
+    B200BT_REQUIRE(S >= 1 && pop >= 1 && N >= 1 && ld_price >= N, B200BT_EINVAL, "%s: bad sizes", what);
+    B200BT_REQUIRE(N < (1ll << 30), B200BT_ELIMIT, "%s: N must be < 2^30 bars", what);
+    B200BT_REQUIRE(start_bar >= 0 && start_bar < N, B200BT_EINVAL, "%s: start_bar = %lld outside [0, N = %lld)", what,
                    (long long)start_bar, (long long)N);
-    B200BT_REQUIRE(bar_minutes > 0 && minute0 >= 0 && minute0 + N * (int64_t)bar_minutes < (1ll << 62), B200BT_EINVAL,
-                   "grid_sweep: bad bar clock (bar_minutes > 0, minute0 >= 0)");
-    B200BT_REQUIRE(!labels_or_null || ld_labels == 0 || ld_labels >= N, B200BT_EINVAL,
-                   "grid_sweep: ld_labels must be 0 (one shared row) or >= N");
-    const int64_t first_day = minute0 / 1440;
-    const int64_t need_days = (minute0 + (N - 1) * (int64_t)bar_minutes) / 1440 - first_day + 1;
-    B200BT_REQUIRE(!day_profit_or_null || D >= need_days, B200BT_EINVAL,
-                   "grid_sweep: D = %lld days, the series spans %lld", (long long)D, (long long)need_days);
-    GridArgs a;
-    if (regime_table_host_or_null) {
-        for (int r = 0; r < B200BT_GRID_REGIME_RULES; ++r) {
-            const b200bt_grid_regime_rule& q = regime_table_host_or_null[r];
-            B200BT_REQUIRE(!q.apply || (q.num_grids >= 1 && q.num_grids <= B200BT_GRID_MAX_GRIDS), B200BT_EINVAL,
-                           "grid_sweep: regime rule %d sets num_grids = %d outside 1 .. %d", r, q.num_grids,
-                           B200BT_GRID_MAX_GRIDS);
-            a.rules[r] = q;
-        }
+    B200BT_REQUIRE(bar_clock_ok(minute0, N, bar_minutes), B200BT_EINVAL,
+                   "%s: bad bar clock (bar_minutes > 0, minute0 >= 0)", what);
+    if (service) {
+        B200BT_REQUIRE(!labels_or_null || ld_labels == 0, B200BT_EINVAL,
+                       "%s: ld_labels must be 0: the service reads one regime label row", what);
     } else {
-        for (int r = 0; r < B200BT_GRID_REGIME_RULES; ++r) a.rules[r] = b200bt_grid_regime_rule{0, 0, 0.0, 0.0};
+        B200BT_REQUIRE(!labels_or_null || ld_labels == 0 || ld_labels >= N, B200BT_EINVAL,
+                       "%s: ld_labels must be 0 (one shared row) or >= N", what);
+    }
+    const int64_t need_days = series_days(minute0, N, bar_minutes);
+    B200BT_REQUIRE(!day_profit_or_null || D >= need_days, B200BT_EINVAL, "%s: D = %lld days, the series spans %lld", what,
+                   (long long)D, (long long)need_days);
+    for (int r = 0; r < B200BT_GRID_REGIME_RULES; ++r) {
+        a.rules[r] = regime_table_host_or_null ? regime_table_host_or_null[r] : b200bt_grid_regime_rule{0, 0, 0.0, 0.0};
+        B200BT_REQUIRE(!a.rules[r].apply || (a.rules[r].num_grids >= 1 && a.rules[r].num_grids <= B200BT_GRID_MAX_GRIDS),
+                       B200BT_EINVAL, "%s: regime rule %d sets num_grids = %d outside 1 .. %d", what, r,
+                       a.rules[r].num_grids, B200BT_GRID_MAX_GRIDS);
     }
     int rc = check_device();
     if (rc) return rc;
@@ -564,9 +564,9 @@ extern "C" int b200bt_grid_sweep(const float* price, int64_t ld_price, int S, in
     a.N = N;
     a.start_bar = start_bar;
     a.minute0 = minute0;
-    a.ld_labels = ld_labels;
+    a.ld_labels = service ? 0 : ld_labels;
     a.D = D;
-    a.first_day = first_day;
+    a.first_day = minute0 / 1440;
     a.S = S;
     a.pop = pop;
     a.bar_minutes = bar_minutes;
@@ -577,6 +577,18 @@ extern "C" int b200bt_grid_sweep(const float* price, int64_t ld_price, int S, in
     a.labels = labels_or_null;
     a.stats = stats;
     a.day = day_profit_or_null;
+    return B200BT_OK;
+}
+
+extern "C" int b200bt_grid_sweep(const float* price, int64_t ld_price, int S, int64_t N, int64_t start_bar, int bar_minutes,
+                                 int64_t minute0, const b200bt_grid_individual* indiv, int pop, const double* qty,
+                                 const double* init_bounds, const uint8_t* labels_or_null, int64_t ld_labels,
+                                 const b200bt_grid_regime_rule* regime_table_host_or_null, b200bt_grid_stats* stats,
+                                 double* day_profit_or_null, int64_t D, b200bt_stream_t stream) {
+    GridArgs a;
+    int rc = grid_args("grid_sweep", false, price, ld_price, S, N, start_bar, bar_minutes, minute0, indiv, pop, qty,
+                       init_bounds, labels_or_null, ld_labels, regime_table_host_or_null, stats, day_profit_or_null, D, a);
+    if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     const unsigned groups = (unsigned)((pop + GR_WARPS - 1) / GR_WARPS);
     if (day_profit_or_null) {
@@ -594,46 +606,10 @@ extern "C" int b200bt_grid_service_sweep(const float* price, int64_t ld_price, i
                                          int64_t ld_labels, const b200bt_grid_regime_rule* regime_table_host_or_null,
                                          b200bt_grid_stats* stats, b200bt_grid_service_stats* service_or_null,
                                          double* day_profit_or_null, int64_t D, b200bt_stream_t stream) {
-    B200BT_REQUIRE(price && indiv && qty && init_bounds && stats, B200BT_EINVAL, "grid_service_sweep: null pointer");
-    B200BT_REQUIRE(S >= 1 && pop >= 1 && N >= 1 && ld_price >= N, B200BT_EINVAL, "grid_service_sweep: bad sizes");
-    B200BT_REQUIRE(N < (1ll << 30), B200BT_ELIMIT, "grid_service_sweep: N must be < 2^30 bars");
-    B200BT_REQUIRE(start_bar >= 0 && start_bar < N, B200BT_EINVAL,
-                   "grid_service_sweep: start_bar = %lld outside [0, N = %lld)", (long long)start_bar, (long long)N);
-    B200BT_REQUIRE(bar_minutes > 0 && minute0 >= 0 && minute0 + N * (int64_t)bar_minutes < (1ll << 62), B200BT_EINVAL,
-                   "grid_service_sweep: bad bar clock (bar_minutes > 0, minute0 >= 0)");
-    B200BT_REQUIRE(!labels_or_null || ld_labels == 0, B200BT_EINVAL,
-                   "grid_service_sweep: ld_labels must be 0: the service reads one regime label row");
-    const int64_t first_day = minute0 / 1440;
-    const int64_t need_days = (minute0 + (N - 1) * (int64_t)bar_minutes) / 1440 - first_day + 1;
-    B200BT_REQUIRE(!day_profit_or_null || D >= need_days, B200BT_EINVAL,
-                   "grid_service_sweep: D = %lld days, the series spans %lld", (long long)D, (long long)need_days);
     GridArgs a;
-    for (int r = 0; r < B200BT_GRID_REGIME_RULES; ++r) {
-        a.rules[r] = regime_table_host_or_null ? regime_table_host_or_null[r] : b200bt_grid_regime_rule{0, 0, 0.0, 0.0};
-        B200BT_REQUIRE(!a.rules[r].apply || (a.rules[r].num_grids >= 1 && a.rules[r].num_grids <= B200BT_GRID_MAX_GRIDS),
-                       B200BT_EINVAL, "grid_service_sweep: regime rule %d sets num_grids = %d outside 1 .. %d", r,
-                       a.rules[r].num_grids, B200BT_GRID_MAX_GRIDS);
-    }
-    int rc = check_device();
+    int rc = grid_args("grid_service_sweep", true, price, ld_price, S, N, start_bar, bar_minutes, minute0, indiv, pop, qty,
+                       init_bounds, labels_or_null, ld_labels, regime_table_host_or_null, stats, day_profit_or_null, D, a);
     if (rc) return rc;
-    a.price = price;
-    a.ld_price = ld_price;
-    a.N = N;
-    a.start_bar = start_bar;
-    a.minute0 = minute0;
-    a.ld_labels = 0;
-    a.D = D;
-    a.first_day = first_day;
-    a.S = S;
-    a.pop = pop;
-    a.bar_minutes = bar_minutes;
-    a.use_rules = regime_table_host_or_null != nullptr;
-    a.indiv = indiv;
-    a.qty = qty;
-    a.bounds = init_bounds;
-    a.labels = labels_or_null;
-    a.stats = stats;
-    a.day = day_profit_or_null;
     cudaStream_t st = (cudaStream_t)stream;
     if (day_profit_or_null) {
         grid_service_kernel<true><<<(unsigned)pop, 32, 0, st>>>(a, service_or_null);

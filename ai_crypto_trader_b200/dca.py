@@ -22,18 +22,18 @@ import copy
 import ctypes as C
 import logging
 import math
-from datetime import datetime, timedelta, timezone
+from datetime import datetime, timedelta
 from typing import Dict, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 import torch
 
 from . import _lib
+from .population import StrategySweep, iso_minute
 
 logger = logging.getLogger("b200bt.dca")
 
 FIELDS = _lib.DCA_STATS_FIELDS
-WORDS = len(FIELDS)
 OBJECTIVE_FIELDS = FIELDS[:-3]          # purchase_hash, n_ticks and reserved describe the run, not the strategy
 SERVICE_FIELDS = _lib.DCA_SERVICE_FIELDS
 REGIMES = _lib.REGIMES
@@ -232,7 +232,7 @@ def decode_individual(params: Dict, block: Dict, symbols: Sequence[str], bar_min
     return {"individual": iv, "first_us": first, "target": target, "service": svc}
 
 
-class DCASweep:
+class DCASweep(StrategySweep):
     """b200bt_dca_sweep for populations of DCA parameter dicts on one market.
 
     market              MarketData (device closes and highs, bar clock); every close from start_bar on must be > 0
@@ -247,6 +247,10 @@ class DCASweep:
 
     The rebalance targets depend on the config alone, so they are the same for every individual.  Individuals that
     decode alike are evaluated once."""
+
+    FIELDS, OBJECTIVE_FIELDS, SERVICE_FIELDS = FIELDS, OBJECTIVE_FIELDS, SERVICE_FIELDS
+    SERVICE_OBJECTIVE_FIELDS = SERVICE_FIELDS
+    service = True
 
     def __init__(self, market, config: Optional[Dict] = None, regime=None, start_bar: int = 0, usdc_balance: float = 0.0,
                  quantity_precision: Union[None, int, Sequence[int]] = None, objective: str = "total_profit_pct"):
@@ -280,17 +284,6 @@ class DCASweep:
         self.dip = dip_pct(market)
         self._ws = torch.empty(max(1, _lib.load().b200bt_dca_workspace_bytes(S, N)), dtype=torch.uint8,
                                device=market.device)
-        self._stats = self._service = None
-        self._inverse = None
-
-    @staticmethod
-    def _column(name: str) -> Tuple[str, int]:
-        if name in OBJECTIVE_FIELDS:
-            return "stats", OBJECTIVE_FIELDS.index(name)
-        if name in SERVICE_FIELDS:
-            return "service", SERVICE_FIELDS.index(name)
-        raise ValueError(f"{name!r} is neither a DCA stats field ({', '.join(OBJECTIVE_FIELDS)}) nor a service field "
-                         f"({', '.join(SERVICE_FIELDS)})")
 
     # -- host decoding --------------------------------------------------------------------------------------------
     def decode(self, population: List[Dict]) -> Tuple[np.ndarray, np.ndarray, np.ndarray, bool]:
@@ -308,122 +301,28 @@ class DCASweep:
         flags = np.array([r.flags for r in rows])
         return packed, first, target, bool(np.any(flags & _lib.DCA_REBALANCE))
 
-    # -- device evaluation ----------------------------------------------------------------------------------------
-    def _run(self, population: List[Dict], day: bool = False):
-        if not population:
-            raise ValueError("an empty population")
-        m = self.market
+    def _inputs(self, population: List[Dict]):
         packed, first, target, reb = self.decode(population)
-        key = np.concatenate([packed, first.reshape(len(population), -1).view(np.uint8)], axis=1)
-        _, idx, inverse = np.unique(key, axis=0, return_index=True, return_inverse=True)
-        keep = np.sort(idx)
-        rank = np.empty(len(idx), dtype=np.int64)
-        rank[np.argsort(idx)] = np.arange(len(idx))
-        inverse = rank[inverse.reshape(-1)]
-        U = len(keep)
-        dev = m.device
-        indiv = torch.from_numpy(np.ascontiguousarray(packed[keep])).to(dev)
-        first_us = torch.from_numpy(np.ascontiguousarray(first[keep])).to(dev)
-        tgt = torch.from_numpy(target).to(dev)
-        stats = torch.empty((U, m.S, WORDS), dtype=torch.float64, device=dev)
-        service = torch.empty((U, len(SERVICE_FIELDS)), dtype=torch.float64, device=dev)
-        first_day, D = self.calendar_days()
-        rows = torch.empty((U, D), dtype=torch.float64, device=dev) if day else None
-        close = m.close
-        with torch.cuda.device(dev):
-            _lib.call("b200bt_dca_sweep", close.data_ptr(), _lib.ld(close), self.dip.data_ptr(), m.N, m.S, m.N,
-                      self.start_bar, m.bar_minutes, m.minute0, self._ws.data_ptr(), self._ws.numel(), indiv.data_ptr(),
-                      first_us.data_ptr(), U, int(reb), tgt.data_ptr(), self._pow10.data_ptr(), _lib.ptr(self.labels),
-                      self.ld_labels, self.usdc_balance, stats.data_ptr(), service.data_ptr(), _lib.ptr(rows),
-                      D if day else 0, _lib.current_stream())
-        self._stats, self._service = stats, service
-        self._inverse = None if U == len(population) else inverse
-        return stats, service, rows
+        return [packed, first], {"target": torch.from_numpy(target).to(self.market.device), "rebalance_any": reb}
 
-    def calendar_days(self) -> Tuple[int, int]:
-        """(first_day, D): the calendar day of bar 0 (days since 1970-01-01) and the days from it to the last bar's."""
+    def launch(self, indiv: torch.Tensor, first_us: torch.Tensor, stats: torch.Tensor, service: Optional[torch.Tensor],
+               rows: Optional[torch.Tensor] = None, *, target: torch.Tensor, rebalance_any: bool) -> None:
+        """b200bt_dca_sweep on the current stream for the decoded individuals `indiv` (DcaIndividual bytes [U]), their
+        first intervals `first_us` [U][S][5][2] and the rebalance targets `target` [S], writing `stats` [U][S][20],
+        `service` [U][5] and, when given, the per-day rows `rows` [U][D]."""
         m = self.market
-        first = m.minute0 // 1440
-        return first, (m.minute0 + (m.N - 1) * m.bar_minutes) // 1440 - first + 1
+        _lib.call("b200bt_dca_sweep", m.close.data_ptr(), _lib.ld(m.close), self.dip.data_ptr(), m.N, m.S, m.N,
+                  self.start_bar, m.bar_minutes, m.minute0, self._ws.data_ptr(), self._ws.numel(), indiv.data_ptr(),
+                  first_us.data_ptr(), indiv.shape[0], int(rebalance_any), target.data_ptr(), self._pow10.data_ptr(),
+                  _lib.ptr(self.labels), self.ld_labels, self.usdc_balance, stats.data_ptr(), _lib.ptr(service),
+                  _lib.ptr(rows), 0 if rows is None else rows.shape[1], _lib.current_stream())
 
-    def _expand(self, t: torch.Tensor) -> torch.Tensor:
-        return t if self._inverse is None else t.index_select(0, torch.from_numpy(self._inverse).to(t.device))
-
-    def evaluate(self, population: List[Dict]) -> np.ndarray:
-        """fitness float64 [pop]: the `objective` (a stats field's mean over the symbols, or a service field)."""
-        if not population:
-            return np.zeros(0, dtype=np.float64)
-        return self.evaluate_objectives_device(population, [(self.objective, True)])[:, 0].cpu().numpy()
-
-    def evaluate_objectives_device(self, population: List[Dict], objectives) -> torch.Tensor:
-        """Objective matrix float64 [pop][M] on the device for ParetoGeneticAlgorithm: per objective (field, maximize)
-        a stats field's mean over the symbols (b200bt_objective_matrix) or a service field, in the field's own sense."""
-        objectives = list(objectives)
-        cols = [self._column(name) for name, _ in objectives]
-        M = len(cols)
-        if not 1 <= M <= 8:
-            raise ValueError("1..8 objectives")
-        if not population:
-            return torch.zeros((0, M), dtype=torch.float64, device=self.market.device)
-        stats, service, _ = self._run(population)
-        U = stats.shape[0]
-        fields = [f for kind, f in cols if kind == "stats"]
-        means = None
-        if fields:
-            means = torch.empty((U, len(fields)), dtype=torch.float64, device=stats.device)
-            with torch.cuda.device(stats.device):
-                _lib.call("b200bt_objective_matrix", stats.data_ptr(), U, stats.shape[1],
-                          (C.c_int * len(fields))(*fields), len(fields), means.data_ptr(), len(fields),
-                          _lib.current_stream())
-        out, j = [], 0
-        for kind, f in cols:
-            if kind == "stats":
-                out.append(means[:, j])
-                j += 1
-            else:
-                out.append(service[:, f])
-        return self._expand(torch.stack(out, dim=1))
-
-    def evaluate_objectives(self, population: List[Dict], objectives) -> np.ndarray:
-        return self.evaluate_objectives_device(population, objectives).cpu().numpy()
-
-    def dca_stats(self, population: Optional[List[Dict]] = None) -> Dict[str, np.ndarray]:
-        """dict field -> [pop][S] float64 of `population` (evaluated now) or of the last evaluation."""
-        if population is not None:
-            self._run(population)
-        if self._stats is None:
-            raise RuntimeError("nothing evaluated yet")
-        raw = self._expand(self._stats).cpu().numpy()
-        return {name: raw[:, :, f] for f, name in enumerate(FIELDS)}
-
-    def service_stats(self, population: Optional[List[Dict]] = None) -> Dict[str, np.ndarray]:
-        """dict field -> [pop] float64: _update_performance_metrics' totals at the last tick."""
-        if population is not None:
-            self._run(population)
-        if self._service is None:
-            raise RuntimeError("nothing evaluated yet")
-        raw = self._expand(self._service).cpu().numpy()
-        return {name: raw[:, f] for f, name in enumerate(SERVICE_FIELDS)}
-
-    def stats_device(self) -> torch.Tensor:
-        """The last evaluation's stats float64 [pop][S][20] on the device, in population order."""
-        return self._expand(self._stats)
+    dca_stats = StrategySweep.stats_dict
 
     def day_pnl(self, population: List[Dict]) -> Tuple[torch.Tensor, int]:
         """(rows float64 [pop][D] on the device, first_day): row i, column d = the change of individual i's
         sum_s (Q_s * c_s - I_s) over calendar day first_day + d -- the row shape b200bt_cscv takes."""
-        _, _, rows = self._run(population, day=True)
-        return self._expand(rows), self.calendar_days()[0]
-
-    @property
-    def fitness_function(self):
-        sweep = self
-
-        def fitness(individual: Dict) -> float:
-            return float(sweep.evaluate([individual])[0])
-
-        fitness.batch = lambda population: [float(x) for x in sweep.evaluate(population)]
-        return fitness
+        return self.day_rows(population)
 
 
 def dip_pct(market) -> torch.Tensor:
@@ -438,10 +337,6 @@ def dip_pct(market) -> torch.Tensor:
         _lib.call("b200bt_dca_dip_pct", high.data_ptr(), close.data_ptr(), _lib.ld(close), market.S, market.N,
                   market.minute0, market.bar_minutes, out.data_ptr(), market.N, _lib.current_stream())
     return out
-
-
-def _iso(minute: int) -> str:
-    return (datetime(1970, 1, 1, tzinfo=timezone.utc) + timedelta(minutes=int(minute))).replace(tzinfo=None).isoformat()
 
 
 class DCAStrategy:
@@ -474,7 +369,7 @@ class DCAStrategy:
                 positions[sym] = {
                     "symbol": sym, "total_invested": v["total_invested"], "total_quantity": v["total_quantity"],
                     "average_price": v["average_price"],
-                    "last_purchase_time": _iso(t0 + k * market.bar_minutes) if k >= 0 else None,
+                    "last_purchase_time": iso_minute(t0 + k * market.bar_minutes) if k >= 0 else None,
                     "last_purchase_price": v["last_purchase_price"], "current_price": float(last_close[s]),
                     "current_value": v["current_value"], "profit_loss": v["profit_loss"],
                     "profit_loss_pct": v["profit_loss_pct"],
@@ -482,7 +377,7 @@ class DCAStrategy:
             next_buys = {sym: (datetime(1970, 1, 1) + timedelta(minutes=t0, microseconds=int(stats[sym]["next_scheduled_us"])))
                          .isoformat() for sym in market.symbols}
             performance = {
-                "timestamp": _iso(t1), "start_time": _iso(t0), "running_time_hours": (t1 - t0) * 60 / 3600,
+                "timestamp": iso_minute(t1), "start_time": iso_minute(t0), "running_time_hours": (t1 - t0) * 60 / 3600,
                 "total_purchases": int(sv["total_purchases"]), "total_invested": sv["total_invested"],
                 "total_value": sv["total_value"], "total_profit": sv["total_profit"],
                 "total_profit_pct": sv["total_profit_pct"], "symbols": list(market.symbols),

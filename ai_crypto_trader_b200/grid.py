@@ -25,18 +25,17 @@ import ctypes as C
 import logging
 import math
 import os
-from datetime import datetime, timedelta, timezone
 from typing import Dict, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 import torch
 
 from . import _lib
+from .population import StrategySweep, iso_minute
 
 logger = logging.getLogger("b200bt.grid")
 
 FIELDS = _lib.GRID_STATS_FIELDS
-WORDS = len(FIELDS)
 OBJECTIVE_FIELDS = FIELDS[:-1]          # near_ties describes the arithmetic, not the strategy
 SERVICE_FIELDS = _lib.GRID_SERVICE_FIELDS
 GRID_TYPES = _lib.GRID_TYPES
@@ -172,7 +171,7 @@ def symbol_quantity(block: Dict, symbol: str) -> float:
     return float(block.get("quantity_per_grid", DEFAULTS["quantity_per_grid"]))
 
 
-class GridSweep:
+class GridSweep(StrategySweep):
     """b200bt_grid_sweep for populations of grid parameter dicts on one market.
 
     market      MarketData (device closes, bar clock)
@@ -189,6 +188,8 @@ class GridSweep:
                 default BTCUSDC), which must be one of the market's symbols, and per-symbol label rows are refused.
 
     Individuals that decode alike (same kernel fields and initial boundaries) are evaluated once."""
+
+    FIELDS, OBJECTIVE_FIELDS, SERVICE_FIELDS = FIELDS, OBJECTIVE_FIELDS, SERVICE_FIELDS
 
     def __init__(self, market, quantity: Union[None, float, Sequence[float]] = None, start_bar: Optional[int] = None,
                  regime=None, config: Optional[Dict] = None, objective: str = "total_profit", service: bool = False):
@@ -229,18 +230,9 @@ class GridSweep:
                 raise ValueError("service mode reads one regime label row (market_regime_history): pass [1][N] labels")
         self.table = regime_table(self.block)
         self.objective = objective
-        self._field(objective)
+        self._column(objective)
         self._closes = None                      # host closes up to the start bar (auto boundaries)
         self._vol_cache: Dict[Tuple[int, int], List[float]] = {}
-        self._stats = None
-        self._service = None
-        self._inverse = None
-
-    @staticmethod
-    def _field(name: str) -> int:
-        if name not in OBJECTIVE_FIELDS:
-            raise ValueError(f"{name!r} is not a grid stats field; one of {', '.join(OBJECTIVE_FIELDS)}")
-        return OBJECTIVE_FIELDS.index(name)
 
     # -- host decoding --------------------------------------------------------------------------------------------
     def _history(self, s: int, lookback: int) -> List[float]:
@@ -275,123 +267,30 @@ class GridSweep:
         packed = np.frombuffer(bytes(rows), dtype=np.uint8).reshape(len(population), C.sizeof(_lib.GridIndividual))
         return packed, bounds
 
-    # -- device evaluation ----------------------------------------------------------------------------------------
-    def _run(self, population: List[Dict], day: bool = False):
-        if not population:
-            raise ValueError("an empty population")
+    def _inputs(self, population: List[Dict]):
+        return list(self.decode(population)), {}
+
+    def launch(self, indiv: torch.Tensor, bounds: torch.Tensor, stats: torch.Tensor,
+               service: Optional[torch.Tensor] = None, rows: Optional[torch.Tensor] = None) -> None:
+        """One launch on the current stream for the decoded individuals `indiv` (GridIndividual bytes [U]) and their
+        initial boundaries `bounds` [U][S][2], writing `stats` [U][S][20] and, when given, the per-day rows `rows` [U][D]:
+        b200bt_grid_service_sweep when `service` [U][12] is given, else b200bt_grid_sweep."""
         m = self.market
-        packed, bounds = self.decode(population)
-        key = np.concatenate([packed, bounds.reshape(len(population), -1).view(np.uint8)], axis=1)
-        _, first, inverse = np.unique(key, axis=0, return_index=True, return_inverse=True)
-        keep = np.sort(first)
-        rank = np.empty(len(first), dtype=np.int64)
-        rank[np.argsort(first)] = np.arange(len(first))
-        inverse = rank[inverse.reshape(-1)]
-        U = len(keep)
-        indiv = torch.from_numpy(np.ascontiguousarray(packed[keep])).to(m.device)
-        bnd = torch.from_numpy(np.ascontiguousarray(bounds[keep])).to(m.device)
-        stats = torch.empty((U, m.S, WORDS), dtype=torch.float64, device=m.device)
-        first_day, D = self.calendar_days()
-        rows = torch.empty((U, D), dtype=torch.float64, device=m.device) if day else None
-        close = m.close
         table = self.table if self.labels is not None else None
-        with torch.cuda.device(m.device):
-            if self.service:
-                service = torch.empty((U, len(SERVICE_FIELDS)), dtype=torch.float64, device=m.device)
-                _lib.call("b200bt_grid_service_sweep", close.data_ptr(), _lib.ld(close), m.S, m.N, self.start_bar,
-                          m.bar_minutes, m.minute0, indiv.data_ptr(), U, self._qty.data_ptr(), bnd.data_ptr(),
-                          _lib.ptr(self.labels), self.ld_labels, table, stats.data_ptr(), service.data_ptr(),
-                          _lib.ptr(rows), D if day else 0, _lib.current_stream())
-                self._service = service
-            else:
-                _lib.call("b200bt_grid_sweep", close.data_ptr(), _lib.ld(close), m.S, m.N, self.start_bar, m.bar_minutes,
-                          m.minute0, indiv.data_ptr(), U, self._qty.data_ptr(), bnd.data_ptr(), _lib.ptr(self.labels),
-                          self.ld_labels, table, stats.data_ptr(), _lib.ptr(rows), D if day else 0,
-                          _lib.current_stream())
-        self._stats = stats
-        self._inverse = None if U == len(population) else inverse
-        return stats, rows
+        args = [m.close.data_ptr(), _lib.ld(m.close), m.S, m.N, self.start_bar, m.bar_minutes, m.minute0, indiv.data_ptr(),
+                indiv.shape[0], self._qty.data_ptr(), bounds.data_ptr(), _lib.ptr(self.labels), self.ld_labels, table,
+                stats.data_ptr()]
+        if service is not None:
+            args.append(service.data_ptr())
+        _lib.call("b200bt_grid_service_sweep" if service is not None else "b200bt_grid_sweep", *args, _lib.ptr(rows),
+                  0 if rows is None else rows.shape[1], _lib.current_stream())
 
-    def calendar_days(self) -> Tuple[int, int]:
-        """(first_day, D): the calendar day of bar 0 (days since 1970-01-01) and the days from it to the last bar's."""
-        m = self.market
-        first = m.minute0 // 1440
-        return first, (m.minute0 + (m.N - 1) * m.bar_minutes) // 1440 - first + 1
-
-    def _expand(self, t: torch.Tensor) -> torch.Tensor:
-        return t if self._inverse is None else t.index_select(0, torch.from_numpy(self._inverse).to(t.device))
-
-    def evaluate(self, population: List[Dict]) -> np.ndarray:
-        """fitness float64 [pop]: the mean over symbols of the `objective` field (b200bt_objective_matrix)."""
-        if not population:
-            return np.zeros(0, dtype=np.float64)
-        return self.evaluate_objectives_device(population, [(self.objective, True)])[:, 0].cpu().numpy()
-
-    def evaluate_objectives_device(self, population: List[Dict], objectives) -> torch.Tensor:
-        """Objective matrix float64 [pop][M] on the device for ParetoGeneticAlgorithm: per objective (field, maximize)
-        the field's mean over the symbols, in the field's own sense (b200bt_objective_matrix on the grid stats, whose
-        160-byte rows it reads as it reads lane stats)."""
-        objectives = list(objectives)
-        fields = [self._field(name) for name, _ in objectives]
-        M = len(fields)
-        if not 1 <= M <= 8:
-            raise ValueError("1..8 objectives")
-        if not population:
-            return torch.zeros((0, M), dtype=torch.float64, device=self.market.device)
-        stats, _ = self._run(population)
-        out = torch.empty((stats.shape[0], M), dtype=torch.float64, device=stats.device)
-        with torch.cuda.device(stats.device):
-            _lib.call("b200bt_objective_matrix", stats.data_ptr(), stats.shape[0], stats.shape[1], (C.c_int * M)(*fields),
-                      M, out.data_ptr(), M, _lib.current_stream())
-        return self._expand(out)
-
-    def evaluate_objectives(self, population: List[Dict], objectives) -> np.ndarray:
-        return self.evaluate_objectives_device(population, objectives).cpu().numpy()
-
-    def grid_stats(self, population: Optional[List[Dict]] = None) -> Dict[str, np.ndarray]:
-        """dict field -> [pop][S] float64 of `population` (evaluated now) or of the last evaluation."""
-        if population is not None:
-            self._run(population)
-        if self._stats is None:
-            raise RuntimeError("nothing evaluated yet")
-        raw = self._expand(self._stats).cpu().numpy()
-        return {name: raw[:, :, f] for f, name in enumerate(FIELDS)}
-
-    def service_stats(self, population: Optional[List[Dict]] = None) -> Dict[str, np.ndarray]:
-        """Service mode: dict field -> [pop] float64 of b200bt_grid_service_stats (the reference's grid_performance plus
-        the service's final num_grids / pcts and its adjustment counts) of `population` or of the last evaluation."""
-        if not self.service:
-            raise RuntimeError("service_stats() needs GridSweep(..., service=True)")
-        if population is not None:
-            self._run(population)
-        if self._service is None:
-            raise RuntimeError("nothing evaluated yet")
-        raw = self._expand(self._service).cpu().numpy()
-        return {name: raw[:, f] for f, name in enumerate(SERVICE_FIELDS)}
-
-    def stats_device(self) -> torch.Tensor:
-        """The last evaluation's stats float64 [pop][S][20] on the device, in population order."""
-        return self._expand(self._stats)
+    grid_stats = StrategySweep.stats_dict
 
     def day_profit(self, population: List[Dict]) -> Tuple[torch.Tensor, int]:
         """(rows float64 [pop][D] on the device, first_day): row i, column d = individual i's realised grid profit on
         calendar day first_day + d, summed over its symbols -- the row shape b200bt_cscv takes."""
-        _, rows = self._run(population, day=True)
-        return self._expand(rows), self.calendar_days()[0]
-
-    @property
-    def fitness_function(self):
-        sweep = self
-
-        def fitness(individual: Dict) -> float:
-            return float(sweep.evaluate([individual])[0])
-
-        fitness.batch = lambda population: [float(x) for x in sweep.evaluate(population)]
-        return fitness
-
-
-def _iso(minute: int) -> str:
-    return (datetime(1970, 1, 1, tzinfo=timezone.utc) + timedelta(minutes=int(minute))).replace(tzinfo=None).isoformat()
+        return self.day_rows(population)
 
 
 class GridTradingStrategy:
@@ -419,8 +318,9 @@ class GridTradingStrategy:
             trades, prof = int(v["total_trades"]), int(v["profitable_trades"])
             return {
                 "grid_profits": {"total_profit": v["total_profit"], "total_trades": trades, "profitable_trades": prof,
-                                 "start_time": _iso(t0)},
-                "performance": {"timestamp": _iso(t1), "start_time": _iso(t0), "running_time_hours": (t1 - t0) * 60 / 3600,
+                                 "start_time": iso_minute(t0)},
+                "performance": {"timestamp": iso_minute(t1), "start_time": iso_minute(t0),
+                                "running_time_hours": (t1 - t0) * 60 / 3600,
                                 "total_trades": trades, "profitable_trades": prof, "win_rate": v["win_rate"],
                                 "total_profit": v["total_profit"], "profit_per_day": v["profit_per_day"],
                                 "symbols": [symbol], "simulation_mode": True, "symbol_profits": {symbol: v["total_profit"]}},
@@ -447,9 +347,10 @@ class GridTradingStrategy:
             lanes = {sym: {k: float(a[0, s]) for k, a in st.items()} for s, sym in enumerate(market.symbols)}
             return {
                 "grid_profits": {sym: {"total_profit": v["total_profit"], "total_trades": int(v["total_trades"]),
-                                       "profitable_trades": int(v["profitable_trades"]), "start_time": _iso(t0)}
+                                       "profitable_trades": int(v["profitable_trades"]), "start_time": iso_minute(t0)}
                                  for sym, v in lanes.items()},
-                "performance": {"timestamp": _iso(t1), "start_time": _iso(t0), "running_time_hours": (t1 - t0) * 60 / 3600,
+                "performance": {"timestamp": iso_minute(t1), "start_time": iso_minute(t0),
+                                "running_time_hours": (t1 - t0) * 60 / 3600,
                                 "total_trades": int(sv["total_trades"]), "profitable_trades": int(sv["profitable_trades"]),
                                 "win_rate": sv["win_rate"], "total_profit": sv["total_profit"],
                                 "profit_per_day": sv["profit_per_day"], "symbols": list(market.symbols),

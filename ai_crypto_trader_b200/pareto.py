@@ -7,7 +7,7 @@ A Pareto front keeps the trade-off instead: every strategy that no other beats i
 
 pareto_rank            b200bt_pareto_rank on a device [n][M] float64 matrix (contract: include/b200bt.h)
 objectives_from_goals  goals dict -> [(lane-stat field, maximize)]
-objective_matrix       b200bt_objective_matrix: the per-individual mean over symbols of lane-stat fields
+objective_matrix       b200bt_objective_matrix: the per-individual mean over symbols of lane-stat (or other stats) fields
 """
 from __future__ import annotations
 
@@ -28,10 +28,10 @@ OBJECTIVE_FIELDS = _lib.LANE_STATS_FIELDS[:-1]          # trade_hash is a hash, 
 Objective = Tuple[str, bool]
 
 
-def _field(name: str) -> int:
-    if name not in OBJECTIVE_FIELDS:
-        raise ValueError(f"{name!r} is not a lane-stat field; objectives are one of {', '.join(OBJECTIVE_FIELDS)}")
-    return OBJECTIVE_FIELDS.index(name)
+def _field(name: str, fields: Sequence[str] = OBJECTIVE_FIELDS) -> int:
+    if name not in fields:
+        raise ValueError(f"{name!r} is not a stats field; objectives are one of {', '.join(fields)}")
+    return fields.index(name)
 
 
 def objectives_from_goals(goals: Union[Dict, Sequence]) -> List[Objective]:
@@ -66,10 +66,12 @@ def objectives_from_goals(goals: Union[Dict, Sequence]) -> List[Objective]:
     return out
 
 
-def objective_matrix(stats: torch.Tensor, objectives: Sequence[Objective], out: Optional[torch.Tensor] = None) -> torch.Tensor:
+def objective_matrix(stats: torch.Tensor, objectives: Sequence[Objective], out: Optional[torch.Tensor] = None,
+                     fields: Sequence[str] = OBJECTIVE_FIELDS) -> torch.Tensor:
     """b200bt_objective_matrix: [pop][M] float64 on the device, out[i][j] = mean over the S symbols of stats[i][s].<field j>
     (the ascending sum of b200bt_fitness_reduce), in the metric's own sense.  stats: device [pop][S][20] float64 lane stats,
-    or [pop][20] book stats."""
+    or [pop][20] book stats; `fields` names the record's words (another 20-word stats record, such as the grid's or the
+    DCA's, passes its own names)."""
     if not (isinstance(stats, torch.Tensor) and stats.is_cuda and stats.dtype == torch.float64):
         raise TypeError("objective_matrix: stats must be a float64 CUDA tensor")
     if stats.dim() == 2:
@@ -80,7 +82,7 @@ def objective_matrix(stats: torch.Tensor, objectives: Sequence[Objective], out: 
     stats = stats.contiguous()
     pop, S = stats.shape[0], stats.shape[1]
     M = len(objectives)
-    fields = (C.c_int * M)(*[_field(name) for name, _ in objectives])
+    index = (C.c_int * M)(*[_field(name, fields) for name, _ in objectives])
     if out is None:
         out = torch.empty((pop, M), dtype=torch.float64, device=stats.device)
     elif not (isinstance(out, torch.Tensor) and out.device == stats.device and out.dtype == torch.float64 and
@@ -88,7 +90,7 @@ def objective_matrix(stats: torch.Tensor, objectives: Sequence[Objective], out: 
         raise ValueError(f"objective_matrix: out must be a float64 [{pop}][{M}] tensor with unit column stride on "
                          f"{stats.device}")
     with torch.cuda.device(stats.device):
-        _lib.call("b200bt_objective_matrix", stats.data_ptr(), pop, S, fields, M, out.data_ptr(), _lib.ld(out),
+        _lib.call("b200bt_objective_matrix", stats.data_ptr(), pop, S, index, M, out.data_ptr(), _lib.ld(out),
                   _lib.current_stream())
     return out
 

@@ -29,6 +29,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from .population import calendar_days, fitness_callable, unique_rows
 from .synth import EPOCH_2024_MINUTES
 
 DEFAULT_GOALS = {  # config.json: evolution.optimization_goals
@@ -271,25 +272,11 @@ def lane_costs(population: List[Dict]) -> np.ndarray:
     return _band_costs(g("rsi_period", 14).astype(np.int64), g("rsi_oversold", 30), g("rsi_overbought", 70))
 
 
-_HASH_MULTIPLIERS = np.array([0x9E3779B97F4A7C15, 0xC2B2AE3D27D4EB4F, 0x165667B19E3779F9, 0x27D4EB2F165667C5,
-                              0x85EBCA77C2B2AE63], dtype=np.uint64)
-
-
 def _duplicate_classes(packed: np.ndarray):
-    """(first index of each distinct record, class of every record), or None when all records are distinct.
-    Records are compared through a 64-bit multiplicative hash of their 40 bytes (3x faster than sorting the structured
-    array); a hash class is only trusted after every member is compared with its representative."""
-    words = packed.view(np.uint64).reshape(len(packed), -1)
-    with np.errstate(over="ignore"):
-        key = (words * _HASH_MULTIPLIERS[:words.shape[1]]).sum(axis=1, dtype=np.uint64)
-    uk, first, inverse = np.unique(key, return_index=True, return_inverse=True)
-    if len(uk) == len(packed):
-        return None
-    inverse = inverse.reshape(-1)
-    if not bool((packed[first][inverse] == packed).all()):       # a collision merged different records: exact path
-        _, first, inverse = np.unique(packed, return_index=True, return_inverse=True)
-        inverse = inverse.reshape(-1)
-    return (first, inverse) if len(first) < len(packed) else None
+    """(first index of each distinct record, class of every record) of decoded records, in population order, or None
+    when all records are distinct (population.unique_rows)."""
+    keep, expand = unique_rows(packed)
+    return None if expand is None else (keep, expand)
 
 
 def costs_from_packed(packed: np.ndarray, periods: Sequence[int], timeframes: Sequence[int] = (1,)) -> np.ndarray:
@@ -844,11 +831,8 @@ class PopulationSweep:
         dup = _duplicate_classes(packed)
         if dup is None:
             return packed, population, None
-        first, inverse = dup
-        keep = np.sort(first)
-        rank = np.empty(len(first), dtype=np.int64)
-        rank[np.argsort(first)] = np.arange(len(first))
-        return np.ascontiguousarray(packed[keep]), [population[i] for i in keep], rank[inverse.reshape(-1)]
+        keep, expand = dup
+        return np.ascontiguousarray(packed[keep]), [population[i] for i in keep], expand
 
     def evaluate(self, population: List[Dict]) -> np.ndarray:
         """fitness (float64[pop]) of a list of parameter dicts; H2D of the decoded
@@ -1065,10 +1049,8 @@ class PopulationSweep:
     def calendar_days(self) -> Tuple[int, int]:
         """(first_day, D): the calendar day of bar 0 (days since 1970-01-01 of the market's minute clock) and the number of
         days from it to the day of the last bar, the skipped days of a glued series (set_gap) included."""
-        c, last = self.cfg, self.market.N - 1
-        first = c.minute0 // 1440
-        gap = c.gap_minutes if (c.gap_bar > 0 and last >= c.gap_bar) else 0
-        return first, (c.minute0 + last * c.bar_minutes + gap) // 1440 - first + 1
+        c = self.cfg
+        return calendar_days(c.minute0, c.bar_minutes, self.market.N, c.gap_bar, c.gap_minutes)
 
     def daily_pnl(self, population: List[Dict], max_bytes: int = DAILY_PNL_MAX_BYTES):
         """Per-day PnL of every individual's book and of its lanes, on the device, in the order of `population`:
@@ -1173,10 +1155,4 @@ class PopulationSweep:
 
     @property
     def fitness_function(self):
-        sweep = self
-
-        def fitness(individual: Dict) -> float:
-            return float(sweep.evaluate([individual])[0])
-
-        fitness.batch = lambda population: [float(x) for x in sweep.evaluate(population)]
-        return fitness
+        return fitness_callable(self.evaluate)

@@ -43,7 +43,7 @@ def main():
     a = ap.parse_args()
     import numpy as np
     import torch
-    from ai_crypto_trader_b200 import _lib, synth
+    from ai_crypto_trader_b200 import synth
     from ai_crypto_trader_b200.dca import DCASweep, dca_param_ranges, dip_pct
     from ai_crypto_trader_b200.sweep import MarketData
     torch.cuda.set_device(0)
@@ -81,16 +81,8 @@ def main():
         tgt = torch.from_numpy(target).to(dev)
         stats = torch.empty((a.pop, a.symbols, 20), dtype=torch.float64, device=dev)
         service = torch.empty((a.pop, 5), dtype=torch.float64, device=dev)
-        _, D = sweep.calendar_days()
-        rows = torch.empty((a.pop, D), dtype=torch.float64, device=dev) if day else None
-
-        def run():
-            _lib.call("b200bt_dca_sweep", market.close.data_ptr(), _lib.ld(market.close), sweep.dip.data_ptr(),
-                      market.N, a.symbols, market.N, sweep.start_bar, market.bar_minutes, market.minute0,
-                      sweep._ws.data_ptr(), sweep._ws.numel(), indiv.data_ptr(), first_us.data_ptr(), a.pop, int(reb),
-                      tgt.data_ptr(), sweep._pow10.data_ptr(), None, 0, sweep.usdc_balance, stats.data_ptr(),
-                      service.data_ptr(), _lib.ptr(rows), D if day else 0, _lib.current_stream())
-
+        rows = torch.empty((a.pop, sweep.calendar_days()[1]), dtype=torch.float64, device=dev) if day else None
+        run = lambda: sweep.launch(indiv, first_us, stats, service, rows, target=tgt, rebalance_any=reb)
         report(name, timed(torch, run, a.reps), per_lane)
 
 

@@ -29,7 +29,7 @@ def main():
     a = ap.parse_args()
     import numpy as np
     import torch
-    from ai_crypto_trader_b200 import _lib, synth
+    from ai_crypto_trader_b200 import synth
     from ai_crypto_trader_b200.grid import GridSweep, grid_param_ranges
     from ai_crypto_trader_b200.sweep import MarketData
     torch.cuda.set_device(0)
@@ -43,15 +43,13 @@ def main():
     indiv = torch.from_numpy(packed).to(market.device)
     bnd = torch.from_numpy(bounds).to(market.device)
     stats = torch.empty((a.pop, a.symbols, 20), dtype=torch.float64, device=market.device)
-    first_day, D = sweep.calendar_days()
+    D = sweep.calendar_days()[1]
     rows = torch.empty((a.pop, D), dtype=torch.float64, device=market.device) if a.day_profit else None
     times = []
     for _ in range(a.reps):
         t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         t0.record()
-        _lib.call("b200bt_grid_sweep", market.close.data_ptr(), market.N, a.symbols, market.N, sweep.start_bar, 1,
-                  market.minute0, indiv.data_ptr(), a.pop, sweep._qty.data_ptr(), bnd.data_ptr(), None, 0, None,
-                  stats.data_ptr(), _lib.ptr(rows), D if a.day_profit else 0, _lib.current_stream())
+        sweep.launch(indiv, bnd, stats, rows=rows)
         t1.record()
         torch.cuda.synchronize()
         times.append(t0.elapsed_time(t1))

@@ -29,7 +29,7 @@ def main():
     a = ap.parse_args()
     import numpy as np
     import torch
-    from ai_crypto_trader_b200 import _lib, synth
+    from ai_crypto_trader_b200 import synth
     from ai_crypto_trader_b200.grid import GridSweep, grid_param_ranges
     from ai_crypto_trader_b200.sweep import MarketData
     torch.cuda.set_device(0)
@@ -50,22 +50,15 @@ def main():
         bnd = torch.from_numpy(bounds).to(market.device)
         stats = torch.empty((a.pop, S, 20), dtype=torch.float64, device=market.device)
         service = torch.empty((a.pop, 12), dtype=torch.float64, device=market.device)
-        first_day, D = sweep.calendar_days()
-        rows = torch.empty((a.pop, D), dtype=torch.float64, device=market.device)
+        rows = torch.empty((a.pop, sweep.calendar_days()[1]), dtype=torch.float64, device=market.device)
         res = {"symbols": S}
-        for name, fn, day in (("service_ms", "b200bt_grid_service_sweep", False),
-                              ("service_day_ms", "b200bt_grid_service_sweep", True),
-                              ("lane_ms", "b200bt_grid_sweep", False), ("lane_day_ms", "b200bt_grid_sweep", True)):
+        for name, sv_out, day in (("service_ms", service, False), ("service_day_ms", service, True),
+                                  ("lane_ms", None, False), ("lane_day_ms", None, True)):      # None: b200bt_grid_sweep
             times = []
             for r in range(a.reps + 1):
                 t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                args = [market.close.data_ptr(), market.N, S, market.N, sweep.start_bar, 1, market.minute0,
-                        indiv.data_ptr(), a.pop, sweep._qty.data_ptr(), bnd.data_ptr(), None, 0, None, stats.data_ptr()]
-                if fn == "b200bt_grid_service_sweep":
-                    args.append(service.data_ptr())
-                args += [rows.data_ptr() if day else None, D if day else 0, _lib.current_stream()]
                 t0.record()
-                _lib.call(fn, *args)
+                sweep.launch(indiv, bnd, stats, sv_out, rows if day else None)
                 t1.record()
                 torch.cuda.synchronize()
                 if r:
