@@ -11,6 +11,7 @@ from pathlib import Path
 
 _HERE = Path(__file__).resolve().parent
 LIB_PATH = Path(os.environ.get("B200BT_LIB", _HERE / "libb200bt.so"))
+ABI_VERSION = 1                                                       # B200BT_ABI_VERSION
 
 
 class B200btError(RuntimeError):
@@ -368,7 +369,7 @@ def load():
         fn = getattr(lib, name)  # AttributeError if the symbol is not exported
         fn.restype = res
         fn.argtypes = args
-    if lib.b200bt_abi_version() != 1:
+    if lib.b200bt_abi_version() != ABI_VERSION:
         raise ImportError("libb200bt.so ABI version mismatch; rebuild")
     _lib = lib
     return lib

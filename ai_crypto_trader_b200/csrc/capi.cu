@@ -3,6 +3,29 @@
 #include <string.h>
 #include "common.cuh"
 
+// Every struct of the C-ABI at the size its declaration in b200bt.h states (tests/test_abi_header.py holds the Python
+// mirrors to the same layouts), so that a change to a struct that leaves its size comment behind fails the build.
+static_assert(sizeof(b200bt_individual) == 40, "b200bt_individual layout");
+static_assert(sizeof(b200bt_lane_stats) == 160, "b200bt_lane_stats layout");
+static_assert(sizeof(b200bt_sweep_config) == 40, "b200bt_sweep_config layout");
+static_assert(sizeof(b200bt_chunk_item) == 16, "b200bt_chunk_item layout");
+static_assert(sizeof(b200bt_bt_params) == 56, "b200bt_bt_params layout");
+static_assert(sizeof(b200bt_regime_params) == 64, "b200bt_regime_params layout");
+static_assert(sizeof(b200bt_regime_window) == 64, "b200bt_regime_window layout");
+static_assert(sizeof(b200bt_grid_individual) == 40, "b200bt_grid_individual layout");
+static_assert(sizeof(b200bt_grid_regime_rule) == 24, "b200bt_grid_regime_rule layout");
+static_assert(sizeof(b200bt_grid_stats) == 160, "b200bt_grid_stats layout");
+static_assert(sizeof(b200bt_grid_service_stats) == 96, "b200bt_grid_service_stats layout");
+static_assert(sizeof(b200bt_dca_individual) == 272, "b200bt_dca_individual layout");
+static_assert(sizeof(b200bt_dca_stats) == 160, "b200bt_dca_stats layout");
+static_assert(sizeof(b200bt_dca_service) == 40, "b200bt_dca_service layout");
+static_assert(sizeof(b200bt_rl_agent) == 64, "b200bt_rl_agent layout");
+static_assert(sizeof(b200bt_rl_agent_state) == 64, "b200bt_rl_agent_state layout");
+static_assert(sizeof(b200bt_vp_params) == 32, "b200bt_vp_params layout");
+static_assert(sizeof(b200bt_vp_row) == 384, "b200bt_vp_row layout");
+static_assert(sizeof(b200bt_monitor_params) == 24, "b200bt_monitor_params layout");
+static_assert(sizeof(b200bt_monitor_row) == 352, "b200bt_monitor_row layout");
+
 namespace b200bt {
 
 static thread_local char t_err[512] = "";

@@ -485,9 +485,6 @@ combinations_kernel(b200bt_monitor_row* __restrict__ rows, int64_t n) {
 
 using namespace b200bt;
 
-static_assert(sizeof(b200bt_monitor_row) == 352, "b200bt_monitor_row layout");
-static_assert(sizeof(b200bt_monitor_params) == 24, "b200bt_monitor_params layout");
-
 extern "C" int b200bt_market_monitor(const float* ohlcv, int S, int64_t N, int64_t minute0, int bar_minutes,
                                      const float* ohlcv_3m, int64_t M3, const float* ohlcv_5m, int64_t M5,
                                      const float* ohlcv_15m, int64_t M15, const b200bt_monitor_params* params,

@@ -473,9 +473,6 @@ vp_frame_kernel(const VpArgs a) {
 
 using namespace b200bt;
 
-static_assert(sizeof(b200bt_vp_params) == 32, "b200bt_vp_params layout");
-static_assert(sizeof(b200bt_vp_row) == 384, "b200bt_vp_row layout");
-
 // services/utils/volume_profile_analyzer.py :43-394, :487-562, :564-684 (see b200bt.h)
 extern "C" int b200bt_volume_profile(const float* ohlcv, int64_t ld, int S, int64_t N, const b200bt_vp_params* params,
                                      b200bt_vp_row* rows_or_null, double* bins_or_null, uint8_t* labels_or_null,

@@ -23,7 +23,8 @@ def _rows(*ts):
     copied to contiguous rows first."""
     S, N = ts[0].shape
     for t in ts:
-        assert t.is_cuda and t.dtype == torch.float32 and t.dim() == 2 and tuple(t.shape) == (S, N) and t.stride(1) == 1
+        if not (t.is_cuda and t.dtype == torch.float32 and t.dim() == 2 and tuple(t.shape) == (S, N) and t.stride(1) == 1):
+            raise ValueError(f"inputs must be device float32 tensors [{S}][{N}] with unit stride along the bars")
     if len({_lib.ld(t) for t in ts}) > 1:
         ts = tuple(t.contiguous() for t in ts)
     return S, N, _lib.ld(ts[0]), ts
@@ -35,7 +36,8 @@ def _ints(v: Sequence[int]):
 
 def nanfill_(x: torch.Tensor) -> torch.Tensor:
     """In-place ffill -> bfill -> 0 along the last axis of a contiguous fp32 CUDA tensor."""
-    assert x.is_cuda and x.dtype == torch.float32 and x.is_contiguous()
+    if not (x.is_cuda and x.dtype == torch.float32 and x.is_contiguous()):
+        raise ValueError("x must be a contiguous device float32 tensor")
     N = x.shape[-1]
     rows = x.numel() // N
     ws = torch.empty(int(_lib.load().b200bt_nanfill_workspace_floats(rows, N)), dtype=torch.float32, device=x.device)

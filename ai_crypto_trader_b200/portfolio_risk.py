@@ -28,7 +28,8 @@ class ReturnBank:
     """Device-resident simple returns of S assets: fp32 [S][N], NaN where undefined (bar 0, missing data)."""
 
     def __init__(self, symbols: Sequence[str], returns: torch.Tensor):
-        assert returns.dim() == 2 and returns.dtype == torch.float32 and returns.is_cuda and len(symbols) == returns.shape[0]
+        if not (returns.dim() == 2 and returns.dtype == torch.float32 and returns.is_cuda and len(symbols) == returns.shape[0]):
+            raise ValueError(f"returns must be a device float32 tensor with one row per symbol ({len(symbols)})")
         self.symbols = list(symbols)
         self.returns = returns.contiguous()
         self.row = {s: i for i, s in enumerate(self.symbols)}

@@ -37,6 +37,9 @@ DEFAULT_GOALS = {  # config.json: evolution.optimization_goals
     "secondary": ["max_drawdown", "win_rate", "profit_factor"],
 }
 
+INDIVIDUAL_DTYPE = np.dtype([("rsi_row", "<i4"), ("rsi_lo", "<f4"), ("rsi_hi", "<f4"), ("reserved", "<i4"),  # b200bt_individual
+                             ("take_profit", "<f8"), ("stop_loss", "<f8"), ("position_size", "<f8")])
+
 
 def _f32_up(x: float) -> np.float32:
     """Smallest float32 >= x."""
@@ -106,7 +109,8 @@ class MarketData:
     @classmethod
     def from_close(cls, close: torch.Tensor, minute0: int = EPOCH_2024_MINUTES, bar_minutes: int = 1,
                    symbols: Optional[Sequence[str]] = None) -> "MarketData":
-        assert close.is_cuda and close.dtype == torch.float32 and close.dim() == 2
+        if not (close.is_cuda and close.dtype == torch.float32 and close.dim() == 2):
+            raise ValueError("close must be a device float32 tensor [S][N]")
         ohlcv = torch.zeros((5,) + tuple(close.shape), dtype=torch.float32, device=close.device)
         ohlcv[3] = close
         return cls(ohlcv, symbols=symbols, minute0=minute0, bar_minutes=bar_minutes, device=close.device)
@@ -183,18 +187,21 @@ def rsi_bank(close: torch.Tensor, periods: Sequence[int], fill: bool = True,
     [first_symbol, first_symbol + S) are written in the same pass (b200bt_rsi_bank_zones; needs fill=True).
     A `close` whose bars are not consecutive in memory (a time-strided view) is copied to contiguous rows first.
     """
-    assert close.is_cuda and close.dtype == torch.float32 and close.dim() == 2
+    if not (close.is_cuda and close.dtype == torch.float32 and close.dim() == 2):
+        raise ValueError("close must be a device float32 tensor [S][N]")
     if close.stride(-1) != 1:
         close = close.contiguous()
     S, N = close.shape
     P = len(periods)
     if out is None:
         out = torch.empty((S, P, N), dtype=torch.float32, device=close.device)
-    assert out.device == close.device and out.dtype == torch.float32 and tuple(out.shape) == (S, P, N) and out.is_contiguous()
+    if not (out.device == close.device and out.dtype == torch.float32 and tuple(out.shape) == (S, P, N) and out.is_contiguous()):
+        raise ValueError(f"out must be a contiguous float32 tensor [{S}][{P}][{N}] on the device of close")
     arr = (C.c_int * P)(*[int(p) for p in periods])
     with torch.cuda.device(close.device):
         if zones is not None:
-            assert fill, "zone rows describe the NaN-filled bank"
+            if not fill:
+                raise ValueError("zones need fill=True: zone rows describe the NaN-filled bank")
             _lib.call("b200bt_rsi_bank_zones", close.data_ptr(), S, N, _lib.ld(close), arr, P, out.data_ptr(), zones.data_ptr(),
                       int(zones_symbols), int(first_symbol), _lib.current_stream())
         else:
@@ -208,10 +215,7 @@ def decode_population(population: List[Dict], period_row: Dict[int, int], n_time
 
     With `n_timeframes` > 1 the bank holds one block of len(period_row) rows per timeframe and the gene
     `rsi_timeframe` (an index into PopulationSweep.timeframes, default 0 = the base clock) selects the block."""
-    dt = np.dtype([("rsi_row", "<i4"), ("rsi_lo", "<f4"), ("rsi_hi", "<f4"), ("reserved", "<i4"),
-                   ("take_profit", "<f8"), ("stop_loss", "<f8"), ("position_size", "<f8")])
-    assert dt.itemsize == C.sizeof(_lib.Individual)
-    out = np.zeros(len(population), dtype=dt)
+    out = np.zeros(len(population), dtype=INDIVIDUAL_DTYPE)
     g = lambda key, default: np.array([p.get(key, default) for p in population], dtype=np.float64)
     period = g("rsi_period", 14).astype(np.int64)
     rows = np.full(int(period.max()) + 2 if len(period) else 1, -1, dtype=np.int64)
@@ -637,7 +641,8 @@ class PopulationSweep:
         """Sweep over a caller-supplied RSI bank [S][P][N] (e.g. the 'rsi' field of the reference's
         market-data points) instead of one computed from the close prices."""
         periods = [int(p) for p in periods]
-        assert bank.is_cuda and bank.dtype == torch.float32 and tuple(bank.shape) == (market.S, len(periods), market.N)
+        if not (bank.is_cuda and bank.dtype == torch.float32 and tuple(bank.shape) == (market.S, len(periods), market.N)):
+            raise ValueError(f"bank must be a device float32 tensor [{market.S}][{len(periods)}][{market.N}]")
         self = cls.__new__(cls)
         self._setup(market, periods, optimization_goals, initial_capital, event_cap, mode, None, score_on_advanced, (),
                     bank=bank.contiguous(), aggregation=aggregation, max_event_bytes=max_event_bytes)

@@ -6,18 +6,15 @@ from pathlib import Path
 
 import pytest
 
-ROOT = Path(__file__).resolve().parents[1]
+import abi_header
+from abi_header import DEV, EINVAL, ELIMIT, ENODEVICE
 
 
 def test_library_exports_every_declared_symbol(native_lib):
-    header = (ROOT / "include" / "b200bt.h").read_text()
-    declared = set(re.findall(r"\b(b200bt_[a-z0-9_]+)\s*\(", header))
-    assert declared, "no declarations parsed"
-    from ai_crypto_trader_b200 import _lib
-    assert set(_lib.exported_symbols()) == declared
-    for name in declared:
+    header = abi_header.parse()
+    for name in header.prototypes:
         assert hasattr(native_lib, name), name
-    assert native_lib.b200bt_abi_version() == 1
+    assert native_lib.b200bt_abi_version() == header.defines["B200BT_ABI_VERSION"]
 
 
 def test_library_holds_sm90a_code_only(native_lib):
@@ -33,20 +30,6 @@ def test_library_holds_sm90a_code_only(native_lib):
     assert set(re.findall(r"\.(sm_\w+)\.cubin", out)) == {"sm_90a"}, out
 
 
-def test_event_word_constants_match_header():
-    header = (ROOT / "include" / "b200bt.h").read_text()
-    defined = {k: int(v, 16) for k, v in re.findall(r"#define B200BT_EVENT_(\w+)\s+(0x[0-9a-fA-F]+)u", header)}
-    from ai_crypto_trader_b200 import _lib
-    assert defined == {"EXIT": _lib.EVENT_EXIT, "SELL": _lib.EVENT_SELL, "BAR_MASK": _lib.EVENT_BAR_MASK}
-
-
-def test_struct_layouts_match_header(native_lib):
-    from ai_crypto_trader_b200 import _lib
-    assert C.sizeof(_lib.Individual) == 40
-    assert C.sizeof(_lib.SweepConfig) == 40
-    assert len(_lib.LANE_STATS_FIELDS) * 8 == 160
-
-
 def test_no_cpu_fallback(native_lib):
     import torch
     if torch.cuda.is_available():
@@ -56,7 +39,7 @@ def test_no_cpu_fallback(native_lib):
     buf = (C.c_float * 64)()
     with pytest.raises(_lib.B200btError) as ei:
         _lib.call("b200bt_rsi_bank", C.addressof(buf), 1, 64, 64, periods, 1, 1, C.addressof(buf), None)
-    assert ei.value.status == 10002  # B200BT_ENODEVICE
+    assert ei.value.status == ENODEVICE
     from ai_crypto_trader_b200.sweep import MarketData
     import numpy as np
     with pytest.raises(RuntimeError):
@@ -67,10 +50,31 @@ def test_argument_validation(native_lib):
     from ai_crypto_trader_b200 import _lib
     with pytest.raises(_lib.B200btError) as ei:
         _lib.call("b200bt_rsi_bank", None, 1, 64, 64, (C.c_int * 1)(14), 1, 1, None, None)
-    assert ei.value.status == 10001
+    assert ei.value.status == EINVAL
 
 
-_EINVAL, _ELIMIT = 10001, 10003
+_CPU_TENSOR_CALLS = """
+import torch
+from ai_crypto_trader_b200 import indicators, sweep
+x = torch.zeros((2, 64), dtype=torch.float32)
+for name, call in (("nanfill_", lambda: indicators.nanfill_(x)), ("rsi_bank", lambda: sweep.rsi_bank(x, [14])),
+                   ("from_close", lambda: sweep.MarketData.from_close(x))):
+    try:
+        call()
+    except ValueError:
+        continue
+    raise SystemExit(name + " accepted a host tensor")
+"""
+
+
+def test_host_wrappers_refuse_host_tensors_under_python_O():
+    """The wrappers check a tensor's device and dtype before its pointer goes to C with raises, not assert statements,
+    which `python -O` strips."""
+    import subprocess
+    import sys
+    subprocess.run([sys.executable, "-O", "-c", _CPU_TENSOR_CALLS], cwd=Path(__file__).resolve().parents[1], check=True)
+
+
 _CLOCK_N, _CLOCK_BAR = 200_000, 7
 _CLOCK_END = (1 << 32) - 1440          # minute0 + N * bar_minutes + gap_minutes must stay below this
 
@@ -82,27 +86,26 @@ def _sweep_calls(cfg):
     from ai_crypto_trader_b200 import _lib
     lib = _lib.load()
     P, S, N, pop, K, n_seg, pool = 26, 2, _CLOCK_N, 64, 8, 64 * 8, 4096
-    dev = 1 << 20                                              # 16-byte aligned, never read
     ws_c = int(lib.b200bt_sweep_chunked_workspace_bytes(pool, S, n_seg))
     ws_t = int(lib.b200bt_sweep_tiled_workspace_bytes(pool, S, pop, K))
     ref = C.byref(cfg)
     return {
-        "b200bt_sweep": (dev, N, dev, N, P, S, N, dev, None, pop, ref, dev, None, 0, None),
-        "b200bt_sweep_chunked": (dev, N, dev, N, P, S, N, dev, None, pop, dev, n_seg, dev, dev, n_seg, 2048, 8, pool, dev,
-                                 ws_c, ref, dev, None, 0, dev, None, None),
-        "b200bt_sweep_tiled": (dev, N, dev, N, P, S, N, None, dev, dev, pop, None, pop, K, 1536, 2, pool, dev, ws_t, ref,
-                               dev, None, 0, dev, None, None),
+        "b200bt_sweep": (DEV, N, DEV, N, P, S, N, DEV, None, pop, ref, DEV, None, 0, None),
+        "b200bt_sweep_chunked": (DEV, N, DEV, N, P, S, N, DEV, None, pop, DEV, n_seg, DEV, DEV, n_seg, 2048, 8, pool, DEV,
+                                 ws_c, ref, DEV, None, 0, DEV, None, None),
+        "b200bt_sweep_tiled": (DEV, N, DEV, N, P, S, N, None, DEV, DEV, pop, None, pop, K, 1536, 2, pool, DEV, ws_t, ref,
+                               DEV, None, 0, DEV, None, None),
     }
 
 
 @pytest.mark.parametrize("case, minute0, gap_minutes, bar_minutes, status", [
-    ("sum at 2^32 - 1440", _CLOCK_END - _CLOCK_N * _CLOCK_BAR - 1441, 1441, _CLOCK_BAR, _ELIMIT),
-    ("minute0 at 2^32 - 1440", _CLOCK_END, 0, _CLOCK_BAR, _ELIMIT),
-    ("minute0 near 2^62", 1 << 62, 0, _CLOCK_BAR, _ELIMIT),
-    ("negative minute0", -1, 0, _CLOCK_BAR, _EINVAL),
-    ("negative gap_minutes", 0, -1, _CLOCK_BAR, _EINVAL),
-    ("negative gap_minutes, large minute0", _CLOCK_END - _CLOCK_N * _CLOCK_BAR, -1, _CLOCK_BAR, _EINVAL),
-    ("zero bar_minutes", 0, 0, 0, _EINVAL),
+    ("sum at 2^32 - 1440", _CLOCK_END - _CLOCK_N * _CLOCK_BAR - 1441, 1441, _CLOCK_BAR, ELIMIT),
+    ("minute0 at 2^32 - 1440", _CLOCK_END, 0, _CLOCK_BAR, ELIMIT),
+    ("minute0 near 2^62", 1 << 62, 0, _CLOCK_BAR, ELIMIT),
+    ("negative minute0", -1, 0, _CLOCK_BAR, EINVAL),
+    ("negative gap_minutes", 0, -1, _CLOCK_BAR, EINVAL),
+    ("negative gap_minutes, large minute0", _CLOCK_END - _CLOCK_N * _CLOCK_BAR, -1, _CLOCK_BAR, EINVAL),
+    ("zero bar_minutes", 0, 0, 0, EINVAL),
 ])
 def test_sweep_entry_points_reject_an_out_of_range_calendar(native_lib, case, minute0, gap_minutes, bar_minutes, status):
     """The kernels form calendar minutes in unsigned 32 bits: the three sweep entry points refuse a clock that leaves that
@@ -125,12 +128,12 @@ def test_resample_and_align_reject_a_negative_clock(native_lib, minute0):
     touched; the dummy pointers are never read) and b200bt_resample_bars reports no bars."""
     from ai_crypto_trader_b200 import _lib
     lib = _lib.load()
-    N, bar, k, dev = 1000, 5, 15, 1 << 20
+    N, bar, k = 1000, 5, 15
     assert lib.b200bt_resample_bars(N, minute0, bar, k) == 0
     assert lib.b200bt_resample_bars(N, 0, bar, k) == (N * bar + k - 1) // k
     M = int(lib.b200bt_resample_bars(N, 0, bar, k))
-    for name, args in (("b200bt_resample", (dev, 2, N, minute0, bar, k, dev, M, None)),
-                       ("b200bt_align", (dev, 2, M, N, minute0, bar, k, dev, None))):
+    for name, args in (("b200bt_resample", (DEV, 2, N, minute0, bar, k, DEV, M, None)),
+                       ("b200bt_align", (DEV, 2, M, N, minute0, bar, k, DEV, None))):
         with pytest.raises(_lib.B200btError) as ei:
             _lib.call(name, *args)
-        assert ei.value.status == _EINVAL and "minute0" in str(ei.value), (name, str(ei.value))
+        assert ei.value.status == EINVAL and "minute0" in str(ei.value), (name, str(ei.value))

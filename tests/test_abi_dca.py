@@ -1,21 +1,10 @@
-"""CPU-side checks of the DCA entry points (csrc/dca.cu): struct layouts and every argument refusal, which happens before
-the device is touched (so these run without a GPU; the dummy device pointers are never dereferenced)."""
-import ctypes as C
-
+"""CPU-side checks of the DCA entry points (csrc/dca.cu): workspace sizing and every argument refusal, which happens
+before the device is touched (so these run without a GPU; the dummy device pointers are never dereferenced)."""
 import pytest
 
-_EINVAL, _ENODEVICE, _ELIMIT = 10001, 10002, 10003
-DEV = 1 << 20
+from abi_header import DEV, EINVAL, ELIMIT, ENODEVICE, status
+
 M0 = 28_401_120
-
-
-def _status(fn, *args):
-    from ai_crypto_trader_b200 import _lib
-    try:
-        _lib.call(fn, *args)
-    except _lib.B200btError as e:
-        return e.status
-    return 0
 
 
 def _ws(S=2, N=10_000):
@@ -28,21 +17,12 @@ def _sweep(close=DEV, ld=10_000, dip=DEV, ld_dip=10_000, S=2, N=10_000, start_ba
            stats=DEV, service=None, day=None, D=0):
     if ws_bytes is None:
         ws_bytes = _ws(S, N)
-    return _status("b200bt_dca_sweep", close, ld, dip, ld_dip, S, N, start_bar, bar_minutes, minute0, ws, ws_bytes, indiv,
-                   first, pop, reb, target, pow10, labels, ld_labels, usdc, stats, service, day, D, None)
+    return status("b200bt_dca_sweep", close, ld, dip, ld_dip, S, N, start_bar, bar_minutes, minute0, ws, ws_bytes, indiv,
+                  first, pop, reb, target, pow10, labels, ld_labels, usdc, stats, service, day, D, None)
 
 
 def _dip(high=DEV, close=DEV, ld=10_000, S=2, N=10_000, minute0=M0, bar_minutes=1, out=DEV, ld_out=10_000):
-    return _status("b200bt_dca_dip_pct", high, close, ld, S, N, minute0, bar_minutes, out, ld_out, None)
-
-
-def test_struct_layouts(native_lib):
-    from ai_crypto_trader_b200 import _lib
-    assert C.sizeof(_lib.DcaIndividual) == 272
-    assert _lib.DcaIndividual.order.offset == 160 and _lib.DcaIndividual.flags.offset == 264
-    assert len(_lib.DCA_STATS_FIELDS) * 8 == 160 == len(_lib.LANE_STATS_FIELDS) * 8
-    assert _lib.DCA_STATS_FIELDS[-3:] == ("purchase_hash", "n_ticks", "reserved")
-    assert len(_lib.DCA_SERVICE_FIELDS) == 5
+    return status("b200bt_dca_dip_pct", high, close, ld, S, N, minute0, bar_minutes, out, ld_out, None)
 
 
 def test_workspace_bytes(native_lib):
@@ -60,32 +40,32 @@ def test_dca_refusals(native_lib):
     if torch.cuda.is_available():
         pytest.skip("GPU present: the accepted call would run")
     days = (M0 + 9_999) // 1440 - M0 // 1440 + 1
-    assert _sweep() == _ENODEVICE                                         # every check passed
-    assert _sweep(labels=DEV, ld_labels=0) == _ENODEVICE and _sweep(labels=DEV, ld_labels=10_000) == _ENODEVICE
-    assert _sweep(day=DEV, D=days, service=DEV) == _ENODEVICE
-    assert _sweep(start_bar=0) == _ENODEVICE and _sweep(start_bar=9_999) == _ENODEVICE
+    assert _sweep() == ENODEVICE                                         # every check passed
+    assert _sweep(labels=DEV, ld_labels=0) == ENODEVICE and _sweep(labels=DEV, ld_labels=10_000) == ENODEVICE
+    assert _sweep(day=DEV, D=days, service=DEV) == ENODEVICE
+    assert _sweep(start_bar=0) == ENODEVICE and _sweep(start_bar=9_999) == ENODEVICE
     for kw in ({"close": None}, {"dip": None}, {"ws": None}, {"indiv": None}, {"first": None}, {"target": None},
                {"pow10": None}, {"stats": None}):
-        assert _sweep(**kw) == _EINVAL, kw
-    assert _sweep(S=0) == _EINVAL
-    assert _sweep(pop=0) == _EINVAL
-    assert _sweep(N=0) == _EINVAL
-    assert _sweep(ld=9_999) == _EINVAL and _sweep(ld_dip=9_999) == _EINVAL
-    assert _sweep(start_bar=-1) == _EINVAL and _sweep(start_bar=10_000) == _EINVAL
-    assert _sweep(bar_minutes=0) == _EINVAL and _sweep(minute0=-1) == _EINVAL
-    assert _sweep(bar_minutes=1 << 26, ws_bytes=_ws()) == _EINVAL                     # the clock in us overflows
-    assert _sweep(labels=DEV, ld_labels=9_999) == _EINVAL
-    assert _sweep(day=DEV, D=days - 1) == _EINVAL
-    assert _sweep(ws_bytes=_ws() - 1) == _EINVAL
-    assert _sweep(N=1 << 30, ld=1 << 30, ld_dip=1 << 30, ws_bytes=1 << 40) == _ELIMIT
+        assert _sweep(**kw) == EINVAL, kw
+    assert _sweep(S=0) == EINVAL
+    assert _sweep(pop=0) == EINVAL
+    assert _sweep(N=0) == EINVAL
+    assert _sweep(ld=9_999) == EINVAL and _sweep(ld_dip=9_999) == EINVAL
+    assert _sweep(start_bar=-1) == EINVAL and _sweep(start_bar=10_000) == EINVAL
+    assert _sweep(bar_minutes=0) == EINVAL and _sweep(minute0=-1) == EINVAL
+    assert _sweep(bar_minutes=1 << 26, ws_bytes=_ws()) == EINVAL                     # the clock in us overflows
+    assert _sweep(labels=DEV, ld_labels=9_999) == EINVAL
+    assert _sweep(day=DEV, D=days - 1) == EINVAL
+    assert _sweep(ws_bytes=_ws() - 1) == EINVAL
+    assert _sweep(N=1 << 30, ld=1 << 30, ld_dip=1 << 30, ws_bytes=1 << 40) == ELIMIT
     # S > 32: refused with rebalancing or day rows, accepted without
-    assert _sweep(S=33, reb=1) == _ELIMIT
-    assert _sweep(S=33, reb=0, day=DEV, D=days) == _ELIMIT
-    assert _sweep(S=33, reb=0) == _ENODEVICE
-    assert _sweep(S=32, reb=1, day=DEV, D=days) == _ENODEVICE
+    assert _sweep(S=33, reb=1) == ELIMIT
+    assert _sweep(S=33, reb=0, day=DEV, D=days) == ELIMIT
+    assert _sweep(S=33, reb=0) == ENODEVICE
+    assert _sweep(S=32, reb=1, day=DEV, D=days) == ENODEVICE
     # the drop series
-    assert _dip() == _ENODEVICE
+    assert _dip() == ENODEVICE
     for kw in ({"high": None}, {"close": None}, {"out": None}, {"S": 0}, {"N": 0}, {"ld": 9_999}, {"ld_out": 9_999},
                {"bar_minutes": 0}, {"minute0": -1}):
-        assert _dip(**kw) == _EINVAL, kw
-    assert _dip(N=1 << 30, ld=1 << 30, ld_out=1 << 30) == _ELIMIT
+        assert _dip(**kw) == EINVAL, kw
+    assert _dip(N=1 << 30, ld=1 << 30, ld_out=1 << 30) == ELIMIT

@@ -1,21 +1,10 @@
-"""CPU-side checks of the grid-trading entry point (csrc/grid.cu): struct layouts and every argument refusal, which happens
-before the device is touched (so these run without a GPU; the dummy device pointers are never dereferenced)."""
-import ctypes as C
-
+"""CPU-side checks of the grid-trading entry point (csrc/grid.cu): every argument refusal, which happens before the
+device is touched (so these run without a GPU; the dummy device pointers are never dereferenced)."""
 import pytest
 
-_EINVAL, _ENODEVICE, _ELIMIT = 10001, 10002, 10003
-DEV = 1 << 20
+from abi_header import DEV, EINVAL, ELIMIT, ENODEVICE, status
+
 M0 = 28_401_120
-
-
-def _status(fn, *args):
-    from ai_crypto_trader_b200 import _lib
-    try:
-        _lib.call(fn, *args)
-    except _lib.B200btError as e:
-        return e.status
-    return 0
 
 
 def _table(n=15):
@@ -27,16 +16,8 @@ def _table(n=15):
 
 def _grid(price=DEV, ld=10_000, S=2, N=10_000, start_bar=100, bar_minutes=1, minute0=M0, indiv=DEV, pop=4, qty=DEV,
           bounds=DEV, labels=None, ld_labels=0, table=None, stats=DEV, day=None, D=0):
-    return _status("b200bt_grid_sweep", price, ld, S, N, start_bar, bar_minutes, minute0, indiv, pop, qty, bounds, labels,
-                   ld_labels, table, stats, day, D, None)
-
-
-def test_struct_layouts(native_lib):
-    from ai_crypto_trader_b200 import _lib
-    assert C.sizeof(_lib.GridIndividual) == 40
-    assert C.sizeof(_lib.GridRegimeRule) == 24
-    assert len(_lib.GRID_STATS_FIELDS) * 8 == 160 == len(_lib.LANE_STATS_FIELDS) * 8
-    assert _lib.GRID_STATS_FIELDS[-1] == "near_ties"
+    return status("b200bt_grid_sweep", price, ld, S, N, start_bar, bar_minutes, minute0, indiv, pop, qty, bounds, labels,
+                  ld_labels, table, stats, day, D, None)
 
 
 def test_grid_sweep_refusals(native_lib):
@@ -44,24 +25,24 @@ def test_grid_sweep_refusals(native_lib):
     if torch.cuda.is_available():
         pytest.skip("GPU present: the accepted call would run")
     days = (M0 + 9_999) // 1440 - M0 // 1440 + 1
-    assert _grid() == _ENODEVICE                                         # every check passed
-    assert _grid(labels=DEV, ld_labels=0, table=_table()) == _ENODEVICE
-    assert _grid(labels=DEV, ld_labels=10_000) == _ENODEVICE
-    assert _grid(day=DEV, D=days) == _ENODEVICE
-    assert _grid(start_bar=0) == _ENODEVICE and _grid(start_bar=9_999) == _ENODEVICE
+    assert _grid() == ENODEVICE                                         # every check passed
+    assert _grid(labels=DEV, ld_labels=0, table=_table()) == ENODEVICE
+    assert _grid(labels=DEV, ld_labels=10_000) == ENODEVICE
+    assert _grid(day=DEV, D=days) == ENODEVICE
+    assert _grid(start_bar=0) == ENODEVICE and _grid(start_bar=9_999) == ENODEVICE
     for kw in ({"price": None}, {"indiv": None}, {"qty": None}, {"bounds": None}, {"stats": None}):
-        assert _grid(**kw) == _EINVAL, kw
-    assert _grid(S=0) == _EINVAL
-    assert _grid(pop=0) == _EINVAL
-    assert _grid(N=0) == _EINVAL
-    assert _grid(ld=9_999) == _EINVAL
-    assert _grid(start_bar=-1) == _EINVAL
-    assert _grid(start_bar=10_000) == _EINVAL
-    assert _grid(bar_minutes=0) == _EINVAL
-    assert _grid(minute0=-1) == _EINVAL
-    assert _grid(labels=DEV, ld_labels=9_999) == _EINVAL
-    assert _grid(day=DEV, D=days - 1) == _EINVAL
-    assert _grid(table=_table(0)) == _EINVAL
-    assert _grid(table=_table(128)) == _EINVAL
-    assert _grid(table=_table(127)) == _ENODEVICE
-    assert _grid(N=1 << 30, ld=1 << 30) == _ELIMIT
+        assert _grid(**kw) == EINVAL, kw
+    assert _grid(S=0) == EINVAL
+    assert _grid(pop=0) == EINVAL
+    assert _grid(N=0) == EINVAL
+    assert _grid(ld=9_999) == EINVAL
+    assert _grid(start_bar=-1) == EINVAL
+    assert _grid(start_bar=10_000) == EINVAL
+    assert _grid(bar_minutes=0) == EINVAL
+    assert _grid(minute0=-1) == EINVAL
+    assert _grid(labels=DEV, ld_labels=9_999) == EINVAL
+    assert _grid(day=DEV, D=days - 1) == EINVAL
+    assert _grid(table=_table(0)) == EINVAL
+    assert _grid(table=_table(128)) == EINVAL
+    assert _grid(table=_table(127)) == ENODEVICE
+    assert _grid(N=1 << 30, ld=1 << 30) == ELIMIT

@@ -4,7 +4,8 @@ import ctypes as C
 
 import pytest
 
-EINVAL, ENODEVICE, ELIMIT = 10001, 10002, 10003
+from abi_header import EINVAL, ELIMIT, ENODEVICE, status
+
 MINUTE0 = 1440 * 19_000 + 600
 
 
@@ -30,50 +31,41 @@ def _cscv(N=4, T=40, B=4, ld=None, ws=True, ws_bytes=None, out=True):
             need if ws_bytes is None else ws_bytes, dev if out else None, dev, dev, dev, dev, dev, dev, dev, dev, dev, None)
 
 
-def _status(args):
-    from ai_crypto_trader_b200 import _lib
-    try:
-        _lib.call(*args)
-    except _lib.B200btError as e:
-        return e.status
-    return 0
-
-
 def test_entry_points_refuse_without_device(native_lib):
     import torch
     if torch.cuda.is_available():
         pytest.skip("GPU present: the no-device path cannot be exercised")
     # 2000 one-minute bars from 10:00 end on the next calendar day: D = 2 columns cover them
-    assert _status(_daily(D=2)) == ENODEVICE
-    assert _status(_cscv()) == ENODEVICE
+    assert status(*_daily(D=2)) == ENODEVICE
+    assert status(*_cscv()) == ENODEVICE
 
 
 def test_daily_pnl_validates_arguments(native_lib):
-    assert _status(_daily(S=0)) == EINVAL
-    assert _status(_daily(pop=0)) == EINVAL
-    assert _status(_daily(ld=100)) == EINVAL                    # row stride below N
-    assert _status(_daily(events=False)) == EINVAL
-    assert _status(_daily(out=False)) == EINVAL
-    assert _status(_daily(D=1)) == EINVAL                       # the series spans two calendar days
-    assert _status(_daily(D=5, cfg=_cfg(gap_bar=10, gap_minutes=4 * 1440))) == EINVAL    # the gap adds four more
-    assert _status(_daily(N=1 << 30, ld=1 << 30, D=1 << 20)) == ELIMIT
-    assert _status(_daily(cfg=_cfg(bar_minutes=0))) == EINVAL   # the sweeps' clock check
-    assert _status(_daily(cfg=_cfg(minute0=-1))) == EINVAL
-    assert _status(_daily(cfg=_cfg(minute0=(1 << 32) - 1440))) == ELIMIT
+    assert status(*_daily(S=0)) == EINVAL
+    assert status(*_daily(pop=0)) == EINVAL
+    assert status(*_daily(ld=100)) == EINVAL                    # row stride below N
+    assert status(*_daily(events=False)) == EINVAL
+    assert status(*_daily(out=False)) == EINVAL
+    assert status(*_daily(D=1)) == EINVAL                       # the series spans two calendar days
+    assert status(*_daily(D=5, cfg=_cfg(gap_bar=10, gap_minutes=4 * 1440))) == EINVAL    # the gap adds four more
+    assert status(*_daily(N=1 << 30, ld=1 << 30, D=1 << 20)) == ELIMIT
+    assert status(*_daily(cfg=_cfg(bar_minutes=0))) == EINVAL   # the sweeps' clock check
+    assert status(*_daily(cfg=_cfg(minute0=-1))) == EINVAL
+    assert status(*_daily(cfg=_cfg(minute0=(1 << 32) - 1440))) == ELIMIT
 
 
 def test_cscv_validates_arguments(native_lib):
     from ai_crypto_trader_b200 import _lib
     lib = _lib.load()
-    assert _status(_cscv(B=3)) == EINVAL                        # odd
-    assert _status(_cscv(B=0)) == EINVAL
-    assert _status(_cscv(B=22, T=440)) == ELIMIT                # more than 20 blocks
-    assert _status(_cscv(T=7, B=4)) == EINVAL                   # L = 1
-    assert _status(_cscv(N=1)) == EINVAL
-    assert _status(_cscv(ws=False)) == EINVAL
-    assert _status(_cscv(out=False)) == EINVAL
-    assert _status(_cscv(ld=30)) == EINVAL                      # row stride below T
-    assert _status(_cscv(ws_bytes=8)) == EINVAL                 # workspace too small
+    assert status(*_cscv(B=3)) == EINVAL                        # odd
+    assert status(*_cscv(B=0)) == EINVAL
+    assert status(*_cscv(B=22, T=440)) == ELIMIT                # more than 20 blocks
+    assert status(*_cscv(T=7, B=4)) == EINVAL                   # L = 1
+    assert status(*_cscv(N=1)) == EINVAL
+    assert status(*_cscv(ws=False)) == EINVAL
+    assert status(*_cscv(out=False)) == EINVAL
+    assert status(*_cscv(ld=30)) == EINVAL                      # row stride below T
+    assert status(*_cscv(ws_bytes=8)) == EINVAL                 # workspace too small
     for args in ((4, 7, 4), (1, 40, 4), (4, 40, 3), (4, 440, 22)):
         assert lib.b200bt_cscv_workspace_bytes(*args) == 0, args
     assert lib.b200bt_cscv_workspace_bytes(1000, 700, 16) >= 2 * 16 * 1000 * 8 + 12870 * 4 * 12

@@ -5,7 +5,7 @@ import ctypes as C
 
 import pytest
 
-EINVAL, ENODEVICE, ELIMIT = 10001, 10002, 10003
+from abi_header import EINVAL, ELIMIT, ENODEVICE, status
 
 
 def _d(*v):
@@ -28,41 +28,32 @@ def _boot(S=2, R=16, block_len=1, returns=True, n_paths=8):
             _d(*[1.0] * S), _d(*[1.0] * S), n_paths, 4, 1, 0, C.addressof(buf), C.addressof(buf), None, None)
 
 
-def _status(args):
-    from ai_crypto_trader_b200 import _lib
-    try:
-        _lib.call(*args)
-    except _lib.B200btError as e:
-        return e.status
-    return 0
-
-
 def test_portfolio_entry_points_refuse_without_device(native_lib):
     import torch
     if torch.cuda.is_available():
         pytest.skip("GPU present: the no-device path cannot be exercised")
-    assert _status(_gbm()) == ENODEVICE
-    assert _status(_boot()) == ENODEVICE
+    assert status(*_gbm()) == ENODEVICE
+    assert status(*_boot()) == ENODEVICE
 
 
 def test_portfolio_entry_points_validate_arguments(native_lib):
-    assert _status(_gbm(S=0)) == EINVAL
-    assert _status(_gbm(n_paths=0)) == EINVAL
-    assert _status(_gbm(steps=-1)) == EINVAL
-    assert _status(_gbm(finals=False)) == EINVAL
-    assert _status(_gbm(s0=_d(1.0, 0.0))) == EINVAL                  # a price must be positive
-    assert _status(_gbm(qty=_d(1.0, -1.0))) == EINVAL                # no short positions
-    assert _status(_gbm(qty=_d(0.0, 0.0))) == EINVAL                 # V_0 = 0
-    assert _status(_gbm(chol=(C.c_float * 4)(1.0, 0.0, float("nan"), 1.0))) == EINVAL
-    assert _status(_boot(returns=False)) == EINVAL
-    assert _status(_boot(R=0)) == EINVAL
-    assert _status(_boot(block_len=0)) == EINVAL
+    assert status(*_gbm(S=0)) == EINVAL
+    assert status(*_gbm(n_paths=0)) == EINVAL
+    assert status(*_gbm(steps=-1)) == EINVAL
+    assert status(*_gbm(finals=False)) == EINVAL
+    assert status(*_gbm(s0=_d(1.0, 0.0))) == EINVAL                  # a price must be positive
+    assert status(*_gbm(qty=_d(1.0, -1.0))) == EINVAL                # no short positions
+    assert status(*_gbm(qty=_d(0.0, 0.0))) == EINVAL                 # V_0 = 0
+    assert status(*_gbm(chol=(C.c_float * 4)(1.0, 0.0, float("nan"), 1.0))) == EINVAL
+    assert status(*_boot(returns=False)) == EINVAL
+    assert status(*_boot(R=0)) == EINVAL
+    assert status(*_boot(block_len=0)) == EINVAL
 
 
 def test_portfolio_entry_points_limits(native_lib):
-    assert _status(_gbm(S=33)) == ELIMIT
-    assert _status(_boot(S=33)) == ELIMIT
-    assert _status(_boot(S=4, R=3073)) == ELIMIT                      # R x S > 12288 table entries
+    assert status(*_gbm(S=33)) == ELIMIT
+    assert status(*_boot(S=33)) == ELIMIT
+    assert status(*_boot(S=4, R=3073)) == ELIMIT                      # R x S > 12288 table entries
 
 
 _BUF = (C.c_float * 64)()
@@ -72,19 +63,19 @@ _P = C.addressof(_BUF)           # any non-null pointer: the arguments are refus
 def test_risk_entry_points_validate_arguments(native_lib):
     lib = native_lib
     ws = int(lib.b200bt_correlation_workspace_bytes(4, 100))
-    assert _status(("b200bt_correlation", _P, 100, 513, 100, _P, _P, 1 << 40, None)) == EINVAL      # S > 512
-    assert _status(("b200bt_correlation", _P, 99, 4, 100, _P, _P, ws, None)) == EINVAL              # ld < N
-    assert _status(("b200bt_correlation", _P, 100, 4, 100, _P, _P, ws - 8, None)) == EINVAL         # workspace
+    assert status(*("b200bt_correlation", _P, 100, 513, 100, _P, _P, 1 << 40, None)) == EINVAL      # S > 512
+    assert status(*("b200bt_correlation", _P, 99, 4, 100, _P, _P, ws, None)) == EINVAL              # ld < N
+    assert status(*("b200bt_correlation", _P, 100, 4, 100, _P, _P, ws - 8, None)) == EINVAL         # workspace
     need = int(lib.b200bt_select_workspace_bytes(3))
-    assert _status(("b200bt_select", _P, 10, _P, 0, _P, _P, 1 << 40, None)) == EINVAL               # no rank
-    assert _status(("b200bt_select", _P, 10, _P, 65, _P, _P, 1 << 40, None)) == EINVAL              # > 64 ranks
-    assert _status(("b200bt_select", _P, 10, _P, 3, _P, _P, need - 1, None)) == EINVAL              # workspace
-    assert _status(("b200bt_tail_stats", _P, 0, 0.0, _P, _P, 1 << 20, None)) == EINVAL              # empty input
-    assert _status(("b200bt_pct_change", _P, 99, 2, 100, _P, 100, None)) == EINVAL                  # ld < N
+    assert status(*("b200bt_select", _P, 10, _P, 0, _P, _P, 1 << 40, None)) == EINVAL               # no rank
+    assert status(*("b200bt_select", _P, 10, _P, 65, _P, _P, 1 << 40, None)) == EINVAL              # > 64 ranks
+    assert status(*("b200bt_select", _P, 10, _P, 3, _P, _P, need - 1, None)) == EINVAL              # workspace
+    assert status(*("b200bt_tail_stats", _P, 0, 0.0, _P, _P, 1 << 20, None)) == EINVAL              # empty input
+    assert status(*("b200bt_pct_change", _P, 99, 2, 100, _P, 100, None)) == EINVAL                  # ld < N
 
 
 def test_risk_entry_points_limits(native_lib):
     def boot(R):
         return ("b200bt_mc_bootstrap", _P, R, 1, 1, 100.0, 8, 4, 1, 0, _P, _P, None, None)
-    assert _status(boot(12289)) == ELIMIT                                # more than 48 KB of table
-    assert _status(("b200bt_pct_change", _P, 10, 65536, 10, _P, 10, None)) == ELIMIT   # S rides on gridDim.y
+    assert status(*boot(12289)) == ELIMIT                                # more than 48 KB of table
+    assert status(*("b200bt_pct_change", _P, 10, 65536, 10, _P, 10, None)) == ELIMIT   # S rides on gridDim.y

@@ -4,7 +4,7 @@ import ctypes as C
 
 import pytest
 
-EINVAL, ENODEVICE, ELIMIT = 10001, 10002, 10003
+from abi_header import EINVAL, ELIMIT, ENODEVICE, status
 
 
 def _mc(T=4, L=1, block_len=1, n_paths=8, method=0, trips=True, counts=True, fees=True, out=True, ld=None, capital=1e4):
@@ -24,47 +24,38 @@ def _pnl(S=1, pop=1, N=16, ld=None, event_cap=4, ld_trip=2, events=True):
             C.addressof(buf), C.addressof(buf), None)
 
 
-def _status(args):
-    from ai_crypto_trader_b200 import _lib
-    try:
-        _lib.call(*args)
-    except _lib.B200btError as e:
-        return e.status
-    return 0
-
-
 def test_trade_mc_entry_points_refuse_without_device(native_lib):
     import torch
     if torch.cuda.is_available():
         pytest.skip("GPU present: the no-device path cannot be exercised")
-    assert _status(_mc()) == ENODEVICE
-    assert _status(_mc(method=1)) == ENODEVICE
-    assert _status(_pnl()) == ENODEVICE
+    assert status(*_mc()) == ENODEVICE
+    assert status(*_mc(method=1)) == ENODEVICE
+    assert status(*_pnl()) == ENODEVICE
 
 
 def test_trade_mc_validates_arguments(native_lib):
-    assert _status(_mc(trips=False)) == EINVAL
-    assert _status(_mc(counts=False)) == EINVAL
-    assert _status(_mc(fees=False)) == EINVAL
-    assert _status(_mc(out=False)) == EINVAL
-    assert _status(_mc(L=0)) == EINVAL
-    assert _status(_mc(method=2)) == EINVAL
-    assert _status(_mc(block_len=0)) == EINVAL
-    assert _status(_mc(n_paths=0)) == EINVAL
-    assert _status(_mc(T=-1)) == EINVAL
-    assert _status(_mc(T=5, ld=4)) == EINVAL                # more trips than the row stride holds
-    assert _status(_mc(capital=0.0)) == EINVAL
+    assert status(*_mc(trips=False)) == EINVAL
+    assert status(*_mc(counts=False)) == EINVAL
+    assert status(*_mc(fees=False)) == EINVAL
+    assert status(*_mc(out=False)) == EINVAL
+    assert status(*_mc(L=0)) == EINVAL
+    assert status(*_mc(method=2)) == EINVAL
+    assert status(*_mc(block_len=0)) == EINVAL
+    assert status(*_mc(n_paths=0)) == EINVAL
+    assert status(*_mc(T=-1)) == EINVAL
+    assert status(*_mc(T=5, ld=4)) == EINVAL                # more trips than the row stride holds
+    assert status(*_mc(capital=0.0)) == EINVAL
 
 
 def test_trade_mc_limits(native_lib):
-    assert _status(_mc(T=1 << 30, ld=1 << 30)) == ELIMIT
-    assert _status(_mc(n_paths=(1 << 38) + 1)) == ELIMIT
+    assert status(*_mc(T=1 << 30, ld=1 << 30)) == ELIMIT
+    assert status(*_mc(n_paths=(1 << 38) + 1)) == ELIMIT
 
 
 def test_trade_pnl_validates_arguments(native_lib):
-    assert _status(_pnl(S=0)) == EINVAL
-    assert _status(_pnl(pop=0)) == EINVAL
-    assert _status(_pnl(ld=8)) == EINVAL                    # row stride below N
-    assert _status(_pnl(events=False)) == EINVAL
-    assert _status(_pnl(event_cap=6, ld_trip=2)) == EINVAL  # event_cap / 2 trips do not fit a row
-    assert _status(_pnl(N=1 << 30, ld=1 << 30)) == ELIMIT
+    assert status(*_pnl(S=0)) == EINVAL
+    assert status(*_pnl(pop=0)) == EINVAL
+    assert status(*_pnl(ld=8)) == EINVAL                    # row stride below N
+    assert status(*_pnl(events=False)) == EINVAL
+    assert status(*_pnl(event_cap=6, ld_trip=2)) == EINVAL  # event_cap / 2 trips do not fit a row
+    assert status(*_pnl(N=1 << 30, ld=1 << 30)) == ELIMIT

@@ -8,8 +8,7 @@ import pytest
 
 import ga_ref
 from oracle import mc_ref
-
-EINVAL, ENODEVICE, ELIMIT = 10001, 10002, 10003
+from abi_header import EINVAL, ELIMIT, ENODEVICE, status
 
 
 # -- fma ---------------------------------------------------------------------------------------------------------------
@@ -160,47 +159,38 @@ def _next(pop=8, genes=2, lo=(0.0, 1.0), hi=(1.0, 5.0), is_int=(0, 1), elitism=0
             (C.c_double * G)(*hi), (C.c_int * G)(*is_int), elitism, tournament, 0.8, 0.2, 1, 1, _DEV + 3072, out, None)
 
 
-def _status(args):
-    from ai_crypto_trader_b200 import _lib
-    try:
-        _lib.call(*args)
-    except _lib.B200btError as e:
-        return e.status
-    return 0
-
-
 def _wide(n, lo, hi, is_int):
     return dict(lo=(lo,) * n, hi=(hi,) * n, is_int=(is_int,) * n)
 
 
 @pytest.mark.parametrize("entry", [_init, _next])
 def test_ga_entry_points_validate_ranges(native_lib, entry):
-    assert _status(entry(genes=0)) == EINVAL
-    assert _status(entry(genes=65, **_wide(65, 0.0, 1.0, 0))) == EINVAL
-    assert _status(entry(lo=(0.0, 2.0), hi=(1.0, 1.0))) == EINVAL                       # hi < lo
-    assert _status(entry(lo=(0.0, 0.0), hi=(1.0, 4.0e9), is_int=(0, 1))) == ELIMIT        # integer span >= 4e9
-    assert _status(entry(lo=(0.0, -2.0e9), hi=(1.0, 2.0e9), is_int=(0, 1))) == ELIMIT
+    assert status(*entry(genes=0)) == EINVAL
+    assert status(*entry(genes=65, **_wide(65, 0.0, 1.0, 0))) == EINVAL
+    assert status(*entry(lo=(0.0, 2.0), hi=(1.0, 1.0))) == EINVAL                       # hi < lo
+    assert status(*entry(lo=(0.0, 0.0), hi=(1.0, 4.0e9), is_int=(0, 1))) == ELIMIT        # integer span >= 4e9
+    assert status(*entry(lo=(0.0, -2.0e9), hi=(1.0, 2.0e9), is_int=(0, 1))) == ELIMIT
 
 
 def test_ga_init_validates_arguments(native_lib):
-    assert _status(_init(n_seeded=9)) == EINVAL                  # more seeded rows than the population
-    assert _status(_init(n_seeded=-1)) == EINVAL
-    assert _status(_init(pop=0)) == EINVAL
+    assert status(*_init(n_seeded=9)) == EINVAL                  # more seeded rows than the population
+    assert status(*_init(n_seeded=-1)) == EINVAL
+    assert status(*_init(pop=0)) == EINVAL
 
 
 @pytest.mark.parametrize("tournament", [0, 9, 5])
 def test_ga_next_generation_validates_tournament(native_lib, tournament):
-    assert _status(_next(pop=4, tournament=tournament)) == EINVAL
+    assert status(*_next(pop=4, tournament=tournament)) == EINVAL
 
 
 @pytest.mark.parametrize("elitism", [math.nan, math.inf, -math.inf])
 def test_ga_next_generation_refuses_a_non_finite_elitism(native_lib, elitism):
-    assert _status(_next(elitism=elitism)) == EINVAL
+    assert status(*_next(elitism=elitism)) == EINVAL
 
 
 def test_ga_next_generation_refuses_aliased_or_null_buffers(native_lib):
-    assert _status(_next(out=_DEV)) == EINVAL                    # params == params_out
-    assert _status(_next(out=None)) == EINVAL
+    assert status(*_next(out=_DEV)) == EINVAL                    # params == params_out
+    assert status(*_next(out=None)) == EINVAL
 
 
 def test_ga_entry_points_refuse_without_device(native_lib):
@@ -209,10 +199,10 @@ def test_ga_entry_points_refuse_without_device(native_lib):
     import torch
     if torch.cuda.is_available():
         pytest.skip("GPU present: the no-device path cannot be exercised")
-    assert _status(_init()) == ENODEVICE
-    assert _status(_init(n_seeded=8)) == ENODEVICE
-    assert _status(_init(lo=(0.0, 0.0), hi=(1.0, 4.0e9), is_int=(0, 0))) == ENODEVICE
-    assert _status(_next(lo=(0.0, 0.0), hi=(1.0, 4.0e9), is_int=(0, 0))) == ENODEVICE
+    assert status(*_init()) == ENODEVICE
+    assert status(*_init(n_seeded=8)) == ENODEVICE
+    assert status(*_init(lo=(0.0, 0.0), hi=(1.0, 4.0e9), is_int=(0, 0))) == ENODEVICE
+    assert status(*_next(lo=(0.0, 0.0), hi=(1.0, 4.0e9), is_int=(0, 0))) == ENODEVICE
     for elitism in (0.1, 0.0, -5.0, 1.0, 1e300):
-        assert _status(_next(elitism=elitism)) == ENODEVICE
-    assert _status(_next(pop=8, tournament=8)) == ENODEVICE
+        assert status(*_next(elitism=elitism)) == ENODEVICE
+    assert status(*_next(pop=8, tournament=8)) == ENODEVICE

@@ -11,6 +11,8 @@ import ctypes
 import numpy as np
 import pytest
 
+from gpu_fixtures import torch_cuda
+
 pytestmark = pytest.mark.gpu
 
 EXACT = ("n_records", "trade_hash", "n_wins", "n_losses", "n_days", "n_negative_days", "sum_duration_bars")
@@ -21,14 +23,6 @@ SOURCE = [0, 1, 0, 2, 0]          # symbol s is a copy of synthetic series SOURC
 QUIET = 4                         # this symbol's RSI rows are NaN: no threshold compare is true, it never trades
 DENSE = dict(rsi_period=5, rsi_oversold=99, rsi_overbought=101, take_profit=0.0001, stop_loss=0.0001)
 NEVER = dict(rsi_period=14, rsi_oversold=0, rsi_overbought=100)
-
-
-@pytest.fixture(scope="module")
-def torch_cuda(native_lib):
-    import torch
-    assert torch.cuda.is_available(), "gpu-marked tests need a CUDA device"
-    torch.cuda.set_device(0)
-    return torch
 
 
 def _population(n=22, seed=11):

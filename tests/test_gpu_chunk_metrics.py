@@ -12,6 +12,8 @@ bars per day (a first chunk inside one day, days spanning several steps) and 7-m
 import numpy as np
 import pytest
 
+from gpu_fixtures import torch_cuda
+
 pytestmark = pytest.mark.gpu
 
 K, CHUNK = 12, 1024               # tiled chunks: chunk c is bars [1024 c, 1024 (c + 1)) (group aligned)
@@ -22,14 +24,6 @@ WINDOW = [20, -1, 96, 97, 128, 224, 225, 256, 32, 169, 300, 61]
 RISE = [1, 0, 1, 1, 0, 1, 1, 0, 1, 1, 0, 0]
 EDGES = {1, 127, 128, 129, 255, 256, 257}
 LONG = dict(rsi_period=5, rsi_oversold=99, rsi_overbought=101, take_profit=0.0001, stop_loss=0.0001)
-
-
-@pytest.fixture(scope="module")
-def torch_cuda(native_lib):
-    import torch
-    assert torch.cuda.is_available(), "gpu-marked tests need a CUDA device"
-    torch.cuda.set_device(0)
-    return torch
 
 
 def _close():

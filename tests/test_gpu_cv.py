@@ -6,17 +6,10 @@ import numpy as np
 import pytest
 
 from conftest import unjson
+from gpu_fixtures import torch_cuda
 
 GOLD = Path(__file__).parent / "golden"
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def torch_cuda(native_lib):
-    import torch
-    assert torch.cuda.is_available(), "gpu-marked tests need a CUDA device"
-    torch.cuda.set_device(0)
-    return torch
 
 
 def _points(ref, params):

@@ -3,15 +3,9 @@ determinism, elitism, range / integrality invariants, and a real optimisation ru
 import numpy as np
 import pytest
 
+from gpu_fixtures import torch_cuda
+
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def torch_cuda(native_lib):
-    import torch
-    assert torch.cuda.is_available(), "gpu-marked tests need a CUDA device"
-    torch.cuda.set_device(0)
-    return torch
 
 
 def _toy_fitness(population):

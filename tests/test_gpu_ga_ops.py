@@ -10,18 +10,11 @@ import numpy as np
 import pytest
 
 import ga_ref
+from gpu_fixtures import torch_cuda
 
 pytestmark = pytest.mark.gpu
 
 SEED = 0x9E3779B97F4A7C15                  # both key words non-zero
-
-
-@pytest.fixture(scope="module")
-def torch_cuda(native_lib):
-    import torch
-    assert torch.cuda.is_available(), "gpu-marked tests need a CUDA device"
-    torch.cuda.set_device(0)
-    return torch
 
 
 # -- gene sets ---------------------------------------------------------------------------------------------------------

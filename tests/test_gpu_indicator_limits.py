@@ -11,6 +11,9 @@ import numpy as np
 import pandas as pd
 import pytest
 
+from abi_header import EINVAL, ELIMIT
+from gpu_fixtures import torch_cuda
+
 pytestmark = pytest.mark.gpu
 
 # kernel constants (csrc/indicators.cu, csrc/indicators2.cu)
@@ -55,14 +58,6 @@ def _rsi_halo(w):
 ATR_MAX_WINDOW = max(w for w in range(1, IND_MAX_WINDOW + 1)
                      if (_wilder_halo(w) + IND_TILE + IND_MAX_WINDOW + 8) * 8 <= SMEM_LIMIT)
 assert ATR_MAX_WINDOW == 541
-
-
-@pytest.fixture(scope="module")
-def torch_cuda(native_lib):
-    import torch
-    assert torch.cuda.is_available(), "gpu-marked tests need a CUDA device"
-    torch.cuda.set_device(0)
-    return torch
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -379,7 +374,6 @@ def test_each_bound_is_accepted_at_the_limit_and_refused_past_it(torch_cuda):
     from ai_crypto_trader_b200 import _lib, indicators as ind
     from ai_crypto_trader_b200._lib import B200btError
     from ai_crypto_trader_b200.sweep import rsi_bank
-    ELIMIT, EINVAL = 10003, 10001
     N = 300
     o, h, l, c, v = _dev(torch, _ohlcv(2, N))
 

@@ -8,18 +8,12 @@ it opened, ordinary lanes, and one lane whose price screen passes on a bar that 
 import numpy as np
 import pytest
 
+from gpu_fixtures import torch_cuda
+
 N_BARS = 40_001               # not a multiple of the 128-bar tile: a ragged last tile
 PERIODS = (5, 7)              # at most two RSI rows per warp (the scan's packing rule)
 NEAR_BAND = 3                 # the lane whose planted bar sits inside the fp32 screening band
 SW_MARGIN = 1e-6              # relative width of that band (csrc/sweep_dev.cuh)
-
-
-@pytest.fixture(scope="module")
-def torch_cuda(native_lib):
-    import torch
-    assert torch.cuda.is_available(), "gpu-marked tests need a CUDA device"
-    torch.cuda.set_device(0)
-    return torch
 
 
 def _population():

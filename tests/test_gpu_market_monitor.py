@@ -16,19 +16,12 @@ import pytest
 
 import market_monitor_ref as ref
 import regime_ref
+from gpu_fixtures import torch_cuda
 from test_market_monitor_host import DICTS, FIXTURE, _equal, _leaves
 
 pytestmark = pytest.mark.gpu
 
 MINUTE0 = 28_401_120
-
-
-@pytest.fixture(scope="module")
-def torch_cuda(native_lib):
-    import torch
-    assert torch.cuda.is_available(), "gpu-marked tests need a CUDA device"
-    torch.cuda.set_device(0)
-    return torch
 
 
 def _synth(S, N, minute0=MINUTE0, seed=1234):

@@ -12,6 +12,7 @@ import numpy as np
 import pytest
 
 import cscv_ref
+from gpu_fixtures import torch_cuda
 
 pytestmark = pytest.mark.gpu
 
@@ -21,14 +22,6 @@ SOURCE = [0, 1, 0, 2, 0]
 QUIET = 4
 DENSE = dict(rsi_period=5, rsi_oversold=99, rsi_overbought=101, take_profit=0.0001, stop_loss=0.0001)
 NEVER = dict(rsi_period=14, rsi_oversold=0, rsi_overbought=100)
-
-
-@pytest.fixture(scope="module")
-def torch_cuda(native_lib):
-    import torch
-    assert torch.cuda.is_available(), "gpu-marked tests need a CUDA device"
-    torch.cuda.set_device(0)
-    return torch
 
 
 def _population(n=22, seed=11):

@@ -6,18 +6,12 @@ initial capital) after chunks without records, a lane whose equity never moves (
 import numpy as np
 import pytest
 
+from gpu_fixtures import torch_cuda
+
 pytestmark = pytest.mark.gpu
 
 N = 140_000
 QUIET = 30_000          # constant price before this bar: RSI stays at 100, the long-only lanes do not trade
-
-
-@pytest.fixture(scope="module")
-def torch_cuda(native_lib):
-    import torch
-    assert torch.cuda.is_available(), "gpu-marked tests need a CUDA device"
-    torch.cuda.set_device(0)
-    return torch
 
 
 def _close():

@@ -22,6 +22,7 @@ import pytest
 import cscv_ref
 import record_buffers as rb
 import trade_mc_ref
+from gpu_fixtures import torch_cuda
 from oracle import sim_oracle
 
 pytestmark = pytest.mark.gpu
@@ -336,14 +337,6 @@ SCALES = (2.0 ** -12, 2.0 ** 10)
 
 
 # ---- device calls --------------------------------------------------------------------------------------------------
-@pytest.fixture(scope="module")
-def torch_cuda(native_lib):
-    import torch
-    assert torch.cuda.is_available(), "gpu-marked tests need a CUDA device"
-    torch.cuda.set_device(0)
-    return torch
-
-
 def run(torch, case):
     """All four passes on the case's buffer -> host arrays."""
     from ai_crypto_trader_b200 import _lib

@@ -15,6 +15,7 @@ import numpy as np
 import pytest
 
 import regime_ref
+from gpu_fixtures import torch_cuda
 
 pytestmark = pytest.mark.gpu
 
@@ -27,14 +28,6 @@ COUNTS = ("n_records", "n_wins", "n_losses", "n_days", "sum_duration_bars")
 FLOATS = ("total_profit", "total_loss", "net_profit", "max_drawdown", "sharpe_ratio", "largest_profit", "largest_loss",
           "score", "win_rate", "profit_factor", "sortino_ratio", "n_negative_days", "downside_deviation",
           "mean_daily_pnl")
-
-
-@pytest.fixture(scope="module")
-def torch_cuda(native_lib):
-    import torch
-    assert torch.cuda.is_available(), "gpu-marked tests need a CUDA device"
-    torch.cuda.set_device(0)
-    return torch
 
 
 def _population(n=22, seed=11):

@@ -13,6 +13,7 @@ import pandas as pd
 import pytest
 
 import mc_joint_ref
+from gpu_fixtures import torch_cuda
 from oracle import mc_ref, portfolio_ref
 
 pytestmark = pytest.mark.gpu
@@ -46,14 +47,6 @@ def corr_smem(S):
 
 def tail_blocks(n):
     return min(TAIL_GRID, (n + 255) // 256)
-
-
-@pytest.fixture(scope="module")
-def torch_cuda(native_lib):
-    import torch
-    assert torch.cuda.is_available(), "gpu-marked tests need a CUDA device"
-    torch.cuda.set_device(0)
-    return torch
 
 
 @pytest.fixture(scope="module")

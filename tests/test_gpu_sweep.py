@@ -4,16 +4,9 @@ import numpy as np
 import pytest
 
 from conftest import unjson
+from gpu_fixtures import torch_cuda
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def torch_cuda(native_lib):
-    import torch
-    assert torch.cuda.is_available(), "gpu-marked tests need a CUDA device"
-    torch.cuda.set_device(0)
-    return torch
 
 
 def _bank_mismatch(got, want):

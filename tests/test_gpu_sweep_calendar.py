@@ -25,6 +25,8 @@ from pathlib import Path
 import numpy as np
 import pytest
 
+from gpu_fixtures import torch_cuda
+
 pytestmark = pytest.mark.gpu
 
 GOLD = Path(__file__).parent / "golden"
@@ -43,14 +45,6 @@ N1 = 1 << 16                      # section 1: tiled chunk c starts at 4096 c
 CHUNK = N1 // 16
 CAP = 2048                        # event words kept per lane
 DENSE = dict(rsi_period=5, rsi_oversold=99, rsi_overbought=101, take_profit=0.0001, stop_loss=0.0001)
-
-
-@pytest.fixture(scope="module")
-def torch_cuda(native_lib):
-    import torch
-    assert torch.cuda.is_available(), "gpu-marked tests need a CUDA device"
-    torch.cuda.set_device(0)
-    return torch
 
 
 # -- shared helpers ------------------------------------------------------------------------------------------------------

@@ -22,6 +22,7 @@ import numpy as np
 import pandas as pd
 import pytest
 
+from gpu_fixtures import torch_cuda
 from test_oracle_indicators import DAY0, grid_cases
 
 pytestmark = pytest.mark.gpu
@@ -33,14 +34,6 @@ SCHEDULES = {
     "chunked": dict(mode="chunked", chunk_options=dict(target_events=300, max_chunks=64, warm=256, pool_scale=4.0)),
     "tiled": dict(mode="tiled", chunk_options=dict(chunks=16, warm=1024, pool_scale=4.0)),
 }
-
-
-@pytest.fixture(scope="module")
-def torch_cuda(native_lib):
-    import torch
-    assert torch.cuda.is_available(), "gpu-marked tests need a CUDA device"
-    torch.cuda.set_device(0)
-    return torch
 
 
 # -- 1. resample and align -----------------------------------------------------------------------------------------------

@@ -5,18 +5,11 @@ import pytest
 
 import trade_mc_ref as R
 from conftest import unjson
+from gpu_fixtures import torch_cuda
 
 pytestmark = pytest.mark.gpu
 
 SMEM_TRIPS = 6144          # csrc/trade_mc.cu TMC_SMEM_TRIPS: larger lanes take the L2 form
-
-
-@pytest.fixture(scope="module")
-def torch_cuda(native_lib):
-    import torch
-    assert torch.cuda.is_available(), "gpu-marked tests need a CUDA device"
-    torch.cuda.set_device(0)
-    return torch
 
 
 @pytest.fixture(scope="module")

@@ -12,19 +12,12 @@ import pytest
 
 import regime_ref
 import volume_profile_ref as ref
+from gpu_fixtures import torch_cuda
 from test_volume_profile_host import CASES, IDS, _close, frame_of
 
 pytestmark = pytest.mark.gpu
 
 MINUTE0 = 28_401_120
-
-
-@pytest.fixture(scope="module")
-def torch_cuda(native_lib):
-    import torch
-    assert torch.cuda.is_available(), "gpu-marked tests need a CUDA device"
-    torch.cuda.set_device(0)
-    return torch
 
 
 def _synth(torch, S, N, bar_minutes=1, seed=1234, minute0=MINUTE0):

@@ -7,6 +7,8 @@ import ctypes as C
 import numpy as np
 import pytest
 
+from abi_header import DEV, EINVAL, ELIMIT, ENODEVICE
+
 PERIODS = (5, 9, 14)
 SOURCE = [0, 1, 0, 2]            # symbols 0 and 2 are the same series: their records tie on the same bars
 
@@ -80,28 +82,24 @@ def test_single_symbol_book_is_the_oracle_lane():
                 assert got[f] == pytest.approx(float(want[f]), rel=1e-12, abs=1e-12, nan_ok=True), f
 
 
-_EINVAL, _ENODEVICE, _ELIMIT = 10001, 10002, 10003
-
-
-def _book_args(S=10, N=200_000, pop=64, cap=4096, minute0=0, bar_minutes=1, price=1 << 20):
+def _book_args(S=10, N=200_000, pop=64, cap=4096, minute0=0, bar_minutes=1, price=DEV):
     """b200bt_book_metrics arguments with non-null dummy device pointers (never dereferenced: every call below is
     rejected before the device is touched)."""
     from ai_crypto_trader_b200 import _lib
     cfg = _lib.SweepConfig(initial_capital=10000.0, minute0=minute0, bar_minutes=bar_minutes, primary=0, secondary_mask=7,
                            variant=0, gap_bar=0, gap_minutes=0)
-    dev = 1 << 20
-    return (price, N, S, N, dev, pop, C.byref(cfg), dev, dev, cap, dev, None, None)
+    return (price, N, S, N, DEV, pop, C.byref(cfg), DEV, DEV, cap, DEV, None, None)
 
 
 @pytest.mark.parametrize("case, kw, status", [
-    ("null price", dict(price=None), _EINVAL),
-    ("no individuals", dict(pop=0), _EINVAL),
-    ("negative event cap", dict(cap=-1), _EINVAL),
-    ("65 symbols", dict(S=65), _ELIMIT),
-    ("N = 2^30", dict(N=1 << 30), _ELIMIT),
-    ("S * (N + 1) records beyond 2^32", dict(S=64, N=(1 << 26)), _ELIMIT),
-    ("zero bar_minutes", dict(bar_minutes=0), _EINVAL),
-    ("clock beyond 2^32 minutes", dict(minute0=1 << 32), _ELIMIT),
+    ("null price", dict(price=None), EINVAL),
+    ("no individuals", dict(pop=0), EINVAL),
+    ("negative event cap", dict(cap=-1), EINVAL),
+    ("65 symbols", dict(S=65), ELIMIT),
+    ("N = 2^30", dict(N=1 << 30), ELIMIT),
+    ("S * (N + 1) records beyond 2^32", dict(S=64, N=(1 << 26)), ELIMIT),
+    ("zero bar_minutes", dict(bar_minutes=0), EINVAL),
+    ("clock beyond 2^32 minutes", dict(minute0=1 << 32), ELIMIT),
 ])
 def test_book_metrics_rejects_bad_arguments(native_lib, case, kw, status):
     from ai_crypto_trader_b200 import _lib
@@ -117,4 +115,4 @@ def test_book_metrics_needs_a_device(native_lib):
     from ai_crypto_trader_b200 import _lib
     with pytest.raises(_lib.B200btError) as ei:
         _lib.call("b200bt_book_metrics", *_book_args(S=64))
-    assert ei.value.status == _ENODEVICE
+    assert ei.value.status == ENODEVICE

@@ -6,13 +6,12 @@ import numpy as np
 import pytest
 
 import pareto_ref as pr
+from abi_header import EINVAL, ELIMIT, ENODEVICE, status
 
 # config.json evolution.optimization_goals of the reference
 REFERENCE_GOALS = {"primary": "sharpe_ratio", "secondary": ["max_drawdown", "win_rate", "profit_factor"],
                    "constraints": {"min_trades_per_day": 20, "max_trades_per_day": 50, "min_holding_period": "1m",
                                    "max_holding_period": "15m"}}
-
-EINVAL, ENODEVICE, ELIMIT = 10001, 10002, 10003
 
 
 def _same(a, b):
@@ -131,15 +130,6 @@ def test_objectives_from_goals():
             objectives_from_goals(bad)
 
 
-def _status(*args):
-    from ai_crypto_trader_b200 import _lib
-    try:
-        _lib.call(*args)
-    except _lib.B200btError as e:
-        return e.status
-    return 0
-
-
 def _rank_args(n=4, M=2, ld=None, ws_bytes=None, maximize=None, null_out=False):
     import ctypes as C
     from ai_crypto_trader_b200 import _lib
@@ -164,19 +154,19 @@ def test_entry_points_refuse_without_device(native_lib):
     import torch
     if torch.cuda.is_available():
         pytest.skip("GPU present: the no-device path cannot be exercised")
-    assert _status(*_rank_args()) == ENODEVICE
-    assert _status(*_matrix_args()) == ENODEVICE
+    assert status(*_rank_args()) == ENODEVICE
+    assert status(*_matrix_args()) == ENODEVICE
 
 
 def test_pareto_rank_validates_arguments(native_lib):
     lib = native_lib
-    assert _status(*_rank_args(n=0)) == EINVAL
-    assert _status(*_rank_args(n=65537)) == ELIMIT
-    assert _status(*_rank_args(M=0)) == EINVAL
-    assert _status(*_rank_args(M=9)) == ELIMIT
-    assert _status(*_rank_args(M=3, ld=2)) == EINVAL
-    assert _status(*_rank_args(ws_bytes=64)) == EINVAL
-    assert _status(*_rank_args(null_out=True)) == EINVAL
+    assert status(*_rank_args(n=0)) == EINVAL
+    assert status(*_rank_args(n=65537)) == ELIMIT
+    assert status(*_rank_args(M=0)) == EINVAL
+    assert status(*_rank_args(M=9)) == ELIMIT
+    assert status(*_rank_args(M=3, ld=2)) == EINVAL
+    assert status(*_rank_args(ws_bytes=64)) == EINVAL
+    assert status(*_rank_args(null_out=True)) == EINVAL
     for n, M in ((0, 2), (65537, 2), (10, 0), (10, 9)):
         assert lib.b200bt_pareto_workspace_bytes(n, M) == 0, (n, M)
     assert lib.b200bt_pareto_workspace_bytes(65536, 8) >= 65536 * 65536 // 8
@@ -184,13 +174,13 @@ def test_pareto_rank_validates_arguments(native_lib):
 
 
 def test_objective_matrix_validates_arguments(native_lib):
-    assert _status(*_matrix_args(pop=0)) == EINVAL
-    assert _status(*_matrix_args(S=0)) == EINVAL
-    assert _status(*_matrix_args(fields=())) == EINVAL
-    assert _status(*_matrix_args(fields=tuple(range(9)))) == ELIMIT
-    assert _status(*_matrix_args(fields=(12, 19))) == EINVAL       # trade_hash is not a field
-    assert _status(*_matrix_args(fields=(-1,))) == EINVAL
-    assert _status(*_matrix_args(fields=(0, 1), ld=1)) == EINVAL
+    assert status(*_matrix_args(pop=0)) == EINVAL
+    assert status(*_matrix_args(S=0)) == EINVAL
+    assert status(*_matrix_args(fields=())) == EINVAL
+    assert status(*_matrix_args(fields=tuple(range(9)))) == ELIMIT
+    assert status(*_matrix_args(fields=(12, 19))) == EINVAL       # trade_hash is not a field
+    assert status(*_matrix_args(fields=(-1,))) == EINVAL
+    assert status(*_matrix_args(fields=(0, 1), ld=1)) == EINVAL
 
 
 def test_host_wrappers_refuse_host_tensors():
