@@ -15,55 +15,21 @@ with the card's name, power limit, the SM clock sampled while timing and the boo
 Needs an H100; no fallback.
 """
 import argparse
-import json
-import re
-import subprocess
-import sys
-import time
-from pathlib import Path
-
-ROOT = Path(__file__).resolve().parents[1]
-sys.path.insert(0, str(ROOT))
-sys.path.insert(0, str(ROOT / "tests"))
 import ctypes as C
+import json
+import sys
 
 import numpy as np
 import torch
 
-
-def _card():
-    out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i",
-                          str(torch.cuda.current_device())], capture_output=True, text=True, timeout=30).stdout
-    name, power = [x.strip() for x in out.strip().splitlines()[0].split(",")]
-    return name, power
-
-
-def _resources():
-    from ai_crypto_trader_b200 import _lib
-    import shutil
-    tool = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
-    try:
-        text = subprocess.run([tool, "-res-usage", str(_lib.LIB_PATH)], capture_output=True, text=True, timeout=120).stdout
-    except OSError:
-        return None
-    fn = None
-    for line in text.splitlines():
-        m = re.search(r"Function (\S+):", line)
-        if m:
-            fn = m.group(1)
-            continue
-        if fn and "book_kernel" in fn:
-            r, loc, sh = re.search(r"REG:(\d+)", line), re.search(r"LOCAL:(\d+)", line), re.search(r"SHARED:(\d+)", line)
-            if r:
-                return {"registers": int(r.group(1)), "local_bytes": int(loc.group(1)) if loc else None,
-                        "shared_bytes": int(sh.group(1)) if sh else None}
-    return None
+import harness
 
 
 def _check(sweep, population, idx, close, bank):
     """Largest relative deviation of the GPU books `idx` (of the last book evaluation) from the oracle's."""
-    import book_ref
     from oracle import sim_oracle
+    sys.path.insert(0, str(harness.ROOT / "tests"))
+    import book_ref
     got = sweep.book_stats()
     cfg = sim_oracle.config_of(sweep.market.minute0, sweep.market.bar_minutes)
     worst, exact = 0.0, True
@@ -95,22 +61,17 @@ def main():
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("book_bench needs a CUDA device (H100); there is no CPU path")
-    from bench import ClockSampler
-    from ai_crypto_trader_b200 import _lib, synth
-    from ai_crypto_trader_b200.genetic_algorithm import GeneticAlgorithm
-    from ai_crypto_trader_b200.sweep import MarketData, PopulationSweep, decode_population
+    from ai_crypto_trader_b200 import _lib
+    from ai_crypto_trader_b200.sweep import PopulationSweep, decode_population
     torch.cuda.set_device(0)
-    ohlcv = synth.synth_ohlcv(a.symbols, a.bars)
-    market = MarketData(ohlcv)
-    random_pop = synth.random_population(a.pop, seed=42)
-    ga = GeneticAlgorithm(synth.param_ranges(), PopulationSweep(market).fitness_function, population_size=a.pop,
-                          generations=3, random_seed=42)
-    ga.run(seeded_individuals=random_pop)
-    name, power = _card()
+    market, random_pop = harness.configs1(a.symbols, a.bars, a.pop)
+    close = market.close.cpu().numpy()
+    evolved = harness.generation3(PopulationSweep(market).fitness_function, random_pop)
+    resources = harness.kernel_resources(["book_kernel"])
     out = {"workload": f"configs[1]: population {a.pop} x {a.symbols} symbols x {a.bars} 1-minute bars",
-           "card": name, "power_limit": power, "book_kernel": _resources(), "populations": {}}
+           **harness.card(), "book_kernel": resources and resources.get("book_kernel"), "populations": {}}
     rng = np.random.default_rng(7)
-    for label, population in (("random", random_pop), ("generation_3", list(ga.population))):
+    for label, population in (("random", random_pop), ("generation_3", list(evolved))):
         sweep = PopulationSweep(market, aggregation="book")
         sweep.evaluate(population)                        # plans, buffers, zone map, learnt cap
         sweep.evaluate(population)
@@ -146,21 +107,12 @@ def main():
         legs = {"sweep_no_events": sweep_plain, "sweep_with_events": sweep_events, "book_metrics": book_pass}
         sweep_plain(); sweep_events(); book_pass(); torch.cuda.synchronize()
         times = {k: [] for k in legs}
-        clocks = ClockSampler(torch.cuda.current_device())
-        clocks.start()
-        time.sleep(0.3)
-        w0 = time.time()
-        for _ in range(a.reps):
-            for k, fn in legs.items():
-                if k == "book_metrics":
-                    sweep_events()                        # the book reads the buffers this sweep wrote
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record()
-                fn()
-                e1.record()
-                torch.cuda.synchronize()
-                times[k].append(e0.elapsed_time(e1))
-        w1 = time.time()
+        with harness.sampled_clocks() as clocks:
+            for _ in range(a.reps):
+                for k, fn in legs.items():
+                    if k == "book_metrics":
+                        sweep_events()                    # the book reads the buffers this sweep wrote
+                    times[k] += harness.event_ms(fn, 1, warmup=0)
         res = {k: {"ms_median": float(np.median(v)), "ms_runs": v, "records_per_s": records / (float(np.median(v)) * 1e-3)}
                for k, v in times.items()}
         # the timed book equals the one evaluate() returned
@@ -170,9 +122,9 @@ def main():
                                              np.array_equal(mine[:, -1].view(np.uint64), ref[:, -1].view(np.uint64)))
         busiest = list(np.argsort(-sweep.book_stats()["n_records"])[:max(1, a.check // 2)])
         sample = busiest + list(rng.choice(pop, size=max(0, a.check - len(busiest)), replace=False))
-        check = _check(sweep, population, sample, ohlcv[3], sweep.bank.cpu().numpy()) if a.check else None
+        check = _check(sweep, population, sample, close, sweep.bank.cpu().numpy()) if a.check else None
         out["populations"][label] = {"records": records, "busiest_lane": cap, "event_buffer_bytes": pop * market.S * cap * 4,
-                                     "legs": res, "sm_clock": clocks.stop(w0, w1), "timed_book_equals_evaluate": same,
+                                     "legs": res, "sm_clock": clocks.sm_clock, "timed_book_equals_evaluate": same,
                                      "oracle_check": check}
     print(json.dumps(out))
 

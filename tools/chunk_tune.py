@@ -1,34 +1,23 @@
 #!/usr/bin/env python
 """Sweep of the time-chunking knobs on the bench workload (pop 1024 x 10 symbols x 1M bars)."""
 import sys, itertools
-from pathlib import Path
-sys.path.insert(0, str(Path(__file__).resolve().parents[1]))
 import numpy as np, torch
-from ai_crypto_trader_b200 import synth
-from ai_crypto_trader_b200.sweep import MarketData, PopulationSweep, decode_population
+import harness
+from ai_crypto_trader_b200.sweep import PopulationSweep, decode_population
 
 S, N, POP = 10, 1_000_000, 1024
-m = MarketData(synth.synth_ohlcv(S, N)); sw = PopulationSweep(m, mode="fused")
-pop = synth.random_population(POP, seed=42)
+m, pop = harness.configs1(S, N, POP); sw = PopulationSweep(m, mode="fused")
+print(", ".join(harness.card().values()))
 packed = decode_population(pop, sw.period_row)
 indiv = torch.from_numpy(packed.view(np.uint8)).cuda()
 fit = torch.empty(POP, dtype=torch.float64, device="cuda")
 
-def timed(plan, reps=3):
-    for _ in range(2): sw.evaluate_device(indiv, None, POP, fit, plan=plan)
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps): sw.evaluate_device(indiv, None, POP, fit, plan=plan)
-    e1.record(); torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / reps
+def timed(plan, order=None, reps=3):
+    return float(np.mean(harness.event_ms(lambda: sw.evaluate_device(indiv, order, POP, fit, plan=plan), reps, warmup=2)))
 
 from ai_crypto_trader_b200.sweep import evaluation_order
 order = torch.from_numpy(evaluation_order(pop)).cuda()
-for _ in range(2): sw.evaluate_device(indiv, order, POP, fit)
-torch.cuda.synchronize(); e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-e0.record(); [sw.evaluate_device(indiv, order, POP, fit) for _ in range(3)]; e1.record(); torch.cuda.synchronize()
-ref = fit.clone(); print("fused %.2f ms" % (e0.elapsed_time(e1) / 3))
+print("fused %.2f ms" % timed(None, order)); ref = fit.clone()
 targets = [int(x) for x in sys.argv[1].split(",")] if len(sys.argv) > 1 else (2048, 4096, 8192, 16384)
 warms = [int(x) for x in sys.argv[2].split(",")] if len(sys.argv) > 2 else (2048, 4096, 8192)
 for target, warm in itertools.product(targets, warms):

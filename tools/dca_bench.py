@@ -12,26 +12,8 @@ from __future__ import annotations
 import argparse
 import json
 import random
-import subprocess
-import sys
-from pathlib import Path
 
-ROOT = Path(__file__).resolve().parents[1]
-sys.path.insert(0, str(ROOT))
-
-
-def timed(torch, fn, reps):
-    fn()
-    torch.cuda.synchronize()
-    times = []
-    for _ in range(reps):
-        t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        t0.record()
-        fn()
-        t1.record()
-        torch.cuda.synchronize()
-        times.append(t0.elapsed_time(t1))
-    return sorted(times)
+import harness
 
 
 def main():
@@ -50,9 +32,7 @@ def main():
     ohlcv = synth.synth_ohlcv(a.symbols, a.bars)
     ohlcv[1] = np.maximum(ohlcv[1], ohlcv[3])
     market = MarketData(ohlcv)
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    gpu = q[0] if q else "unknown"
+    gpu = ", ".join(harness.card().values())
     sweep = DCASweep(market, start_bar=7 * 1440, usdc_balance=5000.0)
     T = a.bars - sweep.start_bar
 
@@ -65,7 +45,7 @@ def main():
             row["purchases_per_lane"] = purchases
         print(json.dumps(row), flush=True)
 
-    report("dca_dip_pct", timed(torch, lambda: dip_pct(market), a.reps))
+    report("dca_dip_pct", sorted(harness.event_ms(lambda: dip_pct(market), a.reps)))
     rng = random.Random(1)
     random_pop = [{k: (rng.randint(lo, hi) if isinstance(lo, int) else rng.uniform(lo, hi))
                    for k, (lo, hi) in dca_param_ranges().items()} for _ in range(a.pop)]
@@ -83,7 +63,7 @@ def main():
         service = torch.empty((a.pop, 5), dtype=torch.float64, device=dev)
         rows = torch.empty((a.pop, sweep.calendar_days()[1]), dtype=torch.float64, device=dev) if day else None
         run = lambda: sweep.launch(indiv, first_us, stats, service, rows, target=tgt, rebalance_any=reb)
-        report(name, timed(torch, run, a.reps), per_lane)
+        report(name, sorted(harness.event_ms(run, a.reps)), per_lane)
 
 
 if __name__ == "__main__":

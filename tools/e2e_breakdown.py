@@ -1,19 +1,16 @@
 #!/usr/bin/env python
 """Where the end-to-end generation time goes (bench.py's e2e leg, phase by phase; wall clock with syncs)."""
-import sys, time
-from pathlib import Path
-sys.path.insert(0, str(Path(__file__).resolve().parents[1]))
 import numpy as np, torch
+import harness
 from ai_crypto_trader_b200 import synth
 from ai_crypto_trader_b200.sweep import MarketData, PopulationSweep, decode_population, evaluation_order, predicted_events
 S, N, POP = 10, 1_000_000, 1024
 ohlcv_host = torch.from_numpy(synth.synth_ohlcv(S, N)).pin_memory()
 pop = synth.random_population(POP, seed=42)
+print(", ".join(harness.card().values()))
 def T(f, n=5):
-    f(); torch.cuda.synchronize()
-    t = time.perf_counter()
-    for _ in range(n): r = f(); torch.cuda.synchronize()
-    return (time.perf_counter() - t) / n * 1e3, r
+    ms, r = harness.wall_ms(f, n, warmup=1)
+    return float(np.mean(ms)), r
 ms, mk = T(lambda: MarketData(ohlcv_host)); print(f"MarketData (H2D 200 MB)      {ms:7.2f} ms")
 ms, sw = T(lambda: PopulationSweep(mk)); print(f"PopulationSweep (RSI bank)   {ms:7.2f} ms")
 ms, _ = T(lambda: sw.evaluate(pop)); print(f"evaluate (total)             {ms:7.2f} ms")

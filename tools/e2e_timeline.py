@@ -1,15 +1,15 @@
 #!/usr/bin/env python
 """Host timeline of one end-to-end generation (bench.py's e2e leg) without intermediate synchronisation:
 when does the host reach each point, and when is the device done."""
-import sys, time
-from pathlib import Path
-sys.path.insert(0, str(Path(__file__).resolve().parents[1]))
+import time
 import numpy as np, torch
+import harness
 from ai_crypto_trader_b200 import synth, sweep as sw_mod
 from ai_crypto_trader_b200.sweep import MarketData, PopulationSweep
 S, N, POP = 10, 1_000_000, 1024
 ohlcv_host = torch.from_numpy(synth.synth_ohlcv(S, N)).pin_memory()
 pop = synth.random_population(POP, seed=42)
+print(", ".join(harness.card().values()))
 marks = []
 def mark(name): marks.append((name, time.perf_counter()))
 orig_plan, orig_dev, orig_decode = PopulationSweep.plan, PopulationSweep.evaluate_device, sw_mod.decode_population
@@ -32,11 +32,7 @@ for name, t in marks: print(f"{(t - t0) * 1e3:8.2f} ms  {name}")
 
 # where do the extra ~2 ms of the sweep inside the e2e step come from?
 def timed(fn, n=5):
-    fn(); torch.cuda.synchronize()
-    t = time.perf_counter()
-    for _ in range(n): fn()
-    torch.cuda.synchronize()
-    return (time.perf_counter() - t) / n * 1e3
+    return float(np.mean(harness.wall_ms(fn, n, warmup=1)[0]))
 PopulationSweep.plan, PopulationSweep.evaluate_device, sw_mod.decode_population = orig_plan, orig_dev, orig_decode
 mk = MarketData(ohlcv_host); sw = PopulationSweep(mk); sw.use_zones = False
 print(f"evaluate() on a resident market / bank, no zone map : {timed(lambda: sw.evaluate(pop)):6.2f} ms")
@@ -44,26 +40,15 @@ dev_ohlcv = mk.ohlcv.clone()
 print(f"MarketData(device tensor) + bank + evaluate          : {timed(lambda: PopulationSweep(MarketData(dev_ohlcv)).evaluate(pop)):6.2f} ms")
 print(f"MarketData(pinned host) + bank + evaluate            : {timed(lambda: PopulationSweep(MarketData(ohlcv_host)).evaluate(pop)):6.2f} ms")
 pinned_close = ohlcv_host[3]
-def close_only_step():
+def close_copy():
     c = torch.empty((S, N), dtype=torch.float32, device="cuda")
     c.copy_(pinned_close, non_blocking=True)
-    return PopulationSweep(MarketData.from_close(c)).evaluate(pop)
+    return c
+def close_and_bank(): return PopulationSweep(MarketData.from_close(close_copy()))
+def close_only_step(): return close_and_bank().evaluate(pop)
 print(f"pinned close only (40 MB) + bank + evaluate          : {timed(close_only_step):6.2f} ms")
 
-def event_timeline():
-    ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
-    torch.cuda.synchronize()
-    t0 = time.perf_counter()
-    ev[0].record()
-    c = torch.empty((S, N), dtype=torch.float32, device="cuda")
-    c.copy_(pinned_close, non_blocking=True)
-    ev[1].record()
-    sw2 = PopulationSweep(MarketData.from_close(c))
-    ev[2].record()
-    sw2.evaluate(pop)
-    ev[3].record()
-    torch.cuda.synchronize()
-    wall = (time.perf_counter() - t0) * 1e3
-    return [ev[0].elapsed_time(e) for e in ev[1:]] + [wall]
-for _ in range(3): r = event_timeline()
+# device time from the start of the step to the end of each of its prefixes, no synchronisation inside a prefix
+r = [harness.event_ms(f, 1, warmup=2)[0] for f in (close_copy, close_and_bank, close_only_step)]
+r.append(harness.wall_ms(close_only_step, 1, warmup=2)[0][0])
 print("device timeline (ms since start): close copied %.2f, bank built %.2f, sweep done %.2f; wall %.2f" % tuple(r))

@@ -7,10 +7,9 @@ Prints one JSON line: per-generation wall time split into the device fitness swe
 planning, and the reference-compatible host GA operators (selection, crossover, mutation).  Under torchrun the
 population is sharded over ranks (ShardedFitness, one all-gather per generation).
 """
-import argparse, json, os, sys, time
-from pathlib import Path
-sys.path.insert(0, str(Path(__file__).resolve().parents[1]))
+import argparse, json, os, time
 import numpy as np, torch
+import harness
 from ai_crypto_trader_b200 import synth
 from ai_crypto_trader_b200.dist import ShardedFitness
 from ai_crypto_trader_b200.genetic_algorithm import DeviceGeneticAlgorithm, GeneticAlgorithm
@@ -37,15 +36,14 @@ torch.cuda.synchronize(); t2 = time.perf_counter()
 fit = ShardedFitness(sweep.evaluate, device=market.device)
 sweep_ms = []; diag = []
 def batch(population):
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    w0 = time.perf_counter(); e0.record()
-    out = fit.batch(population)
-    e1.record(); torch.cuda.synchronize()
-    sweep_ms.append((e0.elapsed_time(e1), (time.perf_counter() - w0) * 1e3))
+    out = []
+    w0 = time.perf_counter()
+    [ms] = harness.event_ms(lambda: out.append(fit.batch(population)), 1, warmup=0)
+    sweep_ms.append((ms, (time.perf_counter() - w0) * 1e3))
     diag.append({"unique": sweep.last_unique, "invalid_lanes": getattr(sweep, "last_invalid_lanes", 0),
                  "pool_overflow": getattr(sweep, "last_pool_overflow", False),
                  "records": float(sweep._stats[:, :, 0].sum().item())})
-    return out
+    return out[0]
 def one(ind): return batch([ind])[0]
 one.batch = batch
 if a.device_ga:
@@ -60,7 +58,7 @@ if rank == 0:
     dev = [m[0] for m in sweep_ms]; wall = [m[1] for m in sweep_ms]
     per_gen = total / evals
     print(json.dumps({"workload": f"GA: pop {a.pop} x {a.symbols} symbols x {a.bars} bars, {a.generations} generations (+1 initial evaluation)",
-                      "n_gpus": world, "generation_wall_s": per_gen, "fitness_device_ms": dev, "fitness_wall_ms": wall,
+                      **harness.card(), "n_gpus": world, "generation_wall_s": per_gen, "fitness_device_ms": dev, "fitness_wall_ms": wall,
                       "host_operator_s_per_generation": (total - sum(wall) / 1e3) / max(1, a.generations),
                       "bar_strategy_evals_per_generation": a.pop * a.symbols * a.bars,
                       "evals_per_s_in_sweep": a.pop * a.symbols * a.bars / (np.median(dev) * 1e-3),

@@ -11,12 +11,8 @@ from __future__ import annotations
 import argparse
 import json
 import random
-import subprocess
-import sys
-from pathlib import Path
 
-ROOT = Path(__file__).resolve().parents[1]
-sys.path.insert(0, str(ROOT))
+import harness
 
 
 def main():
@@ -45,20 +41,11 @@ def main():
     stats = torch.empty((a.pop, a.symbols, 20), dtype=torch.float64, device=market.device)
     D = sweep.calendar_days()[1]
     rows = torch.empty((a.pop, D), dtype=torch.float64, device=market.device) if a.day_profit else None
-    times = []
-    for _ in range(a.reps):
-        t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        t0.record()
-        sweep.launch(indiv, bnd, stats, rows=rows)
-        t1.record()
-        torch.cuda.synchronize()
-        times.append(t0.elapsed_time(t1))
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
+    times = harness.event_ms(lambda: sweep.launch(indiv, bnd, stats, rows=rows), a.reps, warmup=0)
     ticks = a.pop * a.symbols * (a.bars - sweep.start_bar)
     ms = float(np.median(times))
     print(json.dumps({
-        "workload": "grid_sweep" + ("+day_profit" if a.day_profit else ""), "gpu": q[0] if q else "unknown",
+        "workload": "grid_sweep" + ("+day_profit" if a.day_profit else ""), "gpu": ", ".join(harness.card().values()),
         "pop": a.pop, "symbols": a.symbols, "bars": a.bars, "start_bar": sweep.start_bar,
         "ms_median": round(ms, 3), "ms_min": round(min(times), 3), "ms_max": round(max(times), 3),
         "lane_ticks_per_s": ticks / (ms / 1e3),

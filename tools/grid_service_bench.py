@@ -13,12 +13,8 @@ from __future__ import annotations
 import argparse
 import json
 import random
-import subprocess
-import sys
-from pathlib import Path
 
-ROOT = Path(__file__).resolve().parents[1]
-sys.path.insert(0, str(ROOT))
+import harness
 
 
 def main():
@@ -33,9 +29,7 @@ def main():
     from ai_crypto_trader_b200.grid import GridSweep, grid_param_ranges
     from ai_crypto_trader_b200.sweep import MarketData
     torch.cuda.set_device(0)
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    out = {"workload": "grid_service_sweep", "gpu": q[0] if q else "unknown", "pop": a.pop, "bars": a.bars, "runs": []}
+    out = {"workload": "grid_service_sweep", "gpu": ", ".join(harness.card().values()), "pop": a.pop, "bars": a.bars, "runs": []}
     ohlcv = synth.synth_ohlcv(10, a.bars)
     rng = random.Random(1)
     pop = [{k: (rng.randint(lo, hi) if isinstance(lo, int) else rng.uniform(lo, hi))
@@ -54,15 +48,7 @@ def main():
         res = {"symbols": S}
         for name, sv_out, day in (("service_ms", service, False), ("service_day_ms", service, True),
                                   ("lane_ms", None, False), ("lane_day_ms", None, True)):      # None: b200bt_grid_sweep
-            times = []
-            for r in range(a.reps + 1):
-                t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                t0.record()
-                sweep.launch(indiv, bnd, stats, sv_out, rows if day else None)
-                t1.record()
-                torch.cuda.synchronize()
-                if r:
-                    times.append(t0.elapsed_time(t1))
+            times = harness.event_ms(lambda: sweep.launch(indiv, bnd, stats, sv_out, rows if day else None), a.reps)
             res[name] = round(float(np.median(times)), 3)
         res["adjust_ticks_per_individual"] = float(sv["n_adjustments"].mean())
         res["regenerations_per_individual"] = float(st["n_regenerations"].sum(axis=1).mean())

@@ -1,10 +1,9 @@
 #!/usr/bin/env python
 """Pinned host -> device copy bandwidth by size and number of streams (what bounds the upload leg of the e2e step)."""
-import torch, time
-def t(fn, n=10):
-    fn(); torch.cuda.synchronize(); t0=time.perf_counter()
-    for _ in range(n): fn()
-    torch.cuda.synchronize(); return (time.perf_counter()-t0)/n*1e3
+import numpy as np, torch
+import harness
+def t(fn, n=10): return float(np.mean(harness.wall_ms(fn, n, warmup=1)[0]))
+print(", ".join(harness.card().values()))
 for mb in (8, 40, 200):
     h = torch.empty(mb*1024*1024//4, dtype=torch.float32).pin_memory(); d = torch.empty_like(h, device="cuda")
     ms = t(lambda: d.copy_(h, non_blocking=True)); print(f"{mb:4d} MB single copy: {ms:6.2f} ms = {mb/1024/ms*1e3:6.1f} GB/s")

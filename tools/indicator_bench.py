@@ -4,10 +4,9 @@ and GB/s against SURVEY 8(d)'s algorithmic bytes (4 B per input row read + 4 B p
 
     python tools/indicator_bench.py [--symbols 10] [--bars 1000000]
 """
-import argparse, json, sys
-from pathlib import Path
-sys.path.insert(0, str(Path(__file__).resolve().parents[1]))
-import torch
+import argparse, json
+import numpy as np
+import harness
 from ai_crypto_trader_b200 import indicators as ind, synth
 from ai_crypto_trader_b200.sweep import MarketData, rsi_bank
 
@@ -19,18 +18,11 @@ ap.add_argument("--warmup", type=int, default=3)
 a = ap.parse_args()
 m = MarketData(synth.synth_ohlcv(a.symbols, a.bars))
 o, h, l, c, v = m.open, m.high, m.low, m.close, m.volume
-peak = json.loads((Path(__file__).resolve().parents[1] / "MEASURED_PEAKS.json").read_text()).get("hbm_gbs", 3350.0) \
-    if (Path(__file__).resolve().parents[1] / "MEASURED_PEAKS.json").exists() else 3350.0     # H100 SXM data sheet
+peak = json.loads((harness.ROOT / "MEASURED_PEAKS.json").read_text()).get("hbm_gbs", 3350.0) \
+    if (harness.ROOT / "MEASURED_PEAKS.json").exists() else 3350.0     # H100 SXM data sheet
 
-def timed(fn, reps=None):
-    reps = reps or a.reps
-    for _ in range(a.warmup): fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps): fn()
-    e1.record(); torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / reps
+def timed(fn):
+    return float(np.mean(harness.event_ms(fn, a.reps, a.warmup)))
 
 cases = [  # name, callable, input rows, output rows
     ("rsi_bank x26 (no NaN fill)", lambda: rsi_bank(c, list(range(5, 31)), fill=False), 1, 26),
@@ -52,4 +44,5 @@ for name, fn, n_in, n_out in cases:
     rows.append({"kernel": name, "ms": round(ms, 4), "algorithmic_GB": round(gb, 3), "GBps": round(gb / (ms * 1e-3), 1),
                  "frac_of_hbm_peak": round(gb / (ms * 1e-3) / peak, 3)})
     print(f"{name:32s} {ms:8.3f} ms  {gb:6.3f} GB  {gb / (ms * 1e-3):8.1f} GB/s  {gb / (ms * 1e-3) / peak:6.1%}")
-print(json.dumps({"workload": f"{a.symbols} symbols x {a.bars} bars", "hbm_peak_GBps": peak, "indicators": rows}))
+print(json.dumps({"workload": f"{a.symbols} symbols x {a.bars} bars", **harness.card(), "hbm_peak_GBps": peak,
+                  "indicators": rows}))

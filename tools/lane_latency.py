@@ -2,22 +2,18 @@
 """Critical-path probe for the sweep kernel: time a single heavy / mid / light lane alone,
 then one CTA and a full grid of heavy lanes (1M bars).  The heaviest lane's serial event chain is
 the floor of the kernel time at small populations."""
-import sys
-from pathlib import Path
-sys.path.insert(0, str(Path(__file__).resolve().parents[1]))
 import torch
+import harness
 from ai_crypto_trader_b200 import synth
 from ai_crypto_trader_b200.sweep import MarketData, PopulationSweep
 
 m = MarketData(synth.synth_ohlcv(1, 1_000_000))
 sw = PopulationSweep(m)
+print(", ".join(harness.card().values()))
 
 
 def t(pop):
-    sw.evaluate(pop); torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record(); sw.evaluate(pop); e1.record(); torch.cuda.synchronize()
-    return e0.elapsed_time(e1)
+    return harness.event_ms(lambda: sw.evaluate(pop), 1)[0]
 
 
 heavy = dict(synth.random_population(1, seed=1)[0], rsi_period=5, rsi_oversold=35, rsi_overbought=65, take_profit=1, stop_loss=1)

@@ -13,17 +13,16 @@ name, power limit and the SM clock sampled while timing.  Needs an H100; no fall
 import argparse
 import ctypes as C
 import json
-import sys
-import time
-from pathlib import Path
 
-ROOT = Path(__file__).resolve().parents[1]
-sys.path.insert(0, str(ROOT))
-sys.path.insert(0, str(ROOT / "tools"))
-
+import numpy as np
 import torch
 
-from overfitting_bench import _time
+import harness
+
+
+def _time(fn, reps):
+    ms = harness.event_ms(fn, reps)
+    return {"ms_median": float(np.median(ms)), "ms_runs": ms}
 
 
 def main():
@@ -35,14 +34,12 @@ def main():
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("market_monitor_bench needs a CUDA device (H100); there is no CPU path")
-    from bench import ClockSampler
-    from book_bench import _card
-    from ai_crypto_trader_b200 import _lib, synth
+    from ai_crypto_trader_b200 import _lib
     from ai_crypto_trader_b200 import indicators as ind
     from ai_crypto_trader_b200 import market_monitor as mm
-    from ai_crypto_trader_b200.sweep import MarketData, PopulationSweep
+    from ai_crypto_trader_b200.sweep import PopulationSweep
     torch.cuda.set_device(0)
-    market = MarketData(synth.synth_ohlcv(a.symbols, a.bars))
+    market, population = harness.configs1(a.symbols, a.bars, a.pop)
     S, N = market.S, market.N
     k3, k5, k15 = (ind.resample(market, k) for k in (3, 5, 15))
     rows = torch.empty((S, N, mm.ROW_DTYPE.itemsize // 8), dtype=torch.float64, device=market.device)
@@ -54,22 +51,17 @@ def main():
                   k5.ohlcv.data_ptr(), k5.N, k15.ohlcv.data_ptr(), k15.N, C.byref(params),
                   rows.data_ptr() if with_rows else None, labels.data_ptr(), _lib.current_stream())
 
-    name, power = _card()
-    out = {"workload": f"configs[1]: {S} symbols x {N} 1-minute bars, W = 100", "card": name, "power_limit": power}
-    clocks = ClockSampler(torch.cuda.current_device())
-    clocks.start()
-    time.sleep(0.3)
-    w0 = time.time()
-    for with_rows in (True, False):
-        t = _time(lambda: launch(with_rows), a.reps)
-        out["rows" if with_rows else "labels_only"] = dict(t, updates=S * N, updates_per_s=S * N / (t["ms_median"] * 1e-3))
-    trend, names = mm.monitor_labels(market, "trend")
-    sweep = PopulationSweep(market)
-    population = synth.random_population(a.pop, seed=42)
-    out["class_stats_trend"] = _time(lambda: sweep.class_stats(population, trend, len(names)), a.reps)
-    _, views = sweep.class_stats(population, trend, len(names))
-    out["records_per_trend"] = [float(v["n_records"].sum()) for v in views]
-    out["sm_clock"] = clocks.stop(w0, time.time())
+    out = {"workload": f"configs[1]: {S} symbols x {N} 1-minute bars, W = 100", **harness.card()}
+    with harness.sampled_clocks() as clocks:
+        for with_rows in (True, False):
+            t = _time(lambda: launch(with_rows), a.reps)
+            out["rows" if with_rows else "labels_only"] = dict(t, updates=S * N, updates_per_s=S * N / (t["ms_median"] * 1e-3))
+        trend, names = mm.monitor_labels(market, "trend")
+        sweep = PopulationSweep(market)
+        out["class_stats_trend"] = _time(lambda: sweep.class_stats(population, trend, len(names)), a.reps)
+        _, views = sweep.class_stats(population, trend, len(names))
+        out["records_per_trend"] = [float(v["n_records"].sum()) for v in views]
+    out["sm_clock"] = clocks.sm_clock
     print(json.dumps(out))
 
 

@@ -10,12 +10,11 @@ stage time, and the reference's NumPy GBM timed on the host on a bounded sample.
 With --assets: the joint (portfolio) GBM for each asset count S, in path-asset-steps/s, next to the
 single-asset kernel on the same paths and steps, with the card's name and power limit.
 """
-import argparse, json, sys, time
-from pathlib import Path
-ROOT = Path(__file__).resolve().parents[1]
-sys.path.insert(0, str(ROOT))
+import argparse, json, time
 import numpy as np
 import torch
+
+import harness
 
 
 def main():
@@ -46,31 +45,26 @@ def main():
             f, d, _ = eng.gbm(100.0, mu, sigma, 1 / 252, hi - lo, a.steps, 2024, path_offset=lo)
             f, d = gather_paths(f, d, a.paths)
             return risk_statistics(eng, f, d, 100.0, 0.95)
-        job(); dist.barrier(); torch.cuda.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(a.reps): st = job()
-        e1.record(); dist.barrier(); torch.cuda.synchronize()
-        t = torch.tensor([e0.elapsed_time(e1) / a.reps], dtype=torch.float64, device="cuda")
+        job(); dist.barrier()
+        ms = harness.event_ms(job, a.reps, warmup=0)
+        st = job()
+        dist.barrier()
+        t = torch.tensor([float(np.mean(ms))], dtype=torch.float64, device="cuda")
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
         if rank == 0:
             print(json.dumps({"workload": f"GBM {a.paths} paths x {a.steps} steps, risk statistics, {world} GPUs (paths sharded, strong scaling)",
-                              "n_gpus": world, "ms": float(t.item()), "path_steps_per_s": a.paths * a.steps / (float(t.item()) * 1e-3),
+                              **harness.card(), "n_gpus": world, "ms": float(t.item()), "path_steps_per_s": a.paths * a.steps / (float(t.item()) * 1e-3),
                               "var_pct": abs(st["var"]), "mdd_mean": st["mdd_mean"]}))
         dist.destroy_process_group()
         return
     eng = PathEngine()
-    def timed(fn, reps):
-        fn(); torch.cuda.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(reps): out = fn()
-        e1.record(); torch.cuda.synchronize()
-        return e0.elapsed_time(e1) / reps, out
-    ms, (f, d, _) = timed(lambda: eng.gbm(100.0, mu, sigma, 1 / 252, a.paths, a.steps, 2024), a.reps)
-    ms_store, _ = timed(lambda: eng.gbm(100.0, mu, sigma, 1 / 252, a.paths, a.store_steps, 2024, store_paths=True), 3)
+    risk_only = lambda: eng.gbm(100.0, mu, sigma, 1 / 252, a.paths, a.steps, 2024)
+    ms = float(np.mean(harness.event_ms(risk_only, a.reps)))
+    f, d, _ = risk_only()
+    ms_store = float(np.mean(harness.event_ms(
+        lambda: eng.gbm(100.0, mu, sigma, 1 / 252, a.paths, a.store_steps, 2024, store_paths=True), 3)))
     t0 = time.perf_counter(); st = risk_statistics(eng, f, d, 100.0, 0.95); torch.cuda.synchronize(); ms_stats = (time.perf_counter() - t0) * 1e3
-    peak = json.loads((ROOT / "MEASURED_PEAKS.json").read_text())["hbm_gbs"] if (ROOT / "MEASURED_PEAKS.json").exists() else 3350.0     # H100 SXM data sheet
+    peak = json.loads((harness.ROOT / "MEASURED_PEAKS.json").read_text())["hbm_gbs"] if (harness.ROOT / "MEASURED_PEAKS.json").exists() else 3350.0     # H100 SXM data sheet
     # reference generator (NumPy, monte_carlo_service.py:266-273) on a bounded sample
     n_ref, days_ref = 100_000, 101
     t0 = time.perf_counter()
@@ -81,7 +75,7 @@ def main():
     ref_s = time.perf_counter() - t0
     store_bytes = a.paths * (a.store_steps + 1) * 4
     print(json.dumps({
-        "workload": f"GBM {a.paths} paths x {a.steps} steps, risk-only",
+        "workload": f"GBM {a.paths} paths x {a.steps} steps, risk-only", **harness.card(),
         "risk_only": {"ms": ms, "path_steps_per_s": a.paths * a.steps / (ms * 1e-3), "bound": "fp32/fp64 ALU (Philox4x32-10 + Box-Muller + fp64 log-price)"},
         "path_store": {"steps": a.store_steps, "ms": ms_store, "GBps": store_bytes / (ms_store * 1e-3) / 1e9, "hbm_peak_GBps": peak,
                        "frac": store_bytes / (ms_store * 1e-3) / 1e9 / peak},
@@ -90,31 +84,13 @@ def main():
     }))
 
 
-def _card():
-    """(name, power limit) of the card the numbers were taken on (read-only query)."""
-    import subprocess
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i",
-                              str(torch.cuda.current_device())], capture_output=True, text=True, timeout=30).stdout
-        name, power = [x.strip() for x in out.strip().splitlines()[0].split(",")]
-        return name, power
-    except Exception:
-        return torch.cuda.get_device_name(), "unknown"
-
-
 def joint(a, assets):
     from ai_crypto_trader_b200.monte_carlo import PathEngine
     torch.cuda.set_device(0)
     eng = PathEngine()
     reps = max(1, min(a.reps, 3))
 
-    def timed(fn):
-        fn(); torch.cuda.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(reps): fn()
-        e1.record(); torch.cuda.synchronize()
-        return e0.elapsed_time(e1) / reps
+    timed = lambda fn: float(np.mean(harness.event_ms(fn, reps)))
 
     ms1 = timed(lambda: eng.gbm(100.0, 0.08, 0.35, 1 / 252, a.paths, a.steps, 2024))
     rows = []
@@ -127,10 +103,9 @@ def joint(a, assets):
         ms = timed(lambda: eng.portfolio_gbm(s0, qty, mu, sigma, 1 / 252, L, a.paths, a.steps, 2024))
         rows.append({"assets": S, "ms": ms, "path_asset_steps_per_s": a.paths * a.steps * S / (ms * 1e-3),
                      "vs_single_asset_per_asset_step": (ms1 / ms) * S})
-    name, power = _card()
     print(json.dumps({
         "workload": f"joint GBM {a.paths} paths x {a.steps} steps, portfolio value + drawdown every step",
-        "card": name, "power_limit": power, "reps": reps,
+        **harness.card(), "reps": reps,
         "single_asset": {"ms": ms1, "path_steps_per_s": a.paths * a.steps / (ms1 * 1e-3)},
         "joint": rows,
     }))

@@ -2,23 +2,18 @@
 """Fused vs warp-per-chunk vs thread-per-lane sweep across population sizes (10 symbols x N bars).
     python tools/mode_crossover.py [N bars]"""
 import sys
-from pathlib import Path
-sys.path.insert(0, str(Path(__file__).resolve().parents[1]))
 import numpy as np, torch
-from ai_crypto_trader_b200 import synth
-from ai_crypto_trader_b200.sweep import MarketData, PopulationSweep, decode_population, evaluation_order
+import harness
+from ai_crypto_trader_b200.sweep import PopulationSweep, decode_population, evaluation_order
 S, N = 10, (int(sys.argv[1]) if len(sys.argv) > 1 else 1_000_000)
-m = MarketData(synth.synth_ohlcv(S, N)); sw = PopulationSweep(m, mode="fused")
-allpop = synth.random_population(8192, seed=42)
+m, allpop = harness.configs1(S, N, 8192); sw = PopulationSweep(m, mode="fused")
+print(", ".join(harness.card().values()))
 def run(pop, plan):
     indiv = torch.from_numpy(decode_population(pop, sw.period_row).view(np.uint8)).cuda()
     order = torch.from_numpy(evaluation_order(pop)).cuda()
     fit = torch.empty(len(pop), dtype=torch.float64, device="cuda")
     f = lambda: sw.evaluate_device(indiv, order, len(pop), fit, plan=plan)
-    f(); f(); torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record(); f(); f(); f(); e1.record(); torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / 3
+    return float(np.mean(harness.event_ms(f, 3, warmup=2)))
 for P in (8, 32, 128, 512, 1024, 2048, 8192):
     pop = allpop[:P]
     tf = run(pop, None)

@@ -14,30 +14,16 @@ import argparse
 import ctypes as C
 import json
 import math
-import sys
-import time
-from pathlib import Path
-
-ROOT = Path(__file__).resolve().parents[1]
-sys.path.insert(0, str(ROOT))
-sys.path.insert(0, str(ROOT / "tools"))
 
 import numpy as np
 import torch
 
+import harness
+
 
 def _time(fn, reps):
-    fn()
-    torch.cuda.synchronize()
-    out = []
-    for _ in range(reps):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        fn()
-        e1.record()
-        torch.cuda.synchronize()
-        out.append(e0.elapsed_time(e1))
-    return {"ms_median": float(np.median(out)), "ms_runs": out}
+    ms = harness.event_ms(fn, reps)
+    return {"ms_median": float(np.median(ms)), "ms_runs": ms}
 
 
 def main():
@@ -49,60 +35,50 @@ def main():
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("overfitting_bench needs a CUDA device (H100); there is no CPU path")
-    from bench import ClockSampler
-    from book_bench import _card
-    from ai_crypto_trader_b200 import _lib, synth
-    from ai_crypto_trader_b200.genetic_algorithm import GeneticAlgorithm
-    from ai_crypto_trader_b200.sweep import MarketData, PopulationSweep, decode_population
-    torch.cuda.set_device(0)
-    market = MarketData(synth.synth_ohlcv(a.symbols, a.bars))
-    random_pop = synth.random_population(a.pop, seed=42)
-    ga = GeneticAlgorithm(synth.param_ranges(), PopulationSweep(market).fitness_function, population_size=a.pop,
-                          generations=3, random_seed=42)
-    ga.run(seeded_individuals=random_pop)
-    name, power = _card()
-    out = {"workload": f"configs[1]: population {a.pop} x {a.symbols} symbols x {a.bars} 1-minute bars",
-           "card": name, "power_limit": power, "daily_pnl": {}, "cscv": {}}
-    clocks = ClockSampler(torch.cuda.current_device())
-    clocks.start()
-    time.sleep(0.3)
-    w0 = time.time()
-    st = _lib.current_stream()
-    D = 0
-    for label, population in (("random", random_pop), ("generation_3", list(ga.population))):
-        sweep = PopulationSweep(market)
-        sweep.daily_pnl(population)                                   # plans, zone map
-        pop = len(population)
-        indiv = torch.from_numpy(decode_population(population, sweep.period_row).view(np.uint8)).to(market.device)
-        cap = sweep._exact_cap(sweep._stats)
-        records = float(sweep._stats[:, :, 0].sum().item())
-        first, D = sweep.calendar_days()
-        plan = sweep.plan(population)
-        fit = torch.empty(pop, dtype=torch.float64, device=market.device)
-        lanes = torch.empty((pop, market.S, D), dtype=torch.float64, device=market.device)
-        book = torch.empty((pop, D), dtype=torch.float64, device=market.device)
-
-        def sweep_events():
-            sweep.evaluate_device(indiv, None, pop, fit, plan=plan, event_cap=cap)
-
-        def rows():
-            _lib.call("b200bt_daily_pnl", market.close.data_ptr(), _lib.ld(market.close), market.S, market.N,
-                      indiv.data_ptr(), pop, C.byref(sweep.cfg), sweep._stats.data_ptr(), sweep._events.data_ptr(), cap,
-                      lanes.data_ptr(), D, book.data_ptr(), st)
-
-        t_sweep = _time(sweep_events, a.reps)
-        t_rows = _time(rows, a.reps)
-        out["daily_pnl"][label] = {"records": records, "days": D, "busiest_lane": cap, "sweep_with_events": t_sweep,
-                                   "daily_pnl": t_rows,
-                                   "records_per_s": records / (t_rows["ms_median"] * 1e-3)}
+    from ai_crypto_trader_b200 import _lib
     from ai_crypto_trader_b200.overfitting import cscv
-    rng = np.random.default_rng(3)
-    for N, B in ((1024, 16), (1024, 20), (10_000, 16)):
-        x = torch.from_numpy(rng.normal(0.0, 1.0, (N, D))).cuda()
-        t = _time(lambda: cscv(x, B), a.reps)
-        C_ = math.comb(B, B // 2)
-        out["cscv"][f"N={N},B={B}"] = {"days": D, "combinations": C_, "trial_splits": N * C_, "cscv_call": t}
-    out["sm_clock"] = clocks.stop(w0, time.time())
+    from ai_crypto_trader_b200.sweep import PopulationSweep, decode_population
+    torch.cuda.set_device(0)
+    market, random_pop = harness.configs1(a.symbols, a.bars, a.pop)
+    evolved = harness.generation3(PopulationSweep(market).fitness_function, random_pop)
+    out = {"workload": f"configs[1]: population {a.pop} x {a.symbols} symbols x {a.bars} 1-minute bars",
+           **harness.card(), "daily_pnl": {}, "cscv": {}}
+    with harness.sampled_clocks() as clocks:
+        st = _lib.current_stream()
+        D = 0
+        for label, population in (("random", random_pop), ("generation_3", list(evolved))):
+            sweep = PopulationSweep(market)
+            sweep.daily_pnl(population)                                   # plans, zone map
+            pop = len(population)
+            indiv = torch.from_numpy(decode_population(population, sweep.period_row).view(np.uint8)).to(market.device)
+            cap = sweep._exact_cap(sweep._stats)
+            records = float(sweep._stats[:, :, 0].sum().item())
+            first, D = sweep.calendar_days()
+            plan = sweep.plan(population)
+            fit = torch.empty(pop, dtype=torch.float64, device=market.device)
+            lanes = torch.empty((pop, market.S, D), dtype=torch.float64, device=market.device)
+            book = torch.empty((pop, D), dtype=torch.float64, device=market.device)
+
+            def sweep_events():
+                sweep.evaluate_device(indiv, None, pop, fit, plan=plan, event_cap=cap)
+
+            def rows():
+                _lib.call("b200bt_daily_pnl", market.close.data_ptr(), _lib.ld(market.close), market.S, market.N,
+                          indiv.data_ptr(), pop, C.byref(sweep.cfg), sweep._stats.data_ptr(), sweep._events.data_ptr(), cap,
+                          lanes.data_ptr(), D, book.data_ptr(), st)
+
+            t_sweep = _time(sweep_events, a.reps)
+            t_rows = _time(rows, a.reps)
+            out["daily_pnl"][label] = {"records": records, "days": D, "busiest_lane": cap, "sweep_with_events": t_sweep,
+                                       "daily_pnl": t_rows,
+                                       "records_per_s": records / (t_rows["ms_median"] * 1e-3)}
+        rng = np.random.default_rng(3)
+        for N, B in ((1024, 16), (1024, 20), (10_000, 16)):
+            x = torch.from_numpy(rng.normal(0.0, 1.0, (N, D))).cuda()
+            t = _time(lambda: cscv(x, B), a.reps)
+            C_ = math.comb(B, B // 2)
+            out["cscv"][f"N={N},B={B}"] = {"days": D, "combinations": C_, "trial_splits": N * C_, "cscv_call": t}
+    out["sm_clock"] = clocks.sm_clock
     print(json.dumps(out))
 
 

@@ -18,29 +18,18 @@ import argparse
 import json
 import sys
 import time
-from pathlib import Path
-
-ROOT = Path(__file__).resolve().parents[1]
-sys.path.insert(0, str(ROOT))
-sys.path.insert(0, str(ROOT / "tools"))
-sys.path.insert(0, str(ROOT / "tests"))
 
 import numpy as np
 import torch
 
+import harness
+
+sys.path.insert(0, str(harness.ROOT / "tests"))        # pareto_ref: the NumPy form of the ranking contract
+
 
 def _time(fn, reps):
-    fn()
-    torch.cuda.synchronize()
-    out = []
-    for _ in range(reps):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        fn()
-        e1.record()
-        torch.cuda.synchronize()
-        out.append(e0.elapsed_time(e1))
-    return {"ms_median": float(np.median(out)), "ms_min": float(min(out)), "ms_max": float(max(out))}
+    ms = harness.event_ms(fn, reps)
+    return {"ms_median": float(np.median(ms)), "ms_min": float(min(ms)), "ms_max": float(max(ms))}
 
 
 def _kernel_split(fn):
@@ -56,14 +45,6 @@ def _kernel_split(fn):
             name = ev.name.split("(")[0].replace("void ", "").replace("b200bt::", "").split("<")[0]
             split[name] = split.get(name, 0.0) + ev.device_time_total / 1e3
     return {k: round(v, 4) for k, v in split.items()}
-
-
-def _wall(fn):
-    torch.cuda.synchronize()
-    t = time.perf_counter()
-    out = fn()
-    torch.cuda.synchronize()
-    return out, (time.perf_counter() - t) * 1e3
 
 
 def rank_leg(reps):
@@ -122,23 +103,23 @@ def generation_leg(pop, symbols, bars, rounds):
                      pop, len(nsga.names), nsga._lo, nsga._hi, nsga._is_int, 0.0, nsga.tournament_size,
                      nsga.crossover_rate, nsga.mutation_rate, nsga.seed, gen, nsga._sel.data_ptr(), nsga._next.data_ptr(),
                      lib.current_stream())
-        _, t_ops = _wall(operators)
+        [t_ops], _ = harness.wall_ms(operators)
         q = nsga._next[1:]
-        fq, t_sweep = _wall(lambda: nsga._evaluate_rows(q))
+        [t_sweep], fq = harness.wall_ms(lambda: nsga._evaluate_rows(q))
         R = torch.cat([nsga.params, q])
         FR = torch.cat([nsga._obj, fq])
-        (front, crowd, order, _), t_rank = _wall(lambda: nsga._ranker.rank(FR, nsga.maximize))
+        [t_rank], (front, crowd, order, _) = harness.wall_ms(lambda: nsga._ranker.rank(FR, nsga.maximize))
 
         def gather():
             keep = order[:pop].long()
             nsga.params = R.index_select(0, keep)
             nsga._obj = FR.index_select(0, keep)
             nsga._front, nsga._crowding = front.index_select(0, keep), crowd.index_select(0, keep)
-        _, t_gather = _wall(gather)
+        [t_gather], _ = harness.wall_ms(gather)
         rows["nsga2"].append({"operators_ms": t_ops, "sweep_and_objectives_ms": t_sweep, "rank_ms": t_rank,
                               "survivor_gather_ms": t_gather, "total_ms": t_ops + t_sweep + t_rank + t_gather})
         # the scalar device GA, one generation: operators + sweep of the whole population
-        _, t_scalar = _wall(lambda: (scalar.evolve_generation(gen), scalar.evaluate_population()))
+        [t_scalar], _ = harness.wall_ms(lambda: (scalar.evolve_generation(gen), scalar.evaluate_population()))
         rows["device_ga"].append({"total_ms": t_scalar})
         gen += 1
     med = lambda key, part: float(np.median([r[part] for r in rows[key]]))
@@ -160,10 +141,8 @@ def main():
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("pareto_bench needs a CUDA device (H100); there is no CPU path")
-    from book_bench import _card
     torch.cuda.set_device(0)
-    name, power = _card()
-    out = {"card": name, "power_limit": power, "rank": rank_leg(a.reps), "host_numpy": host_leg()}
+    out = {**harness.card(), "rank": rank_leg(a.reps), "host_numpy": host_leg()}
     if not a.skip_generation:
         out["generation_configs1"] = generation_leg(1024, 10, 1_000_000, a.rounds)
         if a.c4:

@@ -14,13 +14,10 @@ from __future__ import annotations
 
 import argparse
 import json
-import subprocess
-import sys
 import time
-from pathlib import Path
 
-ROOT = Path(__file__).resolve().parents[1]
-sys.path.insert(0, str(ROOT))
+import harness
+
 FP64_PEAK = 34e12          # H100 SXM data sheet, FP64 (non-tensor), FLOP/s
 
 
@@ -78,20 +75,13 @@ def main():
     from ai_crypto_trader_b200.rl import RLPopulation, rl_states
     from ai_crypto_trader_b200.sweep import MarketData
     torch.cuda.set_device(0)
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    gpu = q[0] if q else "unknown"
+    gpu = ", ".join(harness.card().values())
     market = MarketData(synth.synth_ohlcv(a.symbols, a.bars))
     hourly = resample(market, 60)
-    rl_states(hourly)
-    torch.cuda.synchronize()
-    t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    t0.record()
+    [ms] = harness.event_ms(lambda: rl_states(hourly), 1)
     states = rl_states(hourly)
-    t1.record()
-    torch.cuda.synchronize()
     print(json.dumps({"workload": "rl_states", "gpu": gpu, "symbols": a.symbols, "hourly_bars": hourly.N,
-                      "ms": round(t0.elapsed_time(t1), 3)}), flush=True)
+                      "ms": round(ms, 3)}), flush=True)
     ends = np.arange(19, hourly.N, dtype=np.int64)
     if not a.full:
         ends = ends[:a.calls]

@@ -6,38 +6,24 @@ the random seed-42 population and for the generation-3 population bench.py's `ev
 
 torch.profiler with CUDA activities (CUPTI) records every kernel, memset and copy of the profiled sweeps; the table lists the
 mean device time per sweep of each, the share of the summed device time, and launches per sweep.  The card's name, power
-limit and SM clock (nvidia-smi, sampled right after the profiled sweeps) are printed beside it: the numbers mean nothing
+limit and SM clock (nvidia-smi, sampled during the profiled sweeps) are printed beside it: the numbers mean nothing
 without them.  `peak chunks` is PopulationSweep.last_peak_chunks (time chunks that set a new equity peak and took the
 record-by-record drawdown pass), compared with tools/peak_chunks_model.py's CPU count."""
 import argparse
 import json
 import re
-import subprocess
-import sys
 from collections import defaultdict
 from pathlib import Path
 
-sys.path.insert(0, str(Path(__file__).resolve().parents[1]))
 import numpy as np
 import torch
 from torch.profiler import ProfilerActivity, profile
 
-from ai_crypto_trader_b200 import synth
+import harness
 from ai_crypto_trader_b200.dist import ShardedFitness
-from ai_crypto_trader_b200.genetic_algorithm import GeneticAlgorithm
-from ai_crypto_trader_b200.sweep import MarketData, PopulationSweep, decode_population, evaluation_order
+from ai_crypto_trader_b200.sweep import PopulationSweep, decode_population, evaluation_order
 
 POP, S, N = 1024, 10, 1_000_000
-
-
-def card():
-    q = "name,power.limit,clocks.sm,clocks.max.sm"
-    try:
-        out = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader", "-i", str(torch.cuda.current_device())],
-                             capture_output=True, text=True, timeout=30).stdout.strip()
-        return dict(zip(q.split(","), (x.strip() for x in out.split(","))))
-    except Exception as e:              # (the table is still worth printing)
-        return {"name": torch.cuda.get_device_name(), "nvidia-smi": f"unavailable: {e}"}
 
 
 def short(name: str) -> str:
@@ -50,11 +36,10 @@ def profile_sweeps(sweep, indiv, order, plan, fit, sweeps, warmup):
     for _ in range(warmup):
         sweep.evaluate_device(indiv, order, POP, fit, plan=plan)
     torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+    with profile(activities=[ProfilerActivity.CUDA]) as prof, harness.sampled_clocks() as clocks:
         for _ in range(sweeps):
             sweep.evaluate_device(indiv, order, POP, fit, plan=plan)
         torch.cuda.synchronize()
-    clocks = card()
     total, count = defaultdict(float), defaultdict(int)
     for e in prof.events():
         if e.device_type == torch.autograd.DeviceType.CUDA:
@@ -62,13 +47,13 @@ def profile_sweeps(sweep, indiv, order, plan, fit, sweeps, warmup):
             total[k] += e.time_range.elapsed_us() / 1e3
             count[k] += 1
     rows = sorted(((k, total[k] / sweeps, count[k] / sweeps) for k in total), key=lambda r: -r[1])
-    return rows, clocks
+    return rows, {**harness.card(), "sm_clock": clocks.sm_clock}
 
 
 def report(tag, rows, clocks, extra):
     summed = sum(r[1] for r in rows)
-    print(f"\n== {tag}: {clocks.get('name')}, power limit {clocks.get('power.limit')}, SM clock {clocks.get('clocks.sm')} "
-          f"(max {clocks.get('clocks.max.sm')})")
+    print(f"\n== {tag}: {clocks['card']}, power limit {clocks['power_limit']}, SM clock {clocks['sm_clock']['sm_mhz']} MHz "
+          f"(max {clocks['sm_max_mhz']})")
     print("   " + ", ".join(f"{k} {v}" for k, v in extra.items()))
     print(f"   {'kernel':<44}{'ms/sweep':>10}{'share':>8}{'launches':>10}")
     for k, ms, n in rows:
@@ -84,9 +69,8 @@ def main():
     args = ap.parse_args()
     torch.cuda.set_device(0)
     dev = torch.device("cuda", 0)
-    market = MarketData(torch.from_numpy(synth.synth_ohlcv(S, N)).pin_memory())
+    market, population = harness.configs1(S, N, POP)
     sweep = PopulationSweep(market)
-    population = synth.random_population(POP, seed=42)
     fit = torch.empty(POP, dtype=torch.float64, device=dev)
     out = {}
 
@@ -100,17 +84,14 @@ def main():
         extra = {"path": type(plan[0]).__name__ if plan else "fused", "K": getattr(plan[0], "K", None) if plan else None,
                  "records": float(sweep.lane_stats()["n_records"].sum()), "chunks": segs,
                  "peak chunks": peak if peak is None else f"{peak} ({100 * peak / max(segs, 1):.2f} %)",
-                 "fallback lanes": sweep.last_invalid_lanes}
+                 "fallback lanes": sweep.last_invalid_lanes, "pool blocks planned": [p.pool_blocks for p in plan or []],
+                 "pool blocks used": [int(p.overflow[2]) for p in plan or []]}
         report(tag, rows, clocks, extra)
         out[tag] = {"kernels": [{"kernel": k, "ms_per_sweep": ms, "launches_per_sweep": n} for k, ms, n in rows],
                     "card": clocks, **extra}
 
     leg("random population (seed 42)", population, evaluation_order(population))
-    # bench.py's evolved_population_value: generation 3 of the reference GA started from the random population
-    ga = GeneticAlgorithm(synth.param_ranges(), ShardedFitness(sweep.evaluate, device=dev), population_size=POP,
-                          generations=3, random_seed=42)
-    ga.run(seeded_individuals=population)
-    leg("generation-3 population", ga.population, None)
+    leg("generation-3 population", harness.generation3(ShardedFitness(sweep.evaluate, device=dev), population), None)
     if args.json:
         Path(args.json).parent.mkdir(parents=True, exist_ok=True)
         Path(args.json).write_text(json.dumps(out, indent=1))

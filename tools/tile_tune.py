@@ -2,26 +2,18 @@
 """Sweep of the thread-per-lane knobs on the bench workload (pop 1024 x 10 symbols x 1M bars).
     python tools/tile_tune.py [K list] [warm list]"""
 import sys, itertools
-from pathlib import Path
-sys.path.insert(0, str(Path(__file__).resolve().parents[1]))
 import numpy as np, torch
-from ai_crypto_trader_b200 import synth
-from ai_crypto_trader_b200.sweep import MarketData, PopulationSweep, decode_population, evaluation_order
+import harness
+from ai_crypto_trader_b200.sweep import PopulationSweep, decode_population, evaluation_order
 
 S, N, POP = 10, 1_000_000, 1024
-m = MarketData(synth.synth_ohlcv(S, N)); sw = PopulationSweep(m, mode="fused")
-pop = synth.random_population(POP, seed=42)
+m, pop = harness.configs1(S, N, POP); sw = PopulationSweep(m, mode="fused")
+print(", ".join(harness.card().values()))
 indiv = torch.from_numpy(decode_population(pop, sw.period_row).view(np.uint8)).cuda()
 fit = torch.empty(POP, dtype=torch.float64, device="cuda")
 
 def timed(plan, order=None, reps=3):
-    for _ in range(2): sw.evaluate_device(indiv, order, POP, fit, plan=plan)
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps): sw.evaluate_device(indiv, order, POP, fit, plan=plan)
-    e1.record(); torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / reps
+    return float(np.mean(harness.event_ms(lambda: sw.evaluate_device(indiv, order, POP, fit, plan=plan), reps, warmup=2)))
 
 order = torch.from_numpy(evaluation_order(pop)).cuda()
 print("fused %.2f ms" % timed(None, order)); ref = fit.clone()

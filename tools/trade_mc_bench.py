@@ -15,48 +15,12 @@ counts (min / median / max / sum) and the registers / local memory of the new ke
 """
 import argparse
 import json
-import re
-import subprocess
-import sys
 import time
-from pathlib import Path
 
-ROOT = Path(__file__).resolve().parents[1]
-sys.path.insert(0, str(ROOT))
 import numpy as np
 import torch
 
-
-def _card():
-    out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i",
-                          str(torch.cuda.current_device())], capture_output=True, text=True, timeout=30).stdout
-    name, power = [x.strip() for x in out.strip().splitlines()[0].split(",")]
-    return name, power
-
-
-def _resources():
-    """Registers and local memory (spills) per thread of the new kernels, from the library's own SASS resource table."""
-    from ai_crypto_trader_b200 import _lib
-    import shutil
-    tool = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
-    try:
-        text = subprocess.run([tool, "-res-usage", str(_lib.LIB_PATH)], capture_output=True, text=True, timeout=120).stdout
-    except OSError:
-        return None
-    out, fn = {}, None
-    for line in text.splitlines():
-        m = re.search(r"Function (\S+):", line)
-        if m:
-            fn = m.group(1)
-            continue
-        if fn and ("trade_mc_kernel" in fn or "trade_pnl_kernel" in fn):
-            r = re.search(r"REG:(\d+)", line)
-            loc = re.search(r"LOCAL:(\d+)", line)
-            if r:
-                out["trade_mc_kernel" if "trade_mc_kernel" in fn else "trade_pnl_kernel"] = {
-                    "registers": int(r.group(1)), "local_bytes": int(loc.group(1)) if loc else None}
-                fn = None
-    return out
+import harness
 
 
 def main():
@@ -70,63 +34,44 @@ def main():
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("trade_mc_bench needs a CUDA device (H100); there is no CPU path")
-    from bench import ClockSampler
-    from ai_crypto_trader_b200 import synth
-    from ai_crypto_trader_b200.sweep import MarketData, PopulationSweep
+    from ai_crypto_trader_b200.sweep import PopulationSweep
     from ai_crypto_trader_b200.monte_carlo import risk_statistics
     from ai_crypto_trader_b200.trade_monte_carlo import TradeMonteCarlo
     torch.cuda.set_device(0)
-    market = MarketData(synth.synth_ohlcv(a.symbols, a.bars))
+    market, population = harness.configs1(a.symbols, a.bars, a.pop)
     sweep = PopulationSweep(market)
-    population = synth.random_population(a.pop, seed=42)
     fitness = sweep.evaluate(population)
     rank = np.argsort(-np.nan_to_num(fitness, nan=-np.inf, posinf=np.finfo(np.float64).max), kind="stable")
     top = [population[i] for i in rank[:a.top]]
 
     sweep.trade_pnl(top)                                   # warm-up (plans, buffers)
-    ext = []
-    for _ in range(3):
-        t0 = time.perf_counter()
-        trip, n_trips, fee = sweep.trade_pnl(top)
-        torch.cuda.synchronize()
-        ext.append((time.perf_counter() - t0) * 1e3)
+    ext, (trip, n_trips, fee) = harness.wall_ms(lambda: sweep.trade_pnl(top), 3)
     nt = n_trips.cpu().numpy().reshape(-1).astype(np.int32)
     fe = fee.cpu().numpy().reshape(-1)
     rows = trip.view(len(nt), -1)
     sum_t = int(nt.sum())
 
     mc = TradeMonteCarlo()
-    name, power = _card()
     legs = {}
     for method in ("bootstrap", "shuffle"):
         run = lambda: mc.simulate(rows, nt, fe, a.paths, method, 1, 10000.0, 2024)
-        run(); run(); torch.cuda.synchronize()
-        clocks = ClockSampler(torch.cuda.current_device())
-        clocks.start()
-        time.sleep(0.3)
-        w0 = time.time()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(a.reps):
-            finals, maxdd = run()
-        e1.record()
-        torch.cuda.synchronize()
-        w1 = time.time()
-        ms = e0.elapsed_time(e1) / a.reps
+        with harness.sampled_clocks() as clocks:
+            ms = float(np.mean(harness.event_ms(run, a.reps, warmup=2)))
+        finals, maxdd = run()
         t0 = time.perf_counter()
         p5 = [risk_statistics(mc.engine, finals[r], maxdd[r], 10000.0, 0.95, mdd_percentiles=(95,))["percentile_values"][1]
               for r in range(len(nt))]
         stats_ms = (time.perf_counter() - t0) * 1e3
         legs[method] = {"kernel_ms": ms, "round_trip_steps_per_s": a.paths * sum_t / (ms * 1e-3),
                         "statistics_ms_all_lanes": stats_ms, "statistics_ms_per_lane": stats_ms / len(nt),
-                        "sm_clock": clocks.stop(w0, w1), "p5_final_equity_median": float(np.median(p5))}
+                        "sm_clock": clocks.sm_clock, "p5_final_equity_median": float(np.median(p5))}
     print(json.dumps({
         "workload": f"trade Monte-Carlo: top {a.top} of configs[1] population {a.pop} by fitness x {a.symbols} symbols x "
                     f"{a.bars} bars, {a.paths} paths per lane",
-        "card": name, "power_limit": power, "lanes": int(len(nt)),
+        **harness.card(), "lanes": int(len(nt)),
         "trips": {"min": int(nt.min()), "median": float(np.median(nt)), "max": int(nt.max()), "sum": sum_t},
         "extraction_ms": {"median": float(np.median(ext)), "runs": ext},
-        "methods": legs, "kernels": _resources(),
+        "methods": legs, "kernels": harness.kernel_resources(["trade_mc_kernel", "trade_pnl_kernel"]),
     }))
 
 

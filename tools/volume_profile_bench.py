@@ -13,17 +13,16 @@ name, power limit and the SM clock sampled while timing.  Needs an H100; no fall
 """
 import argparse
 import json
-import sys
-import time
-from pathlib import Path
 
-ROOT = Path(__file__).resolve().parents[1]
-sys.path.insert(0, str(ROOT))
-sys.path.insert(0, str(ROOT / "tools"))
-
+import numpy as np
 import torch
 
-from overfitting_bench import _time
+import harness
+
+
+def _time(fn, reps):
+    ms = harness.event_ms(fn, reps)
+    return {"ms_median": float(np.median(ms)), "ms_runs": ms}
 
 
 def main():
@@ -35,34 +34,26 @@ def main():
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("volume_profile_bench needs a CUDA device (H100); there is no CPU path")
-    from bench import ClockSampler
-    from book_bench import _card
-    from ai_crypto_trader_b200 import synth
     from ai_crypto_trader_b200 import volume_profile as vp
-    from ai_crypto_trader_b200.sweep import MarketData, PopulationSweep
+    from ai_crypto_trader_b200.sweep import PopulationSweep
     torch.cuda.set_device(0)
-    market = MarketData(synth.synth_ohlcv(a.symbols, a.bars))
-    name, power = _card()
+    market, population = harness.configs1(a.symbols, a.bars, a.pop)
     out = {"workload": f"configs[1]: {a.symbols} symbols x {a.bars} 1-minute bars, 100-bar frames, 20 bins",
-           "card": name, "power_limit": power}
-    clocks = ClockSampler(torch.cuda.current_device())
-    clocks.start()
-    time.sleep(0.3)
-    w0 = time.time()
-    for tf in (5, 1):
-        frames = a.symbols * (a.bars // tf)
-        for rows in (True, False):
-            key = f"history_{tf}m_{'rows' if rows else 'labels_only'}"
-            t = _time(lambda: vp.volume_profile_history(market, tf, rows=rows), a.reps)
-            out[key] = dict(t, frames=frames, frames_per_s=frames / (t["ms_median"] * 1e-3))
-    out["labels_base_clock"] = _time(lambda: vp.volume_profile_labels(market), a.reps)
-    labels = vp.volume_profile_labels(market)
-    sweep = PopulationSweep(market)
-    population = synth.random_population(a.pop, seed=42)
-    out["class_stats_6_zones"] = _time(lambda: sweep.class_stats(population, labels, 6), a.reps)
-    _, views = sweep.class_stats(population, labels, 6)
-    out["records_per_zone"] = [float(v["n_records"].sum()) for v in views]
-    out["sm_clock"] = clocks.stop(w0, time.time())
+           **harness.card()}
+    with harness.sampled_clocks() as clocks:
+        for tf in (5, 1):
+            frames = a.symbols * (a.bars // tf)
+            for rows in (True, False):
+                key = f"history_{tf}m_{'rows' if rows else 'labels_only'}"
+                t = _time(lambda: vp.volume_profile_history(market, tf, rows=rows), a.reps)
+                out[key] = dict(t, frames=frames, frames_per_s=frames / (t["ms_median"] * 1e-3))
+        out["labels_base_clock"] = _time(lambda: vp.volume_profile_labels(market), a.reps)
+        labels = vp.volume_profile_labels(market)
+        sweep = PopulationSweep(market)
+        out["class_stats_6_zones"] = _time(lambda: sweep.class_stats(population, labels, 6), a.reps)
+        _, views = sweep.class_stats(population, labels, 6)
+        out["records_per_zone"] = [float(v["n_records"].sum()) for v in views]
+    out["sm_clock"] = clocks.sm_clock
     print(json.dumps(out))
 
 
