@@ -14,9 +14,11 @@
 //     independent by a warm-up halo that attenuates the unknown state below 2^-60;
 //   * window sums (SMA, Bollinger, VWAP, %D): fp64 prefix sums of tile-offset values in
 //     shared memory, window sum = difference of two prefixes;
-//   * window extrema (stochastic, Williams, Ichimoku): direct scan of the window in shared
-//     memory (exact: min/max do not round).
+//   * window extrema (stochastic, Williams, Ichimoku): one backward walk per bar over the staged
+//     highs / lows captures every window (exact: min/max do not round).
+// The single-indicator kernels and the fused TechnicalAnalyzer kernels call the same tile functions.
 #include <math.h>
+#include <algorithm>
 #include "common.cuh"
 
 namespace b200bt {
@@ -262,206 +264,198 @@ __device__ void block_prefix_sum(double* __restrict__ s, int n, double* __restri
 }
 
 // ---------------------------------------------------------------------------------
-// SMA bank (ta.trend.SMAIndicator = rolling(w, min_periods=w).mean(); :67-76).
+// Window sums.  The CTA stages row[s0, tile_end) as offsets d = x - c from the tile's first value c (small prefixes: Σd²
+// without cancellation) and forms the inclusive fp64 prefixes p1[i + 1] = Σ_{k<=i} d_k, p1[0] = 0, and the same of d² into
+// p2 when it is given; a window sum is the difference of two prefixes.  Σd² is not exact in fp64, so the staged span
+// decides the last bits of Bollinger's deviation: each caller keeps its own s0.  Returns c.
 // ---------------------------------------------------------------------------------
+__device__ __forceinline__ double stage_prefixes(const float* __restrict__ row, int64_t s0, int64_t tile_start, int64_t tile_end,
+                                                 double* __restrict__ p1, double* __restrict__ p2, double* __restrict__ s_warp) {
+    const double c = (double)__ldg(row + tile_start);
+    const int n = (int)(tile_end - s0);
+    if (threadIdx.x == 0) {
+        p1[0] = 0.0;
+        if (p2) p2[0] = 0.0;
+    }
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        const double d = (double)__ldg(row + s0 + i) - c;
+        p1[i + 1] = d;
+        if (p2) p2[i + 1] = d * d;
+    }
+    __syncthreads();
+    block_prefix_sum(p1 + 1, n, s_warp);
+    if (p2) block_prefix_sum(p2 + 1, n, s_warp);
+    return c;
+}
+
+// SMA (ta.trend.SMAIndicator = rolling(w, min_periods=w).mean(); :67-76) at bar t, staged index i
+__device__ __forceinline__ float sma_at(const double* __restrict__ p1, int i, int64_t t, int w, double c) {
+    return t >= w - 1 ? (float)((p1[i + 1] - p1[i + 1 - w]) / (double)w + c) : nanf32();
+}
+
+// Bollinger bands (ta.volatility.BollingerBands(close, 20, 2); :148-156) at bar t, staged index i, output offset o:
+// mid = rolling mean, std = rolling std(ddof=0), high/low = mid +- k*std,
+// width = (high-low)/mid, position = (close-low)/(high-low) with NaN where the range is 0.
+__device__ __forceinline__ void bollinger_at(const double* __restrict__ p1, const double* __restrict__ p2, int i, int64_t t, int w,
+                                             double c, double kdev, const float* __restrict__ row, int64_t o,
+                                             float* __restrict__ o_high, float* __restrict__ o_mid, float* __restrict__ o_low,
+                                             float* __restrict__ o_width, float* __restrict__ o_pos) {
+    if (t < w - 1) {
+        o_high[o] = o_mid[o] = o_low[o] = o_width[o] = o_pos[o] = nanf32();
+        return;
+    }
+    const double close = (double)__ldg(row + t);
+    double mid = close, sd = 0.0;     // one bar is its own mean and has no deviation (the prefix differences leave a residue)
+    if (w > 1) {
+        const double m1 = (p1[i + 1] - p1[i + 1 - w]) / (double)w;   // mean of d
+        const double m2 = (p2[i + 1] - p2[i + 1 - w]) / (double)w;   // mean of d^2
+        double var = m2 - m1 * m1;
+        if (var < 0.0) var = 0.0;
+        sd = sqrt(var);
+        mid = m1 + c;
+    }
+    const double hi = mid + kdev * sd, lo = mid - kdev * sd;
+    const double rng = hi - lo;
+    o_high[o] = (float)hi;
+    o_mid[o] = (float)mid;
+    o_low[o] = (float)lo;
+    o_width[o] = (float)(rng / mid);
+    o_pos[o] = rng == 0.0 ? nanf32() : (float)((close - lo) / rng);
+}
+
+// SMA bank: the staged span follows the longest window (halo_max = its w - 1)
 __global__ void __launch_bounds__(IND_THREADS)
 sma_bank_kernel(const float* __restrict__ x, int64_t N, int64_t ld, const __grid_constant__ BankParams prm, int P,
                 int halo_max, float* __restrict__ out) {
-    extern __shared__ double s_pre[];  // s_pre[i+1] = sum_{k<=i} (x[s0+k] - c), s_pre[0] = 0
+    extern __shared__ double s_pre[];  // prefix of d
     __shared__ double s_warp[32];
     const int sym = blockIdx.y;
     const int64_t tile_start = (int64_t)blockIdx.x * IND_TILE;
     const int64_t tile_end = min(tile_start + (int64_t)IND_TILE, N);
     const int64_t s0 = max((int64_t)0, tile_start - halo_max);
-    const int n_stage = (int)(tile_end - s0);
-    const float* row = x + (int64_t)sym * ld;
-    const double c = (double)__ldg(row + tile_start);  // tile offset keeps the prefix small
-    if (threadIdx.x == 0) s_pre[0] = 0.0;
-    for (int i = threadIdx.x; i < n_stage; i += blockDim.x) s_pre[i + 1] = (double)__ldg(row + s0 + i) - c;
-    __syncthreads();
-    block_prefix_sum(s_pre + 1, n_stage, s_warp);
+    const double c = stage_prefixes(x + (int64_t)sym * ld, s0, tile_start, tile_end, s_pre, nullptr, s_warp);
     for (int pi = 0; pi < P; ++pi) {
         const int w = prm.window[pi];
         float* orow = out + ((int64_t)sym * P + pi) * N;
-        for (int64_t t = tile_start + threadIdx.x; t < tile_end; t += blockDim.x) {
-            float v = nanf32();
-            if (t >= w - 1) {
-                const int i = (int)(t - s0);
-                v = (float)((s_pre[i + 1] - s_pre[i + 1 - w]) / (double)w + c);
-            }
-            orow[t] = v;
-        }
+        for (int64_t t = tile_start + threadIdx.x; t < tile_end; t += blockDim.x) orow[t] = sma_at(s_pre, (int)(t - s0), t, w, c);
     }
 }
 
-// ---------------------------------------------------------------------------------
-// Bollinger bands (ta.volatility.BollingerBands(close, 20, 2); :148-156):
-// mid = rolling mean, std = rolling std(ddof=0), high/low = mid +- k*std,
-// width = (high-low)/mid, position = (close-low)/(high-low) with NaN where the range is 0.
-// ---------------------------------------------------------------------------------
+// Bollinger bands: the staged span is the window's own w - 1 bars before the tile
 __global__ void __launch_bounds__(IND_THREADS)
 bollinger_kernel(const float* __restrict__ x, int64_t N, int64_t ld, int w, double kdev, float* __restrict__ o_high,
                  float* __restrict__ o_mid, float* __restrict__ o_low, float* __restrict__ o_width,
                  float* __restrict__ o_pos) {
-    extern __shared__ double s_buf[];  // [0, n+1): prefix of d, [n+1, 2n+2): prefix of d^2
+    extern __shared__ double s_buf[];  // prefix of d, then prefix of d^2 (IND_TILE + IND_MAX_WINDOW + 1 each)
     __shared__ double s_warp[32];
     const int sym = blockIdx.y;
     const int64_t tile_start = (int64_t)blockIdx.x * IND_TILE;
     const int64_t tile_end = min(tile_start + (int64_t)IND_TILE, N);
     const int64_t s0 = max((int64_t)0, tile_start - (w - 1));
-    const int n = (int)(tile_end - s0);
     double* p1 = s_buf;
     double* p2 = s_buf + (IND_TILE + IND_MAX_WINDOW + 1);
     const float* row = x + (int64_t)sym * ld;
-    const double c = (double)__ldg(row + tile_start);
-    if (threadIdx.x == 0) { p1[0] = 0.0; p2[0] = 0.0; }
-    for (int i = threadIdx.x; i < n; i += blockDim.x) {
-        const double d = (double)__ldg(row + s0 + i) - c;
-        p1[i + 1] = d;
-        p2[i + 1] = d * d;
-    }
-    __syncthreads();
-    block_prefix_sum(p1 + 1, n, s_warp);
-    block_prefix_sum(p2 + 1, n, s_warp);
-    for (int64_t t = tile_start + threadIdx.x; t < tile_end; t += blockDim.x) {
-        const int64_t o = (int64_t)sym * N + t;
-        if (t < w - 1) {
-            o_high[o] = o_mid[o] = o_low[o] = o_width[o] = o_pos[o] = nanf32();
-            continue;
-        }
-        const int i = (int)(t - s0);
-        const double close = (double)__ldg(row + t);
-        double mid = close, sd = 0.0;     // one bar is its own mean and has no deviation (the prefix differences leave a residue)
-        if (w > 1) {
-            const double m1 = (p1[i + 1] - p1[i + 1 - w]) / (double)w;   // mean of d
-            const double m2 = (p2[i + 1] - p2[i + 1 - w]) / (double)w;   // mean of d^2
-            double var = m2 - m1 * m1;
-            if (var < 0.0) var = 0.0;
-            sd = sqrt(var);
-            mid = m1 + c;
-        }
-        const double hi = mid + kdev * sd, lo = mid - kdev * sd;
-        const double rng = hi - lo;
-        o_high[o] = (float)hi;
-        o_mid[o] = (float)mid;
-        o_low[o] = (float)lo;
-        o_width[o] = (float)(rng / mid);
-        o_pos[o] = rng == 0.0 ? nanf32() : (float)((close - lo) / rng);
-    }
+    const double c = stage_prefixes(row, s0, tile_start, tile_end, p1, p2, s_warp);
+    for (int64_t t = tile_start + threadIdx.x; t < tile_end; t += blockDim.x)
+        bollinger_at(p1, p2, (int)(t - s0), t, w, c, kdev, row, (int64_t)sym * N + t, o_high, o_mid, o_low, o_width, o_pos);
 }
 
 // ---------------------------------------------------------------------------------
-// Rolling extrema helpers + stochastic / Williams %R / Ichimoku.
+// Window extrema: stochastic %K / %D (:121-127), Williams %R (:135-140), Ichimoku a / b (conversion, base, span b;
+// :102-104).  ONE backward walk per staged bar extends a running (max high, min low) over the bar's last k bars and
+// captures it at each window in ascending order, so a bar costs its longest window once, whatever the number of
+// outputs.  Exact: min and max do not round.  %D averages the float64 %K of the bar and the smooth - 1 bars before it
+// (the reference averages float64 %K), kept in shared memory.
 // ---------------------------------------------------------------------------------
-__device__ __forceinline__ float window_max(const float* __restrict__ s, int i, int w) {
-    float m = s[i];
-    for (int k = 1; k < w; ++k) m = fmaxf(m, s[i - k]);
-    return m;
-}
-__device__ __forceinline__ float window_min(const float* __restrict__ s, int i, int w) {
-    float m = s[i];
-    for (int k = 1; k < w; ++k) m = fminf(m, s[i - k]);
-    return m;
-}
+struct ExtremaArgs {
+    int w_st, smooth;                        // %K / Williams window, %D smoothing
+    int w_conv, w_base, w_span;              // Ichimoku windows
+    int walk[4];                             // w_st, w_conv, w_base, w_span in ascending order: where the walk captures
+    int halo;                                // bars staged before the tile
+    float *o_k, *o_d, *o_wr, *o_ia, *o_ib;   // [S][N] outputs, null if not wanted (a call sets the windows it does not use to 1)
+};
 
-// mode 0: stochastic (%K into o_a, %D = rolling mean(smooth) of %K into o_b)   :121-127
-// mode 1: Williams %R into o_a                                                 :135-140
-// mode 2: Ichimoku a, b (w1 conversion, w2 base, w3 span b)                    :102-104
-// (whole CTA; s_hl: 3 (IND_TILE + 2 IND_MAX_WINDOW) floats of shared memory -- highs, lows, %K scratch; ends with every
-// thread past its last shared-memory access only after the caller's next barrier)
+// (whole CTA; s_raw: `cap` >= IND_TILE + halo floats each of highs, lows and closes, then `cap` doubles of %K when o_d is
+// given, `cap` even; ends with threads still reading shared memory: a caller that reuses it syncs first)
 __device__ __forceinline__ void extrema_tile(const float* __restrict__ high, const float* __restrict__ low, const float* __restrict__ close,
-                                             int64_t N, int64_t ld, int mode, int w1, int w2, int w3, float* __restrict__ o_a,
-                                             float* __restrict__ o_b, float* __restrict__ s_hl, int sym, int64_t tile_start) {
+                                             int64_t N, int64_t ld, const ExtremaArgs& a, int cap, unsigned char* __restrict__ s_raw,
+                                             int sym, int64_t tile_start) {
     const int64_t tile_end = min(tile_start + (int64_t)IND_TILE, N);
-    const int wmax = max(w1, max(w2, w3));
-    const int extra = (mode == 0) ? (w2 - 1) : 0;  // %D needs %K of the previous smooth-1 bars
-    const int64_t s0 = max((int64_t)0, tile_start - (wmax - 1) - extra);
+    const int64_t s0 = max((int64_t)0, tile_start - a.halo);
     const int n = (int)(tile_end - s0);
-    float* sh = s_hl;
-    float* sl = s_hl + (IND_TILE + 2 * IND_MAX_WINDOW);
-    float* sk = sl + (IND_TILE + 2 * IND_MAX_WINDOW);
-    stage_row(high + (int64_t)sym * ld, N, s0, n, sh);
-    stage_row(low + (int64_t)sym * ld, N, s0, n, sl);
+    const int64_t ro = (int64_t)sym * ld;
+    float* sh = reinterpret_cast<float*>(s_raw);
+    float* sl = sh + cap;
+    float* sc = sl + cap;
+    double* skd = reinterpret_cast<double*>(sc + cap);
+    stage_row(high + ro, N, s0, n, sh);
+    stage_row(low + ro, N, s0, n, sl);
+    if (close) stage_row(close + ro, N, s0, n, sc);
     __syncthreads();
-    const float* crow = close ? close + (int64_t)sym * ld : nullptr;
-    if (mode == 0) {
-        for (int i = threadIdx.x; i < n; i += blockDim.x) {
-            const int64_t t = s0 + i;
-            float k = nanf32();
-            if (i >= w1 - 1) {  // (s0 == 0: same as t >= w1-1; s0 > 0: the window must lie inside the staged halo)
-                const double lo = (double)window_min(sl, i, w1), hi = (double)window_max(sh, i, w1);
-                k = (float)(100.0 * ((double)__ldg(crow + t) - lo) / (hi - lo));   // 0/0 -> NaN as in pandas
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        const int64_t t = s0 + i;
+        float mh = sh[i], ml = sl[i], hs, ls, hc, lc, hb, lb, hp, lp;
+        int k = 1;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int w = a.walk[j];
+            for (const int lim = min(w, i + 1); k < lim; ++k) {      // (i + 1: the staged bars at or before this one)
+                mh = fmaxf(mh, sh[i - k]);
+                ml = fminf(ml, sl[i - k]);
             }
-            sk[i] = k;
+            if (w == a.w_st) { hs = mh; ls = ml; }
+            if (w == a.w_conv) { hc = mh; lc = ml; }
+            if (w == a.w_base) { hb = mh; lb = ml; }
+            if (w == a.w_span) { hp = mh; lp = ml; }
         }
+        const double c = close ? (double)sc[i] : 0.0;
+        // (s0 == 0: "i >= w - 1" is "t >= w - 1"; s0 > 0: every window lies inside the staged halo)
+        double kk = (double)nanf32();
+        if ((a.o_k || a.o_d) && i >= a.w_st - 1) kk = 100.0 * (c - (double)ls) / ((double)hs - (double)ls);   // 0/0 -> NaN as in pandas
+        if (a.o_d) skd[i] = kk;
+        if (t >= tile_start) {
+            const int64_t o = (int64_t)sym * N + t;
+            if (a.o_k) a.o_k[o] = (t >= a.w_st - 1) ? (float)kk : nanf32();
+            if (a.o_wr) a.o_wr[o] = (t >= a.w_st - 1) ? (float)(-100.0 * ((double)hs - c) / ((double)hs - (double)ls)) : nanf32();
+            if (a.o_ia)
+                a.o_ia[o] = (t >= max(a.w_conv, a.w_base) - 1)
+                    ? (float)(0.5 * (0.5 * ((double)hc + (double)lc) + 0.5 * ((double)hb + (double)lb))) : nanf32();
+            if (a.o_ib) a.o_ib[o] = (t >= a.w_span - 1) ? (float)(0.5 * ((double)hp + (double)lp)) : nanf32();
+        }
+    }
+    if (a.o_d) {
         __syncthreads();
         for (int64_t t = tile_start + threadIdx.x; t < tile_end; t += blockDim.x) {
             const int i = (int)(t - s0);
-            const int64_t o = (int64_t)sym * N + t;
-            o_a[o] = sk[i];
             float d = nanf32();
-            if (t >= w1 - 1 + w2 - 1) {
-                // %D over the float64 %K values (recomputed: the reference averages float64 %K)
+            if (t >= a.w_st - 1 + a.smooth - 1) {
                 double acc = 0.0;
-                for (int k = 0; k < w2; ++k) {
-                    const int ii = i - k;
-                    const double lo = (double)window_min(sl, ii, w1), hi = (double)window_max(sh, ii, w1);
-                    acc += 100.0 * ((double)__ldg(crow + s0 + ii) - lo) / (hi - lo);
-                }
-                d = (float)(acc / (double)w2);
+                for (int q = 0; q < a.smooth; ++q) acc += skd[i - q];
+                d = (float)(acc / (double)a.smooth);
             }
-            o_b[o] = d;
-        }
-    } else if (mode == 1) {
-        for (int64_t t = tile_start + threadIdx.x; t < tile_end; t += blockDim.x) {
-            const int i = (int)(t - s0);
-            float v = nanf32();
-            if (t >= w1 - 1) {
-                const double hi = (double)window_max(sh, i, w1), lo = (double)window_min(sl, i, w1);
-                v = (float)(-100.0 * (hi - (double)__ldg(crow + t)) / (hi - lo));
-            }
-            o_a[(int64_t)sym * N + t] = v;
-        }
-    } else {
-        for (int64_t t = tile_start + threadIdx.x; t < tile_end; t += blockDim.x) {
-            const int i = (int)(t - s0);
-            const int64_t o = (int64_t)sym * N + t;
-            float a = nanf32(), b = nanf32();
-            if (t >= max(w1, w2) - 1) {
-                const double conv = 0.5 * ((double)window_max(sh, i, w1) + (double)window_min(sl, i, w1));
-                const double base = 0.5 * ((double)window_max(sh, i, w2) + (double)window_min(sl, i, w2));
-                a = (float)(0.5 * (conv + base));
-            }
-            if (t >= w3 - 1) b = (float)(0.5 * ((double)window_max(sh, i, w3) + (double)window_min(sl, i, w3)));
-            o_a[o] = a;
-            o_b[o] = b;
+            a.o_d[(int64_t)sym * N + t] = d;
         }
     }
 }
 
 __global__ void __launch_bounds__(IND_THREADS)
 extrema_kernel(const float* __restrict__ high, const float* __restrict__ low, const float* __restrict__ close,
-               int64_t N, int64_t ld, int mode, int w1, int w2, int w3, float* __restrict__ o_a, float* __restrict__ o_b) {
-    extern __shared__ float s_hl[];  // [halo + tile] highs, then lows, then %K scratch
-    extrema_tile(high, low, close, N, ld, mode, w1, w2, w3, o_a, o_b, s_hl, blockIdx.y, (int64_t)blockIdx.x * IND_TILE);
+               int64_t N, int64_t ld, const __grid_constant__ ExtremaArgs a, int cap) {
+    extern __shared__ __align__(16) unsigned char s_raw[];
+    extrema_tile(high, low, close, N, ld, a, cap, s_raw, blockIdx.y, (int64_t)blockIdx.x * IND_TILE);
 }
 
 // ---------------------------------------------------------------------------------
-// ATR bank (ta.volatility.AverageTrueRange; :164): TR_t = max(h-l, |h-c_{t-1}|, |l-c_{t-1}|),
+// ATR (ta.volatility.AverageTrueRange; :164): TR_t = max(h-l, |h-c_{t-1}|, |l-c_{t-1}|),
 // TR_0 = h_0-l_0; atr[t<w-1] = 0, atr[w-1] = mean(TR[0:w]), atr[i] = (atr[i-1](w-1)+TR[i])/w.
 // ---------------------------------------------------------------------------------
-// (whole CTA; `tr`: (halo_max + IND_TILE + IND_MAX_WINDOW + 8) doubles of shared memory; window i of `prm` goes to warp i % nwarp
-// and is written to out + ((sym * P + i) * N))
-__device__ __forceinline__ void atr_tile(const float* __restrict__ high, const float* __restrict__ low, const float* __restrict__ close,
-                                         int64_t N, int64_t ld, const BankParams& prm, int P, int halo_max,
-                                         float* __restrict__ out, double* __restrict__ tr, int sym, int64_t tile_start) {
-    const int64_t tile_end = min(tile_start + (int64_t)IND_TILE, N);
-    int64_t s0 = max((int64_t)0, tile_start - halo_max) & ~(int64_t)3;
+// (whole CTA) TR over [s0, tile_start + IND_TILE) into `tr` as float64, 0 past the row's end: (halo + IND_TILE + IND_MAX_WINDOW
+// + 8) doubles of shared memory.  s0 is `halo` bars before the tile, down to a multiple of 4.  Returns s0.
+__device__ __forceinline__ int64_t stage_true_range(const float* __restrict__ hr, const float* __restrict__ lr, const float* __restrict__ cr,
+                                                    int64_t N, int64_t tile_start, int halo, double* __restrict__ tr) {
+    int64_t s0 = max((int64_t)0, tile_start - halo) & ~(int64_t)3;
     if (s0 < IND_MAX_WINDOW) s0 = 0;  // a pass that crosses a seed bar t = w-1 needs TR from bar 0
     const int n_stage = (int)(tile_start + IND_TILE - s0);
-    const float* hr = high + (int64_t)sym * ld;
-    const float* lr = low + (int64_t)sym * ld;
-    const float* cr = close + (int64_t)sym * ld;
     for (int i = threadIdx.x; i < n_stage; i += blockDim.x) {
         const int64_t t = s0 + i;
         double v = 0.0;
@@ -476,38 +470,42 @@ __device__ __forceinline__ void atr_tile(const float* __restrict__ high, const f
         tr[i] = v;
     }
     __syncthreads();
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarp = blockDim.x >> 5;
+    return s0;
+}
+
+// (one warp) ATR of window w over bars [range_start, range_end) into orow, from the true range staged over [s0, s0 + n_stage).
+// The scan starts `halo` bars before range_start, or at bar 0 when it crosses the seed bar: its start decides the rounding,
+// so each caller keeps its own ranges.
+__device__ __forceinline__ void atr_scan(const double* __restrict__ tr, int64_t s0, int n_stage, int64_t N, int w, int halo,
+                                         int64_t range_start, int64_t range_end, float* __restrict__ orow) {
+    const int lane = threadIdx.x & 31;
     constexpr int K = 4;
-    for (int pi = warp; pi < P; pi += nwarp) {
-        const int w = prm.window[pi];
-        float* orow = out + ((int64_t)sym * P + pi) * N;
-        const double alpha = 1.0 / (double)w, om = ((double)w - 1.0) / (double)w;
-        AffineScan<K> sc;
-        sc.init(om, lane);
-        int64_t start = max(s0, tile_start - prm.halo[pi]) & ~(int64_t)3;
-        const bool has_seed = (start <= w - 1);     // this pass crosses the seed bar t = w-1
-        double seed = 0.0;
-        if (has_seed && w - 1 < N) {
-            for (int k = 0; k < w; ++k) seed += tr[(int)(k - s0)];   // s0 == 0 whenever has_seed
-            seed /= (double)w;
-        }
-        if (has_seed) start = 0;
-        double carry = 0.0;
-        for (int64_t base = start; base < tile_end; base += 32 * K) {
-            const int64_t t = base + lane * K;
-            double b[K], y[K];
+    const double alpha = 1.0 / (double)w, om = ((double)w - 1.0) / (double)w;
+    AffineScan<K> sc;
+    sc.init(om, lane);
+    int64_t start = max(s0, range_start - halo) & ~(int64_t)3;
+    const bool has_seed = (start <= w - 1);     // this pass crosses the seed bar t = w-1
+    double seed = 0.0;
+    if (has_seed && w - 1 < N) {
+        for (int k = 0; k < w; ++k) seed += tr[(int)(k - s0)];   // s0 == 0 whenever has_seed
+        seed /= (double)w;
+    }
+    if (has_seed) start = 0;
+    double carry = 0.0;
+    for (int64_t base = start; base < range_end; base += 32 * K) {
+        const int64_t t = base + lane * K;
+        double b[K], y[K];
 #pragma unroll
-            for (int j = 0; j < K; ++j) {
-                const int64_t tt = t + j;
-                double v = alpha * tr[min((int)(tt - s0), n_stage - 1)];
-                if (has_seed) v = tt < w - 1 ? 0.0 : (tt == w - 1 ? seed : v);   // zeros, then the seed, then the recurrence
-                b[j] = v;
-            }
-            sc.run(b, carry, y, lane);
-#pragma unroll
-            for (int j = 0; j < K; ++j)
-                if (t + j >= tile_start && t + j < tile_end) orow[t + j] = (t + j >= w - 1) ? (float)y[j] : 0.0f;
+        for (int j = 0; j < K; ++j) {
+            const int64_t tt = t + j;
+            double v = alpha * tr[min((int)(tt - s0), n_stage - 1)];
+            if (has_seed) v = tt < w - 1 ? 0.0 : (tt == w - 1 ? seed : v);   // zeros, then the seed, then the recurrence
+            b[j] = v;
         }
+        sc.run(b, carry, y, lane);
+#pragma unroll
+        for (int j = 0; j < K; ++j)
+            if (t + j >= range_start && t + j < range_end) orow[t + j] = (t + j >= w - 1) ? (float)y[j] : 0.0f;
     }
 }
 
@@ -515,8 +513,14 @@ __global__ void __launch_bounds__(IND_THREADS)
 atr_bank_kernel(const float* __restrict__ high, const float* __restrict__ low, const float* __restrict__ close,
                 int64_t N, int64_t ld, const __grid_constant__ BankParams prm, int P, int halo_max,
                 float* __restrict__ out) {
-    extern __shared__ float s_tr[];  // true range over [s0, tile_end), float64
-    atr_tile(high, low, close, N, ld, prm, P, halo_max, out, reinterpret_cast<double*>(s_tr), blockIdx.y, (int64_t)blockIdx.x * IND_TILE);
+    extern __shared__ double s_tr[];  // true range over [s0, tile_start + IND_TILE)
+    const int sym = blockIdx.y;
+    const int64_t tile_start = (int64_t)blockIdx.x * IND_TILE, tile_end = min(tile_start + (int64_t)IND_TILE, N);
+    const int64_t ro = (int64_t)sym * ld;
+    const int64_t s0 = stage_true_range(high + ro, low + ro, close + ro, N, tile_start, halo_max, s_tr);
+    const int n_stage = (int)(tile_start + IND_TILE - s0);
+    for (int pi = threadIdx.x >> 5; pi < P; pi += blockDim.x >> 5)
+        atr_scan(s_tr, s0, n_stage, N, prm.window[pi], prm.halo[pi], tile_start, tile_end, out + ((int64_t)sym * P + pi) * N);
 }
 
 // ---------------------------------------------------------------------------------
@@ -728,50 +732,23 @@ analyzer_b_kernel(const float* __restrict__ x, int64_t N, int64_t ld, int w0, in
                   float* __restrict__ o_s0, float* __restrict__ o_s1, float* __restrict__ o_s2, float* __restrict__ o_high,
                   float* __restrict__ o_mid, float* __restrict__ o_low, float* __restrict__ o_width, float* __restrict__ o_pos,
                   int halo, const LeadFill lf) {
-    extern __shared__ double s_buf[];   // prefix of d = x - c, then prefix of d^2 (IND_TILE + IND_MAX_WINDOW + 1 each)
+    extern __shared__ double s_buf[];   // prefix of d, then prefix of d^2 (IND_TILE + IND_MAX_WINDOW + 1 each)
     __shared__ double s_warp[32];
     const int sym = blockIdx.y;
     const int64_t tile_start = (int64_t)blockIdx.x * IND_TILE, tile_end = min(tile_start + (int64_t)IND_TILE, N);
-    const int64_t s0 = max((int64_t)0, tile_start - halo);
-    const int n = (int)(tile_end - s0);
+    const int64_t s0 = max((int64_t)0, tile_start - halo);    // the longest SMA's span serves Bollinger too
     double* p1 = s_buf;
     double* p2 = s_buf + (IND_TILE + IND_MAX_WINDOW + 1);
     const float* row = x + (int64_t)sym * ld;
-    const double c = (double)__ldg(row + tile_start);   // tile offset keeps the prefixes small (sum of squares without cancellation)
-    if (threadIdx.x == 0) { p1[0] = 0.0; p2[0] = 0.0; }
-    for (int i = threadIdx.x; i < n; i += blockDim.x) {
-        const double d = (double)__ldg(row + s0 + i) - c;
-        p1[i + 1] = d;
-        p2[i + 1] = d * d;
-    }
-    __syncthreads();
-    block_prefix_sum(p1 + 1, n, s_warp);
-    block_prefix_sum(p2 + 1, n, s_warp);
+    const double c = stage_prefixes(row, s0, tile_start, tile_end, p1, p2, s_warp);
     const int ws[3] = {w0, w1, w2};
     float* const os[3] = {o_s0, o_s1, o_s2};
     for (int64_t t = tile_start + threadIdx.x; t < tile_end; t += blockDim.x) {
         const int i = (int)(t - s0);
         const int64_t o = (int64_t)sym * N + t;
 #pragma unroll
-        for (int k = 0; k < 3; ++k)      // ta.trend.SMAIndicator (:67-76)
-            os[k][o] = (t >= ws[k] - 1) ? (float)((p1[i + 1] - p1[i + 1 - ws[k]]) / (double)ws[k] + c) : nanf32();
-        if (t < w_bb - 1) {              // ta.volatility.BollingerBands (:148-156)
-            o_high[o] = o_mid[o] = o_low[o] = o_width[o] = o_pos[o] = nanf32();
-            continue;
-        }
-        const double m1 = (p1[i + 1] - p1[i + 1 - w_bb]) / (double)w_bb;
-        const double m2 = (p2[i + 1] - p2[i + 1 - w_bb]) / (double)w_bb;
-        double var = m2 - m1 * m1;
-        if (var < 0.0) var = 0.0;
-        const double sd = sqrt(var), mid = m1 + c;
-        const double hi = mid + kdev * sd, lo = mid - kdev * sd;
-        const double rng = hi - lo;
-        const double close = (double)__ldg(row + t);
-        o_high[o] = (float)hi;
-        o_mid[o] = (float)mid;
-        o_low[o] = (float)lo;
-        o_width[o] = (float)(rng / mid);
-        o_pos[o] = rng == 0.0 ? nanf32() : (float)((close - lo) / rng);
+        for (int k = 0; k < 3; ++k) os[k][o] = sma_at(p1, i, t, ws[k], c);
+        bollinger_at(p1, p2, i, t, w_bb, c, kdev, row, o, o_high, o_mid, o_low, o_width, o_pos);
     }
     if (tile_start == 0) {
         __syncthreads();
@@ -779,131 +756,28 @@ analyzer_b_kernel(const float* __restrict__ x, int64_t N, int64_t ld, int w0, in
     }
 }
 
-// C: one backward walk of the staged highs / lows per bar serves every window (the reference's are nested: 9 <= 14 <= 26 <= 52),
-// %D averages the float64 %K values kept in shared memory, the ATR recurrence runs on all eight warps (a 256-bar sub-tile
-// each, its own warm-up halo) instead of one, VWAP on block-wide prefix sums.  Phases reuse the shared memory.
+// C: one backward walk of the staged highs / lows per bar serves every window, the ATR recurrence runs on all eight warps (a
+// 256-bar sub-tile each, its own warm-up halo) instead of one, VWAP on block-wide prefix sums.  Phases reuse the shared memory.
 __global__ void __launch_bounds__(IND_THREADS)
 analyzer_c_kernel(const float* __restrict__ high, const float* __restrict__ low, const float* __restrict__ close,
-                  const float* __restrict__ volume, int64_t N, int64_t ld, int w_st, int smooth, int i1, int i2, int i3,
-                  int w_atr, int atr_halo, int w_vwap, float* __restrict__ o_k, float* __restrict__ o_d,
-                  float* __restrict__ o_wr, float* __restrict__ o_ia, float* __restrict__ o_ib, float* __restrict__ o_atr,
-                  float* __restrict__ o_vwap, const LeadFill lf) {
+                  const float* __restrict__ volume, int64_t N, int64_t ld, const __grid_constant__ ExtremaArgs ext,
+                  int w_atr, int atr_halo, int w_vwap, float* __restrict__ o_atr, float* __restrict__ o_vwap, const LeadFill lf) {
     extern __shared__ __align__(16) unsigned char s_raw[];
     __shared__ double s_warp[32];
     const int sym = blockIdx.y;
     const int64_t tile_start = (int64_t)blockIdx.x * IND_TILE, tile_end = min(tile_start + (int64_t)IND_TILE, N);
     const int64_t ro = (int64_t)sym * ld;
     // ---- phase 1: window extrema -> stochastic %K / %D, Williams %R, Ichimoku a / b ----
-    {
-        const int halo = max(i3 - 1, w_st - 1 + smooth - 1);
-        const int64_t s0 = max((int64_t)0, tile_start - halo);
-        const int n = (int)(tile_end - s0);
-        constexpr int CAP = IND_TILE + 256;                         // (the host checks halo <= 256)
-        float* sh = reinterpret_cast<float*>(s_raw);
-        float* sl = sh + CAP;
-        float* sc = sl + CAP;
-        double* skd = reinterpret_cast<double*>(sc + CAP);          // float64 %K of the staged bars
-        stage_row(high + ro, N, s0, n, sh);
-        stage_row(low + ro, N, s0, n, sl);
-        stage_row(close + ro, N, s0, n, sc);
-        __syncthreads();
-        for (int i = threadIdx.x; i < n; i += blockDim.x) {
-            const int64_t t = s0 + i;
-            // running (max high, min low) over the last k bars, captured at the windows in ascending order
-            float mh = -INFINITY, ml = INFINITY;
-            int k = 0;
-            const int have = i + 1;                                  // staged bars at or before this one
-            auto upto = [&](int w) { const int lim = min(w, have); for (; k < lim; ++k) { mh = fmaxf(mh, sh[i - k]); ml = fminf(ml, sl[i - k]); } };
-            upto(i1);
-            const double h1 = (double)mh, l1 = (double)ml;
-            upto(w_st);
-            const double hs = (double)mh, ls = (double)ml;
-            upto(i2);
-            const double h2 = (double)mh, l2 = (double)ml;
-            upto(i3);
-            const double h3 = (double)mh, l3 = (double)ml;
-            const double c = (double)sc[i];
-            // (s0 == 0: "i >= w - 1" is "t >= w - 1"; s0 > 0: every window lies inside the staged halo)
-            const double kk = (i >= w_st - 1) ? 100.0 * (c - ls) / (hs - ls) : (double)nanf32();       // 0/0 -> NaN as in pandas
-            skd[i] = kk;
-            if (t >= tile_start) {
-                const int64_t o = (int64_t)sym * N + t;
-                o_k[o] = (float)kk;
-                o_wr[o] = (t >= w_st - 1) ? (float)(-100.0 * (hs - c) / (hs - ls)) : nanf32();
-                float a = nanf32(), b = nanf32();
-                if (t >= max(i1, i2) - 1) a = (float)(0.5 * (0.5 * (h1 + l1) + 0.5 * (h2 + l2)));
-                if (t >= i3 - 1) b = (float)(0.5 * (h3 + l3));
-                o_ia[o] = a;
-                o_ib[o] = b;
-            }
-        }
-        __syncthreads();
-        for (int64_t t = tile_start + threadIdx.x; t < tile_end; t += blockDim.x) {
-            const int i = (int)(t - s0);
-            float d = nanf32();
-            if (t >= w_st - 1 + smooth - 1) {
-                double acc = 0.0;
-                for (int q = 0; q < smooth; ++q) acc += skd[i - q];
-                d = (float)(acc / (double)smooth);
-            }
-            o_d[(int64_t)sym * N + t] = d;
-        }
-        __syncthreads();
-    }
-    // ---- phase 2: ATR (ta.volatility.AverageTrueRange; :164), a 256-bar sub-tile per warp ----
+    extrema_tile(high, low, close, N, ld, ext, IND_TILE + 256, s_raw, sym, tile_start);    // (the host checks halo <= 256)
+    __syncthreads();
+    // ---- phase 2: ATR, a 256-bar sub-tile per warp ----
     {
         double* tr = reinterpret_cast<double*>(s_raw);
-        int64_t s0 = max((int64_t)0, tile_start - atr_halo) & ~(int64_t)3;
-        if (s0 < IND_MAX_WINDOW) s0 = 0;                             // a pass that crosses the seed bar t = w-1 needs TR from bar 0
-        const int n_stage = (int)(tile_start + IND_TILE - s0);
-        for (int i = threadIdx.x; i < n_stage; i += blockDim.x) {
-            const int64_t t = s0 + i;
-            double v = 0.0;
-            if (t < N) {
-                const double h = (double)__ldg(high + ro + t), l = (double)__ldg(low + ro + t);
-                v = h - l;
-                if (t > 0) {
-                    const double pc = (double)__ldg(close + ro + t - 1);
-                    v = fmax(v, fmax(fabs(h - pc), fabs(l - pc)));
-                }
-            }
-            tr[i] = v;
-        }
-        __syncthreads();
-        const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarp = blockDim.x >> 5;
-        constexpr int K = 4;
-        const int w = w_atr;
-        const double alpha = 1.0 / (double)w, om = ((double)w - 1.0) / (double)w;
-        AffineScan<K> scn;
-        scn.init(om, lane);
-        const int sub = IND_TILE / (int)nwarp;
-        const int64_t sub_start = tile_start + (int64_t)warp * sub, sub_end = min(sub_start + sub, tile_end);
-        if (sub_start < sub_end) {
-            int64_t start = max(s0, sub_start - atr_halo) & ~(int64_t)3;
-            const bool has_seed = (start <= w - 1);                  // this pass crosses the seed bar t = w-1
-            double seed = 0.0;
-            if (has_seed && w - 1 < N) {
-                for (int q = 0; q < w; ++q) seed += tr[(int)(q - s0)];   // s0 == 0 whenever has_seed
-                seed /= (double)w;
-            }
-            if (has_seed) start = 0;
-            double carry = 0.0;
-            for (int64_t base = start; base < sub_end; base += 32 * K) {
-                const int64_t t = base + lane * K;
-                double b[K], y[K];
-#pragma unroll
-                for (int j = 0; j < K; ++j) {
-                    const int64_t tt = t + j;
-                    double v = alpha * tr[min((int)(tt - s0), n_stage - 1)];
-                    if (has_seed) v = tt < w - 1 ? 0.0 : (tt == w - 1 ? seed : v);   // zeros, then the seed, then the recurrence
-                    b[j] = v;
-                }
-                scn.run(b, carry, y, lane);
-#pragma unroll
-                for (int j = 0; j < K; ++j)
-                    if (t + j >= sub_start && t + j < sub_end) o_atr[(int64_t)sym * N + t + j] = (t + j >= w - 1) ? (float)y[j] : 0.0f;
-            }
-        }
+        const int64_t s0 = stage_true_range(high + ro, low + ro, close + ro, N, tile_start, atr_halo, tr);
+        const int sub = IND_TILE / (int)(blockDim.x >> 5);
+        const int64_t sub_start = tile_start + (int64_t)(threadIdx.x >> 5) * sub, sub_end = min(sub_start + sub, tile_end);
+        if (sub_start < sub_end)
+            atr_scan(tr, s0, (int)(tile_start + IND_TILE - s0), N, w_atr, atr_halo, sub_start, sub_end, o_atr + (int64_t)sym * N);
         __syncthreads();
     }
     // ---- phase 3: VWAP ----
@@ -930,6 +804,17 @@ using namespace b200bt;
 static unsigned bank_threads(int P) { return 32u * (unsigned)(P < 2 ? 2 : (P > 8 ? 8 : P)); }
 static dim3 ind_grid(int64_t N, int S) { return dim3((unsigned)((N + IND_TILE - 1) / IND_TILE), (unsigned)S); }
 
+// opts `kern` in to `smem` bytes of dynamic shared memory, launches it with one CTA per (tile, symbol) and checks the launch
+template <typename Kernel, typename... Args>
+static int launch_with_smem(Kernel kern, int64_t N, int S, unsigned threads, size_t smem, b200bt_stream_t stream,
+                            const char* what, Args... args) {
+    const int rc = cuda_status(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), what);
+    if (rc) return rc;
+    kern<<<ind_grid(N, S), threads, smem, (cudaStream_t)stream>>>(args...);
+    B200BT_LAUNCH_CHECK(what);
+    return B200BT_OK;
+}
+
 extern "C" int b200bt_nanfill(float* x, int64_t rows, int64_t N, float* workspace, b200bt_stream_t stream) {
     B200BT_REQUIRE(x && workspace && rows > 0 && N > 0, B200BT_EINVAL, "nanfill: bad argument");
     int rc = check_device();
@@ -951,15 +836,18 @@ extern "C" int64_t b200bt_nanfill_workspace_floats(int64_t rows, int64_t N) {
     return 3 * rows * ((N + NF_TILE - 1) / NF_TILE);
 }
 
-static int fill_bank_params(const int* w_host, int P, bool wilder, BankParams& prm, int& halo_max, const char* name) {
+// the warm-up each window of a bank is started with: an EMA or Wilder recurrence's (halo_for), or the window's own w - 1 bars
+enum class BankHalo { ema, wilder, window };
+
+static int fill_bank_params(const int* w_host, int P, BankHalo rule, BankParams& prm, int& halo_max, const char* name) {
     B200BT_REQUIRE(w_host && P > 0 && P <= IND_MAX_P, B200BT_ELIMIT, "%s: 1..%d windows per call", name, IND_MAX_P);
     halo_max = 0;
     for (int i = 0; i < P; ++i) {
         const int w = w_host[i];
         B200BT_REQUIRE(w >= 1 && w <= IND_MAX_WINDOW, B200BT_ELIMIT, "%s: window %d outside [1,%d]", name, w, IND_MAX_WINDOW);
         prm.window[i] = w;
-        const double om = wilder ? ((double)w - 1.0) / (double)w : 1.0 - 2.0 / ((double)w + 1.0);
-        prm.halo[i] = halo_for(om);
+        if (rule == BankHalo::window) prm.halo[i] = w - 1;
+        else prm.halo[i] = halo_for(rule == BankHalo::wilder ? ((double)w - 1.0) / (double)w : 1.0 - 2.0 / ((double)w + 1.0));
         if (prm.halo[i] > halo_max) halo_max = prm.halo[i];
     }
     return B200BT_OK;
@@ -971,15 +859,11 @@ extern "C" int b200bt_ema_bank(const float* x, int S, int64_t N, int64_t ld, con
     IND_COMMON_CHECKS("ema_bank");
     BankParams prm;
     int halo_max;
-    int rc = fill_bank_params(spans_host, P, false, prm, halo_max, "ema_bank");
+    int rc = fill_bank_params(spans_host, P, BankHalo::ema, prm, halo_max, "ema_bank");
     if (rc) return rc;
     const size_t smem = (size_t)(halo_max + IND_TILE + 8) * sizeof(float);
     B200BT_REQUIRE(smem <= 200 * 1024, B200BT_ELIMIT, "ema_bank: span too long for the shared-memory tile");
-    cudaError_t e = cudaFuncSetAttribute(ema_bank_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return cuda_status(e, "ema_bank: cudaFuncSetAttribute");
-    ema_bank_kernel<<<ind_grid(N, S), bank_threads(P), smem, (cudaStream_t)stream>>>(x, N, ld, prm, P, halo_max, out);
-    B200BT_LAUNCH_CHECK("ema_bank launch");
-    return B200BT_OK;
+    return launch_with_smem(ema_bank_kernel, N, S, bank_threads(P), smem, stream, "ema_bank launch", x, N, ld, prm, P, halo_max, out);
 }
 
 extern "C" int b200bt_macd(const float* x, int S, int64_t N, int64_t ld, int fast, int slow, int sign, float* line,
@@ -992,12 +876,8 @@ extern "C" int b200bt_macd(const float* x, int S, int64_t N, int64_t ld, int fas
     const int halo_sig = halo_for(1.0 - 2.0 / ((double)sign + 1.0));
     const size_t smem = (size_t)(halo_sig + IND_TILE + 8) * sizeof(double);
     B200BT_REQUIRE(smem <= 200 * 1024, B200BT_ELIMIT, "macd: signal span too long for the shared-memory tile");
-    cudaError_t e = cudaFuncSetAttribute(macd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return cuda_status(e, "macd: cudaFuncSetAttribute");
-    macd_kernel<<<ind_grid(N, S), 32, smem, (cudaStream_t)stream>>>(x, N, ld, fast, slow, sign, halo_ema, halo_sig, line,
-                                                                     signal, diff);
-    B200BT_LAUNCH_CHECK("macd launch");
-    return B200BT_OK;
+    return launch_with_smem(macd_kernel, N, S, 32, smem, stream, "macd launch", x, N, ld, fast, slow, sign, halo_ema, halo_sig,
+                            line, signal, diff);
 }
 
 extern "C" int b200bt_sma_bank(const float* x, int S, int64_t N, int64_t ld, const int* windows_host, int P, float* out,
@@ -1005,21 +885,11 @@ extern "C" int b200bt_sma_bank(const float* x, int S, int64_t N, int64_t ld, con
     B200BT_REQUIRE(x && out, B200BT_EINVAL, "sma_bank: null pointer");
     IND_COMMON_CHECKS("sma_bank");
     BankParams prm;
-    int halo_max = 0;
-    B200BT_REQUIRE(windows_host && P > 0 && P <= IND_MAX_P, B200BT_ELIMIT, "sma_bank: 1..%d windows per call", IND_MAX_P);
-    for (int i = 0; i < P; ++i) {
-        B200BT_REQUIRE(windows_host[i] >= 1 && windows_host[i] <= IND_MAX_WINDOW, B200BT_ELIMIT, "sma_bank: window %d outside [1,%d]",
-                       windows_host[i], IND_MAX_WINDOW);
-        prm.window[i] = windows_host[i];
-        prm.halo[i] = windows_host[i] - 1;
-        if (prm.halo[i] > halo_max) halo_max = prm.halo[i];
-    }
+    int halo_max;
+    int rc = fill_bank_params(windows_host, P, BankHalo::window, prm, halo_max, "sma_bank");
+    if (rc) return rc;
     const size_t smem = (size_t)(halo_max + IND_TILE + 2) * sizeof(double);
-    cudaError_t e = cudaFuncSetAttribute(sma_bank_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return cuda_status(e, "sma_bank: cudaFuncSetAttribute");
-    sma_bank_kernel<<<ind_grid(N, S), IND_THREADS, smem, (cudaStream_t)stream>>>(x, N, ld, prm, P, halo_max, out);
-    B200BT_LAUNCH_CHECK("sma_bank launch");
-    return B200BT_OK;
+    return launch_with_smem(sma_bank_kernel, N, S, IND_THREADS, smem, stream, "sma_bank launch", x, N, ld, prm, P, halo_max, out);
 }
 
 extern "C" int b200bt_bollinger(const float* x, int S, int64_t N, int64_t ld, int window, double k, float* high,
@@ -1028,45 +898,51 @@ extern "C" int b200bt_bollinger(const float* x, int S, int64_t N, int64_t ld, in
     IND_COMMON_CHECKS("bollinger");
     B200BT_REQUIRE(window >= 1 && window <= IND_MAX_WINDOW, B200BT_ELIMIT, "bollinger: window outside [1,%d]", IND_MAX_WINDOW);
     const size_t smem = (size_t)2 * (IND_TILE + IND_MAX_WINDOW + 1) * sizeof(double);
-    cudaError_t e = cudaFuncSetAttribute(bollinger_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return cuda_status(e, "bollinger: cudaFuncSetAttribute");
-    bollinger_kernel<<<ind_grid(N, S), IND_THREADS, smem, (cudaStream_t)stream>>>(x, N, ld, window, k, high, mid, low, width, pos);
-    B200BT_LAUNCH_CHECK("bollinger launch");
-    return B200BT_OK;
+    return launch_with_smem(bollinger_kernel, N, S, IND_THREADS, smem, stream, "bollinger launch", x, N, ld, window, k, high, mid,
+                            low, width, pos);
 }
 
-static int launch_extrema(const float* high, const float* low, const float* close, int S, int64_t N, int64_t ld, int mode,
-                          int w1, int w2, int w3, float* a, float* b, b200bt_stream_t stream, const char* name) {
-    B200BT_REQUIRE(high && low && a, B200BT_EINVAL, "%s: null pointer", name);
+// the windows the extrema walk captures at, in ascending order, and the bars it stages before a tile
+static ExtremaArgs extrema_args(int w_st, int smooth, int w_conv, int w_base, int w_span, float* k, float* d, float* wr,
+                                float* ia, float* ib) {
+    ExtremaArgs a{w_st, smooth, w_conv, w_base, w_span, {w_st, w_conv, w_base, w_span}, 0, k, d, wr, ia, ib};
+    std::sort(a.walk, a.walk + 4);
+    a.halo = std::max(a.walk[3] - 1, d ? w_st - 1 + smooth - 1 : 0);   // %D needs %K of the previous smooth - 1 bars
+    return a;
+}
+
+// stochastic, Williams %R or Ichimoku: the windows a call does not use are 1
+static int launch_extrema(const float* high, const float* low, const float* close, int S, int64_t N, int64_t ld,
+                          const ExtremaArgs& a, b200bt_stream_t stream, const char* name) {
     B200BT_REQUIRE(S > 0 && N > 0 && ld >= N, B200BT_EINVAL, "%s: bad sizes", name);
-    B200BT_REQUIRE(w1 >= 1 && w2 >= 1 && w3 >= 1 && w1 <= IND_MAX_WINDOW && w2 <= IND_MAX_WINDOW && w3 <= IND_MAX_WINDOW,
-                   B200BT_ELIMIT, "%s: window outside [1,%d]", name, IND_MAX_WINDOW);
+    const int ws[5] = {a.w_st, a.smooth, a.w_conv, a.w_base, a.w_span};
+    for (int w : ws) B200BT_REQUIRE(w >= 1 && w <= IND_MAX_WINDOW, B200BT_ELIMIT, "%s: window outside [1,%d]", name, IND_MAX_WINDOW);
     int rc = check_device();
     if (rc) return rc;
-    const size_t smem = (size_t)3 * (IND_TILE + 2 * IND_MAX_WINDOW) * sizeof(float);
-    cudaError_t e = cudaFuncSetAttribute(extrema_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return cuda_status(e, "extrema: cudaFuncSetAttribute");
-    extrema_kernel<<<ind_grid(N, S), IND_THREADS, smem, (cudaStream_t)stream>>>(high, low, close, N, ld, mode, w1, w2, w3, a, b);
-    B200BT_LAUNCH_CHECK("extrema launch");
-    return B200BT_OK;
+    const int cap = IND_TILE + ((a.halo + 1) & ~1);          // even: the %K doubles follow three float rows
+    const size_t smem = (size_t)cap * (3 * sizeof(float) + (a.o_d ? sizeof(double) : 0));
+    return launch_with_smem(extrema_kernel, N, S, IND_THREADS, smem, stream, "extrema launch", high, low, close, N, ld, a, cap);
 }
 
 extern "C" int b200bt_stochastic(const float* high, const float* low, const float* close, int S, int64_t N, int64_t ld,
                                  int window, int smooth, float* k, float* d, b200bt_stream_t stream) {
-    B200BT_REQUIRE(close && d, B200BT_EINVAL, "stochastic: null pointer");
-    return launch_extrema(high, low, close, S, N, ld, 0, window, smooth, 1, k, d, stream, "stochastic");
+    B200BT_REQUIRE(high && low && close && k && d, B200BT_EINVAL, "stochastic: null pointer");
+    return launch_extrema(high, low, close, S, N, ld, extrema_args(window, smooth, 1, 1, 1, k, d, nullptr, nullptr, nullptr),
+                          stream, "stochastic");
 }
 
 extern "C" int b200bt_williams_r(const float* high, const float* low, const float* close, int S, int64_t N, int64_t ld,
                                  int lbp, float* out, b200bt_stream_t stream) {
-    B200BT_REQUIRE(close, B200BT_EINVAL, "williams_r: null pointer");
-    return launch_extrema(high, low, close, S, N, ld, 1, lbp, 1, 1, out, nullptr, stream, "williams_r");
+    B200BT_REQUIRE(high && low && close && out, B200BT_EINVAL, "williams_r: null pointer");
+    return launch_extrema(high, low, close, S, N, ld, extrema_args(lbp, 1, 1, 1, 1, nullptr, nullptr, out, nullptr, nullptr),
+                          stream, "williams_r");
 }
 
 extern "C" int b200bt_ichimoku(const float* high, const float* low, int S, int64_t N, int64_t ld, int w1, int w2, int w3,
                                float* a, float* b, b200bt_stream_t stream) {
-    B200BT_REQUIRE(b, B200BT_EINVAL, "ichimoku: null pointer");
-    return launch_extrema(high, low, nullptr, S, N, ld, 2, w1, w2, w3, a, b, stream, "ichimoku");
+    B200BT_REQUIRE(high && low && a && b, B200BT_EINVAL, "ichimoku: null pointer");
+    return launch_extrema(high, low, nullptr, S, N, ld, extrema_args(1, 1, w1, w2, w3, nullptr, nullptr, nullptr, a, b), stream,
+                          "ichimoku");
 }
 
 extern "C" int b200bt_atr_bank(const float* high, const float* low, const float* close, int S, int64_t N, int64_t ld,
@@ -1075,16 +951,13 @@ extern "C" int b200bt_atr_bank(const float* high, const float* low, const float*
     IND_COMMON_CHECKS("atr_bank");
     BankParams prm;
     int halo_max;
-    int rc = fill_bank_params(windows_host, P, true, prm, halo_max, "atr_bank");
+    int rc = fill_bank_params(windows_host, P, BankHalo::wilder, prm, halo_max, "atr_bank");
     if (rc) return rc;
     for (int i = 0; i < P; ++i) B200BT_REQUIRE(prm.window[i] <= IND_TILE / 2, B200BT_ELIMIT, "atr_bank: window too long");
     const size_t smem = (size_t)(halo_max + IND_TILE + IND_MAX_WINDOW + 8) * sizeof(double);
     B200BT_REQUIRE(smem <= 200 * 1024, B200BT_ELIMIT, "atr_bank: window too long for the shared-memory tile");
-    cudaError_t e = cudaFuncSetAttribute(atr_bank_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return cuda_status(e, "atr_bank: cudaFuncSetAttribute");
-    atr_bank_kernel<<<ind_grid(N, S), IND_THREADS, smem, (cudaStream_t)stream>>>(high, low, close, N, ld, prm, P, halo_max, out);
-    B200BT_LAUNCH_CHECK("atr_bank launch");
-    return B200BT_OK;
+    return launch_with_smem(atr_bank_kernel, N, S, IND_THREADS, smem, stream, "atr_bank launch", high, low, close, N, ld, prm, P,
+                            halo_max, out);
 }
 
 extern "C" int b200bt_vwap(const float* high, const float* low, const float* close, const float* volume, int S, int64_t N,
@@ -1093,11 +966,7 @@ extern "C" int b200bt_vwap(const float* high, const float* low, const float* clo
     IND_COMMON_CHECKS("vwap");
     B200BT_REQUIRE(window >= 1 && window <= IND_MAX_WINDOW, B200BT_ELIMIT, "vwap: window outside [1,%d]", IND_MAX_WINDOW);
     const size_t smem = (size_t)2 * (IND_TILE + IND_MAX_WINDOW + 1) * sizeof(double);
-    cudaError_t e = cudaFuncSetAttribute(vwap_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return cuda_status(e, "vwap: cudaFuncSetAttribute");
-    vwap_kernel<<<ind_grid(N, S), IND_THREADS, smem, (cudaStream_t)stream>>>(high, low, close, volume, N, ld, window, out);
-    B200BT_LAUNCH_CHECK("vwap launch");
-    return B200BT_OK;
+    return launch_with_smem(vwap_kernel, N, S, IND_THREADS, smem, stream, "vwap launch", high, low, close, volume, N, ld, window, out);
 }
 
 // TechnicalAnalyzer._calculate_all_indicators for S symbols: three fused launches + one batched NaN-policy call.
@@ -1109,71 +978,66 @@ extern "C" int b200bt_analyzer(const float* high, const float* low, const float*
                                int64_t ld, float* cols, float* workspace, b200bt_stream_t stream) {
     B200BT_REQUIRE(high && low && close && volume && cols && workspace, B200BT_EINVAL, "analyzer: null pointer");
     IND_COMMON_CHECKS("analyzer");
-    cudaStream_t st = (cudaStream_t)stream;
     const int64_t plane = (int64_t)S * N;
     auto col = [&](int c) { return cols + (int64_t)c * plane; };
     // the reference's windows (binance_ml_strategy.py:67-179)
     const int fast = 12, slow = 26, sign = 9, w_rsi = 14, w_bb = 20, w_st = 14, smooth = 3, w_wr = 14, w_atr = 14, w_vwap = 14;
     const int sma_w[3] = {20, 50, 200}, ich[3] = {9, 26, 52};
+    int rc;
     // A: close -> ema_12, ema_26, macd, macd_signal, macd_diff, rsi
     {
         const int halo_ema = halo_for(1.0 - 2.0 / ((double)slow + 1.0)), halo_sig = halo_for(1.0 - 2.0 / ((double)sign + 1.0));
         const int halo_rsi = halo_for(((double)w_rsi - 1.0) / (double)w_rsi);
         const size_t smem = (size_t)(halo_sig + IND_TILE + 8) * sizeof(double);
-        cudaError_t e = cudaFuncSetAttribute(analyzer_a_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return cuda_status(e, "analyzer: cudaFuncSetAttribute");
         LeadFill lf{};
         const int cs[6] = {B200BT_COL_EMA_12, B200BT_COL_EMA_26, B200BT_COL_MACD, B200BT_COL_MACD_SIGNAL, B200BT_COL_MACD_DIFF, B200BT_COL_RSI};
         const int fs[6] = {fast - 1, slow - 1, slow - 1, slow - 1 + sign - 1, slow - 1 + sign - 1, w_rsi - 1};
         lf.n = 6;
         for (int i = 0; i < 6; ++i) { lf.col[i] = col(cs[i]); lf.first[i] = fs[i]; }
-        analyzer_a_kernel<<<ind_grid(N, S), 64, smem, st>>>(close, N, ld, fast, slow, sign, halo_ema, halo_sig, w_rsi, halo_rsi,
-                                                           col(B200BT_COL_EMA_12), col(B200BT_COL_EMA_26), col(B200BT_COL_MACD),
-                                                           col(B200BT_COL_MACD_SIGNAL), col(B200BT_COL_MACD_DIFF), col(B200BT_COL_RSI), lf);
-        B200BT_LAUNCH_CHECK("analyzer A launch");
+        if ((rc = launch_with_smem(analyzer_a_kernel, N, S, 64, smem, stream, "analyzer A launch", close, N, ld, fast, slow, sign,
+                                   halo_ema, halo_sig, w_rsi, halo_rsi, col(B200BT_COL_EMA_12), col(B200BT_COL_EMA_26),
+                                   col(B200BT_COL_MACD), col(B200BT_COL_MACD_SIGNAL), col(B200BT_COL_MACD_DIFF),
+                                   col(B200BT_COL_RSI), lf)))
+            return rc;
     }
     // B: close -> sma_20, sma_50, sma_200, Bollinger
     {
         const int halo = sma_w[2] - 1;
         const size_t smem = (size_t)2 * (IND_TILE + IND_MAX_WINDOW + 1) * sizeof(double);
-        cudaError_t e = cudaFuncSetAttribute(analyzer_b_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return cuda_status(e, "analyzer: cudaFuncSetAttribute");
         LeadFill lf{};
         const int cs[7] = {B200BT_COL_SMA_20, B200BT_COL_SMA_50, B200BT_COL_SMA_200, B200BT_COL_BB_HIGH, B200BT_COL_BB_MID, B200BT_COL_BB_LOW,
                            B200BT_COL_BB_WIDTH};
         const int fs[7] = {sma_w[0] - 1, sma_w[1] - 1, sma_w[2] - 1, w_bb - 1, w_bb - 1, w_bb - 1, w_bb - 1};
         lf.n = 7;
         for (int i = 0; i < 7; ++i) { lf.col[i] = col(cs[i]); lf.first[i] = fs[i]; }
-        analyzer_b_kernel<<<ind_grid(N, S), IND_THREADS, smem, st>>>(close, N, ld, sma_w[0], sma_w[1], sma_w[2], w_bb, 2.0,
-                                                                    col(B200BT_COL_SMA_20), col(B200BT_COL_SMA_50), col(B200BT_COL_SMA_200),
-                                                                    col(B200BT_COL_BB_HIGH), col(B200BT_COL_BB_MID), col(B200BT_COL_BB_LOW),
-                                                                    col(B200BT_COL_BB_WIDTH), col(B200BT_COL_BB_POSITION), halo, lf);
-        B200BT_LAUNCH_CHECK("analyzer B launch");
+        if ((rc = launch_with_smem(analyzer_b_kernel, N, S, IND_THREADS, smem, stream, "analyzer B launch", close, N, ld, sma_w[0],
+                                   sma_w[1], sma_w[2], w_bb, 2.0, col(B200BT_COL_SMA_20), col(B200BT_COL_SMA_50),
+                                   col(B200BT_COL_SMA_200), col(B200BT_COL_BB_HIGH), col(B200BT_COL_BB_MID), col(B200BT_COL_BB_LOW),
+                                   col(B200BT_COL_BB_WIDTH), col(B200BT_COL_BB_POSITION), halo, lf)))
+            return rc;
     }
     // C: high, low, close, volume -> stochastic, Williams %R, Ichimoku, ATR, VWAP
     {
         B200BT_REQUIRE(w_wr == w_st && ich[0] <= w_st && w_st <= ich[1] && ich[1] <= ich[2], B200BT_EINVAL, "analyzer: windows must nest");
         BankParams prm;
         int atr_halo;
-        int rc = fill_bank_params(&w_atr, 1, true, prm, atr_halo, "analyzer");
+        rc = fill_bank_params(&w_atr, 1, BankHalo::wilder, prm, atr_halo, "analyzer");
         if (rc) return rc;
-        B200BT_REQUIRE(ich[2] - 1 <= 256 && w_st + smooth - 2 <= 256, B200BT_ELIMIT, "analyzer: window too long");
+        const ExtremaArgs ext = extrema_args(w_st, smooth, ich[0], ich[1], ich[2], col(B200BT_COL_STOCH_K), col(B200BT_COL_STOCH_D),
+                                             col(B200BT_COL_WILLIAMS_R), col(B200BT_COL_ICHIMOKU_A), col(B200BT_COL_ICHIMOKU_B));
+        B200BT_REQUIRE(ext.halo <= 256, B200BT_ELIMIT, "analyzer: window too long");
         size_t smem = (size_t)3 * (IND_TILE + 256) * sizeof(float) + (size_t)(IND_TILE + 256) * sizeof(double);
         const size_t smem_atr = (size_t)(atr_halo + IND_TILE + IND_MAX_WINDOW + 8) * sizeof(double);
         const size_t smem_vwap = (size_t)2 * (IND_TILE + IND_MAX_WINDOW + 1) * sizeof(double);
         if (smem_atr > smem) smem = smem_atr;
         if (smem_vwap > smem) smem = smem_vwap;
-        cudaError_t e = cudaFuncSetAttribute(analyzer_c_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return cuda_status(e, "analyzer: cudaFuncSetAttribute");
         LeadFill lf{};
         lf.n = 2;
         lf.col[0] = col(B200BT_COL_ICHIMOKU_A); lf.first[0] = ich[1] - 1;
         lf.col[1] = col(B200BT_COL_ICHIMOKU_B); lf.first[1] = ich[2] - 1;
-        analyzer_c_kernel<<<ind_grid(N, S), IND_THREADS, smem, st>>>(high, low, close, volume, N, ld, w_st, smooth, ich[0], ich[1], ich[2],
-                                                                    w_atr, atr_halo, w_vwap, col(B200BT_COL_STOCH_K), col(B200BT_COL_STOCH_D),
-                                                                    col(B200BT_COL_WILLIAMS_R), col(B200BT_COL_ICHIMOKU_A),
-                                                                    col(B200BT_COL_ICHIMOKU_B), col(B200BT_COL_ATR), col(B200BT_COL_VWAP), lf);
-        B200BT_LAUNCH_CHECK("analyzer C launch");
+        if ((rc = launch_with_smem(analyzer_c_kernel, N, S, IND_THREADS, smem, stream, "analyzer C launch", high, low, close, volume,
+                                   N, ld, ext, w_atr, atr_halo, w_vwap, col(B200BT_COL_ATR), col(B200BT_COL_VWAP), lf)))
+            return rc;
     }
     // NaN policy of the five columns that can be undefined in mid-series (they are the last five of the allocation)
     return b200bt_nanfill(col(B200BT_COL_VWAP), (int64_t)5 * S, N, workspace, stream);

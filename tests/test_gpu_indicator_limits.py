@@ -528,3 +528,30 @@ def test_rsi_bank_copies_a_time_strided_close_to_contiguous_rows(torch_cuda):
     assert _same_bits(got, want)
     for s in range(2):
         np.testing.assert_allclose(got[s], ref.rsi_bank(data[3, s, ::2], periods), rtol=2e-7, atol=0)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# 6. the fused analyzer and the entry points run the same tile functions
+# ---------------------------------------------------------------------------------------------------------------------
+def test_analyzer_columns_equal_the_single_indicator_entry_points(torch_cuda):
+    """Over several tiles at both price scales, wherever an entry point's output is defined, the analyzer's column (NaN
+    policy applied) is the same bit for bit: sma_20 / 50 / 200 (the bank of those windows stages the analyzer's 199-bar
+    span), stoch_k, stoch_d, williams_r, ichimoku_a, ichimoku_b (exact extrema, one walk) and vwap (vwap_tile, same span).
+    The other columns differ in their last bits by design: Bollinger's Σd² rounds with the staged span (19 bars alone, 199
+    in the analyzer), ATR's and the EMAs' scans start at other bars (sub-tiles, the MACD halo), RSI is another kernel."""
+    torch = torch_cuda
+    from ai_crypto_trader_b200.indicators import TechnicalAnalyzer
+    from ai_crypto_trader_b200.sweep import MarketData
+    N = 3 * IND_TILE + 777
+    data = _two_scales(N, seed=12)
+    t = _dev(torch, data)
+    cols = {name: x.cpu().numpy() for name, x in TechnicalAnalyzer(MarketData(data)).data.items()}
+    sma = _gpu("sma", [20, 50, 200], t)["sma"]
+    alone = {"sma_20": sma[:, 0], "sma_50": sma[:, 1], "sma_200": sma[:, 2], **_gpu("stochastic", (14, 3), t),
+             **_gpu("williams_r", 14, t), **_gpu("ichimoku", (9, 26, 52), t), **_gpu("vwap", 14, t)}
+    for name, want in alone.items():
+        defined = ~np.isnan(want)
+        assert defined.sum() >= 2 * (N - 200), name
+        got = cols[name]
+        assert _same_bits(got[defined], want[defined]), (name, "bars that differ:",
+                                                         np.flatnonzero((got != want) & defined)[:8])
