@@ -3,6 +3,7 @@ from __future__ import annotations
 
 import ctypes as C
 import subprocess
+from concurrent.futures import ThreadPoolExecutor
 from pathlib import Path
 
 import numpy as np
@@ -109,3 +110,75 @@ def lanes(price32: np.ndarray, rsi32: np.ndarray, plist: list, cfg: Config) -> n
     lib().oracle_lanes(price32.ctypes.data, rsi32.ctypes.data, len(price32), arr, len(plist), C.byref(cfg),
                        out.ctypes.data)
     return out
+
+
+def population(close: np.ndarray, bank: np.ndarray, row_of, population: list, cfg: Config, event_cap: int = 0,
+               workers: int | None = None):
+    """`lane` on every (individual, symbol) of `population`, on the host fp32 rows a sweep reads: close [S][N], RSI bank
+    [S][R][N].  `row_of`: {rsi_period: bank row} (an individual without the gene reads period 14) or a callable
+    individual -> bank row.
+    -> (stats STATS_DTYPE [pop][S], events, pnl): with event_cap > 0 events[i][s] / pnl[i][s] are the lane's first
+    min(n_records, event_cap) event words / record pnl, else both are None.  `workers` > 1 runs the individuals in that
+    many threads (ctypes releases the GIL); the results do not depend on it."""
+    row = row_of if callable(row_of) else (lambda p: row_of[int(p.get("rsi_period", 14))])
+
+    def one(p):
+        r = row(p)
+        # copies: a lane's slices would keep its whole event_cap buffers alive
+        return [(st, np.array(ev), np.array(pn)) if event_cap else (st, None, None)
+                for st, ev, pn in (lane(close[s], bank[s][r], p, cfg, event_cap) for s in range(len(close)))]
+
+    if workers is not None and workers > 1:
+        with ThreadPoolExecutor(max_workers=workers) as ex:
+            out = list(ex.map(one, population))
+    else:
+        out = [one(p) for p in population]
+    stats = np.zeros((len(population), len(close)), dtype=STATS_DTYPE)
+    for i, lanes_i in enumerate(out):
+        stats[i] = [st for st, _, _ in lanes_i]
+    if not event_cap:
+        return stats, None, None
+    return stats, [[ev for _, ev, _ in lanes_i] for lanes_i in out], [[pn for _, _, pn in lanes_i] for lanes_i in out]
+
+
+# The sweep-against-oracle check (DESIGN.md section 5): counts, days, durations and the trade hash exact, every float
+# statistic to max(rtol |want|, atol).
+EXACT_FIELDS = ("n_records", "n_wins", "n_losses", "n_days", "sum_duration_bars", "n_negative_days", "trade_hash")
+CLOSE_FIELDS = tuple(f for f in STATS_FIELDS if f not in EXACT_FIELDS)
+
+
+def _column(x, f: str) -> np.ndarray:
+    """Field `f` of a STATS_DTYPE array, a mapping field -> array, or a sequence of dicts; trade_hash as uint64."""
+    if isinstance(x, np.ndarray) or hasattr(x, "keys"):
+        col = x[f]
+    else:
+        col = [d[f] for d in x]
+    return np.asarray(col, dtype=np.uint64 if f == "trade_hash" else np.float64)
+
+
+def assert_lanes(got, want, where: str, exact=EXACT_FIELDS, close=CLOSE_FIELDS, rtol: float = 1e-9,
+                 atol: float = 1e-11) -> None:
+    """Fields `exact` equal and fields `close` within max(rtol |want|, atol) (NaN equals NaN, an infinity must match in
+    sign) between two sets of lanes or books: STATS_DTYPE arrays, mappings field -> array (lane_stats(),
+    book_stats()) or sequences of dicts (tests/book_ref.book), of the same shape."""
+    for f in exact + close:
+        g, w = _column(got, f), _column(want, f)
+        assert g.shape == w.shape, f"{where}: {f} has shape {g.shape}, want {w.shape}"
+        if f in exact:
+            bad = g != w
+        else:
+            with np.errstate(invalid="ignore"):
+                near = np.isfinite(w) & (np.abs(g - w) <= np.maximum(rtol * np.abs(w), atol))
+                bad = ~((g == w) | (np.isnan(g) & np.isnan(w)) | near)
+        if bad.any():
+            k = tuple(int(j) for j in np.argwhere(bad)[0])
+            raise AssertionError(f"{where}: {f} differs in {int(bad.sum())} of {bad.size} lanes, first at {k}: "
+                                 f"got {g[k]!r}, want {w[k]!r}")
+
+
+def assert_events(events, want_events, where: str) -> None:
+    """The first n_records event words of every lane: `events` [pop][S][cap] (PopulationSweep.events()) against the
+    ragged want_events[i][s] of `population`."""
+    for i, lanes_i in enumerate(want_events):
+        for s, ev in enumerate(lanes_i):
+            np.testing.assert_array_equal(events[i][s][:len(ev)], ev, err_msg=f"{where}: events of lane {(i, s)}")

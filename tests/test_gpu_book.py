@@ -15,9 +15,6 @@ from gpu_fixtures import torch_cuda
 
 pytestmark = pytest.mark.gpu
 
-EXACT = ("n_records", "trade_hash", "n_wins", "n_losses", "n_days", "n_negative_days", "sum_duration_bars")
-CLOSE = ("net_profit", "total_profit", "total_loss", "largest_profit", "largest_loss", "max_drawdown", "sharpe_ratio",
-         "sortino_ratio", "downside_deviation", "mean_daily_pnl", "win_rate", "profit_factor", "score")
 PERIODS = (5, 9, 14, 21)
 SOURCE = [0, 1, 0, 2, 0]          # symbol s is a copy of synthetic series SOURCE[s]
 QUIET = 4                         # this symbol's RSI rows are NaN: no threshold compare is true, it never trades
@@ -46,30 +43,13 @@ def _market(torch, n_bars, bar_minutes=1, minute0=None, source=SOURCE, quiet=QUI
     return market, bank, close, bank.cpu().numpy()
 
 
-def _oracle(close, bank, population, cfg):
+def _books(close, bank, population, cfg):
     """Oracle books [pop] (dicts) and lanes [pop][S] of `population`."""
     import book_ref
     from oracle import sim_oracle
-    S, N = close.shape
-    row = {p: i for i, p in enumerate(PERIODS)}
-    books, lanes = [], np.zeros((len(population), S), dtype=sim_oracle.STATS_DTYPE)
-    for i, p in enumerate(population):
-        evs, pns = [], []
-        for s in range(S):
-            lanes[i, s], ev, pn = sim_oracle.lane(close[s], bank[s, row[int(p["rsi_period"])]], p, cfg, event_cap=N + 2)
-            evs.append(ev)
-            pns.append(pn)
-        books.append(book_ref.book(evs, pns, cfg))
-    return books, lanes
-
-
-def _compare(got, want, where):
-    for f in EXACT:
-        np.testing.assert_array_equal(np.asarray(got[f]), np.array([w[f] for w in want], dtype=np.asarray(got[f]).dtype),
-                                      err_msg=f"{where}: {f}")
-    for f in CLOSE:
-        np.testing.assert_allclose(np.asarray(got[f], dtype=np.float64), np.array([w[f] for w in want]), rtol=1e-9,
-                                   atol=1e-11, equal_nan=True, err_msg=f"{where}: {f}")
+    lanes, evs, pns = sim_oracle.population(close, bank, {p: i for i, p in enumerate(PERIODS)}, population, cfg,
+                                            event_cap=close.shape[1] + 2)
+    return [book_ref.book(e, p, cfg) for e, p in zip(evs, pns)], lanes
 
 
 def _book_sweep(market, bank, **kw):
@@ -94,9 +74,9 @@ def test_book_matches_the_oracle(torch_cuda, case, bar_minutes, gap):
         sweep.set_gap(*gap)
         cfg.gap_bar, cfg.gap_minutes = gap
     fit = sweep.evaluate(pop)
-    want, lanes = _oracle(close, bank_h, pop, cfg)
+    want, lanes = _books(close, bank_h, pop, cfg)
     got = sweep.book_stats()
-    _compare(got, want, case)
+    sim_oracle.assert_lanes(got, want, case)
     np.testing.assert_allclose(fit, [w["score"] for w in want], rtol=1e-9, atol=1e-11, equal_nan=True)
     # the planted shapes are there: ties across symbols, the last bar's entry + force-close, a quiet symbol, an empty book
     i_dense = len(pop) - 3
@@ -105,9 +85,7 @@ def test_book_matches_the_oracle(torch_cuda, case, bar_minutes, gap):
     assert np.array_equal(got["profitable_symbols"][:, 0], got["profitable_symbols"][:, 2])
     assert not got["profitable_symbols"][:, QUIET].any()
     # lane_stats() keeps describing the per-symbol lanes of the same sweep
-    ls = sweep.lane_stats()
-    np.testing.assert_array_equal(ls["n_records"], lanes["n_records"])
-    np.testing.assert_array_equal(ls["trade_hash"], lanes["trade_hash"])
+    sim_oracle.assert_lanes(sweep.lane_stats(), lanes, f"{case}: lanes")
 
 
 def test_last_bar_entry_and_force_close_across_symbols(torch_cuda):
@@ -126,20 +104,18 @@ def test_last_bar_entry_and_force_close_across_symbols(torch_cuda):
     pop = _population()
     sweep = _book_sweep(market, bank)
     sweep.evaluate(pop)
-    want, _ = _oracle(close, bank_h, pop, cfg)
-    _compare(sweep.book_stats(), want, f"N = {N}")
+    want, _ = _books(close, bank_h, pop, cfg)
+    sim_oracle.assert_lanes(sweep.book_stats(), want, f"N = {N}")
 
 
 def test_single_symbol_book_is_its_lane(torch_cuda):
+    from oracle import sim_oracle
     N = 30_000
     market, bank, _, _ = _market(torch_cuda, N, source=[1], quiet=None)
     sweep = _book_sweep(market, bank)
     sweep.evaluate(_population())
     got, lane = sweep.book_stats(), sweep.lane_stats()
-    for f in EXACT:
-        np.testing.assert_array_equal(got[f], lane[f][:, 0], err_msg=f)
-    for f in CLOSE:
-        np.testing.assert_allclose(got[f], lane[f][:, 0], rtol=1e-9, atol=1e-11, equal_nan=True, err_msg=f)
+    sim_oracle.assert_lanes(got, {f: lane[f][:, 0] for f in lane}, "one symbol")
 
 
 @pytest.mark.parametrize("schedule", ["fused", "chunked", "tiled"])
@@ -156,8 +132,8 @@ def test_every_schedule_gives_the_oracle_books(torch_cuda, schedule):
     if schedule != "fused":
         sweep.chunk_options = dict(pool_scale=4.0, **({"chunks": 16} if schedule == "tiled" else {"target_events": 2000}))
     fit = sweep.evaluate(pop)
-    want, _ = _oracle(close, bank_h, pop, sim_oracle.config_of(market.minute0, 1))
-    _compare(sweep.book_stats(), want, schedule)
+    want, _ = _books(close, bank_h, pop, sim_oracle.config_of(market.minute0, 1))
+    sim_oracle.assert_lanes(sweep.book_stats(), want, schedule)
     np.testing.assert_allclose(fit, [w["score"] for w in want], rtol=1e-9, atol=1e-11, equal_nan=True)
 
 
@@ -187,7 +163,7 @@ def test_every_score_rule(torch_cuda, advanced):
                                           score_on_advanced=advanced)
         fit = sweep.evaluate(pop)
         cfg = sim_oracle.config_of(market.minute0, 7, goals=goals, advanced=advanced)
-        want, _ = _oracle(close, bank_h, pop, cfg)
+        want, _ = _books(close, bank_h, pop, cfg)
         np.testing.assert_allclose(fit, [w["score"] for w in want], rtol=1e-9, atol=1e-11, equal_nan=True,
                                    err_msg=str(goals))
 

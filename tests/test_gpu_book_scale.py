@@ -22,39 +22,22 @@ from gpu_fixtures import torch_cuda
 pytestmark = pytest.mark.gpu
 
 GOLD = Path(__file__).parent / "golden"
-EXACT = ("n_records", "trade_hash", "n_wins", "n_losses", "n_days", "n_negative_days", "sum_duration_bars")
-CLOSE = ("net_profit", "total_profit", "total_loss", "largest_profit", "largest_loss", "max_drawdown", "sharpe_ratio",
-         "sortino_ratio", "downside_deviation", "mean_daily_pnl", "win_rate", "profit_factor", "score")
 DENSE = dict(rsi_period=5, rsi_oversold=99, rsi_overbought=101, take_profit=0.0001, stop_loss=0.0001)
 
 
-def _oracle_books(close, bank, period_row, population, cfg, workers=None):
-    """Oracle books of `population` (list of dicts); lanes run in threads (ctypes releases the GIL)."""
+def _books(close, bank, period_row, population, cfg):
+    """Oracle books of `population` (list of dicts).  Lanes and books run in threads (ctypes and NumPy release the GIL),
+    128 individuals at a time: their event lists are held at once."""
     import book_ref
     from oracle import sim_oracle
-    S, N = close.shape
-
-    def one(p):
-        evs, pns = [], []
-        for s in range(S):
-            _, ev, pn = sim_oracle.lane(close[s], bank[s, period_row[int(p.get("rsi_period", 14))]], p, cfg,
-                                        event_cap=N + 2)
-            evs.append(ev)
-            pns.append(pn)
-        return book_ref.book(evs, pns, cfg)
-
-    with ThreadPoolExecutor(max_workers=workers or min(32, os.cpu_count() or 1)) as ex:
-        return list(ex.map(one, population))
-
-
-def _compare(got, want, where, rows=None):
-    rows = range(len(want)) if rows is None else rows
-    for f in EXACT:
-        g = np.asarray(got[f])[list(rows)]
-        np.testing.assert_array_equal(g, np.array([w[f] for w in want], dtype=g.dtype), err_msg=f"{where}: {f}")
-    for f in CLOSE:
-        np.testing.assert_allclose(np.asarray(got[f], dtype=np.float64)[list(rows)], [w[f] for w in want], rtol=1e-9,
-                                   atol=1e-11, equal_nan=True, err_msg=f"{where}: {f}")
+    workers = min(32, os.cpu_count() or 1)
+    books = []
+    with ThreadPoolExecutor(max_workers=workers) as ex:
+        for k in range(0, len(population), 128):
+            _, evs, pns = sim_oracle.population(close, bank, period_row, population[k:k + 128], cfg,
+                                                event_cap=close.shape[1] + 2, workers=workers)
+            books += ex.map(lambda ev, pn: book_ref.book(ev, pn, cfg), evs, pns)
+    return books
 
 
 def test_reference_books(torch_cuda):
@@ -105,8 +88,8 @@ def test_sixty_four_symbols(torch_cuda):
     pop += [dict(DENSE), dict(DENSE, rsi_overbought=55, take_profit=0.5)]
     sweep = PopulationSweep.from_bank(market, bank, periods, aggregation="book")
     fit = sweep.evaluate(pop)
-    want = _oracle_books(close, bank.cpu().numpy(), {5: 0, 14: 1}, pop, sim_oracle.config_of(market.minute0, 1))
-    _compare(sweep.book_stats(), want, "S = 64")
+    want = _books(close, bank.cpu().numpy(), {5: 0, 14: 1}, pop, sim_oracle.config_of(market.minute0, 1))
+    sim_oracle.assert_lanes(sweep.book_stats(), want, "S = 64")
     np.testing.assert_allclose(fit, [w["score"] for w in want], rtol=1e-9, atol=1e-11, equal_nan=True)
     assert want[len(pop) - 2]["n_records"] > S * N // 4          # the dense books fill windows of 8 records per symbol
 
@@ -129,8 +112,8 @@ def test_full_size_every_book(torch_cuda):
     for label, pop in (("random", random_pop), ("generation 3", list(ga.population))):
         sweep = PopulationSweep(market, aggregation="book")
         fit = sweep.evaluate(pop)
-        want = _oracle_books(ohlcv[3], sweep.bank.cpu().numpy(), sweep.period_row, pop, cfg)
-        _compare(sweep.book_stats(), want, label)
+        want = _books(ohlcv[3], sweep.bank.cpu().numpy(), sweep.period_row, pop, cfg)
+        sim_oracle.assert_lanes(sweep.book_stats(), want, label)
         np.testing.assert_allclose(fit, [w["score"] for w in want], rtol=1e-9, atol=1e-11, equal_nan=True)
         records[label] = sum(w["n_records"] for w in want)
     assert records["generation 3"] > 3 * records["random"], records
@@ -175,7 +158,7 @@ def test_ga_run_reports_the_oracle_book_score(torch_cuda):
     ga = GeneticAlgorithm(synth.param_ranges(), sweep.fitness_function, population_size=32, generations=3, random_seed=7)
     best = ga.run()
     top = ga.get_generation_history()[-1]
-    want = _oracle_books(ohlcv[3], sweep.bank.cpu().numpy(), sweep.period_row, [top["best_individual"]],
+    want = _books(ohlcv[3], sweep.bank.cpu().numpy(), sweep.period_row, [top["best_individual"]],
                          sim_oracle.config_of(market.minute0, 1))[0]
     assert top["best_fitness"] == pytest.approx(want["score"], rel=1e-9, abs=1e-11)
     assert best == top["best_individual"] or ga.best_fitness >= top["best_fitness"]

@@ -61,6 +61,7 @@ def _chunk_counts(events, n):
 def test_chunk_metrics_match_fused_at_step_edges(torch_cuda, bar_minutes, warm):
     torch = torch_cuda
     from ai_crypto_trader_b200.sweep import MarketData, PopulationSweep
+    from oracle import sim_oracle
     close = _close()
     market = MarketData.from_close(torch.from_numpy(close).cuda(), minute0=0, bar_minutes=bar_minutes)
     population = _population()
@@ -97,14 +98,12 @@ def test_chunk_metrics_match_fused_at_step_edges(torch_cuda, bar_minutes, warm):
         per_day = np.unique(chunk_of.astype(np.int64) * 1_000_000 + day, return_counts=True)[1]
         assert per_day.max() > 2 * STEP                                          # a day across three steps of one chunk
 
-    for f in ("n_records", "trade_hash", "n_wins", "n_losses", "n_days", "n_negative_days", "sum_duration_bars"):
-        np.testing.assert_array_equal(st_t[f], st_f[f], err_msg=f)
+    sim_oracle.assert_lanes(st_t, st_f, "tiled against fused")
     live = np.arange(cap)[None, None, :] < st_f["n_records"][:, :, None]
     np.testing.assert_array_equal(ev_t[live], ev_f[live])
     worst = 0.0
-    for f in ("net_profit", "total_profit", "total_loss", "max_drawdown", "sharpe_ratio", "sortino_ratio", "score"):
+    for f in sim_oracle.CLOSE_FIELDS:
         a, b = np.asarray(st_t[f], dtype=np.float64), np.asarray(st_f[f], dtype=np.float64)
-        np.testing.assert_allclose(a, b, rtol=1e-9, atol=1e-11, equal_nan=True, err_msg=f)
         both = np.isfinite(a) & np.isfinite(b)
         worst = max(worst, float(np.max(np.abs(a - b)[both] / np.maximum(np.abs(b[both]), 1e-300), initial=0.0)))
     np.testing.assert_allclose(f_t, f_f, rtol=1e-9, atol=1e-11, equal_nan=True)

@@ -10,6 +10,7 @@ from gpu_fixtures import torch_cuda
 
 GOLD = Path(__file__).parent / "golden"
 pytestmark = pytest.mark.gpu
+CV_CLOSE = ("sharpe_ratio", "max_drawdown", "win_rate", "profit_factor", "score")    # the lane fields a fold reports
 
 
 def _points(ref, params):
@@ -63,20 +64,17 @@ def test_cross_validate_population_vs_oracle_with_gap(torch_cuda):
     population[0].update(rsi_oversold=35, rsi_overbought=65, rsi_period=5, take_profit=1, stop_loss=1)
     ses = StrategyEvaluationSystem(config={})
     cv = ses.cross_validate_population(population, market.close, sweep.bank, sweep.periods, market.minute0, 1, K)
+    bank = np.stack([indicators_ref.rsi_bank(ohlcv[3, s], sweep.periods) for s in range(S)])
     fold = N // K
     for f in range(K):
         a, b = f * fold, (f + 1) * fold if f < K - 1 else N
-        for s in range(S):
-            bank = indicators_ref.rsi_bank(ohlcv[3, s], sweep.periods)
-            for i, p in enumerate(population):
-                row = bank[sweep.period_row[p["rsi_period"]]]
-                price_tr = np.concatenate([ohlcv[3, s, :a], ohlcv[3, s, b:]])
-                rsi_tr = np.concatenate([row[:a], row[b:]])
-                gap = (a, b - a) if 0 < a and b < N else (0, 0)
-                m0 = market.minute0 + (b if a == 0 else 0)
-                want_tr, _, _ = sim_oracle.lane(price_tr, rsi_tr, p, sim_oracle.config_of(m0, 1, gap_bar=gap[0], gap_minutes=gap[1]))
-                want_te, _, _ = sim_oracle.lane(ohlcv[3, s, a:b], row[a:b], p, sim_oracle.config_of(market.minute0 + a, 1))
-                for side, want in (("train", want_tr), ("test", want_te)):
-                    assert cv[f"{side}_n_records"][f, i, s] == want["n_records"], (f, i, s, side)
-                    for k in ("sharpe_ratio", "max_drawdown", "win_rate", "score"):
-                        assert cv[f"{side}_{k}"][f, i, s] == pytest.approx(float(want[k]), rel=1e-9, abs=1e-11), (f, i, s, side, k)
+        gap = (a, b - a) if 0 < a and b < N else (0, 0)
+        m0 = market.minute0 + (b if a == 0 else 0)
+        train = [np.concatenate([x[..., :a], x[..., b:]], axis=-1) for x in (ohlcv[3], bank)]
+        want_tr, _, _ = sim_oracle.population(*train, sweep.period_row, population,
+                                              sim_oracle.config_of(m0, 1, gap_bar=gap[0], gap_minutes=gap[1]))
+        want_te, _, _ = sim_oracle.population(ohlcv[3, :, a:b], bank[..., a:b], sweep.period_row, population,
+                                              sim_oracle.config_of(market.minute0 + a, 1))
+        for side, want in (("train", want_tr), ("test", want_te)):
+            sim_oracle.assert_lanes({k: cv[f"{side}_{k}"][f] for k in ("n_records",) + CV_CLOSE}, want,
+                                    f"fold {f} {side}", exact=("n_records",), close=CV_CLOSE)

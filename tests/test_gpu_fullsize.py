@@ -28,22 +28,11 @@ def cuda(native_lib):
     return torch
 
 
-def _compare_lanes(stats, want, what):
-    """bit-exact record counts and trade hashes (every entry / exit bar and side), float64 score rel 1e-9."""
-    n_bad = int((stats["n_records"] != want["n_records"]).sum())
-    h_bad = int((stats["trade_hash"] != want["trade_hash"]).sum())
-    assert n_bad == 0 and h_bad == 0, f"{what}: {n_bad} lanes differ in record count, {h_bad} in trade hash"
-    for f in ("n_wins", "n_losses", "n_days", "sum_duration_bars", "n_negative_days"):
-        assert np.array_equal(stats[f], want[f]), (what, f)
-    for f in ("net_profit", "max_drawdown", "sharpe_ratio", "win_rate", "profit_factor", "score", "sortino_ratio"):
-        np.testing.assert_allclose(stats[f], want[f], rtol=1e-9, atol=1e-11, equal_nan=True, err_msg=f"{what}: {f}")
-
-
 def test_c2_full_parity(cuda):
     torch = cuda
     from ai_crypto_trader_b200 import synth
     from ai_crypto_trader_b200.sweep import MarketData, PopulationSweep, TilePlan
-    from oracle import parallel
+    from oracle import parallel, sim_oracle
     S, POP = 10, 1024
     ohlcv_host = torch.from_numpy(synth.synth_ohlcv(S, N_BARS)).pin_memory()      # as bench.py
     market = MarketData(ohlcv_host)
@@ -61,7 +50,7 @@ def test_c2_full_parity(cuda):
     np.testing.assert_allclose(f2, f1, rtol=1e-12, atol=0, equal_nan=True)
     assert sweep.last_pool_overflow is False
     want = parallel.population_stats(population, range(S), N_BARS, market.minute0)
-    _compare_lanes(stats, want, "configs[1]")
+    sim_oracle.assert_lanes(stats, want, "configs[1]")
     with np.errstate(invalid="ignore"):
         np.testing.assert_allclose(f2, want["score"].mean(axis=1), rtol=1e-9, atol=1e-11, equal_nan=True)
     assert int(want["n_records"].sum()) > 100_000_000        # the workload is what the bench says it is
@@ -71,7 +60,7 @@ def test_c5_slice_parity_through_plan_batches(cuda):
     torch = cuda
     from ai_crypto_trader_b200 import synth
     from ai_crypto_trader_b200.sweep import MarketData, PopulationSweep, TilePlan
-    from oracle import parallel
+    from oracle import parallel, sim_oracle
     S, POP = 50, 256
     close = np.stack([synth.synth_symbol(s, N_BARS)["close"] for s in range(S)])
     market = MarketData.from_close(torch.from_numpy(close).cuda())
@@ -85,7 +74,7 @@ def test_c5_slice_parity_through_plan_batches(cuda):
         fit = sweep.evaluate(population)
     stats = sweep.lane_stats()
     want = parallel.population_stats(population, range(S), N_BARS, market.minute0)
-    _compare_lanes(stats, want, "configs[4] slice")
+    sim_oracle.assert_lanes(stats, want, "configs[4] slice")
     with np.errstate(invalid="ignore"):
         np.testing.assert_allclose(fit, want["score"].mean(axis=1), rtol=1e-9, atol=1e-11, equal_nan=True)
 

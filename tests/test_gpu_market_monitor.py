@@ -15,8 +15,8 @@ import numpy as np
 import pytest
 
 import market_monitor_ref as ref
-import regime_ref
 from gpu_fixtures import torch_cuda
+from test_gpu_regime import check_classes
 from test_market_monitor_host import DICTS, FIXTURE, _equal, _leaves
 
 pytestmark = pytest.mark.gpu
@@ -162,21 +162,9 @@ def test_class_stats_by_trend(torch_cuda):
     _, views = sweep.class_stats(pop, labels, len(names))
     lab = labels.cpu().numpy()
     cfg = sim_oracle.config_of(market.minute0, 1)
-    row = {p: k for k, p in enumerate(periods)}
-    n_records = 0
-    for i, p in enumerate(pop):
-        for s in range(market.S):
-            _, ev, pn = sim_oracle.lane(x[3, s], bank_h[s, row[p["rsi_period"]]], p, cfg, event_cap=market.N + 2)
-            want = regime_ref.class_stats(np.asarray(ev), np.asarray(pn), lab[s], len(names), cfg)
-            for r in range(len(names)):
-                got = {k: views[r][k][i, s] for k in views[r]}
-                n_records += int(got["n_records"])
-                for k in ("n_records", "n_wins", "n_losses", "n_days", "sum_duration_bars"):
-                    assert got[k] == want[r][k], (i, s, r, k)
-                assert int(got["trade_hash"]) == int(want[r]["trade_hash"]), (i, s, r)
-                for k in ("net_profit", "max_drawdown", "sharpe_ratio", "score"):
-                    g, w = float(got[k]), float(want[r][k])
-                    assert g == w or (np.isnan(g) and np.isnan(w)) or abs(g - w) <= 1e-9 * abs(w), (i, s, r, k, g, w)
+    _, evs, pns = sim_oracle.population(x[3], bank_h, sweep.period_row, pop, cfg, event_cap=market.N + 2)
+    check_classes(views, evs, pns, lab, len(names), cfg, "labels")
+    n_records = sum(int(v["n_records"].sum()) for v in views)
     assert n_records > 100
 
 

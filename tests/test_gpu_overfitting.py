@@ -42,18 +42,12 @@ def _market(torch, n_bars, bar_minutes=1):
     return market, bank, close, bank.cpu().numpy()
 
 
-def _oracle_rows(close, bank, population, cfg, row_of):
+def _day_rows(close, bank, population, cfg, row_of):
     """Host lane rows [pop][S][D] of the C oracle's records."""
     from oracle import sim_oracle
-    S, N = close.shape
-    out = []
-    for p in population:
-        rows = []
-        for s in range(S):
-            _, ev, pn = sim_oracle.lane(close[s], bank[s, row_of[int(p.get("rsi_period", 14))]], p, cfg, event_cap=N + 2)
-            rows.append(cscv_ref.lane_rows(ev, pn, cfg, N))
-        out.append(rows)
-    return np.array(out)
+    N = close.shape[1]
+    _, evs, pns = sim_oracle.population(close, bank, row_of, population, cfg, event_cap=N + 2)
+    return np.array([[cscv_ref.lane_rows(ev, pn, cfg, N) for ev, pn in zip(*lanes)] for lanes in zip(evs, pns)])
 
 
 def _close_rows(got, want, where):
@@ -112,7 +106,7 @@ def test_lane_rows_match_the_oracle(torch_cuda, case, bar_minutes, n_bars, gap):
         sweep.set_gap(gap[0], gap_minutes)
         cfg.gap_bar, cfg.gap_minutes = gap[0], gap_minutes
     book, lanes, first = sweep.daily_pnl(pop)
-    want = _oracle_rows(close, bank_h, pop, cfg, sweep.period_row)
+    want = _day_rows(close, bank_h, pop, cfg, sweep.period_row)
     first_w, D = cscv_ref.calendar(cfg, n_bars)
     assert first == first_w and lanes.shape == (len(pop), market.S, D)
     got = lanes.cpu().numpy()
@@ -139,7 +133,7 @@ def test_last_bar_entry_and_force_close(torch_cuda):
         pytest.fail("no length in 3000..3039 puts an entry on the last bar")
     pop = _population()
     _, lanes, _ = PopulationSweep.from_bank(market, bank, PERIODS).daily_pnl(pop)
-    _close_rows(lanes.cpu().numpy(), _oracle_rows(close, bank_h, pop, cfg, {p: i for i, p in enumerate(PERIODS)}),
+    _close_rows(lanes.cpu().numpy(), _day_rows(close, bank_h, pop, cfg, {p: i for i, p in enumerate(PERIODS)}),
                 f"N = {N}")
 
 
@@ -240,16 +234,8 @@ def test_backtest_overfitting_end_to_end(torch_cuda):
     # the oracle pipeline: C-oracle records -> host rows -> cscv_exact
     _, unique, expand = sweep._unique(pop)
     cfg = sim_oracle.config_of(market.minute0, 1)
-    banks = sweep.bank.cpu().numpy()
-    rows = []
-    for p in unique:
-        lane = []
-        for s in range(S):
-            _, ev, pn = sim_oracle.lane(ohlcv[3, s], banks[s][sweep.period_row[int(p["rsi_period"])]], p, cfg,
-                                        event_cap=N + 2)
-            lane.append(cscv_ref.lane_rows(ev, pn, cfg, N))
-        rows.append(cscv_ref.book_row(lane))
-    want = cscv_ref.cscv_exact(np.array(rows), 16)
+    lanes = _day_rows(ohlcv[3], sweep.bank.cpu().numpy(), unique, cfg, sweep.period_row)
+    want = cscv_ref.cscv_exact(np.array([cscv_ref.book_row(list(g)) for g in lanes]), 16)
     summ = summarize(want["is_sr"], want["oos_sr"], want["n_below"], want["n_tied"], len(unique))
     dsr = deflated_sharpe(want, len(unique))
     assert res["n_trials"] == len(unique) < len(pop) and res["n_combinations"] == 12870

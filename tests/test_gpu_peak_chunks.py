@@ -35,17 +35,10 @@ def _population():
 def _check_vs_oracle(sweep, population, close):
     from ai_crypto_trader_b200 import synth
     from oracle import indicators_ref, sim_oracle
-    stats = sweep.lane_stats()
-    cfg = sim_oracle.config_of(synth.EPOCH_2024_MINUTES, 1)
-    for s in range(close.shape[0]):
-        bank = indicators_ref.rsi_bank(close[s], sweep.periods)
-        for i, p in enumerate(population):
-            want, _, _ = sim_oracle.lane(close[s], bank[sweep.period_row[p["rsi_period"]]], p, cfg)
-            for f in ("n_records", "trade_hash", "n_wins", "n_losses", "n_days", "n_negative_days", "sum_duration_bars"):
-                assert stats[f][i, s] == want[f], (i, s, f)
-            for f in ("max_drawdown", "net_profit", "total_profit", "total_loss", "sharpe_ratio", "sortino_ratio", "score"):
-                got, exp = float(stats[f][i, s]), float(want[f])
-                assert got == pytest.approx(exp, rel=1e-9, abs=1e-11) or (np.isnan(got) and np.isnan(exp)), (i, s, f, got, exp)
+    bank = np.stack([indicators_ref.rsi_bank(close[s], sweep.periods) for s in range(close.shape[0])])
+    want, _, _ = sim_oracle.population(close, bank, sweep.period_row, population,
+                                       sim_oracle.config_of(synth.EPOCH_2024_MINUTES, 1))
+    sim_oracle.assert_lanes(sweep.lane_stats(), want, "lanes")
 
 
 @pytest.mark.parametrize("mode,opts", [

@@ -41,20 +41,15 @@ def book_k(S):
     return BK_CAP // S
 
 
-# tolerances of the existing tests of the same outputs
-BOOK_RTOL, BOOK_ATOL = 1e-9, 1e-11       # test_gpu_book.py _compare
-CLASS_REL = 1e-9                         # test_gpu_regime.py _same
-# Day rows: test_gpu_overfitting.py holds them to rel 1e-12.  The device sums a day in warp-tree order within each
-# batch of 32, the reference in record order; both are within n * eps * sum |pnl| of the exact sum, and these buffers put
-# up to 1024 records of both signs into one day, so the 1e-12 is taken relative to the day's sum of |pnl|, not to the
-# sum itself (which can be much smaller).
+# Books are held to sim_oracle.assert_lanes as in test_gpu_book.py, classes to it without an absolute floor as in
+# test_gpu_regime.py.  Day rows: test_gpu_overfitting.py holds them to rel 1e-12.  The device sums a day in warp-tree
+# order within each batch of 32, the reference in record order; both are within n * eps * sum |pnl| of the exact sum, and
+# these buffers put up to 1024 records of both signs into one day, so the 1e-12 is taken relative to the day's sum of
+# |pnl|, not to the sum itself (which can be much smaller).
 ROW_REL = 1e-12
 
 EPOCH = 28_401_120                       # 2024-01-01T00:00Z in minutes
 MINUTE0 = EPOCH + 777                    # bar 0 is not on a midnight
-EXACT = ("n_records", "n_wins", "n_losses", "n_days", "n_negative_days", "sum_duration_bars")
-CLOSE = ("net_profit", "total_profit", "total_loss", "largest_profit", "largest_loss", "max_drawdown", "sharpe_ratio",
-         "sortino_ratio", "downside_deviation", "mean_daily_pnl", "win_rate", "profit_factor", "score")
 FIELDS = sim_oracle.STATS_FIELDS
 
 
@@ -384,31 +379,6 @@ def _is_lost(row, where):
     assert all(g[f] == 0.0 for f in FIELDS[1:-1] if f != "score") and g["trade_hash"] == 0, where
 
 
-def _book_same(got, want, where):
-    """test_gpu_book.py's _compare for one book."""
-    g = _fields(got)
-    for f in EXACT:
-        assert g[f] == want[f], (where, f, g[f], want[f])
-    assert g["trade_hash"] == int(want["trade_hash"]), (where, "trade_hash")
-    for f in CLOSE:
-        np.testing.assert_allclose(g[f], float(want[f]), rtol=BOOK_RTOL, atol=BOOK_ATOL, equal_nan=True,
-                                   err_msg=f"{where}: {f}")
-
-
-def _class_same(got, want, where):
-    """test_gpu_regime.py's _same for one class of one lane."""
-    g = _fields(got)
-    for f in EXACT:
-        assert g[f] == want[f], (where, f, g[f], want[f])
-    assert g["trade_hash"] == int(want["trade_hash"]), (where, "trade_hash")
-    for f in CLOSE:
-        x, w = g[f], float(want[f])
-        if math.isnan(w) or math.isinf(w) or w == 0.0:
-            assert x == w or (math.isnan(x) and math.isnan(w)), (where, f, x, w)
-        else:
-            assert abs(x - w) <= CLASS_REL * abs(w), (where, f, x, w)
-
-
 def _row_scale(words, pnl, cfg, N, D):
     """float64 [D]: each day's sum of |pnl| (the scale of ROW_REL)."""
     return rb.day_row(words, np.abs(pnl), cfg, N, D)
@@ -426,7 +396,7 @@ def check(case, out, where):
             assert math.isnan(out["fitness"][i])
         else:
             want = rb.book(case.lanes[i], pnls, case.cfg)
-            _book_same(out["book"][i], want, f"{where} book {i}")
+            sim_oracle.assert_lanes(_fields(out["book"][i]), want, f"{where} book {i}")
             assert out["fitness"][i] == out["book"][i][12] or np.isnan(out["fitness"][i]) and np.isnan(out["book"][i][12])
         # day rows, the book row as their sum over symbols in order
         rows = out["lane_pnl"][i]
@@ -448,7 +418,8 @@ def check(case, out, where):
                 continue
             want = rb.classes(case.lanes[i][s], pnls[s], case.labels[s], case.R, case.cfg)
             for r in range(case.R):
-                _class_same(out["classes"][r, i, s], want[r], f"{where} lane ({i}, {s}) class {r}")
+                sim_oracle.assert_lanes(_fields(out["classes"][r, i, s]), want[r], f"{where} lane ({i}, {s}) class {r}",
+                                        atol=0)
         # trip pnl, and the day row's sum against the net profit of the trips
         for s in range(S):
             w = f"{where} lane ({i}, {s})"
@@ -479,7 +450,7 @@ def test_single_symbol_book_is_its_one_class(torch_cuda):
     out = run(torch_cuda, case)
     for i in range(case.pop):
         book, cls = _fields(out["book"][i]), out["classes"][0, i, 0]
-        _class_same(cls, book, f"individual {i}")
+        sim_oracle.assert_lanes(_fields(cls), book, f"individual {i}", atol=0)
 
 
 def test_price_scales_leave_every_output_unchanged(torch_cuda):

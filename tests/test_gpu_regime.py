@@ -24,10 +24,7 @@ SOURCE = [0, 1, 0, 2, 0]
 QUIET = 4
 DENSE = dict(rsi_period=5, rsi_oversold=99, rsi_overbought=101, take_profit=0.0001, stop_loss=0.0001)
 NEVER = dict(rsi_period=14, rsi_oversold=0, rsi_overbought=100)
-COUNTS = ("n_records", "n_wins", "n_losses", "n_days", "sum_duration_bars")
-FLOATS = ("total_profit", "total_loss", "net_profit", "max_drawdown", "sharpe_ratio", "largest_profit", "largest_loss",
-          "score", "win_rate", "profit_factor", "sortino_ratio", "n_negative_days", "downside_deviation",
-          "mean_daily_pnl")
+ROW = {p: k for k, p in enumerate(PERIODS)}
 
 
 def _population(n=22, seed=11):
@@ -48,37 +45,16 @@ def _market(torch, n_bars, bar_minutes=1):
     return market, bank, close, bank.cpu().numpy()
 
 
-def _oracle_lanes(close, bank_h, population, cfg, periods=PERIODS, lanes=None):
-    """{(i, s): (event words, record pnl)} of the C oracle."""
+def check_classes(views, evs, pns, labels, R, cfg, where):
+    """Every class of every lane against regime_ref.class_stats of the oracle's records; float statistics to rel 1e-9 with
+    no absolute floor.  A failure names lane (i, s) by its flat index i S + s."""
     from oracle import sim_oracle
-    S, N = close.shape
-    row = {p: k for k, p in enumerate(periods)}
-    lanes = lanes or [(i, s) for i in range(len(population)) for s in range(S)]
-    out = {}
-    for i, s in lanes:
-        p = population[i]
-        _, ev, pn = sim_oracle.lane(close[s], bank_h[s, row[int(p.get("rsi_period", 14))]], p, cfg, event_cap=N + 2)
-        out[(i, s)] = (np.asarray(ev), np.asarray(pn))
-    return out
-
-
-def _same(got, want, where):
-    for k in COUNTS:
-        assert got[k] == want[k], (where, k, got[k], want[k])
-    assert int(got["trade_hash"]) == int(want["trade_hash"]), (where, "trade_hash")
-    for k in FLOATS:
-        g, w = float(got[k]), float(want[k])
-        if np.isnan(w) or np.isinf(w) or w == 0.0:
-            assert g == w or (np.isnan(g) and np.isnan(w)), (where, k, g, w)
-        else:
-            assert abs(g - w) <= 1e-9 * abs(w), (where, k, g, w)
-
-
-def _check_classes(views, oracle, labels, R, cfg, where):
-    for (i, s), (ev, pn) in oracle.items():
-        want = regime_ref.class_stats(ev, pn, labels[s if labels.shape[0] > 1 else 0], R, cfg)
-        for r in range(R):
-            _same({k: views[r][k][i, s] for k in views[r]}, want[r], f"{where} lane ({i}, {s}) class {r}")
+    S = len(evs[0])
+    want = [regime_ref.class_stats(evs[i][s], pns[i][s], labels[s if labels.shape[0] > 1 else 0], R, cfg)
+            for i in range(len(evs)) for s in range(S)]
+    for r in range(R):
+        sim_oracle.assert_lanes({k: v.reshape(-1) for k, v in views[r].items()}, [w[r] for w in want],
+                                f"{where} class {r}", atol=0)
 
 
 def _labellings(S, N, rng):
@@ -111,13 +87,14 @@ def test_class_stats_match_the_oracle(torch_cuda, case, bar_minutes, n_bars, gap
     if gap is not None:
         sweep.set_gap(*gap)
         cfg.gap_bar, cfg.gap_minutes = gap
-    oracle = _oracle_lanes(close, bank_h, pop, cfg)
-    assert any(len(ev) == 0 for ev, _ in oracle.values()) and max(len(ev) for ev, _ in oracle.values()) > 100
+    _, evs, pns = sim_oracle.population(close, bank_h, ROW, pop, cfg, event_cap=market.N + 2)
+    lengths = [len(ev) for lanes in evs for ev in lanes]
+    assert min(lengths) == 0 and max(lengths) > 100
     rng = np.random.default_rng(bar_minutes + n_bars)
     for name, labels, R in _labellings(market.S, market.N, rng):
         out, views = sweep.class_stats(pop, torch_cuda.from_numpy(labels).cuda(), R)
         assert tuple(out.shape) == (R, len(pop), market.S, 20)
-        _check_classes(views, oracle, labels, R, cfg, f"{case} / {name}")
+        check_classes(views, evs, pns, labels, R, cfg, f"{case} / {name}")
 
 
 def test_last_bar_entry_and_force_close(torch_cuda):
@@ -133,28 +110,26 @@ def test_last_bar_entry_and_force_close(torch_cuda):
         pytest.fail("no length in 3000..3039 puts an entry on the last bar")
     cfg = sim_oracle.config_of(market.minute0, 1)
     pop = _population()
-    oracle = _oracle_lanes(close, bank_h, pop, cfg)
+    _, evs, pns = sim_oracle.population(close, bank_h, ROW, pop, cfg, event_cap=N + 2)
     labels = np.zeros((market.S, N), np.uint8)
     labels[:, -1] = 1                                   # the last bar's entry and force-close form class 1
     labels[:, N // 2:N - 1] = 2
     _, views = PopulationSweep.from_bank(market, bank, PERIODS).class_stats(pop, torch_cuda.from_numpy(labels).cuda(), 3)
-    _check_classes(views, oracle, labels, 3, cfg, "last bar")
+    check_classes(views, evs, pns, labels, 3, cfg, "last bar")
     assert views[1]["n_records"].max() == 2
 
 
 def test_invariants_shared_rows_and_lost_records(torch_cuda):
     from ai_crypto_trader_b200 import _lib
     from ai_crypto_trader_b200.sweep import PopulationSweep
+    from oracle import sim_oracle
     market, bank, close, _ = _market(torch_cuda, 30_000)
     pop = _population()
     sweep = PopulationSweep.from_bank(market, bank, PERIODS)
     S, N = market.S, market.N
     # R = 1, every label 0: the lane's own stats
     _, views = sweep.class_stats(pop, torch_cuda.zeros((S, N), dtype=torch_cuda.uint8, device="cuda"), 1)
-    lanes = sweep.lane_stats()
-    for i in range(len(pop)):
-        for s in range(S):
-            _same({k: views[0][k][i, s] for k in views[0]}, {k: lanes[k][i, s] for k in lanes}, f"R=1 lane ({i}, {s})")
+    sim_oracle.assert_lanes(views[0], sweep.lane_stats(), "R=1", atol=0)
     # a partition (every label < R): class sums of the counts are the lane's, net profit within rounding
     rng = np.random.default_rng(3)
     labels = torch_cuda.from_numpy(rng.integers(0, 6, (S, N)).astype(np.uint8)).cuda()
@@ -283,14 +258,12 @@ def test_service_end_to_end(torch_cuda):
     assert np.array_equal(labels[0], labels[1])                      # PRIMARY_TRADING_SYMBOL's labels everywhere
     cfg = sim_oracle.config_of(market.minute0, 1)
     bank_h = svc.sweep.bank.cpu().numpy()
-    oracle = _oracle_lanes(close, bank_h, pop, cfg, periods=svc.sweep.periods)
+    lanes, evs, pns = sim_oracle.population(close, bank_h, svc.sweep.period_row, pop, cfg, event_cap=market.N + 2)
     seen = set()
     for i, p in enumerate(perf):
-        lanes = [sim_oracle.lane(close[s], bank_h[s, svc.sweep.period_row[pop[i]["rsi_period"]]], pop[i], cfg,
-                                 event_cap=market.N + 2)[0] for s in range(market.S)]
         for k in ("sharpe_ratio", "win_rate", "max_drawdown", "profit_factor"):
-            assert p[k] == pytest.approx(np.mean([float(l[k]) for l in lanes]), rel=1e-9), (i, k)
-        classes = [regime_ref.class_stats(*oracle[(i, s)], labels[s], 4, cfg) for s in range(market.S)]
+            assert p[k] == pytest.approx(np.mean(lanes[k][i]), rel=1e-9), (i, k)
+        classes = [regime_ref.class_stats(evs[i][s], pns[i][s], labels[s], 4, cfg) for s in range(market.S)]
         want = {}
         for r, name in enumerate(SCORED_REGIMES):
             n = sum(c[r]["n_records"] for c in classes)
@@ -345,4 +318,5 @@ def test_full_size_partition_and_oracle_slice(torch_cuda):
         _, ev, pn = sim_oracle.lane(close[s], row, pop[i], cfg, event_cap=N + 2)
         want = regime_ref.class_stats(ev, pn, lab[s], 5, cfg)
         for r in range(5):
-            _same({k: views[r][k][i, s] for k in views[r]}, want[r], f"full size lane ({i}, {s}) class {r}")
+            sim_oracle.assert_lanes({k: v[i, s] for k, v in views[r].items()}, want[r],
+                                    f"full size lane ({i}, {s}) class {r}", atol=0)

@@ -124,9 +124,8 @@ def test_sweep_other_optimisation_goals_match_reference_scores(torch_cuda, sim_g
 
 @pytest.mark.parametrize("n_bars,pop,n_sym", [(1, 4, 1), (31, 8, 2), (33, 8, 1), (1000, 64, 3), (50001, 96, 2)])
 def test_sweep_vs_c_oracle_random_populations(torch_cuda, n_bars, pop, n_sym):
-    from ai_crypto_trader_b200 import _lib, synth
+    from ai_crypto_trader_b200 import synth
     from ai_crypto_trader_b200.sweep import MarketData, PopulationSweep
-    from oracle import indicators_ref, sim_oracle
     ohlcv = synth.synth_ohlcv(n_sym, n_bars, first_symbol=5)
     market = MarketData(ohlcv)
     cap = 512
@@ -136,25 +135,8 @@ def test_sweep_vs_c_oracle_random_populations(torch_cuda, n_bars, pop, n_sym):
     population[0].update(rsi_oversold=35, rsi_overbought=65, rsi_period=5, take_profit=1, stop_loss=1)
     population[1].update(take_profit=0.5, stop_loss=0.5)
     fitness = sweep.evaluate(population)
-    stats, events = sweep.lane_stats(), sweep.events()
-    cfg = sim_oracle.config_of(market.minute0, 1)
-    scores = np.zeros((pop, n_sym))
-    for s in range(n_sym):
-        bank = indicators_ref.rsi_bank(ohlcv[3, s], sweep.periods)
-        for i, p in enumerate(population):
-            want, ev, _ = sim_oracle.lane(ohlcv[3, s], bank[sweep.period_row[p["rsi_period"]]], p, cfg, event_cap=cap)
-            assert int(stats["n_records"][i, s]) == int(want["n_records"]), (i, s)
-            assert int(stats["trade_hash"][i, s]) == int(want["trade_hash"]), (i, s)
-            assert np.array_equal(events[i, s, :len(ev)], ev), (i, s)
-            for f in ("n_wins", "n_losses", "n_days", "sum_duration_bars"):
-                assert stats[f][i, s] == want[f], (i, s, f)
-            for f in ("total_profit", "total_loss", "net_profit", "max_drawdown", "sharpe_ratio", "largest_profit",
-                      "largest_loss", "win_rate", "profit_factor", "score", "sortino_ratio", "downside_deviation",
-                      "mean_daily_pnl"):
-                assert stats[f][i, s] == pytest.approx(float(want[f]), rel=1e-9, abs=1e-11), (i, s, f)
-            assert stats["n_negative_days"][i, s] == want["n_negative_days"], (i, s)
-            scores[i, s] = want["score"]
-    np.testing.assert_allclose(fitness, scores.mean(axis=1), rtol=1e-9, atol=1e-11)
+    want = _check_lanes_vs_oracle(sweep, population, ohlcv, cap)
+    np.testing.assert_allclose(fitness, want["score"].mean(axis=1), rtol=1e-9, atol=1e-11)
 
 
 def test_simulate_trades_dropin_returns_reference_records(torch_cuda, sim_golden):
@@ -200,25 +182,15 @@ def test_evolution_service_runs_ga_on_gpu(torch_cuda):
 
 
 def _check_lanes_vs_oracle(sweep, population, ohlcv, cap):
+    """The sweep's first len(population) lanes and their event words against the C oracle fed the float64 restatement's
+    RSI rows -> the oracle's stats."""
     from oracle import indicators_ref, sim_oracle
-    stats, events = sweep.lane_stats(), sweep.events()
-    cfg = sim_oracle.config_of(sweep.market.minute0, 1)
-    n_sym = ohlcv.shape[1]
-    for s in range(n_sym):
-        bank = indicators_ref.rsi_bank(ohlcv[3, s], sweep.periods)
-        for i, p in enumerate(population):
-            want, ev, _ = sim_oracle.lane(ohlcv[3, s], bank[sweep.period_row[p["rsi_period"]]], p, cfg, event_cap=cap)
-            assert int(stats["n_records"][i, s]) == int(want["n_records"]), (i, s)
-            assert int(stats["trade_hash"][i, s]) == int(want["trade_hash"]), (i, s)
-            if events is not None:
-                assert np.array_equal(events[i, s, :len(ev)], ev), (i, s)
-            for f in ("n_wins", "n_losses", "n_days", "sum_duration_bars"):
-                assert stats[f][i, s] == want[f], (i, s, f)
-            for f in ("total_profit", "total_loss", "net_profit", "max_drawdown", "sharpe_ratio", "largest_profit",
-                      "largest_loss", "win_rate", "profit_factor", "score", "sortino_ratio", "downside_deviation",
-                      "mean_daily_pnl"):
-                assert stats[f][i, s] == pytest.approx(float(want[f]), rel=1e-9, abs=1e-11), (i, s, f)
-            assert stats["n_negative_days"][i, s] == want["n_negative_days"], (i, s)
+    bank = np.stack([indicators_ref.rsi_bank(ohlcv[3, s], sweep.periods) for s in range(ohlcv.shape[1])])
+    want, want_ev, _ = sim_oracle.population(ohlcv[3], bank, sweep.period_row, population,
+                                             sim_oracle.config_of(sweep.market.minute0, 1), event_cap=cap)
+    sim_oracle.assert_lanes({f: v[:len(population)] for f, v in sweep.lane_stats().items()}, want, "lanes")
+    sim_oracle.assert_events(sweep.events(), want_ev, "lanes")
+    return want
 
 
 @pytest.mark.parametrize("n_bars,opts", [
@@ -410,11 +382,10 @@ def test_evaluate_edge_populations(torch_cuda):
         assert sweep.evaluate([]).shape == (0,)
         one = synth.random_population(1, seed=n_bars)
         f = sweep.evaluate(one)
-        bank = indicators_ref.rsi_bank(ohlcv[3, 0], sweep.periods)
-        want, _, _ = sim_oracle.lane(ohlcv[3, 0], bank[sweep.period_row[one[0]["rsi_period"]]], one[0],
-                                     sim_oracle.config_of(market.minute0, 1))
-        assert f.shape == (1,) and f[0] == pytest.approx(float(want["score"]), rel=1e-9, abs=1e-12)
-        assert int(sweep.lane_stats()["n_records"][0, 0]) == int(want["n_records"])
+        bank = indicators_ref.rsi_bank(ohlcv[3, 0], sweep.periods)[None]
+        want, _, _ = sim_oracle.population(ohlcv[3], bank, sweep.period_row, one, sim_oracle.config_of(market.minute0, 1))
+        assert f.shape == (1,) and f[0] == pytest.approx(float(want["score"][0, 0]), rel=1e-9, abs=1e-12)
+        sim_oracle.assert_lanes(sweep.lane_stats(), want, f"{n_bars} bars", atol=1e-12)
 
 
 def test_multi_timeframe_bank_and_sweep(torch_cuda):
@@ -453,17 +424,12 @@ def test_multi_timeframe_bank_and_sweep(torch_cuda):
                     assert np.array_equal(np.isnan(got), np.isnan(ref)), (s, i)
                     neq = (got != ref) & ~np.isnan(ref)
                     assert int(neq.sum()) <= max(2, int(2e-6 * ref.size)), (s, i, int(neq.sum()))   # double-rounding ties only
-            want = np.zeros((POP, S), dtype=sim_oracle.STATS_DTYPE)
-            for s in range(S):
-                for i, p in enumerate(population):
-                    r = rows[s, p["rsi_timeframe"]][sweep.period_row[p["rsi_period"]]]
-                    want[i, s] = sim_oracle.lane(ohlcv[3, s], r, p, cfg)[0]
+            rows = np.stack([np.concatenate([rows[s, i] for i in range(3)]) for s in range(S)])
+            row_of = lambda p: p["rsi_timeframe"] * P + sweep.period_row[p["rsi_period"]]
+            want, _, _ = sim_oracle.population(ohlcv[3], rows, row_of, population, cfg)
         for _ in range(2):
             fit = sweep.evaluate(population)
-        st = sweep.lane_stats()
-        assert np.array_equal(st["n_records"], want["n_records"]), mode
-        assert np.array_equal(st["trade_hash"], want["trade_hash"]), mode
-        np.testing.assert_allclose(st["score"], want["score"], rtol=1e-9, atol=1e-11, equal_nan=True)
+        sim_oracle.assert_lanes(sweep.lane_stats(), want, mode)
         np.testing.assert_allclose(fit, want["score"].mean(axis=1), rtol=1e-9, atol=1e-11, equal_nan=True)
         if mode == "tiled":
             assert sweep.last_invalid_lanes == 0             # packed by bank row: no warp reads more than two rows

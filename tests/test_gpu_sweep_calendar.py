@@ -30,9 +30,6 @@ from gpu_fixtures import torch_cuda
 pytestmark = pytest.mark.gpu
 
 GOLD = Path(__file__).parent / "golden"
-EXACT = ("n_records", "trade_hash", "n_wins", "n_losses", "n_days", "n_negative_days", "sum_duration_bars")
-CLOSE = ("net_profit", "total_profit", "total_loss", "max_drawdown", "sharpe_ratio", "sortino_ratio", "downside_deviation",
-         "mean_daily_pnl", "score")
 SCHEDULES = {
     "fused": dict(mode="fused"),
     "chunked": dict(mode="chunked", chunk_options=dict(target_events=300, max_chunks=64, warm=256, pool_scale=4.0)),
@@ -48,31 +45,6 @@ DENSE = dict(rsi_period=5, rsi_oversold=99, rsi_overbought=101, take_profit=0.00
 
 
 # -- shared helpers ------------------------------------------------------------------------------------------------------
-def _oracle(close, bank, period_row, population, cfg, event_cap=0):
-    """Oracle stats [pop][S] (and event words per lane when event_cap > 0) on the fp32 rows the sweep reads."""
-    from oracle import sim_oracle
-    S = close.shape[0]
-    out = np.zeros((len(population), S), dtype=sim_oracle.STATS_DTYPE)
-    events = {}
-    for i, p in enumerate(population):
-        for s in range(S):
-            out[i, s], ev, _ = sim_oracle.lane(close[s], bank[s, period_row[int(p.get("rsi_period", 14))]], p, cfg, event_cap)
-            if event_cap:
-                events[i, s] = ev
-    return out, events
-
-
-def _compare(st, want, where, events=None, want_events=None):
-    for f in EXACT:
-        np.testing.assert_array_equal(st[f], want[f], err_msg=f"{where}: {f}")
-    for f in CLOSE:
-        np.testing.assert_allclose(np.asarray(st[f], dtype=np.float64), want[f], rtol=1e-9, atol=1e-11, equal_nan=True,
-                                   err_msg=f"{where}: {f}")
-    if events is not None:
-        for (i, s), ev in want_events.items():
-            np.testing.assert_array_equal(events[i, s, :len(ev)], ev, err_msg=f"{where}: events of lane {(i, s)}")
-
-
 def _sweeps(market, bank, periods, goals=None, advanced=False, event_cap=0, gap=(0, 0)):
     """One PopulationSweep per schedule over the same bank."""
     from ai_crypto_trader_b200.sweep import PopulationSweep
@@ -159,8 +131,8 @@ def _seam_case(torch, gap_bar, gap_minutes, m0_mod, bar_minutes, minute0=None):
     base = PopulationSweep(market, mode="fused")
     bank = base.bank.cpu().numpy()
     cfg = sim_oracle.config_of(minute0, bar_minutes, gap_bar=gap_bar, gap_minutes=gap_minutes)
-    want, want_ev = _oracle(close, bank, base.period_row, population, cfg, CAP)
-    plain, _ = _oracle(close, bank, base.period_row, population, sim_oracle.config_of(minute0, bar_minutes))
+    want, want_ev, _ = sim_oracle.population(close, bank, base.period_row, population, cfg, CAP)
+    plain, _, _ = sim_oracle.population(close, bank, base.period_row, population, sim_oracle.config_of(minute0, bar_minutes))
     sweeps = _sweeps(market, base.bank, base.periods, event_cap=CAP, gap=(gap_bar, gap_minutes))
     where = f"gap_bar {gap_bar}, gap_minutes {gap_minutes}, minute0 {minute0}, bar_minutes {bar_minutes}"
     failed = []                       # every schedule is checked, so that a failure names all the schedules it shows on
@@ -168,7 +140,8 @@ def _seam_case(torch, gap_bar, gap_minutes, m0_mod, bar_minutes, minute0=None):
         fit = sw.evaluate(population)
         st = sw.lane_stats()
         try:
-            _compare(st, want, f"{name}, {where}", sw.events(), want_ev)
+            sim_oracle.assert_lanes(st, want, f"{name}, {where}")
+            sim_oracle.assert_events(sw.events(), want_ev, f"{name}, {where}")
             np.testing.assert_allclose(fit, (want["score"][:, 0] + want["score"][:, 1]) / 2, rtol=1e-9, atol=1e-11,
                                        equal_nan=True, err_msg=f"{name}: fitness")
         except AssertionError as e:
@@ -184,7 +157,7 @@ def _seam_case(torch, gap_bar, gap_minutes, m0_mod, bar_minutes, minute0=None):
 def test_glued_series_match_oracle_on_every_schedule(torch_cuda, gap_bar, gap_minutes, m0_mod, bar_minutes, seam_in_day):
     close, population, want, want_ev, plain, minute0 = _seam_case(torch_cuda, gap_bar, gap_minutes, m0_mod, bar_minutes)
     # the dense lane really records on both sides of the seam, across 128-record steps
-    bars = want_ev[0, 0] & 0x3FFFFFFF
+    bars = want_ev[0][0] & 0x3FFFFFFF
     n0 = int(want["n_records"][0, 0])
     assert n0 <= CAP and np.any(bars >= gap_bar)
     if gap_bar > 1:
@@ -307,7 +280,7 @@ def test_score_rules_match_oracle_on_time_chunked_schedules(torch_cuda, score_ma
     saw_nan = saw_inf = False
     for goals, advanced in sets:
         cfg = sim_oracle.config_of(market.minute0, 1, goals, advanced=advanced)
-        want, _ = _oracle(close, bank, period_row, population, cfg)
+        want, _, _ = sim_oracle.population(close, bank, period_row, population, cfg)
         if goals is None:
             # the edge lanes are what they claim to be
             st = want[-n_edge:]
@@ -322,7 +295,7 @@ def test_score_rules_match_oracle_on_time_chunked_schedules(torch_cuda, score_ma
         for name, sw in _sweeps(market, bank_dev, periods, goals=goals, advanced=advanced).items():
             fit = sw.evaluate(population)
             where = f"{name}, goals {goals}, advanced {advanced}"
-            _compare(sw.lane_stats(), want, where)
+            sim_oracle.assert_lanes(sw.lane_stats(), want, where)
             np.testing.assert_allclose(fit, want_fit, rtol=1e-9, atol=1e-11, equal_nan=True, err_msg=f"{where}: fitness")
             _check_path(name, sw, population, 2)
     assert saw_nan and saw_inf
@@ -362,17 +335,16 @@ def test_cross_validation_on_chunked_training_folds_matches_oracle(torch_cuda):
                                          sweep.periods, mode="auto").plan(population) is None
         gap = (a, b - a) if 0 < a and b < N else (0, 0)
         m0 = market.minute0 + (b if a == 0 else 0)
-        want_tr, _ = _oracle(tr_close, tr_bank, sweep.period_row, population,
-                             sim_oracle.config_of(m0, 1, gap_bar=gap[0], gap_minutes=gap[1]))
-        want_te, _ = _oracle(close[:, a:b], bank[:, :, a:b], sweep.period_row, population,
-                             sim_oracle.config_of(market.minute0 + a, 1))
+        want_tr, _, _ = sim_oracle.population(tr_close, tr_bank, sweep.period_row, population,
+                                              sim_oracle.config_of(m0, 1, gap_bar=gap[0], gap_minutes=gap[1]))
+        want_te, _, _ = sim_oracle.population(close[:, a:b], bank[:, :, a:b], sweep.period_row, population,
+                                              sim_oracle.config_of(market.minute0 + a, 1))
         if gap[0]:
-            plain, _ = _oracle(tr_close, tr_bank, sweep.period_row, population, sim_oracle.config_of(m0, 1))
+            plain, _, _ = sim_oracle.population(tr_close, tr_bank, sweep.period_row, population, sim_oracle.config_of(m0, 1))
             assert np.any(plain["sharpe_ratio"] != want_tr["sharpe_ratio"]), f"fold {f}: the gap changes nothing"
         for side, want in (("train", want_tr), ("test", want_te)):
-            np.testing.assert_array_equal(cv[f"{side}_n_records"][f], want["n_records"], err_msg=f"fold {f} {side}")
-            for k in ("sharpe_ratio", "max_drawdown", "win_rate", "profit_factor", "score"):
-                np.testing.assert_allclose(cv[f"{side}_{k}"][f], want[k], rtol=1e-9, atol=1e-11, equal_nan=True,
-                                           err_msg=f"fold {f} {side} {k}")
+            cv_close = ("sharpe_ratio", "max_drawdown", "win_rate", "profit_factor", "score")    # the fields a fold reports
+            sim_oracle.assert_lanes({k: cv[f"{side}_{k}"][f] for k in ("n_records",) + cv_close}, want,
+                                    f"fold {f} {side}", exact=("n_records",), close=cv_close)
             np.testing.assert_allclose(cv[f"{side}_return_pct"][f], want["net_profit"] / 10000.0 * 100, rtol=1e-9,
                                        atol=1e-11, err_msg=f"fold {f} {side} return_pct")

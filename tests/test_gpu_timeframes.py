@@ -28,7 +28,6 @@ from test_oracle_indicators import DAY0, grid_cases
 pytestmark = pytest.mark.gpu
 
 S = 3
-EXACT = ("n_records", "trade_hash")
 SCHEDULES = {
     "fused": dict(mode="fused"),
     "chunked": dict(mode="chunked", chunk_options=dict(target_events=300, max_chunks=64, warm=256, pool_scale=4.0)),
@@ -140,12 +139,8 @@ def mtf(request, torch_cuda):
             c.rows[s, i * P:(i + 1) * P] = indicators_ref.rsi_rows_on_timeframe(c.ohlcv[3, s], c.minute0, k, PERIODS,
                                                                                 bar_minutes=c.bar)
     c.population = _population(len(c.timeframes))
-    cfg = sim_oracle.config_of(c.minute0, c.bar)
-    c.want = np.zeros((len(c.population), c.S), dtype=sim_oracle.STATS_DTYPE)
-    for s in range(c.S):
-        for i, p in enumerate(c.population):
-            row = p["rsi_timeframe"] * P + PERIODS.index(p["rsi_period"])
-            c.want[i, s] = sim_oracle.lane(c.ohlcv[3, s], c.rows[s, row], p, cfg)[0]
+    row_of = lambda p: p["rsi_timeframe"] * P + PERIODS.index(p["rsi_period"])
+    c.want, _, _ = sim_oracle.population(c.ohlcv[3], c.rows, row_of, c.population, sim_oracle.config_of(c.minute0, c.bar))
     return c
 
 
@@ -176,6 +171,7 @@ def test_multi_timeframe_bank_rows(mtf):
 @pytest.mark.parametrize("schedule", sorted(SCHEDULES))
 def test_multi_timeframe_lanes_against_the_c_oracle(mtf, schedule):
     from ai_crypto_trader_b200.sweep import PopulationSweep
+    from oracle import sim_oracle
     c = mtf
     opt = SCHEDULES[schedule]
     sweep = PopulationSweep(_market(c), rsi_periods=PERIODS, timeframes=c.timeframes, mode=opt["mode"],
@@ -190,11 +186,7 @@ def test_multi_timeframe_lanes_against_the_c_oracle(mtf, schedule):
     sweep._zones_if_amortised = spy
     for _ in range(2 if schedule == "tiled" else 1):
         fit = sweep.evaluate(c.population)
-    st = sweep.lane_stats()
-    for f in EXACT:
-        np.testing.assert_array_equal(st[f], c.want[f], err_msg=f"{c.name} {schedule}: {f}")
-    np.testing.assert_allclose(st["score"], c.want["score"], rtol=1e-9, atol=1e-11, equal_nan=True,
-                               err_msg=f"{c.name} {schedule}: score")
+    sim_oracle.assert_lanes(sweep.lane_stats(), c.want, f"{c.name} {schedule}")
     np.testing.assert_allclose(fit, c.want["score"].mean(axis=1), rtol=1e-9, atol=1e-11, equal_nan=True)
     plans = sweep._last_plans
     if schedule == "fused":

@@ -64,13 +64,14 @@ def test_trip_pnl_matches_c_oracle_on_tiled_sweep(torch_cuda):
     pop[2].update(rsi_oversold=35, rsi_overbought=65, rsi_period=5, take_profit=1, stop_loss=1)       # always trading
     trip, n_trips, fee = (t.cpu().numpy() for t in sweep.trade_pnl(pop))
     assert sweep.plan(pop) is not None and type(sweep.plan(pop)[0]).__name__ == "TilePlan"
-    cfg = sim_oracle.config_of(market.minute0, 1)
+    bank = np.stack([indicators_ref.rsi_bank(ohlcv[3, s], sweep.periods) for s in range(S)])
+    want, events, pnls = sim_oracle.population(ohlcv[3], bank, sweep.period_row, pop, sim_oracle.config_of(market.minute0, 1),
+                                               event_cap=N + 1)
     sides = set()
     for s in range(S):
-        bank = indicators_ref.rsi_bank(ohlcv[3, s], sweep.periods)
         for i, p in enumerate(pop):
-            want, ev, pnl = sim_oracle.lane(ohlcv[3, s], bank[sweep.period_row[p["rsi_period"]]], p, cfg, event_cap=N + 1)
-            T = int(want["n_records"]) // 2
+            ev, pnl = events[i][s], pnls[i][s]
+            T = int(want["n_records"][i, s]) // 2
             assert n_trips[i, s] == T, (i, s)
             assert np.array_equal(trip[i, s, :T], pnl[1::2]), (i, s)
             assert fee[i, s] == 10000 * (min(p.get("max_position_size", 5), 20) / 100) * 0.001
@@ -194,16 +195,16 @@ def test_monte_carlo_population_matches_oracle_on_sampled_lanes(torch_cuda):
     ses = StrategyEvaluationSystem(config={})
     out = ses.monte_carlo_population(pop, market, sweep=sweep, num_simulations=M, seed=5)
     assert out["var"].shape == (P, S) and out["percentile_equity"].shape == (P, S, 9)
-    cfg = sim_oracle.config_of(market.minute0, 1)
+    bank = np.stack([indicators_ref.rsi_bank(ohlcv[3, s], sweep.periods) for s in range(S)])
+    want, _, pnls = sim_oracle.population(ohlcv[3], bank, sweep.period_row, pop, sim_oracle.config_of(market.minute0, 1),
+                                          event_cap=N + 1)
     for s in range(S):
-        bank = indicators_ref.rsi_bank(ohlcv[3, s], sweep.periods)
         for i in range(s, P, 7):
             p = pop[i]
-            want, _, pnl = sim_oracle.lane(ohlcv[3, s], bank[sweep.period_row[p["rsi_period"]]], p, cfg, event_cap=N + 1)
-            trips = pnl[1::2]
+            trips = pnls[i][s][1::2]
             fee = 10000 * (min(p.get("max_position_size", 5), 20) / 100) * 0.001
             assert out["num_trades"][i, s] == len(trips)
-            assert out["original_max_drawdown"][i, s] == pytest.approx(float(want["max_drawdown"]), rel=1e-9, abs=1e-12)
+            assert out["original_max_drawdown"][i, s] == pytest.approx(float(want["max_drawdown"][i, s]), rel=1e-9, abs=1e-12)
             finals, maxdd = R.simulate(fee, trips, M, 5, "bootstrap", lane_id=i * S + s)
             st = R.statistics(finals, maxdd, 10000.0, 0.95)
             np.testing.assert_array_equal(out["percentile_equity"][i, s],

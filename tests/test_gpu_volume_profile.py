@@ -10,9 +10,9 @@
 import numpy as np
 import pytest
 
-import regime_ref
 import volume_profile_ref as ref
 from gpu_fixtures import torch_cuda
+from test_gpu_regime import check_classes
 from test_volume_profile_host import CASES, IDS, _close, frame_of
 
 pytestmark = pytest.mark.gpu
@@ -161,21 +161,9 @@ def test_class_stats_by_zone(torch_cuda):
     _, views = sweep.class_stats(pop, labels, 6)
     lab = labels.cpu().numpy()
     cfg = sim_oracle.config_of(market.minute0, 1)
-    row = {p: k for k, p in enumerate(periods)}
-    n_records = 0
-    for i, p in enumerate(pop):
-        for s in range(market.S):
-            _, ev, pn = sim_oracle.lane(x[3, s], bank_h[s, row[p["rsi_period"]]], p, cfg, event_cap=market.N + 2)
-            want = regime_ref.class_stats(np.asarray(ev), np.asarray(pn), lab[s], 6, cfg)
-            for r in range(6):
-                got = {k: views[r][k][i, s] for k in views[r]}
-                n_records += int(got["n_records"])
-                for k in ("n_records", "n_wins", "n_losses", "n_days", "sum_duration_bars"):
-                    assert got[k] == want[r][k], (i, s, r, k)
-                assert int(got["trade_hash"]) == int(want[r]["trade_hash"]), (i, s, r)
-                for k in ("net_profit", "max_drawdown", "sharpe_ratio", "score"):
-                    g, w = float(got[k]), float(want[r][k])
-                    assert g == w or (np.isnan(g) and np.isnan(w)) or abs(g - w) <= 1e-9 * abs(w), (i, s, r, k, g, w)
+    _, evs, pns = sim_oracle.population(x[3], bank_h, sweep.period_row, pop, cfg, event_cap=market.N + 2)
+    check_classes(views, evs, pns, lab, 6, cfg, "labels")
+    n_records = sum(int(v["n_records"].sum()) for v in views)
     assert n_records > 100
 
 

@@ -72,14 +72,10 @@ def test_single_symbol_book_is_the_oracle_lane():
     from oracle import sim_oracle
     close, bank, pop, minute0 = _case(4000, 7)
     cfg = sim_oracle.config_of(minute0, 7)
-    for p in pop:
-        want, ev, pn = sim_oracle.lane(close[1], bank[1, PERIODS.index(p["rsi_period"])], p, cfg, event_cap=4002)
-        got = book_ref.book([ev], [pn], cfg)
-        for f in sim_oracle.STATS_FIELDS:
-            if f in ("n_records", "trade_hash", "n_wins", "n_losses", "n_days", "n_negative_days", "sum_duration_bars"):
-                assert got[f] == want[f], f
-            else:
-                assert got[f] == pytest.approx(float(want[f]), rel=1e-12, abs=1e-12, nan_ok=True), f
+    want, evs, pns = sim_oracle.population(close[1:2], bank[1:2], {p: i for i, p in enumerate(PERIODS)}, pop, cfg,
+                                           event_cap=4002)
+    got = [book_ref.book(ev, pn, cfg) for ev, pn in zip(evs, pns)]
+    sim_oracle.assert_lanes(got, want[:, 0], "one-symbol books", rtol=1e-12, atol=1e-12)
 
 
 def _book_args(S=10, N=200_000, pop=64, cap=4096, minute0=0, bar_minutes=1, price=DEV):

@@ -21,18 +21,16 @@ def test_oracle_lanes_keep_the_invariants_and_the_pricer_is_exact(bar_minutes, g
     cfg = sim_oracle.config_of(limits.MINUTE0, bar_minutes)
     if gap is not None:
         cfg.gap_bar, cfg.gap_minutes = gap
-    n_seen = 0
-    for s in range(S):
-        rsi = rng.uniform(0.0, 100.0, N).astype(np.float32)
-        for p in pop:
-            st, ev, pn = sim_oracle.lane(close[s], rsi, p, cfg, event_cap=N + 2)
-            assert len(ev) == int(st["n_records"])
+    rsi = np.stack([rng.uniform(0.0, 100.0, N).astype(np.float32)[None] for _ in range(S)])      # one row per symbol
+    stats, evs, pns = sim_oracle.population(close, rsi, lambda p: 0, pop, cfg, event_cap=N + 2)
+    for i, p in enumerate(pop):
+        for s in range(S):
+            ev, pn = evs[i][s], pns[i][s]
+            assert len(ev) == int(stats["n_records"][i, s])
             rb.check_lane(ev, N)
-            size = sim_oracle.params_of(p).position_size
-            got = rb.price_lane(ev, close[s], size)
+            got = rb.price_lane(ev, close[s], sim_oracle.params_of(p).position_size)
             assert np.array_equal(got.view(np.uint64), np.asarray(pn, dtype=np.float64).view(np.uint64)), (s, p)
-            n_seen += len(ev)
-    assert n_seen > 10_000                    # the dense lanes trade on most bars
+    assert int(stats["n_records"].sum()) > 10_000                    # the dense lanes trade on most bars
 
 
 @pytest.mark.parametrize("name", list(limits.CASES))

@@ -32,17 +32,12 @@ def _check(sweep, population, idx, close, bank):
     import book_ref
     got = sweep.book_stats()
     cfg = sim_oracle.config_of(sweep.market.minute0, sweep.market.bar_minutes)
-    worst, exact = 0.0, True
-    for i in idx:
-        p = population[i]
-        evs, pns = [], []
-        for s in range(close.shape[0]):
-            _, ev, pn = sim_oracle.lane(close[s], bank[s, sweep.period_row[int(p["rsi_period"])]], p, cfg,
+    _, evs, pns = sim_oracle.population(close, bank, sweep.period_row, [population[i] for i in idx], cfg,
                                         event_cap=close.shape[1] + 2)
-            evs.append(ev)
-            pns.append(pn)
-        want = book_ref.book(evs, pns, cfg)
-        for f in ("n_records", "trade_hash", "n_wins", "n_losses", "n_days", "n_negative_days", "sum_duration_bars"):
+    worst, exact = 0.0, True
+    for i, ev, pn in zip(idx, evs, pns):
+        want = book_ref.book(ev, pn, cfg)
+        for f in sim_oracle.EXACT_FIELDS:
             exact &= bool(got[f][i] == want[f])
         for f in ("net_profit", "max_drawdown", "sharpe_ratio", "sortino_ratio", "score"):
             a, b = float(got[f][i]), float(want[f])
