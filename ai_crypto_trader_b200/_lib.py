@@ -228,6 +228,9 @@ EVENT_BAR_MASK = 0x3FFFFFFF
 
 TRADE_MC_METHODS = {"bootstrap": 0, "shuffle": 1}     # B200BT_TRADE_MC_*
 
+SEGMENT_DTYPE = [("start", "<i8"), ("end", "<i8"), ("individual", "<i4"), ("reserved", "<i4")]
+                                                      # a segment record of b200bt_sweep_segments, 24 bytes (B200BT_SEGMENT_*)
+
 PRIMARY = {"sharpe_ratio": 0, "return_pct": 1, "profit_factor": 2, "win_rate": 3, "net_profit": 4, "total_trades": 5,
            "max_drawdown": 6, "total_profit": 7, "total_loss": 8, "largest_profit": 9, "largest_loss": 10,
            "average_profit": 11, "average_loss": 12}
@@ -345,6 +348,9 @@ _SIGNATURES = {
     "b200bt_tail_stats": (C.c_int, [_vp, _i64, C.c_double, _vp, _vp, _i64, _vp]),
     "b200bt_correlation_workspace_bytes": (C.c_int64, [_i, _i64]),
     "b200bt_correlation": (C.c_int, [_vp, _i64, _i, _i64, _vp, _vp, _i64, _vp]),
+    "b200bt_sweep_segments": (C.c_int, [_vp, _i64, _vp, _i64, _i, _i, _i64, _vp, _i, _vp, _vp, _i, C.POINTER(SweepConfig),
+                                        _vp, _vp, _i64, _vp]),
+    "b200bt_decode_individuals": (C.c_int, [_vp, _i64, _i, C.POINTER(C.c_int), C.POINTER(C.c_int32), _i, _vp, _vp]),
 }
 
 _lib = None

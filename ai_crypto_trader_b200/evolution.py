@@ -4,6 +4,7 @@ Reference: services/strategy_evolution_service.py.
   param_ranges                       :98-117  (synth.param_ranges)
   optimize_with_genetic_algorithm    :525-694 (GA construction :644-655)
   optimize_with_reinforcement_learning :696-791 (rl.py: the agent on the device, trained on the market's bars)
+  the monitor / re-optimise loop      :1584-1711 (walk_forward: the loop replayed on history, walk_forward.py)
 The reference's fitness closure (:542-641) is a data-free placeholder that raises
 NameError (SURVEY.md 0); the fitness wired in here is the reference's own
 simulate -> metrics -> score composition (strategy_evaluation.py:682-691) evaluated for
@@ -24,6 +25,7 @@ from .pareto import objectives_from_goals
 from .rl import ACTIONS, SERVICE_AGENT, RLPopulation, adjust_params_from_q_values, rl_states
 from .sweep import DEFAULT_GOALS, MarketData, PopulationSweep
 from .synth import param_ranges
+from .walk_forward import WalkForward
 
 logger = logging.getLogger("b200bt.evolution")
 
@@ -113,6 +115,50 @@ class StrategyEvolutionService:
             return front
         except Exception as e:        # reference convention (:692-694): log, return None
             logger.error("Error in Pareto optimization: %s", e)
+            return None
+
+    def walk_forward(self, current_params: Optional[Dict], in_sample_days: int = 30, out_of_sample_days: int = 7,
+                     anchored: bool = False, reoptimize: str = "always") -> Optional[Dict]:
+        """Walk-forward analysis of the evolution loop on the service's market (walk_forward.WalkForward): re-optimise on
+        each in-sample window with the service's GA settings (GA_POPULATION_SIZE, GA_GENERATIONS, rates 0.2 / 0.8 / 0.1,
+        random_seed + window as the seed) and score the re-optimised parameters on the bars after each fit.
+        reoptimize="when_needed" re-fits only where the reference's gate (_needs_improvement at RISK_LEVEL, default MEDIUM,
+        on the thresholds built from the config's evolution block) fires; its performance dict carries "drawdown" =
+        100 x the mean max_drawdown, a key the reference reads but never writes.  Appends one evolution record per
+        re-optimisation, with its window.  Returns the report; on error (and for aggregation="book" or a torch.distributed
+        world of more than one process, which it does not cover) logs the reason and returns None."""
+        try:
+            import torch.distributed as dist
+            if self.aggregation == "book":
+                logger.error("walk_forward scores each symbol's lane; aggregation='book' is not covered")
+                return None
+            if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+                logger.error("walk_forward runs in a single process (world size %d)", dist.get_world_size())
+                return None
+            wf = WalkForward(self.sweep, self.param_ranges, population_size=self.ga_population_size,
+                             generations=self.ga_generations, mutation_rate=0.2, crossover_rate=0.8, elitism_pct=0.1,
+                             random_seed=self.random_seed)
+            report = wf.run(current_params, in_sample_days, out_of_sample_days, anchored, reoptimize,
+                            risk_level=os.getenv("RISK_LEVEL", "MEDIUM"),
+                            evolution_config=self.config.get("evolution", {}), leverage_trading=self.leverage_trading)
+            old = current_params
+            for row in report["windows"]:
+                if row["reoptimized"]:
+                    hist = row["history"]
+                    self.evolution_records.append({
+                        "id": str(uuid.uuid4()), "algorithm": "genetic", "timestamp": datetime.now().isoformat(),
+                        "improvement": hist[-1]["best_fitness"] - hist[0]["best_fitness"],
+                        "initial_fitness": hist[0]["best_fitness"], "final_fitness": hist[-1]["best_fitness"],
+                        "generations": len(hist), "population_size": self.ga_population_size,
+                        "old_params": old, "new_params": row["parameters"],
+                        "window": {k: row[k] for k in ("window", "in_sample", "out_of_sample", "in_sample_time",
+                                                       "out_of_sample_time")}})
+                if reoptimize == "when_needed":
+                    old = row["parameters"]
+            self.last_walk_forward = report
+            return report
+        except Exception as e:        # reference convention (:692-694): log, return None
+            logger.error("Error in walk-forward analysis: %s", e)
             return None
 
     def _states(self):

@@ -1257,6 +1257,57 @@ int b200bt_market_monitor(const float* ohlcv, int S, int64_t N, int64_t minute0,
  * (EINVAL), n < 2^31 (ELIMIT). */
 int b200bt_indicator_combinations(b200bt_monitor_row* rows, int64_t n, b200bt_stream_t stream);
 
+/* ---- walk-forward evaluation (csrc/walk_forward.cu) -----------------------------------------------------------------
+ * The strategy-evolution loop (services/strategy_evolution_service.py:1584-1711) re-fits the deployed parameters and trades
+ * them on the bars that follow; a walk-forward analysis scores that loop on history.  A lane of b200bt_sweep_segments trades
+ * a list of bar segments, each with its own individual. */
+
+/* Schedules of segments.  A segment is one 24-byte record, bars [start, end) of the series traded by indiv[individual]:
+ *     int64_t start;       first bar of the segment                 byte B200BT_SEGMENT_START
+ *     int64_t end;         one past its last bar                    byte B200BT_SEGMENT_END
+ *     int32_t individual;  row of indiv that trades the segment     byte B200BT_SEGMENT_INDIVIDUAL
+ *     int32_t reserved;    0                                        byte B200BT_SEGMENT_RESERVED
+ * segments: device array of n_segments such records (8-byte aligned, declared as their int64_t words; host mirror
+ * _lib.SEGMENT_DTYPE); seg_begin: device int32 [J + 1]; schedule j (0 <= j < J) is records seg_begin[j] .. seg_begin[j + 1].
+ * Lane (j, s) trades schedule j on symbol s.
+ *  stats[j][s]  calculate_metrics + _calculate_strategy_score under cfg's score rule (strategy_evaluation.py:32-228,
+ *               :579-633) over the concatenation, in segment order, of the records _simulate_trades (:746-878) emits for
+ *               indiv[individual] on bars [start, end) of symbol s: the reference function called once per segment, every
+ *               segment starting flat and force-closing at end - 1, all segments' records then scored as one list.
+ *               Equity, peak, drawdown, calendar-day buckets and the trade hash run on across segments; the position does not.
+ *  events       optional [J][S][event_cap] (as b200bt_sweep): the lane's first event_cap event words, with GLOBAL bar indices;
+ *               the calendar is the series' own (bar t on day (minute0 + t * bar_minutes) / 1440) and trade_hash is taken
+ *               over the lane's records in that order with their global words.
+ * Checked on the host, before the device: null pointers, n_indiv < 1, J < 1 and b200bt_sweep's argument checks (EINVAL /
+ * ELIMIT: sizes, strides, N < 2^30, the calendar clock, the event buffer); cfg->gap_bar != 0 (EINVAL: a glued series is not
+ * combined with segments).
+ * Checked on the device, nothing read back: a schedule with no segment, a segment with start < 0, end <= start, end > N
+ * or reserved != 0, a segment starting before the previous one ends (gaps are allowed), an individual outside [0, n_indiv) or an individual
+ * whose rsi_row lies outside [0, P) makes the schedule invalid: its lanes get n_records = -1 and score = NaN (the rest zero),
+ * no events are written for them, and the other lanes are unaffected. */
+#define B200BT_SEGMENT_BYTES 24
+#define B200BT_SEGMENT_START 0
+#define B200BT_SEGMENT_END 8
+#define B200BT_SEGMENT_INDIVIDUAL 16
+#define B200BT_SEGMENT_RESERVED 20
+int b200bt_sweep_segments(const float* price, int64_t ld_price, const float* rsi, int64_t ld_rsi, int P, int S, int64_t N,
+                          const b200bt_individual* indiv, int n_indiv, const int64_t* segments, const int32_t* seg_begin,
+                          int J, const b200bt_sweep_config* cfg_host, b200bt_lane_stats* stats, uint32_t* events,
+                          int64_t event_cap, b200bt_stream_t stream);
+
+/* decode_population (ai_crypto_trader_b200/sweep.py) on the device, byte for byte: params is the GA's device float64 matrix
+ * [n][ld]; gene_cols_host[6] the columns of rsi_period, rsi_oversold, rsi_overbought, take_profit, stop_loss,
+ * max_position_size, -1 = absent (decode_population's defaults 14, 30, 70, 3, 2, 5); period_row_host[n_period_row] the bank
+ * row of each period, -1 = not in the bank.  The period is truncated towards zero; one outside the table, or whose entry is
+ * -1, decodes to rsi_row = -1 (b200bt_sweep_segments reports such a lane as lost; the host decode raises KeyError).
+ * Thresholds are rounded to fp32 towards the side that keeps the compares exact, take_profit / 100, stop_loss / 100,
+ * position_size = 10000 * (min(max_position_size, 20) / 100), reserved = 0.  out: device [n].
+ * Checked before the device: null pointers, n < 1, ld < 1, n_period_row < 1, a column outside [-1, ld) (EINVAL);
+ * n_period_row > 256 (ELIMIT). */
+int b200bt_decode_individuals(const double* params, int64_t ld, int n, const int* gene_cols_host,
+                              const int32_t* period_row_host, int n_period_row, b200bt_individual* out,
+                              b200bt_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
