@@ -116,8 +116,8 @@ __device__ __forceinline__ void grid_pass(const GridArgs& a, const double* L, co
     if (lane < n) {
         const int j = j0 + lane;
         const double last = (double)px[j], cur = (double)px[j + 1];
-        if (cur != last) {
-            const bool upmove = cur > last;
+        const bool upmove = cur > last;
+        if (upmove || cur < last) {                   // a NaN price on either side is not a move (nor a near tie)
             const double x_lo = upmove ? last : cur, x_hi = upmove ? cur : last;
             const int e_lo = level_bound<false>(L, g.n, estimate(g, x_lo), x_lo);   // first L >= x_lo
             const int e_hi = level_bound<true>(L, g.n, estimate(g, x_hi), x_hi);    // first L > x_hi
@@ -126,8 +126,17 @@ __device__ __forceinline__ void grid_pass(const GridArgs& a, const double* L, co
                 ++c.n_tie;
             if (upmove) {
                 for (int l = e_lo; l < e_hi; ++l) {
+                    // the reference prices a level by levels.index(lv): every copy of a repeated level earns the step
+                    // under its first copy f (the lower bound of lv, as the levels are sorted), and nothing when f = 0
                     const double lv = L[l];
-                    const double pr = l > 0 ? __dmul_rn(__dsub_rn(lv, L[l - 1]), qty) : 0.0;
+                    int f = l;
+                    double below = l > 0 ? L[l - 1] : 0.0;
+                    if (l > 0 && below == lv) {
+                        do --f;
+                        while (f > 0 && L[f - 1] == lv);
+                        below = f > 0 ? L[f - 1] : 0.0;
+                    }
+                    const double pr = f > 0 ? __dmul_rn(__dsub_rn(lv, below), qty) : 0.0;
                     if (pr > 0.0) ++c.n_prof;
                     p_tick = __dadd_rn(p_tick, pr);
                     c.cash = __dadd_rn(c.cash, __dmul_rn(lv, qty));
@@ -547,6 +556,8 @@ static int grid_args(const char* what, bool service, const float* price, int64_t
     } else {
         B200BT_REQUIRE(!labels_or_null || ld_labels == 0 || ld_labels >= N, B200BT_EINVAL,
                        "%s: ld_labels must be 0 (one shared row) or >= N", what);
+        // the stats launch's grid.y is S
+        B200BT_REQUIRE(S <= 65535, B200BT_ELIMIT, "%s: at most 65535 symbols (S = %d)", what, S);
     }
     const int64_t need_days = series_days(minute0, N, bar_minutes);
     B200BT_REQUIRE(!day_profit_or_null || D >= need_days, B200BT_EINVAL, "%s: D = %lld days, the series spans %lld", what,

@@ -735,10 +735,13 @@ int b200bt_class_stats(const float* price, int64_t ld_price, int S, int64_t N, c
  * __init__ / _initialize_grid (:245-345) run at tick 0: start_time, last_rebalance and last_adjustment are t0.  On every tick,
  * tick 0 included, the loop body runs, in order:
  *   _process_grid_simulation (:679-779) with last = the previous tick's price (tick 0: last == cur, nothing happens).
- *     Up move (cur > last): every level with last <= L_i <= cur is a trade with profit (L_i - L_{i-1}) * qty (0 for i = 0),
- *     profitable when the profit is > 0.  Down move: every level with cur <= L_i <= last is a trade with no profit.  Equal
- *     prices do nothing; a level equal to the last price is counted again.  qty = qty[s] (symbol_settings' quantity_per_grid,
- *     else the global one, :387-400).
+ *     Up move (cur > last): every level with last <= L_i <= cur is a trade with profit (L_i - L_{f-1}) * qty, f the first
+ *     index holding L_i's value (levels.index, :712: every copy of a repeated level earns the step under the first copy;
+ *     0 for f = 0), profitable when the profit is > 0.  Down move (cur < last): every level with cur <= L_i <= last is a
+ *     trade with no profit.  Equal prices do nothing, and so does a NaN close: the tick with it and the tick after it are
+ *     neither move (the rebalance check's compares are false too, and mark_to_market is NaN when the last close is NaN).
+ *     A level equal to the last price is counted again.  qty = qty[s] (symbol_settings' quantity_per_grid, else the
+ *     global one, :387-400).
  *   The rebalance check (:178-186): (now - last_rebalance) > rebalance_frequency with a strict >, and last_rebalance is reset
  *     whenever the check runs, so it runs on the ticks k = m * rebalance_ticks (m >= 1), rebalance_ticks =
  *     floor(frequency / bar_seconds) + 1 (61 at 1-minute bars and 3600 s).  _rebalance_grid (:781-838): when cur <
@@ -756,7 +759,7 @@ int b200bt_class_stats(const float* price, int64_t ld_price, int S, int64_t N, c
  *     Both take effect at the next regeneration.
  * Levels (_generate_grid_levels :347-385), i = 0 .. n: arithmetic lower + i * step, step = (upper - lower) / n, exact IEEE
  * float64 (no FMA contraction); geometric lower * pow(ratio, i), ratio = pow(upper / lower, 1 / n) with CUDA's pow, which
- * may differ from the C library's by a few ulps.  near_ties counts the ticks on which a price compared with a geometric
+ * may differ from the C library's by a few ulps.  near_ties counts the up or down moves on which a price compared with a geometric
  * level lies within |L| * 2^-50 (<= 4 ulps) of it: only those ticks can decide a compare differently from the reference.
  * Levels must be non-decreasing in i (true for finite lower <= upper); "volatility_based" draws random numbers and is not
  * a grid type here.
@@ -771,7 +774,7 @@ int b200bt_class_stats(const float* price, int64_t ld_price, int S, int64_t N, c
  * With day_profit the symbols of an individual run one after another in one warp; stats are the same either way.
  * An individual outside the limits (num_grids 1 .. B200BT_GRID_MAX_GRIDS, grid_type 0 / 1, periods >= 1) gets NaN stats.
  * Checked before the device: null pointers, sizes, start_bar in [0, N - 1], bar_minutes > 0, minute0 >= 0, ld_labels, D,
- * the table's num_grids (all EINVAL); N >= 2^30 (ELIMIT).  Deterministic: no atomics. */
+ * the table's num_grids (all EINVAL); N >= 2^30, S > 65535 (ELIMIT).  Deterministic: no atomics. */
 #define B200BT_GRID_ARITHMETIC 0
 #define B200BT_GRID_GEOMETRIC 1
 #define B200BT_GRID_ADAPT_REGIME 1       /* adapt_to_market_regime                                          */
@@ -852,7 +855,7 @@ int b200bt_grid_sweep(const float* price, int64_t ld_price, int S, int64_t N, in
  * Schedule: one CTA per individual, min(S, 16) warps, warp w running symbols w, w + W, ... between two adjust ticks, where
  * the warps meet and thread 0 applies the S rule pairs in order; with day rows one warp runs every symbol in order.
  * An individual outside the limits gets NaN stats and a NaN service record.  Checked before the device: as
- * b200bt_grid_sweep, plus labels_or_null with ld_labels != 0 (EINVAL).  Deterministic: no atomics. */
+ * b200bt_grid_sweep but any S, plus labels_or_null with ld_labels != 0 (EINVAL).  Deterministic: no atomics. */
 typedef struct b200bt_grid_service_stats {
     double total_profit;        /* grid_performance (:941-958): the lanes' total_profit summed in symbol order          */
     double total_trades;

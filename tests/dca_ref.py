@@ -52,7 +52,7 @@ def dip_of(klines: List[float], price: float) -> float:
     """_check_for_dips' drop (:841-855), NaN where it makes no check."""
     if not klines or len(klines) < 2:
         return math.nan
-    recent_high = max(klines)
+    recent_high = float(max(klines))                 # a Python float: a 0 high raises, as in the reference
     try:
         return ((recent_high - price) / recent_high) * 100
     except ZeroDivisionError:

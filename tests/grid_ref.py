@@ -72,7 +72,7 @@ def simulate(prices, lower: float, upper: float, n: int, kind: int, qty: float, 
     for k in range(T):
         cur = prices[k]
         p_day = 0.0
-        if cur != last and kind == 1 and (_near(last, lv) or _near(cur, lv)):
+        if (cur > last or cur < last) and kind == 1 and (_near(last, lv) or _near(cur, lv)):
             ties += 1
         if cur > last:
             for level in [lv_ for lv_ in lv if last <= lv_ <= cur]:
@@ -138,7 +138,8 @@ def simulate_fast(prices, lower: float, upper: float, n: int, kind: int, qty: fl
     while k < T:
         stop = min(next_reb, next_adj, T - 1)
         last, cur = p[k - 1:stop], p[k:stop + 1]
-        pl = np.concatenate([[0.0], (lv[1:] - lv[:-1]) * qty])
+        f = np.searchsorted(lv, lv, "left")     # levels.index: a repeated level earns the step under its first copy
+        pl = np.where(f > 0, (lv - lv[np.maximum(f - 1, 0)]) * qty, 0.0)
         cum_p = np.concatenate([[0.0], np.cumsum(pl)])
         cum_w = np.concatenate([[0], np.cumsum(pl > 0)])
         cum_l = np.concatenate([[0.0], np.cumsum(lv * qty)])

@@ -57,7 +57,7 @@ def simulate_service(prices: Sequence[Sequence[float]], bounds: Sequence[Tuple[f
         for s, ln in enumerate(lanes):                      # _process_grid_simulation, symbols in order
             cur, last, lv, st = px[s][k], ln["last"], ln["lv"], ln["st"]
             p_day = 0.0
-            if cur != last and kind == 1 and (grid_ref._near(last, lv) or grid_ref._near(cur, lv)):
+            if (cur > last or cur < last) and kind == 1 and (grid_ref._near(last, lv) or grid_ref._near(cur, lv)):
                 ln["ties"] += 1
             if cur > last:
                 for level in [x for x in lv if last <= x <= cur]:

@@ -88,14 +88,50 @@ def test_fixture_covers_the_rule(fixture):
     assert any(len(c["regenerations"]) > 50 for c in fixture["cases"])
 
 
+NAN = math.nan
+FLAT = dict(rebalance_ticks=10 ** 6, adjust_ticks=10 ** 6, lower_pct=5.0, upper_pct=5.0, qty=1.0)
+# lanes the fixture does not hold: repeated levels (an arithmetic step under an ulp, a geometric ratio of 1.0) and NaN
+# closes (on the first tick, mid-series, on a rebalance tick that would regenerate, and on the last tick)
+EDGE_LANES = {
+    "repeated arithmetic levels": dict(FLAT, prices=[99, 101, 99, 101], lower=100.0, upper=100 * (1 + 6e-16), n=8, kind=0),
+    "geometric ratio 1.0": dict(FLAT, prices=[99, 101, 100, 99, 100, 101], lower=100.0, upper=100.0, n=5, kind=1),
+    "NaN mid-series": dict(FLAT, prices=[100.5, NAN, 100.5, 99], lower=95.0, upper=105.0, n=10, kind=0),
+    "NaN runs": dict(FLAT, prices=[NAN, 101, 97, NAN, NAN, 103, 96, 104, NAN], lower=95.0, upper=105.0, n=10, kind=0),
+    "NaN on a rebalance tick": dict(FLAT, prices=[100, 104, NAN, 90, 100, 110, 90], lower=95.0, upper=105.0, n=4, kind=0,
+                                    rebalance_ticks=2),
+}
+
+
 def test_fast_restatement_matches(fixture):
-    for case in fixture["cases"]:
-        kw, _ = lane_inputs(fixture, case)
+    cases = [(c["name"], lane_inputs(fixture, c)[0]) for c in fixture["cases"]] + list(EDGE_LANES.items())
+    for name, kw in cases:
         a, b = grid_ref.simulate(**kw), grid_ref.simulate_fast(**kw)
         for f in grid_ref.FIELDS:
             if f == "near_ties":
                 continue
-            assert math.isclose(a[f], b[f], rel_tol=1e-9, abs_tol=1e-9), (case["name"], f, a[f], b[f])
+            assert math.isclose(a[f], b[f], rel_tol=1e-9, abs_tol=1e-9) or (math.isnan(a[f]) and math.isnan(b[f])), \
+                (name, f, a[f], b[f])
+        # profits are sums of non-negative steps: no absolute floor, which would hide a step of 1e-14
+        assert a["profitable_trades"] == b["profitable_trades"], name
+        assert math.isclose(a["total_profit"], b["total_profit"], rel_tol=1e-9, abs_tol=0.0), name
+
+
+def test_edge_lanes_follow_the_reference_rule():
+    """levels.index prices every copy of a repeated level by the step under its first copy; a NaN close is no move."""
+    rep = grid_ref.simulate(**EDGE_LANES["repeated arithmetic levels"])
+    lv = grid_ref.levels(100.0, 100 * (1 + 6e-16), 8, 0)
+    assert len(set(lv)) < len(lv)
+    assert (rep["up_crossings"], rep["profitable_trades"]) == (18, 16)
+    assert rep["total_profit"] == 2 * sum(x - lv[lv.index(x) - 1] for x in lv if lv.index(x) > 0)
+    geo = grid_ref.simulate(**EDGE_LANES["geometric ratio 1.0"])
+    assert (geo["up_crossings"], geo["profitable_trades"], geo["total_profit"]) == (18, 0, 0.0)
+    nan = grid_ref.simulate(**EDGE_LANES["NaN mid-series"])
+    assert (nan["down_crossings"], nan["up_crossings"], nan["near_ties"]) == (2, 0, 0)
+    reb = grid_ref.simulate(**EDGE_LANES["NaN on a rebalance tick"])
+    assert reb["regenerations"][1][0] == 4 and reb["n_rebalance_checks"] == 3
+    last = EDGE_LANES["NaN runs"]
+    assert math.isnan(grid_ref.simulate(**last)["mark_to_market"])
+    assert math.isnan(grid_ref.simulate_fast(**last)["mark_to_market"])
 
 
 def test_period_ticks():
