@@ -218,9 +218,10 @@ def decode_population(population: List[Dict], period_row: Dict[int, int], n_time
     out = np.zeros(len(population), dtype=INDIVIDUAL_DTYPE)
     g = lambda key, default: np.array([p.get(key, default) for p in population], dtype=np.float64)
     period = g("rsi_period", 14).astype(np.int64)
-    rows = np.full(int(period.max()) + 2 if len(period) else 1, -1, dtype=np.int64)
+    # the table ends one entry (-1) past the bank's largest period: a larger period, however large, decodes to that entry
+    rows = np.full(max((w for w in period_row if w >= 0), default=-1) + 2, -1, dtype=np.int64)
     for w, r in period_row.items():
-        if 0 <= w < len(rows):
+        if w >= 0:
             rows[w] = r
     row = rows[np.clip(period, 0, len(rows) - 1)]
     if len(period) and (period.min() < 0 or row.min() < 0):

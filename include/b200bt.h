@@ -1298,13 +1298,16 @@ int b200bt_sweep_segments(const float* price, int64_t ld_price, const float* rsi
                           int J, const b200bt_sweep_config* cfg_host, b200bt_lane_stats* stats, uint32_t* events,
                           int64_t event_cap, b200bt_stream_t stream);
 
-/* decode_population (ai_crypto_trader_b200/sweep.py) on the device, byte for byte: params is the GA's device float64 matrix
- * [n][ld]; gene_cols_host[6] the columns of rsi_period, rsi_oversold, rsi_overbought, take_profit, stop_loss,
- * max_position_size, -1 = absent (decode_population's defaults 14, 30, 70, 3, 2, 5); period_row_host[n_period_row] the bank
+/* decode_population (ai_crypto_trader_b200/sweep.py) on the device, byte for byte but for NaN payloads: params is the GA's
+ * device float64 matrix [n][ld]; gene_cols_host[6] the columns of rsi_period, rsi_oversold, rsi_overbought, take_profit,
+ * stop_loss, max_position_size, -1 = absent (decode_population's defaults 14, 30, 70, 3, 2, 5); period_row_host[n_period_row] the bank
  * row of each period, -1 = not in the bank.  The period is truncated towards zero; one outside the table, or whose entry is
  * -1, decodes to rsi_row = -1 (b200bt_sweep_segments reports such a lane as lost; the host decode raises KeyError).
  * Thresholds are rounded to fp32 towards the side that keeps the compares exact, take_profit / 100, stop_loss / 100,
  * position_size = 10000 * (min(max_position_size, 20) / 100), reserved = 0.  out: device [n].
+ * NaN genes: a field decode_population gives as NaN is a NaN here too, but its bits may differ (NumPy keeps the operand's
+ * payload, the device's conversion and division need not); every other field, and every field of a row without NaN, is
+ * byte for byte.  A NaN or infinite period decodes to rsi_row = -1.
  * Checked before the device: null pointers, n < 1, ld < 1, n_period_row < 1, a column outside [-1, ld) (EINVAL);
  * n_period_row > 256 (ELIMIT). */
 int b200bt_decode_individuals(const double* params, int64_t ld, int n, const int* gene_cols_host,

@@ -32,6 +32,16 @@ def test_decode_population_matches_the_scalar_rules():
     assert decode_population([], ROWS).shape == (0,)
 
 
+@pytest.mark.filterwarnings("ignore:invalid value encountered in cast")
+def test_decode_population_refuses_any_period_outside_the_bank():
+    """A period however large, or not a number, is a KeyError, found without a table as long as the period (1e9 would
+    be an 8 GB one), next to valid individuals."""
+    for period in (31, 1e9, 2.0 ** 62, 1e300, np.inf, -np.inf, np.nan, -1, 4):
+        with pytest.raises(KeyError):
+            decode_population([{"rsi_period": 14}, {"rsi_period": period}], ROWS)
+    assert decode_population([{"rsi_period": 30.9}, {"rsi_period": 5}], ROWS)["rsi_row"].tolist() == [25, 0]
+
+
 def test_cost_model_variants_agree():
     pop = synth.random_population(500, seed=3)
     scalar = np.array([lane_cost(p) for p in pop])
