@@ -231,6 +231,17 @@ TRADE_MC_METHODS = {"bootstrap": 0, "shuffle": 1}     # B200BT_TRADE_MC_*
 SEGMENT_DTYPE = [("start", "<i8"), ("end", "<i8"), ("individual", "<i4"), ("reserved", "<i4")]
                                                       # a segment record of b200bt_sweep_segments, 24 bytes (B200BT_SEGMENT_*)
 
+# b200bt_selection_replay: parameter slots (B200BT_SEL_P_* = index), gene columns (B200BT_SEL_G_*), check-row columns
+# (B200BT_SEL_R_*)
+SEL_PARAMS = ("start_bar", "check_bars", "cache_expiry", "w_market_regime", "w_historical_performance", "w_risk_profile",
+              "w_social_sentiment", "w_market_volatility", "w_feature_importance", "min_improvement", "min_confidence",
+              "risk_max_drawdown", "risk_min_sharpe", "risk_volatility", "high_vol_start", "high_vol_end",
+              "low_activity_start", "low_activity_end")
+SEL_GENES = ("ema_long", "take_profit", "stop_loss", "rsi_oversold", "bollinger_std", "rsi_period", "atr_multiplier",
+             "atr_period")
+SEL_ROW = ("bar", "regime", "best", "score", "market_regime", "historical_performance", "risk_profile", "social_sentiment",
+           "market_volatility", "feature_importance", "active", "active_score")
+
 PRIMARY = {"sharpe_ratio": 0, "return_pct": 1, "profit_factor": 2, "win_rate": 3, "net_profit": 4, "total_trades": 5,
            "max_drawdown": 6, "total_profit": 7, "total_loss": 8, "largest_profit": 9, "largest_loss": 10,
            "average_profit": 11, "average_loss": 12}
@@ -351,6 +362,9 @@ _SIGNATURES = {
     "b200bt_sweep_segments": (C.c_int, [_vp, _i64, _vp, _i64, _i, _i, _i64, _vp, _i, _vp, _vp, _i, C.POINTER(SweepConfig),
                                         _vp, _vp, _i64, _vp]),
     "b200bt_decode_individuals": (C.c_int, [_vp, _i64, _i, C.POINTER(C.c_int), C.POINTER(C.c_int32), _i, _vp, _vp]),
+    "b200bt_selection_replay": (C.c_int, [_vp, _i64, _i, _i64, _vp, _i, C.POINTER(SweepConfig), _vp, _vp, _i64, _vp, _i64,
+                                          _vp, _vp, _vp, _i, _i, C.POINTER(C.c_double), _i64, _i, _vp, _vp, _vp, _vp]),
+    "b200bt_selection_switch": (C.c_int, [_vp, _i64, C.POINTER(C.c_double), _vp, _vp, _vp]),
 }
 
 _lib = None

@@ -1314,6 +1314,100 @@ int b200bt_decode_individuals(const double* params, int64_t ld, int n, const int
                               const int32_t* period_row_host, int n_period_row, b200bt_individual* out,
                               b200bt_stream_t stream);
 
+/* ---- strategy selection replay (csrc/selection.cu) ------------------------------------------------------------------
+ * StrategySelectionService (services/strategy_selection_service.py) run over history: at every check each candidate's
+ * metrics snapshot (get_strategy_metrics :159-264, cached per candidate), its six factor scores (:299-687, with
+ * market_regime_service.py:734-827), the weighted sum (:821-828), the time adjustments (:689-770), the best candidate
+ * (:846) and the switch rule (:884-934).
+ *
+ * Parameters: a host float64 array [B200BT_SEL_PARAMS] whose slots are named below.  Weights are normalised as :80-83
+ * does.  Risk volatility preference: 0 low, 1 medium, 2 high.  The time windows are [start, end) UTC hours. */
+#define B200BT_SEL_P_START_BAR 0                /* bar of check 0                                              */
+#define B200BT_SEL_P_CHECK_BARS 1               /* bars between checks (STRATEGY_CHECK_INTERVAL / bar seconds) */
+#define B200BT_SEL_P_CACHE_EXPIRY 2             /* seconds a snapshot is reused (:128, :174)                   */
+#define B200BT_SEL_P_W_MARKET_REGIME 3          /* the normalised weights, in the order of :821-828            */
+#define B200BT_SEL_P_W_HISTORICAL_PERFORMANCE 4
+#define B200BT_SEL_P_W_RISK_PROFILE 5
+#define B200BT_SEL_P_W_SOCIAL_SENTIMENT 6
+#define B200BT_SEL_P_W_MARKET_VOLATILITY 7
+#define B200BT_SEL_P_W_FEATURE_IMPORTANCE 8
+#define B200BT_SEL_P_MIN_IMPROVEMENT 9
+#define B200BT_SEL_P_MIN_CONFIDENCE 10
+#define B200BT_SEL_P_RISK_MAX_DRAWDOWN 11       /* the risk profile (:96-112)                                  */
+#define B200BT_SEL_P_RISK_MIN_SHARPE 12
+#define B200BT_SEL_P_RISK_VOLATILITY 13
+#define B200BT_SEL_P_HIGH_VOL_START 14          /* time windows (:90-93)                                       */
+#define B200BT_SEL_P_HIGH_VOL_END 15
+#define B200BT_SEL_P_LOW_ACTIVITY_START 16
+#define B200BT_SEL_P_LOW_ACTIVITY_END 17
+#define B200BT_SEL_PARAMS 18
+/* Genes the scores read, one float64 row [B200BT_SEL_GENES] per candidate; NaN = the key is absent (its .get default). */
+#define B200BT_SEL_G_EMA_LONG 0
+#define B200BT_SEL_G_TAKE_PROFIT 1
+#define B200BT_SEL_G_STOP_LOSS 2
+#define B200BT_SEL_G_RSI_OVERSOLD 3
+#define B200BT_SEL_G_BOLLINGER_STD 4
+#define B200BT_SEL_G_RSI_PERIOD 5
+#define B200BT_SEL_G_ATR_MULTIPLIER 6
+#define B200BT_SEL_G_ATR_PERIOD 7
+#define B200BT_SEL_GENES 8
+/* A check row, float64 [B200BT_SEL_ROW_WORDS]: the check's bar and regime label (>= 4: unknown), the best candidate
+ * (-1: none valid) and its final score and six factor scores (:862-867), and the active candidate (-1: none) and its
+ * score after the switch rule. */
+#define B200BT_SEL_R_BAR 0
+#define B200BT_SEL_R_REGIME 1
+#define B200BT_SEL_R_BEST 2
+#define B200BT_SEL_R_SCORE 3
+#define B200BT_SEL_R_MARKET_REGIME 4
+#define B200BT_SEL_R_HISTORICAL_PERFORMANCE 5
+#define B200BT_SEL_R_RISK_PROFILE 6
+#define B200BT_SEL_R_SOCIAL_SENTIMENT 7
+#define B200BT_SEL_R_MARKET_VOLATILITY 8
+#define B200BT_SEL_R_FEATURE_IMPORTANCE 9
+#define B200BT_SEL_R_ACTIVE 10
+#define B200BT_SEL_R_ACTIVE_SCORE 11
+#define B200BT_SEL_ROW_WORDS 12
+
+/* Scores of n_cand candidates at checks c = 0 .. n_checks - 1 (bar t_c = start_bar + c * check_bars), merged into rows.
+ * Candidate j is global index cand_index[j] in [0, K) and trades as indiv[cand_row[j]]: its records are the event words of
+ * lanes (cand_row[j], s) of a population sweep (lane_stats [n_indiv][S], events [n_indiv][S][event_cap]), merged over the
+ * symbols in book order and priced as b200bt_book_metrics prices them.
+ *  snapshot    at the candidate's refresh checks: a check with no cached snapshot whose prefix (records with bar <= t_c) is
+ *              non-empty, or one at least cache-expiry seconds after the cached fetch; an empty prefix is not cached.  It is
+ *              calculate_advanced_metrics(calculate_metrics(prefix)) plus regime_performance (per scored regime with
+ *              records: trade_count, win_rate, profit_factor = net / |losses| or 1, and calculate_metrics' sharpe_ratio
+ *              and max_drawdown of those records) and hourly_performance (per UTC hour: trade_count, wins = pnl > 0).
+ *  scores      regime (the label of bar t_c in row 0 of labels), historical performance, risk, social 0.5, volatility
+ *              (0.5 empty, else 0.6), feature importance 0.5; the weighted sum; the time adjustments; a clamp to [0, 1].
+ *              float64 in the reference's order of operations, without contraction.
+ *  rows        [n_checks][B200BT_SEL_ROW_WORDS]: merge = 0 first fills every row (no best) and zeroes check_locks; merge = 1
+ *              merges into the rows of an earlier call over other candidates.  The best is the highest score, the lowest
+ *              candidate index among equal ones, whatever the order of calls.  The ACTIVE columns are b200bt_selection_switch's.
+ *  scores_or_null  [n_checks][K]: every candidate's final score (NaN for an invalid candidate).
+ *  check_locks device int32 [n_checks] workspace.
+ * A candidate with a lane whose n_records > event_cap (or a cand_row outside [0, n_indiv)) is invalid: never selected.
+ * labels: device uint8 [S or 1][ld_labels] (ld_labels = 0: one row for every symbol; as b200bt_class_stats); a record's
+ * regime is the label of its bar in its symbol's row.
+ * Checked on the host, before the device: null pointers, the record-pass checks of b200bt_book_metrics (sizes, strides,
+ * N < 2^30, the calendar clock; S > 64 is ELIMIT), event_cap < 1, ld_labels, 1 <= n_cand <= K, merge, check_bars not an
+ * integer in [1, N], start_bar not an integer in [0, N), cache expiry not positive and finite, a zero risk threshold, a
+ * volatility preference outside {0, 1, 2}, non-integer window hours, n_checks outside [1, (N - 1 - start_bar) / check_bars
+ * + 1] (EINVAL). */
+int b200bt_selection_replay(const float* price, int64_t ld_price, int S, int64_t N, const b200bt_individual* indiv,
+                            int n_indiv, const b200bt_sweep_config* cfg, const b200bt_lane_stats* lane_stats,
+                            const uint32_t* events, int64_t event_cap, const uint8_t* labels, int64_t ld_labels,
+                            const int32_t* cand_row, const int32_t* cand_index, const double* genes, int n_cand, int K,
+                            const double* params_host, int64_t n_checks, int merge, double* rows, double* scores_or_null,
+                            int32_t* check_locks, b200bt_stream_t stream);
+
+/* The switch rule over the rows in check order, one warp on the device: with (active, active score) starting at (-1, 0),
+ * check c switches when its best is >= 0 and differs from the active one, score - active score > MIN_STRATEGY_IMPROVEMENT
+ * and score > MIN_STRATEGY_CONFIDENCE; the best then becomes active with its score.  Writes the ACTIVE columns of every
+ * row, the checks that switched in order (switch_checks, device int32 [n_checks]) and their count (n_switches, device
+ * int32).  params_host: the slots of b200bt_selection_replay.  n_checks < 1 is EINVAL, >= 2^31 ELIMIT. */
+int b200bt_selection_switch(double* rows, int64_t n_checks, const double* params_host, int32_t* switch_checks,
+                            int32_t* n_switches, b200bt_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
