@@ -334,6 +334,9 @@ _SIGNATURES = {
                                    _vp]),
     "b200bt_cscv_workspace_bytes": (C.c_int64, [_i, _i64, _i]),
     "b200bt_cscv": (C.c_int, [_vp, _i64, _i, _i64, _i, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "b200bt_spa_moments": (C.c_int, [_vp, _i64, _i, _i, C.c_double, _vp, _vp, _vp]),
+    "b200bt_spa_bootstrap": (C.c_int, [_vp, _i64, _i, _i, C.c_uint64, _i64, C.c_uint64, C.c_uint64, _i, _vp, _vp, _vp,
+                                       _vp]),
     "b200bt_regime_max_windows": (C.c_int64, [_i64, _i]),
     "b200bt_regime_labels": (C.c_int, [_vp, _vp, _vp, _vp, _i, _i64, _i64, _i64, _i, C.POINTER(RegimeParams), _vp, _i64,
                                        _vp, _i64, _vp]),

@@ -9,9 +9,14 @@
 // cscv_*            moments (one thread per trial), a trial-tile-major combination pass that stages a tile's block
 //                   statistics in registers once and walks a run of combinations, a reduction to the selected trial,
 //                   and a second tile pass that counts the trials below / tied with the selected one out of sample.
-// Every fp64 operation of the CSCV path is an explicit _rn intrinsic: nothing is contracted into an FMA, so that
-// tests/cscv_ref.py restates the arithmetic bit for bit.
+// spa_*             data-snooping tests (White's Reality Check, Hansen's SPA, Romano-Wolf StepM): per-trial moments and
+//                   Hansen's stationary-bootstrap variance (one CTA per trial), and the stationary-bootstrap maxima (one
+//                   CTA per 32-trial tile x resample range, one warp per resample, one lane per trial).
+// Every fp64 operation of the CSCV and SPA paths is an explicit _rn intrinsic: nothing is contracted into an FMA, so
+// that tests/cscv_ref.py and tests/spa_ref.py restate the arithmetic bit for bit.
 #include <math.h>
+#include <algorithm>
+#include "philox.cuh"
 #include "sweep_dev.cuh"
 
 namespace b200bt {
@@ -310,6 +315,188 @@ int64_t cscv_layout(int N, int B, int64_t* part_off, int64_t* n_part) {
     return stats + parts * 12;
 }
 
+// ---- data snooping: Reality Check, SPA, StepM -----------------------------------------------------------------------
+constexpr int SPA_MAX_T = 8192;              // 13-bit day indices
+constexpr int SPA_MAX_STATS = 8;
+constexpr int SPA_MOM_THREADS = 256;
+constexpr int SPA_WARPS = 16;                // resamples walked at once per CTA of the bootstrap pass
+constexpr int SPA_TILE = 32;                 // trials per CTA of the bootstrap pass: one per lane
+constexpr int SPA_STAGE_T = 768;             // rows of up to this many days are staged in shared memory (192 KB)
+
+// Moments of trial k (one CTA): the row, then (1-q)^i by running products and the mean (one thread each, ascending),
+// the lag sums (threads over lags, each in ascending t), and the kappa-weighted sum of the lags (one thread, ascending).
+__global__ void __launch_bounds__(SPA_MOM_THREADS)
+spa_moments_kernel(const double* __restrict__ d, int64_t ld, int T, double q, double* __restrict__ mean_out,
+                   double* __restrict__ omega2_out) {
+    extern __shared__ double sm[];
+    double* c = sm;                          // [T] the row, then the row minus its mean
+    double* p = sm + T;                      // [T + 1] (1-q)^i
+    double* g = p + T + 1;                   // [T] gamma_0, then kappa_i * gamma_i
+    __shared__ double mean_s;
+    const double* x = d + (int64_t)blockIdx.x * ld;
+    for (int t = threadIdx.x; t < T; t += blockDim.x) c[t] = x[t];
+    __syncthreads();
+    const double nt = (double)T;
+    if (threadIdx.x == 0) {
+        double s = 0.0;
+        for (int t = 0; t < T; ++t) s = __dadd_rn(s, c[t]);
+        mean_s = __ddiv_rn(s, nt);
+    } else if (threadIdx.x == 32) {
+        const double a = __dsub_rn(1.0, q);
+        double r = 1.0;
+        p[0] = r;
+        for (int i = 1; i <= T; ++i) p[i] = r = __dmul_rn(r, a);
+    }
+    __syncthreads();
+    const double mu = mean_s;
+    for (int t = threadIdx.x; t < T; t += blockDim.x) c[t] = __dsub_rn(c[t], mu);
+    __syncthreads();
+    for (int i = threadIdx.x; i < T; i += blockDim.x) {
+        double s = 0.0;
+        for (int t = 0; t + i < T; ++t) s = __dadd_rn(s, __dmul_rn(c[t], c[t + i]));
+        const double gam = __ddiv_rn(s, nt);
+        if (i == 0) {
+            g[0] = gam;
+        } else {
+            const double kappa = __dadd_rn(__dmul_rn(__ddiv_rn((double)(T - i), nt), p[i]),
+                                           __dmul_rn(__ddiv_rn((double)i, nt), p[T - i]));
+            g[i] = __dmul_rn(kappa, gam);
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double s = 0.0;
+        for (int i = 1; i < T; ++i) s = __dadd_rn(s, g[i]);
+        mean_out[blockIdx.x] = mu;
+        omega2_out[blockIdx.x] = __dadd_rn(g[0], __dmul_rn(2.0, s));
+    }
+}
+
+// Unsigned image of a double whose order is the numeric order (-inf lowest), for the cross-CTA atomicMax.
+__device__ __forceinline__ unsigned long long ordered(double v) {
+    const unsigned long long u = (unsigned long long)__double_as_longlong(v);
+    return (u >> 63) ? ~u : (u | 0x8000000000000000ull);
+}
+
+__device__ __forceinline__ double unordered(unsigned long long o) {
+    return __longlong_as_double((long long)((o >> 63) ? (o & 0x7fffffffffffffffull) : ~o));
+}
+
+// Days 64w + 2*lane and 64w + 2*lane + 1 of the resample whose Philox key is (k0, k1) and counter words 0, 1 are
+// (c0, c1), packed as theta0 | theta1 << 16.  A block start on day t with index s has the key (t + 1) << 13 | s, so the
+// latest start at or before a day is a max-scan of keys; `carry` holds the latest start before the window and is
+// advanced past it.  Days >= T get unspecified values.
+__device__ __forceinline__ unsigned spa_window(uint32_t k0, uint32_t k1, uint32_t c0, uint32_t c1, int w, int T,
+                                               uint64_t q32, int& carry) {
+    const int lane = threadIdx.x & 31;
+    const int t0 = 64 * w + 2 * lane, t1 = t0 + 1;
+    uint32_t x[4];
+    philox4x32_10(c0, c1, (uint32_t)(32 * w + lane), 0u, k0, k1, x);
+    const bool st0 = t0 == 0 || (uint64_t)x[0] < q32;
+    const bool st1 = (uint64_t)x[2] < q32;
+    const int s0 = (int)__umulhi(x[1], (uint32_t)T), s1 = (int)__umulhi(x[3], (uint32_t)T);
+    int inc = st1 ? ((t1 + 1) << 13 | s1) : st0 ? ((t0 + 1) << 13 | s0) : 0;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const int v = __shfl_up_sync(FULL, inc, o);
+        if (lane >= o) inc = max(inc, v);
+    }
+    int prev = __shfl_up_sync(FULL, inc, 1);
+    prev = max(lane == 0 ? 0 : prev, carry);
+    carry = max(carry, __shfl_sync(FULL, inc, 31));
+    const int ls = prev & 8191, lt = (prev >> 13) - 1;
+    int th0 = s0, th1;
+    if (!st0) {
+        th0 = ls + (t0 - lt);
+        th0 = th0 >= T ? th0 - T : th0;
+    }
+    if (st1) {
+        th1 = s1;
+    } else {
+        th1 = th0 + 1;
+        th1 = th1 >= T ? th1 - T : th1;
+    }
+    return (unsigned)(th0 & 0xffff) | (unsigned)(th1 & 0xffff) << 16;
+}
+
+// One CTA: trials [32 * blockIdx.x, +32) x resamples [b_lo, b_hi) of this CTA's range; warp v walks resamples b_lo + v,
+// b_lo + v + SPA_WARPS, ...  STAGED: the tile's rows sit in shared memory as [t][32] (one 256-byte row per day, read
+// without bank conflicts since every lane of a warp reads the same day); otherwise each lane reads its row through L1/L2.
+template <bool STAGED>
+__global__ void __launch_bounds__(SPA_WARPS * 32)
+spa_bootstrap_kernel(const double* __restrict__ d, int64_t ld, int N, int T, uint64_t q32, int64_t n_boot, int64_t per_cta,
+                     uint64_t seed, uint64_t boot_offset, int n_stats, const double* __restrict__ shift,
+                     const double* __restrict__ scale, unsigned long long* __restrict__ out) {
+    extern __shared__ double xs[];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int64_t k0 = (int64_t)blockIdx.x * SPA_TILE;
+    const int64_t k = k0 + lane;
+    const bool valid = k < N;
+    if (STAGED) {
+        for (int i = threadIdx.x; i < SPA_TILE * T; i += blockDim.x) {
+            const int j = i & (SPA_TILE - 1), t = i / SPA_TILE;
+            xs[i] = k0 + j < N ? d[(k0 + j) * ld + t] : 0.0;
+        }
+        __syncthreads();
+    }
+    const double* row = d + (valid ? k : (int64_t)N - 1) * ld;
+    double sh[SPA_MAX_STATS], sc[SPA_MAX_STATS];
+#pragma unroll
+    for (int j = 0; j < SPA_MAX_STATS; ++j) {
+        sh[j] = valid && j < n_stats ? shift[(int64_t)j * N + k] : INFINITY;
+        sc[j] = valid && j < n_stats ? scale[(int64_t)j * N + k] : 0.0;
+    }
+    const uint32_t key0 = (uint32_t)seed, key1 = (uint32_t)(seed >> 32);
+    const int windows = (T + 63) / 64;
+    const double nt = (double)T;
+    const int64_t b_lo = (int64_t)blockIdx.y * per_cta, b_hi = min(n_boot, b_lo + per_cta);
+    for (int64_t b = b_lo + warp; b < b_hi; b += SPA_WARPS) {
+        const uint64_t gid = boot_offset + (uint64_t)b;
+        int carry = 0;
+        double acc = 0.0;
+        for (int w = 0; w < windows; ++w) {
+            const unsigned packed = spa_window(key0, key1, (uint32_t)gid, (uint32_t)(gid >> 32), w, T, q32, carry);
+            const int nd = min(64, T - 64 * w);
+#pragma unroll 4
+            for (int pr = 0; pr < 32; ++pr) {
+                if (2 * pr >= nd) break;
+                const unsigned v = __shfl_sync(FULL, packed, pr);
+                const int a = (int)(v & 0xffffu), e = (int)(v >> 16);
+                acc = __dadd_rn(acc, STAGED ? xs[a * SPA_TILE + lane] : __ldg(row + a));
+                if (2 * pr + 1 < nd) acc = __dadd_rn(acc, STAGED ? xs[e * SPA_TILE + lane] : __ldg(row + e));
+            }
+        }
+        const double m = __ddiv_rn(acc, nt);
+        for (int j = 0; j < n_stats; ++j) {
+            double v = -INFINITY;
+#pragma unroll
+            for (int jj = 0; jj < SPA_MAX_STATS; ++jj)
+                if (jj == j && sh[jj] != INFINITY) v = __dmul_rn(__dsub_rn(m, sh[jj]), sc[jj]);
+            v = warp_max_d(v);                               // fmax: NaN values drop out
+            if (lane == 0 && !isnan(v)) atomicMax(out + (int64_t)j * n_boot + b, ordered(v));
+        }
+    }
+}
+
+__global__ void spa_fill_kernel(unsigned long long* __restrict__ out, int64_t n) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) out[i] = ordered(-INFINITY);
+}
+
+__global__ void spa_decode_kernel(unsigned long long* __restrict__ out, int64_t n) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) reinterpret_cast<double*>(out)[i] = unordered(out[i]);
+}
+
+static int spa_check(const double* d, int64_t ld, int N, int T, const char* fn) {
+    B200BT_REQUIRE(d, B200BT_EINVAL, "%s: null pointer", fn);
+    B200BT_REQUIRE(N >= 1, B200BT_EINVAL, "%s: need at least 1 trial (N = %d)", fn, N);
+    B200BT_REQUIRE(T >= 2, B200BT_EINVAL, "%s: need at least 2 days (T = %d)", fn, T);
+    B200BT_REQUIRE(T <= SPA_MAX_T, B200BT_ELIMIT, "%s: at most %d days (T = %d)", fn, SPA_MAX_T, T);
+    B200BT_REQUIRE(ld >= T, B200BT_EINVAL, "%s: row stride %lld below T = %d", fn, (long long)ld, T);
+    return B200BT_OK;
+}
+
 }  // namespace b200bt
 
 using namespace b200bt;
@@ -413,4 +600,63 @@ extern "C" int b200bt_cscv(const double* pnl, int64_t ld, int N, int64_t T, int 
         case 18: return cscv_passes<18>(A, st);
         default: return cscv_passes<20>(A, st);
     }
+}
+
+extern "C" int b200bt_spa_moments(const double* d, int64_t ld, int N, int T, double q, double* mean, double* omega2,
+                                  b200bt_stream_t stream) {
+    B200BT_REQUIRE(mean && omega2, B200BT_EINVAL, "spa_moments: null pointer");
+    int rc = spa_check(d, ld, N, T, "spa_moments");
+    if (rc) return rc;
+    B200BT_REQUIRE(q > 0.0 && q <= 1.0, B200BT_EINVAL, "spa_moments: q = %g outside (0, 1]", q);
+    rc = check_device();
+    if (rc) return rc;
+    const size_t smem = (size_t)(3 * T + 1) * sizeof(double);
+    rc = cuda_status(cudaFuncSetAttribute(spa_moments_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),
+                     "spa_moments: cudaFuncSetAttribute");
+    if (rc) return rc;
+    spa_moments_kernel<<<(unsigned)N, SPA_MOM_THREADS, smem, (cudaStream_t)stream>>>(d, ld, T, q, mean, omega2);
+    B200BT_LAUNCH_CHECK("spa_moments");
+    return B200BT_OK;
+}
+
+extern "C" int b200bt_spa_bootstrap(const double* d, int64_t ld, int N, int T, uint64_t q32, int64_t n_boot, uint64_t seed,
+                                    uint64_t boot_offset, int n_stats, const double* shift, const double* scale, double* out,
+                                    b200bt_stream_t stream) {
+    B200BT_REQUIRE(shift && scale && out, B200BT_EINVAL, "spa_bootstrap: null pointer");
+    int rc = spa_check(d, ld, N, T, "spa_bootstrap");
+    if (rc) return rc;
+    B200BT_REQUIRE(q32 >= 1 && q32 <= (1ull << 32), B200BT_EINVAL, "spa_bootstrap: q32 = %llu outside [1, 2^32]",
+                   (unsigned long long)q32);
+    B200BT_REQUIRE(n_boot >= 1, B200BT_EINVAL, "spa_bootstrap: n_boot = %lld", (long long)n_boot);
+    B200BT_REQUIRE(n_stats >= 1, B200BT_EINVAL, "spa_bootstrap: n_stats = %d", n_stats);
+    B200BT_REQUIRE(n_stats <= SPA_MAX_STATS, B200BT_ELIMIT, "spa_bootstrap: at most %d statistics (n_stats = %d)",
+                   SPA_MAX_STATS, n_stats);
+    B200BT_REQUIRE(n_boot <= (INT64_MAX >> 3) / n_stats, B200BT_ELIMIT, "spa_bootstrap: n_stats * n_boot too large");
+    rc = check_device();
+    if (rc) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    const int64_t n_out = (int64_t)n_stats * n_boot;
+    unsigned long long* o = reinterpret_cast<unsigned long long*>(out);
+    spa_fill_kernel<<<(unsigned)((n_out + 255) / 256), 256, 0, st>>>(o, n_out);
+    B200BT_LAUNCH_CHECK("spa_bootstrap fill");
+    const int64_t tiles = ((int64_t)N + SPA_TILE - 1) / SPA_TILE;
+    const int64_t want = (8 * (int64_t)device_sm_count() + tiles - 1) / tiles;
+    const int64_t ny = std::max<int64_t>(1, std::min<int64_t>({want, (n_boot + SPA_WARPS - 1) / SPA_WARPS, 65535}));
+    const int64_t per_cta = (n_boot + ny - 1) / ny;
+    const dim3 grid((unsigned)tiles, (unsigned)((n_boot + per_cta - 1) / per_cta));
+    if (T <= SPA_STAGE_T) {
+        const size_t smem = (size_t)SPA_TILE * T * sizeof(double);
+        rc = cuda_status(cudaFuncSetAttribute(spa_bootstrap_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                              (int)smem), "spa_bootstrap: cudaFuncSetAttribute");
+        if (rc) return rc;
+        spa_bootstrap_kernel<true><<<grid, SPA_WARPS * 32, smem, st>>>(d, ld, N, T, q32, n_boot, per_cta, seed, boot_offset,
+                                                                       n_stats, shift, scale, o);
+    } else {
+        spa_bootstrap_kernel<false><<<grid, SPA_WARPS * 32, 0, st>>>(d, ld, N, T, q32, n_boot, per_cta, seed, boot_offset,
+                                                                     n_stats, shift, scale, o);
+    }
+    B200BT_LAUNCH_CHECK("spa_bootstrap");
+    spa_decode_kernel<<<(unsigned)((n_out + 255) / 256), 256, 0, st>>>(o, n_out);
+    B200BT_LAUNCH_CHECK("spa_bootstrap decode");
+    return B200BT_OK;
 }

@@ -1,6 +1,6 @@
 """Backtest overfitting of a searched population: how much of the best backtest's performance is the search itself.
 
-Host side of `b200bt_cscv` (include/b200bt.h):
+Host side of `b200bt_cscv`, `b200bt_spa_moments` and `b200bt_spa_bootstrap` (include/b200bt.h):
 
 * `cscv(pnl, n_blocks)` -- the Probability of Backtest Overfitting by combinatorially symmetric cross-validation
   (Bailey, Borwein, Lopez de Prado, Zhu 2015, "The Probability of Backtest Overfitting").  The kernel gives, for every
@@ -8,8 +8,11 @@ Host side of `b200bt_cscv` (include/b200bt.h):
   Sharpe; the relative rank, its logit and the summary statistics are formed here.
 * `deflated_sharpe(moments, n_trials)` -- the Deflated Sharpe Ratio (Bailey, Lopez de Prado 2014, "The Deflated Sharpe
   Ratio"): the probability that a trial's true Sharpe exceeds the expected maximum of `n_trials` unskilled trials.
+* `spa(rows, benchmark)` -- the data-snooping tests of the best of N trials against a benchmark on the stationary
+  bootstrap: White's Reality Check, Hansen's SPA and Romano and Wolf's StepM.
 
-The per-day rows come from `PopulationSweep.daily_pnl`; StrategyEvaluationSystem.backtest_overfitting chains the two.
+The per-day rows come from `PopulationSweep.daily_pnl`; StrategyEvaluationSystem.backtest_overfitting chains them with
+CSCV and the deflated Sharpe ratio, StrategyEvaluationSystem.data_snooping with `spa`.
 """
 from __future__ import annotations
 
@@ -112,3 +115,141 @@ def deflated_sharpe(moments: Dict, n_trials: int, n_days: Optional[int] = None) 
     for i in np.nonzero(ok & (den > 0))[0]:
         out[i] = 0.5 * math.erfc(-float(z[i]) / math.sqrt(2.0))
     return out
+
+
+SPA_MAX_OUT_BYTES = 1 << 28
+
+
+def spa_q32(block_len: float) -> int:
+    """round(2^32 / block_len) in [1, 2^32]: the restart threshold of the stationary bootstrap's index stream."""
+    if not (block_len >= 1.0 and math.isfinite(block_len)):
+        raise ValueError(f"spa: block_len = {block_len} must be a finite number >= 1")
+    return min(1 << 32, max(1, round(2.0 ** 32 / float(block_len))))
+
+
+def spa_shifts(mean: np.ndarray, omega: np.ndarray, n_days: int):
+    """(shift, scale) rows [4][N] of the first bootstrap launch: Reality Check (shift mean, scale sqrt(T)), then SPA
+    lower / consistent / upper (shifts max(mean, 0), mean * 1{mean > -omega sqrt(2 ln ln T / T)}, mean; scale
+    sqrt(T) / omega).  Trials without a positive variance estimate (omega NaN) are excluded from SPA (shift +inf)."""
+    rt = math.sqrt(n_days)
+    ok = np.isfinite(omega)
+    thr = math.sqrt(max(0.0, 2.0 * math.log(math.log(n_days)) / n_days)) if n_days > 2 else 0.0
+    with np.errstate(invalid="ignore", divide="ignore"):
+        scale_t = np.where(ok, rt / omega, 0.0)
+        consistent = np.where(mean > -omega * thr, mean, 0.0)
+    shift = np.stack([mean, np.maximum(mean, 0.0), consistent, mean])
+    shift[1:, ~ok] = np.inf
+    scale = np.stack([np.full(len(mean), rt), scale_t, scale_t, scale_t])
+    return shift, scale
+
+
+def spa_summary(mean: np.ndarray, omega: np.ndarray, n_days: int, out: np.ndarray, stepm_rows, alpha: float) -> Dict:
+    """Statistics and p-values from the bootstrap maxima.  out: [4][B], the rows of spa_shifts; stepm_rows(active)
+    returns the [B] maxima of (m* - mean) * sqrt(T) / omega over the boolean mask `active` (a further launch); the first
+    StepM step reads the SPA-upper row instead."""
+    B = out.shape[1]
+    rt = math.sqrt(n_days)
+    ok = np.isfinite(omega)
+    with np.errstate(invalid="ignore", divide="ignore"):
+        t_stat = np.where(ok, rt * mean / omega, np.nan)
+    V = float(np.max(rt * mean))
+    rc = dict(stat=V, pvalue=float(np.count_nonzero(out[0] > V)) / B)
+    if ok.any():
+        t_spa = max(0.0, float(np.max(t_stat[ok])))
+        p = [float(np.count_nonzero(np.maximum(0.0, out[j]) > t_spa)) / B for j in (1, 2, 3)]
+    else:
+        t_spa, p = math.nan, [math.nan] * 3
+    spa = dict(stat=t_spa, pvalue_lower=p[0], pvalue_consistent=p[1], pvalue_upper=p[2])
+    rejected = np.zeros(len(mean), dtype=bool)
+    crit = []
+    rank = max(1, math.ceil((1.0 - alpha) * B))
+    active = ok.copy()
+    row = out[3]
+    while active.any():
+        c = float(np.sort(row)[rank - 1])
+        crit.append(c)
+        new = active & (t_stat > c)
+        if not new.any():
+            break
+        rejected |= new
+        active &= ~new
+        if not active.any():
+            break
+        row = stepm_rows(active)
+    best = None
+    if ok.any():
+        i = int(np.argmax(np.where(ok, t_stat, -np.inf)))
+        best = dict(index=i, t_stat=float(t_stat[i]), mean=float(mean[i]))
+    return dict(t_stat=t_stat, reality_check=rc, spa=spa,
+                stepm=dict(alpha=alpha, rejected=rejected, critical_values=crit), best=best)
+
+
+def spa(rows: torch.Tensor, benchmark: Optional[torch.Tensor] = None, n_boot: int = 10_000, block_len: float = 10.0,
+        alpha: float = 0.05, seed: int = 0, max_out_bytes: int = SPA_MAX_OUT_BYTES) -> Dict:
+    """Data-snooping tests of the N trials in the rows of `rows` (device float64 [N][T], one per-period PnL per column,
+    the same periods for every trial) against `benchmark` (a device [T] row; None: flat, zero PnL): is the best trial
+    better than the benchmark once the search over N trials is accounted for?
+
+    On the differentials d = rows - benchmark, with the stationary bootstrap of mean block length `block_len`
+    (q = 1 / block_len) and `n_boot` resamples (b200bt_spa_moments, b200bt_spa_bootstrap; include/b200bt.h):
+      mean, omega (Hansen's stationary-bootstrap standard deviation, NaN where omega^2 <= 0), t_stat = sqrt(T) mean /
+      omega (NaN likewise) per trial;
+      reality_check {stat, pvalue}: White's V = max sqrt(T) mean, p = #{b: V*_b > V} / B;
+      spa {stat, pvalue_lower, pvalue_consistent, pvalue_upper}: Hansen's T = max(0, max t), p = #{b: T*_b > T} / B
+        with T*_b = max(0, max_k (m* - g(mean)) sqrt(T) / omega) for the three recentrings g (NaN with no eligible trial);
+      stepm {alpha, rejected [N], critical_values}: Romano and Wolf's studentized StepM at level alpha: each step's
+        critical value is the ceil((1 - alpha) B)-th smallest bootstrap maximum over the active (not yet rejected,
+        eligible) trials; the active trials with t > c are rejected, until a step rejects nothing;
+      best {index, t_stat, mean}: the trial of highest t_stat (the first on ties; None with no eligible trial);
+      n_trials, n_days, n_boot, block_len, seed.
+    Trials with omega^2 <= 0 (a never-trading row against a flat benchmark) take no part in SPA and StepM.  The
+    resamples are split over launches by their global index when the [4][n_boot] maxima exceed `max_out_bytes`; the
+    result does not depend on the split."""
+    if not (isinstance(rows, torch.Tensor) and rows.is_cuda and rows.dtype == torch.float64 and rows.dim() == 2):
+        raise ValueError("spa needs a device float64 matrix [N][T]")
+    N, T = int(rows.shape[0]), int(rows.shape[1])
+    B = int(n_boot)
+    if N < 1 or B < 1 or not 0.0 < alpha < 1.0:
+        raise ValueError(f"spa: N = {N} trials, n_boot = {B} and alpha = {alpha} need N >= 1, n_boot >= 1, 0 < alpha < 1")
+    q32 = spa_q32(block_len)
+    if benchmark is not None:
+        if not (isinstance(benchmark, torch.Tensor) and benchmark.device == rows.device and benchmark.numel() == T):
+            raise ValueError(f"spa: the benchmark must be a [{T}] row on {rows.device}")
+        d = rows - benchmark.reshape(1, T).to(torch.float64)
+    else:
+        d = rows if rows.stride(1) == 1 else rows.contiguous()
+    if not bool(torch.isfinite(d).all()):
+        raise ValueError("spa: the rows hold NaN or inf (lost records? sweep again with a larger event cap)")
+    dev = d.device
+    per_launch = max(1, int(max_out_bytes) // (4 * 8))
+    mean_d = torch.empty(N, dtype=torch.float64, device=dev)
+    omega2_d = torch.empty(N, dtype=torch.float64, device=dev)
+    with torch.cuda.device(dev):
+        st = _lib.current_stream()
+        _lib.call("b200bt_spa_moments", d.data_ptr(), _lib.ld(d), N, T, q32 / 2.0 ** 32, mean_d.data_ptr(),
+                  omega2_d.data_ptr(), st)
+        mean, omega2 = mean_d.cpu().numpy(), omega2_d.cpu().numpy()
+        omega = np.where(omega2 > 0, np.sqrt(np.where(omega2 > 0, omega2, 1.0)), np.nan)
+
+        def maxima(shift: np.ndarray, scale: np.ndarray) -> np.ndarray:
+            n_stats = shift.shape[0]
+            sh = torch.from_numpy(np.ascontiguousarray(shift)).to(dev)
+            sc = torch.from_numpy(np.ascontiguousarray(scale)).to(dev)
+            res = np.empty((n_stats, B))
+            for lo in range(0, B, per_launch):
+                n = min(per_launch, B - lo)
+                out = torch.empty((n_stats, n), dtype=torch.float64, device=dev)
+                _lib.call("b200bt_spa_bootstrap", d.data_ptr(), _lib.ld(d), N, T, q32, n, seed, lo, n_stats,
+                          sh.data_ptr(), sc.data_ptr(), out.data_ptr(), st)
+                res[:, lo:lo + n] = out.cpu().numpy()
+            return res
+
+        shift, scale = spa_shifts(mean, omega, T)
+        out = maxima(shift, scale)
+
+        def stepm_rows(active: np.ndarray) -> np.ndarray:
+            return maxima(np.where(active, mean, np.inf)[None], scale[1:2])[0]
+
+        res = spa_summary(mean, omega, T, out, stepm_rows, alpha)
+    res.update(mean=mean, omega=omega, n_trials=N, n_days=T, n_boot=B, block_len=float(block_len), seed=int(seed))
+    return res

@@ -490,3 +490,34 @@ class StrategyEvaluationSystem:
         except Exception as e:        # reference convention: log, return an empty result
             logger.error("Error measuring the backtest overfitting of a population: %s", e)
             return {}
+
+    def data_snooping(self, population: List[Dict], market: MarketData, benchmark: Optional[Dict] = None,
+                      n_boot: int = 10_000, block_len: float = 10.0, alpha: float = 0.05, seed: int = 0,
+                      sweep: Optional[PopulationSweep] = None) -> Dict:
+        """Is the best of `population` really better than `benchmark` once the search over the population is accounted
+        for?  White's Reality Check, Hansen's SPA and Romano and Wolf's StepM (overfitting.spa) on the per-day PnL of
+        every individual's book (PopulationSweep.daily_pnl), against the book row of `benchmark` -- the incumbent
+        strategy's parameter dict, swept on the same calendar -- or a flat, zero PnL when it is None.  The trials are the
+        distinct decoded individuals.
+
+        Returns spa()'s result with the per-trial arrays mean, omega, t_stat and stepm.rejected expanded to `population`
+        order, best.index an index into `population` (the first individual of the best trial), and first_day.  Errors:
+        logged, {} returned (the reference's convention)."""
+        from .overfitting import spa
+        try:
+            sweep = sweep or PopulationSweep(market, optimization_goals=self.optimization_goals)
+            _, unique, expand = sweep._unique(population)
+            book, _, first_day = sweep.daily_pnl(unique)
+            bench = None if benchmark is None else sweep.daily_pnl([benchmark])[0][0]
+            res = spa(book, bench, n_boot=n_boot, block_len=block_len, alpha=alpha, seed=seed)
+            idx = np.arange(len(population)) if expand is None else np.asarray(expand)
+            for k in ("mean", "omega", "t_stat"):
+                res[k] = res[k][idx]
+            res["stepm"]["rejected"] = res["stepm"]["rejected"][idx]
+            if res["best"] is not None:
+                res["best"]["index"] = int(np.flatnonzero(idx == res["best"]["index"])[0])
+            res["first_day"] = first_day
+            return res
+        except Exception as e:        # reference convention: log, return an empty result
+            logger.error("Error testing a population for data snooping: %s", e)
+            return {}

@@ -564,6 +564,44 @@ int b200bt_cscv(const double* pnl, int64_t ld, int N, int64_t T, int B, void* wo
                 int32_t* sel, double* is_sr, double* oos_sr, int32_t* n_below, int32_t* n_tied, double* mu, double* m2,
                 double* m3, double* m4, double* sr, b200bt_stream_t stream);
 
+/* Data-snooping tests of N trials against one benchmark: White's Reality Check (2000), Hansen's Superior Predictive
+ * Ability test (2005) and Romano and Wolf's StepM (2005), on the stationary bootstrap of Politis and Romano (1994).
+ * d: device float64 [N][ld >= T] of differentials d[k][t] = x[k][t] - bench[t] (the host forms them); rows finite.
+ * Arithmetic as b200bt_cscv: correctly rounded float64, no FMA contraction, sums in ascending order from +0.0.
+ * Limits: 2 <= T <= 8192 (ELIMIT above, EINVAL below), 1 <= N < 2^31, ld >= T (EINVAL).
+ *
+ * b200bt_spa_moments, per trial k, with 0 < q <= 1 (EINVAL otherwise):
+ *   mean[k] = (sum_t d_t) / T;  c_t = d_t - mean;  gamma_i = (sum_{t=0}^{T-1-i} c_t * c_{t+i}) / T
+ *   p_0 = 1, p_i = p_{i-1} * (1 - q)  (running products, i = 1..T)
+ *   kappa_i = ((T - i) / T) * p_i + (i / T) * p_{T-i}
+ *   omega2[k] = gamma_0 + 2 * sum_{i=1}^{T-1} kappa_i * gamma_i   (Hansen's stationary-bootstrap variance)
+ * mean and omega2 are exact restatements of these expressions.  Against kappa_i formed with pow((1-q), i) instead, the
+ * running product p_i differs by at most i half-ulps (relative i * 2^-53), so omega2 agrees with such a restatement
+ * within T * 2^-52 * (|gamma_0| + 2 sum |kappa_i gamma_i|) plus the rounding of the sums.  O(N T^2): one CTA per trial,
+ * (3T + 1) * 8 bytes of shared memory.
+ *
+ * b200bt_spa_bootstrap: resample b = 0 .. n_boot - 1 draws the index sequence theta_b(0..T-1), forms
+ *   m*[k][b] = (sum_t d[k][theta_b(t)]) / T   (t ascending; the N x n_boot matrix is never stored)
+ * and writes out[j][b] = max over k of (m*[k][b] - shift[j][k]) * scale[j][k] for j < n_stats, 1 <= n_stats <= 8
+ * (ELIMIT above, EINVAL at 0).  shift[j][k] = +inf excludes trial k from statistic j; NaN values are ignored; a
+ * statistic with every trial excluded is -inf.  shift, scale: device float64 [n_stats][N]; out: device float64
+ * [n_stats][n_boot].  The max does not depend on the order, so the output is deterministic.
+ * Index stream: Philox4x32-10, key = seed, counter = (gid lo, gid hi, t >> 1, 0) with gid = boot_offset + b; day t uses
+ * words x[2(t & 1)] (restart) and x[2(t & 1) + 1] (start).  Day 0 starts a block; day t >= 1 starts one iff
+ * (uint64)x_restart < q32.  A block start is __umulhi(x_start, T); otherwise theta(t) = theta(t-1) + 1, wrapping at T.
+ * q32 in [1, 2^32] (EINVAL outside): round(q * 2^32) for a mean block length 1 / q; 2^32 gives the iid bootstrap.  A
+ * resample is a pure function of (seed, gid, T, q32): it does not depend on N, on the other trials, on how the
+ * resamples are split over calls (boot_offset) or on the launch geometry.  n_boot >= 1.
+ * Schedule: one CTA per (32-trial tile, resample range), one warp per resample, one lane per trial; a warp draws 64 days
+ * at a time (one Philox block per lane, a max-scan for the latest block start).  Rows of T <= 768 days are staged in
+ * shared memory as [t][32] (32 * T * 8 bytes); longer rows are read through L1 / L2.  The tiles' maxima meet in an
+ * ordered-integer atomicMax over out (three launches: fill, bootstrap, decode). */
+int b200bt_spa_moments(const double* d, int64_t ld, int N, int T, double q, double* mean, double* omega2,
+                       b200bt_stream_t stream);
+int b200bt_spa_bootstrap(const double* d, int64_t ld, int N, int T, uint64_t q32, int64_t n_boot, uint64_t seed,
+                         uint64_t boot_offset, int n_stats, const double* shift, const double* scale, double* out,
+                         b200bt_stream_t stream);
+
 /* ---- portfolio risk (SURVEY 8-f4) -------------------------------------------------------------------
  * Replaces the numeric core of services/portfolio_risk_service.py. */
 

@@ -20,7 +20,7 @@ from ai_crypto_trader_b200.sweep import MarketData, PopulationSweep
 from oracle import indicators_ref, sim_oracle
 
 legs = sys.argv[1:] or ["sweep", "mc", "joint", "indicators", "pareto", "regime", "dca", "grid_service", "rl",
-                        "volume_profile", "market_monitor"]
+                        "volume_profile", "market_monitor", "spa"]
 torch.cuda.set_device(0)
 
 if "sweep" in legs:
@@ -223,3 +223,18 @@ if "market_monitor" in legs:
         assert np.array_equal(table["valid"][0], want), W
         assert np.array_equal(labels.cpu().numpy(), np.where(table["valid"] == 1, table["drsi_signal"], 255)), W
     print("market_monitor ok: rows and labels equal the restatement", flush=True)
+if "spa" in legs:
+    # data snooping: moments, the staged and the L2 bootstrap schedules, a partial trial tile, StepM steps and chunked
+    # resamples; the Reality Check and the StepM set checked against the exact restatement
+    sys.path.insert(0, str(Path(__file__).resolve().parents[1] / "tests"))
+    import spa_ref
+    from ai_crypto_trader_b200.overfitting import spa
+    rng = np.random.default_rng(6)
+    for N, T in ((45, 120), (3, 900)):
+        x = rng.normal(0.0, 1.0, (N, T))
+        x[:2] += 0.5
+        got = spa(torch.from_numpy(x).cuda(), n_boot=70, block_len=4.0, seed=2, max_out_bytes=4 * 8 * 32)
+        want = spa_ref.spa_exact(x, 70, 4.0, 0.05, 2)
+        assert got["reality_check"] == want["reality_check"] and np.array_equal(got["stepm"]["rejected"],
+                                                                                want["stepm"]["rejected"]), (N, T)
+    print("spa ok: p-values and StepM sets equal the restatement", flush=True)
