@@ -337,6 +337,15 @@ _SIGNATURES = {
     "b200bt_spa_moments": (C.c_int, [_vp, _i64, _i, _i, C.c_double, _vp, _vp, _vp]),
     "b200bt_spa_bootstrap": (C.c_int, [_vp, _i64, _i, _i, C.c_uint64, _i64, C.c_uint64, C.c_uint64, _i, _vp, _vp, _vp,
                                        _vp]),
+    "b200bt_boot_means": (C.c_int, [_vp, _i64, _i, _i, C.c_uint64, _i64, C.c_uint64, C.c_uint64, _vp, _vp, _i64, _i64,
+                                    _vp]),
+    "b200bt_autocov": (C.c_int, [_vp, _i64, _i, _i, _i, _vp, _vp, _vp]),
+    "b200bt_mcs_pairwise": (C.c_int, [_vp, _i64, _i, _i64, _vp, _i64, _vp]),
+    "b200bt_mcs_range_stats": (C.c_int, [_vp, _i, _i64, _vp, _vp, _i64, _vp]),
+    "b200bt_mcs_range_order": (C.c_int, [_vp, _vp, _i, _vp, _vp, _vp, _i64, _vp]),
+    "b200bt_mcs_range_boot": (C.c_int, [_vp, _i64, _i, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _vp]),
+    "b200bt_mcs_max_workspace_bytes": (C.c_int64, [_i, _i64]),
+    "b200bt_mcs_max": (C.c_int, [_vp, _i64, _i, _i64, _vp, _vp, _i64, _vp, _vp, _vp, _i64, _vp]),
     "b200bt_regime_max_windows": (C.c_int64, [_i64, _i]),
     "b200bt_regime_labels": (C.c_int, [_vp, _vp, _vp, _vp, _i, _i64, _i64, _i64, _i, C.POINTER(RegimeParams), _vp, _i64,
                                        _vp, _i64, _vp]),

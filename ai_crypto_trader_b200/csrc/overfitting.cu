@@ -419,9 +419,45 @@ __device__ __forceinline__ unsigned spa_window(uint32_t k0, uint32_t k1, uint32_
     return (unsigned)(th0 & 0xffff) | (unsigned)(th1 & 0xffff) << 16;
 }
 
+// m* of one resample for the lane's trial: (sum_t row[theta(t)]) / T in ascending t.  The warp walks the resample's
+// index stream 64 days at a time (spa_window) and every lane gathers its own row: from the tile's [t][32] shared-memory
+// stage xs (STAGED; every lane of the warp reads the same day, so no bank conflicts) or through L1/L2 from `row`.
+// Called by the SPA maxima and the MCS bootstrap means, so both see the same m*.
+template <bool STAGED>
+__device__ __forceinline__ double spa_gather_mean(const double* __restrict__ xs, const double* __restrict__ row,
+                                                  uint32_t key0, uint32_t key1, uint64_t gid, int T, uint64_t q32) {
+    const int lane = threadIdx.x & 31;
+    const int windows = (T + 63) / 64;
+    int carry = 0;
+    double acc = 0.0;
+    for (int w = 0; w < windows; ++w) {
+        const unsigned packed = spa_window(key0, key1, (uint32_t)gid, (uint32_t)(gid >> 32), w, T, q32, carry);
+        const int nd = min(64, T - 64 * w);
+#pragma unroll 4
+        for (int pr = 0; pr < 32; ++pr) {
+            if (2 * pr >= nd) break;
+            const unsigned v = __shfl_sync(FULL, packed, pr);
+            const int a = (int)(v & 0xffffu), e = (int)(v >> 16);
+            acc = __dadd_rn(acc, STAGED ? xs[a * SPA_TILE + lane] : __ldg(row + a));
+            if (2 * pr + 1 < nd) acc = __dadd_rn(acc, STAGED ? xs[e * SPA_TILE + lane] : __ldg(row + e));
+        }
+    }
+    return __ddiv_rn(acc, (double)T);
+}
+
+// Stage trials [k0, k0 + 32) of d as [t][32] in shared memory (zeros past N).
+__device__ __forceinline__ void spa_stage_tile(double* __restrict__ xs, const double* __restrict__ d, int64_t ld, int N,
+                                               int T, int64_t k0) {
+    for (int i = threadIdx.x; i < SPA_TILE * T; i += blockDim.x) {
+        const int j = i & (SPA_TILE - 1), t = i / SPA_TILE;
+        xs[i] = k0 + j < N ? d[(k0 + j) * ld + t] : 0.0;
+    }
+    __syncthreads();
+}
+
 // One CTA: trials [32 * blockIdx.x, +32) x resamples [b_lo, b_hi) of this CTA's range; warp v walks resamples b_lo + v,
-// b_lo + v + SPA_WARPS, ...  STAGED: the tile's rows sit in shared memory as [t][32] (one 256-byte row per day, read
-// without bank conflicts since every lane of a warp reads the same day); otherwise each lane reads its row through L1/L2.
+// b_lo + v + SPA_WARPS, ...  STAGED: the tile's rows sit in shared memory as [t][32]; otherwise each lane reads its row
+// through L1/L2.
 template <bool STAGED>
 __global__ void __launch_bounds__(SPA_WARPS * 32)
 spa_bootstrap_kernel(const double* __restrict__ d, int64_t ld, int N, int T, uint64_t q32, int64_t n_boot, int64_t per_cta,
@@ -432,13 +468,7 @@ spa_bootstrap_kernel(const double* __restrict__ d, int64_t ld, int N, int T, uin
     const int64_t k0 = (int64_t)blockIdx.x * SPA_TILE;
     const int64_t k = k0 + lane;
     const bool valid = k < N;
-    if (STAGED) {
-        for (int i = threadIdx.x; i < SPA_TILE * T; i += blockDim.x) {
-            const int j = i & (SPA_TILE - 1), t = i / SPA_TILE;
-            xs[i] = k0 + j < N ? d[(k0 + j) * ld + t] : 0.0;
-        }
-        __syncthreads();
-    }
+    if (STAGED) spa_stage_tile(xs, d, ld, N, T, k0);
     const double* row = d + (valid ? k : (int64_t)N - 1) * ld;
     double sh[SPA_MAX_STATS], sc[SPA_MAX_STATS];
 #pragma unroll
@@ -447,26 +477,9 @@ spa_bootstrap_kernel(const double* __restrict__ d, int64_t ld, int N, int T, uin
         sc[j] = valid && j < n_stats ? scale[(int64_t)j * N + k] : 0.0;
     }
     const uint32_t key0 = (uint32_t)seed, key1 = (uint32_t)(seed >> 32);
-    const int windows = (T + 63) / 64;
-    const double nt = (double)T;
     const int64_t b_lo = (int64_t)blockIdx.y * per_cta, b_hi = min(n_boot, b_lo + per_cta);
     for (int64_t b = b_lo + warp; b < b_hi; b += SPA_WARPS) {
-        const uint64_t gid = boot_offset + (uint64_t)b;
-        int carry = 0;
-        double acc = 0.0;
-        for (int w = 0; w < windows; ++w) {
-            const unsigned packed = spa_window(key0, key1, (uint32_t)gid, (uint32_t)(gid >> 32), w, T, q32, carry);
-            const int nd = min(64, T - 64 * w);
-#pragma unroll 4
-            for (int pr = 0; pr < 32; ++pr) {
-                if (2 * pr >= nd) break;
-                const unsigned v = __shfl_sync(FULL, packed, pr);
-                const int a = (int)(v & 0xffffu), e = (int)(v >> 16);
-                acc = __dadd_rn(acc, STAGED ? xs[a * SPA_TILE + lane] : __ldg(row + a));
-                if (2 * pr + 1 < nd) acc = __dadd_rn(acc, STAGED ? xs[e * SPA_TILE + lane] : __ldg(row + e));
-            }
-        }
-        const double m = __ddiv_rn(acc, nt);
+        const double m = spa_gather_mean<STAGED>(xs, row, key0, key1, boot_offset + (uint64_t)b, T, q32);
         for (int j = 0; j < n_stats; ++j) {
             double v = -INFINITY;
 #pragma unroll
@@ -496,6 +509,470 @@ static int spa_check(const double* d, int64_t ld, int N, int T, const char* fn) 
     B200BT_REQUIRE(ld >= T, B200BT_EINVAL, "%s: row stride %lld below T = %d", fn, (long long)ld, T);
     return B200BT_OK;
 }
+
+// ---- model confidence set ---------------------------------------------------------------------------------------------
+constexpr int MCS_MAX_N = 16384;
+constexpr int MCS_TILE = 64;                 // pairwise and range-maxima tiles: 64 x 64 cells, 4 x 4 per thread
+constexpr int MCS_CHUNK = 16;                // resamples (pairwise) or columns (range maxima) staged per step
+constexpr int MCS_THREADS = 256;
+constexpr int MCS_ORDER_THREADS = 1024;
+
+// Bootstrap means: spa_bootstrap_kernel's schedule, writing m* (minus center[k] when given) at out[b][k].
+template <bool STAGED>
+__global__ void __launch_bounds__(SPA_WARPS * 32)
+boot_means_kernel(const double* __restrict__ d, int64_t ld, int N, int T, uint64_t q32, int64_t n_boot, int64_t per_cta,
+                  uint64_t seed, uint64_t boot_offset, const double* __restrict__ center, double* __restrict__ out,
+                  int64_t ld_out) {
+    extern __shared__ double xs[];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int64_t k0 = (int64_t)blockIdx.x * SPA_TILE;
+    const int64_t k = k0 + lane;
+    const bool valid = k < N;
+    if (STAGED) spa_stage_tile(xs, d, ld, N, T, k0);
+    const double* row = d + (valid ? k : (int64_t)N - 1) * ld;
+    const double c = center && valid ? center[k] : 0.0;
+    const uint32_t key0 = (uint32_t)seed, key1 = (uint32_t)(seed >> 32);
+    const int64_t b_lo = (int64_t)blockIdx.y * per_cta, b_hi = min(n_boot, b_lo + per_cta);
+    for (int64_t b = b_lo + warp; b < b_hi; b += SPA_WARPS) {
+        const double m = spa_gather_mean<STAGED>(xs, row, key0, key1, boot_offset + (uint64_t)b, T, q32);
+        if (valid) out[b * ld_out + k] = center ? __dsub_rn(m, c) : m;
+    }
+}
+
+// Autocovariances of row blockIdx.x: spa_moments_kernel's mean and gamma_i for i = 0..K.
+__global__ void __launch_bounds__(SPA_MOM_THREADS)
+autocov_kernel(const double* __restrict__ d, int64_t ld, int T, int K, double* __restrict__ out,
+               double* __restrict__ mean_out) {
+    extern __shared__ double c[];
+    __shared__ double mean_s;
+    const double* x = d + (int64_t)blockIdx.x * ld;
+    for (int t = threadIdx.x; t < T; t += blockDim.x) c[t] = x[t];
+    __syncthreads();
+    const double nt = (double)T;
+    if (threadIdx.x == 0) {
+        double s = 0.0;
+        for (int t = 0; t < T; ++t) s = __dadd_rn(s, c[t]);
+        mean_s = __ddiv_rn(s, nt);
+    }
+    __syncthreads();
+    const double mu = mean_s;
+    for (int t = threadIdx.x; t < T; t += blockDim.x) c[t] = __dsub_rn(c[t], mu);
+    __syncthreads();
+    for (int i = threadIdx.x; i <= K; i += blockDim.x) {
+        double s = 0.0;
+        for (int t = 0; t + i < T; ++t) s = __dadd_rn(s, __dmul_rn(c[t], c[t + i]));
+        out[(int64_t)blockIdx.x * (K + 1) + i] = __ddiv_rn(s, nt);
+    }
+    if (mean_out && threadIdx.x == 0) mean_out[blockIdx.x] = mu;
+}
+
+// Pairwise pass: s2[i][j] += sum over this launch's resamples b (ascending) of (z[b][j] - z[b][i])^2, for i < j only.
+// One CTA per upper-triangle (i-tile, j-tile) pair; MCS_CHUNK resample rows of both tiles are staged in shared memory
+// and each thread keeps a 4 x 4 register tile of accumulators (rows ty + 16a, columns tx + 16c).
+__global__ void __launch_bounds__(MCS_THREADS, 1)
+mcs_pairwise_kernel(const double* __restrict__ z, int64_t ld_z, int N, int64_t n_boot, int tiles,
+                    double* __restrict__ s2) {
+    __shared__ double zi[MCS_CHUNK][MCS_TILE], zj[MCS_CHUNK][MCS_TILE];
+    int p = blockIdx.x, ti = 0;                   // upper-triangle pair p -> (ti, tj), tj >= ti
+    while (p >= tiles - ti) { p -= tiles - ti; ++ti; }
+    const int tj = ti + p;
+    const int i0 = ti * MCS_TILE, j0 = tj * MCS_TILE;
+    const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+    double acc[4][4];
+#pragma unroll
+    for (int a = 0; a < 4; ++a)
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+            const int i = i0 + ty + 16 * a, j = j0 + tx + 16 * c;
+            acc[a][c] = (i < j && j < N) ? s2[(int64_t)i * N + j] : 0.0;
+        }
+    for (int64_t b0 = 0; b0 < n_boot; b0 += MCS_CHUNK) {
+        const int nb = (int)min((int64_t)MCS_CHUNK, n_boot - b0);
+        for (int e = threadIdx.x; e < MCS_CHUNK * MCS_TILE; e += MCS_THREADS) {
+            const int r = e / MCS_TILE, col = e % MCS_TILE;
+            const bool in = r < nb;
+            const double* zr = z + (b0 + r) * ld_z;
+            zi[r][col] = in && i0 + col < N ? zr[i0 + col] : 0.0;
+            zj[r][col] = in && j0 + col < N ? zr[j0 + col] : 0.0;
+        }
+        __syncthreads();
+        for (int r = 0; r < nb; ++r) {
+            double a4[4], c4[4];
+#pragma unroll
+            for (int a = 0; a < 4; ++a) a4[a] = zi[r][ty + 16 * a];
+#pragma unroll
+            for (int c = 0; c < 4; ++c) c4[c] = zj[r][tx + 16 * c];
+#pragma unroll
+            for (int a = 0; a < 4; ++a)
+#pragma unroll
+                for (int c = 0; c < 4; ++c) {
+                    const double df = __dsub_rn(c4[c], a4[a]);
+                    acc[a][c] = __dadd_rn(acc[a][c], __dmul_rn(df, df));
+                }
+        }
+        __syncthreads();
+    }
+#pragma unroll
+    for (int a = 0; a < 4; ++a)
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+            const int i = i0 + ty + 16 * a, j = j0 + tx + 16 * c;
+            if (i < j && j < N) s2[(int64_t)i * N + j] = acc[a][c];
+        }
+}
+
+// t for a mean difference dm over a standard deviation s, with the zero-variance rule.
+__device__ __forceinline__ double mcs_t(double dm, double s) {
+    if (s > 0.0) return __ddiv_rn(dm, s);
+    return dm == 0.0 ? 0.0 : (dm > 0.0 ? INFINITY : -INFINITY);
+}
+
+// w: s2 (upper triangle) in, rho out (symmetric, zero diagonal); t[i][j] = (mean_j - mean_i) / sigma_ij.
+__global__ void mcs_range_stats_kernel(const double* __restrict__ mean, int N, double nb, double* __restrict__ w,
+                                       double* __restrict__ t) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= (int64_t)N * N) return;
+    const int i = (int)(e / N), j = (int)(e - (int64_t)i * N);
+    if (i == j) {
+        w[e] = 0.0;
+        t[e] = 0.0;
+    }
+    if (i >= j) return;
+    const double sigma = __dsqrt_rn(__ddiv_rn(w[e], nb));
+    const double rho = sigma > 0.0 ? __ddiv_rn(1.0, sigma) : 0.0;
+    w[e] = rho;
+    w[(int64_t)j * N + i] = rho;
+    t[e] = mcs_t(__dsub_rn(mean[j], mean[i]), sigma);
+    t[(int64_t)j * N + i] = mcs_t(__dsub_rn(mean[i], mean[j]), sigma);
+}
+
+__device__ __forceinline__ bool mcs_better(double v, int i, double bv, int bi) { return v > bv || (v == bv && i < bi); }
+
+// Warp-wide (max, lowest index) of row i of t over the live columns.
+__device__ __forceinline__ void mcs_row_max(const double* __restrict__ t, int N, int i, const unsigned char* alive,
+                                            double& v, int& col) {
+    const int lane = threadIdx.x & 31;
+    v = -INFINITY;
+    col = 0x7fffffff;
+    const double* row = t + (int64_t)i * N;
+    for (int j = lane; j < N; j += 32)
+        if (alive[j] && mcs_better(row[j], j, v, col)) { v = row[j]; col = j; }
+#pragma unroll
+    for (int m = 16; m > 0; m >>= 1) {
+        const double ov = shfl_xor_d(v, m);
+        const int oc = __shfl_xor_sync(FULL, col, m);
+        if (mcs_better(ov, oc, v, col)) { v = ov; col = oc; }
+    }
+}
+
+// T_R elimination order in one CTA: each live row keeps its max over the live columns and that column; after e leaves,
+// only the rows whose column was e are rescanned (a warp per row).  Shared memory: rm [N] doubles, col [N] ints,
+// alive [N] bytes.
+__global__ void __launch_bounds__(MCS_ORDER_THREADS)
+mcs_range_order_kernel(const double* __restrict__ t, int N, int32_t* __restrict__ order, double* __restrict__ stat) {
+    extern __shared__ double rm[];
+    int* col = reinterpret_cast<int*>(rm + N);
+    unsigned char* alive = reinterpret_cast<unsigned char*>(col + N);
+    __shared__ double red_v[MCS_ORDER_THREADS / 32];
+    __shared__ int red_i[MCS_ORDER_THREADS / 32];
+    __shared__ int e_s;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, warps = MCS_ORDER_THREADS / 32;
+    for (int i = threadIdx.x; i < N; i += blockDim.x) alive[i] = 1;
+    __syncthreads();
+    for (int i = warp; i < N; i += warps) {
+        double v;
+        int c;
+        mcs_row_max(t, N, i, alive, v, c);
+        if (lane == 0) { rm[i] = v; col[i] = c; }
+    }
+    __syncthreads();
+    for (int k = 0; k + 1 < N; ++k) {
+        double v = -INFINITY;
+        int bi = 0x7fffffff;
+        for (int i = threadIdx.x; i < N; i += blockDim.x)
+            if (alive[i] && mcs_better(rm[i], i, v, bi)) { v = rm[i]; bi = i; }
+#pragma unroll
+        for (int m = 16; m > 0; m >>= 1) {
+            const double ov = shfl_xor_d(v, m);
+            const int oi = __shfl_xor_sync(FULL, bi, m);
+            if (mcs_better(ov, oi, v, bi)) { v = ov; bi = oi; }
+        }
+        if (lane == 0) { red_v[warp] = v; red_i[warp] = bi; }
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            for (int w = 1; w < warps; ++w)
+                if (mcs_better(red_v[w], red_i[w], v, bi)) { v = red_v[w]; bi = red_i[w]; }
+            order[k] = bi;
+            stat[k] = v;
+            alive[bi] = 0;
+            e_s = bi;
+        }
+        __syncthreads();
+        const int e = e_s;
+        for (int i = warp; i < N; i += warps)
+            if (alive[i] && col[i] == e) {
+                double rv;
+                int c;
+                mcs_row_max(t, N, i, alive, rv, c);
+                if (lane == 0) { rm[i] = rv; col[i] = c; }
+            }
+        __syncthreads();
+    }
+    for (int i = threadIdx.x; i < N; i += blockDim.x)
+        if (alive[i]) order[N - 1] = i;
+}
+
+// rho in elimination-rank order, strictly upper triangular: out[r][c] = rho[order[r]][order[c]] for c > r, else 0.
+__global__ void mcs_rank_rho_kernel(const double* __restrict__ rho, const int32_t* __restrict__ order, int N,
+                                   double* __restrict__ out) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= (int64_t)N * N) return;
+    const int r = (int)(e / N), c = (int)(e - (int64_t)r * N);
+    out[e] = c > r ? rho[(int64_t)order[r] * N + order[c]] : 0.0;
+}
+
+// Range maxima: R[b][r] = max over c of |z[b][order[c]] - z[b][order[r]]| * rho_rank[r][c] (0 below the diagonal), for
+// a 64-resample x 64-rank tile per CTA (4 x 4 per thread), columns staged MCS_CHUNK at a time; column chunks wholly at
+// or below the tile's first rank are skipped.
+__global__ void __launch_bounds__(MCS_THREADS, 1)
+mcs_range_boot_kernel(const double* __restrict__ z, int64_t ld_z, int N, int64_t n_boot, const int32_t* __restrict__ order,
+                      const double* __restrict__ rho_rank, double* __restrict__ R) {
+    __shared__ double zc[MCS_TILE][MCS_CHUNK + 1], pc[MCS_TILE][MCS_CHUNK + 1];
+    const int64_t b0 = (int64_t)blockIdx.y * MCS_TILE;
+    const int r0 = blockIdx.x * MCS_TILE;
+    const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;     // ranks r0 + tx + 16c, resamples b0 + ty + 16a
+    double own[4][4], mx[4][4];
+#pragma unroll
+    for (int a = 0; a < 4; ++a)
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+            const int64_t b = b0 + ty + 16 * a;
+            const int r = r0 + tx + 16 * c;
+            own[a][c] = b < n_boot && r < N ? z[b * ld_z + order[r]] : 0.0;
+            mx[a][c] = 0.0;
+        }
+    for (int c0 = (r0 / MCS_CHUNK) * MCS_CHUNK; c0 < N; c0 += MCS_CHUNK) {
+        for (int e = threadIdx.x; e < MCS_TILE * MCS_CHUNK; e += MCS_THREADS) {
+            const int row = e / MCS_CHUNK, cc = e % MCS_CHUNK, cg = c0 + cc;
+            const int64_t b = b0 + row;
+            zc[row][cc] = b < n_boot && cg < N ? z[b * ld_z + order[cg]] : 0.0;
+            pc[row][cc] = r0 + row < N && cg < N ? rho_rank[(int64_t)(r0 + row) * N + cg] : 0.0;
+        }
+        __syncthreads();
+#pragma unroll 4
+        for (int cc = 0; cc < MCS_CHUNK; ++cc) {
+            double zb[4], pr[4];
+#pragma unroll
+            for (int a = 0; a < 4; ++a) zb[a] = zc[ty + 16 * a][cc];
+#pragma unroll
+            for (int c = 0; c < 4; ++c) pr[c] = pc[tx + 16 * c][cc];
+#pragma unroll
+            for (int a = 0; a < 4; ++a)
+#pragma unroll
+                for (int c = 0; c < 4; ++c)
+                    mx[a][c] = fmax(mx[a][c], __dmul_rn(fabs(__dsub_rn(zb[a], own[a][c])), pr[c]));
+        }
+        __syncthreads();
+    }
+#pragma unroll
+    for (int a = 0; a < 4; ++a)
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+            const int64_t b = b0 + ty + 16 * a;
+            const int r = r0 + tx + 16 * c;
+            if (b < n_boot && r < N) R[b * N + r] = mx[a][c];
+        }
+}
+
+// count[k] += #{b : max over r >= k of R[b][r] >= stat[k]}, k = 0..N-2: a warp per resample walks the ranks from the top
+// 32 at a time with a suffix-max scan; counts gather in shared memory (N ints) and go out once per CTA.
+__global__ void __launch_bounds__(MCS_THREADS)
+mcs_range_count_kernel(const double* __restrict__ R, int N, int64_t n_boot, const double* __restrict__ stat,
+                       unsigned long long* __restrict__ count) {
+    extern __shared__ int cnt[];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, warps = MCS_THREADS / 32;
+    for (int k = threadIdx.x; k < N; k += blockDim.x) cnt[k] = 0;
+    __syncthreads();
+    for (int64_t b = (int64_t)blockIdx.x * warps + warp; b < n_boot; b += (int64_t)gridDim.x * warps) {
+        const double* row = R + b * N;
+        double carry = 0.0;
+        for (int top = N; top > 0; top -= 32) {
+            const int r = top - 32 + lane;
+            double v = r >= 0 ? row[r] : 0.0;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const double u = __shfl_down_sync(FULL, v, o);
+                if (lane + o < 32) v = fmax(v, u);
+            }
+            v = fmax(v, carry);
+            carry = __shfl_sync(FULL, v, 0);
+            if (r >= 0 && r + 1 < N && v >= stat[r]) atomicAdd(&cnt[r], 1);
+        }
+    }
+    __syncthreads();
+    for (int k = threadIdx.x; k + 1 < N; k += blockDim.x)
+        if (cnt[k]) atomicAdd(count + k, (unsigned long long)cnt[k]);
+}
+
+// ---- T_max step loop.  Workspace: zbar [B] doubles, s [N] doubles, tv [N] doubles, xbar_M (1 double), two [N] int lists
+// of the live models in ascending index, the eliminated model (1 int).
+struct McsMaxWs {
+    double *zbar, *s, *tv, *xm;
+    int *list0, *list1, *e;
+};
+
+__host__ __device__ inline int64_t mcs_max_ws_layout(int N, int64_t B, McsMaxWs* w, char* base) {
+    const int64_t zb = 0, s = zb + 8 * B, tv = s + 8 * (int64_t)N, xm = tv + 8 * (int64_t)N, l0 = xm + 8,
+                  l1 = l0 + 4 * (int64_t)N, e = l1 + 4 * (int64_t)N, end = e + 4;
+    if (w) {
+        w->zbar = (double*)(base + zb);
+        w->s = (double*)(base + s);
+        w->tv = (double*)(base + tv);
+        w->xm = (double*)(base + xm);
+        w->list0 = (int*)(base + l0);
+        w->list1 = (int*)(base + l1);
+        w->e = (int*)(base + e);
+    }
+    return end;
+}
+
+// list = 0..N-1, xbar_M = (sum of mean ascending) / N.
+__global__ void mcs_max_init_kernel(const double* __restrict__ mean, int N, McsMaxWs w) {
+    for (int i = threadIdx.x; i < N; i += blockDim.x) w.list0[i] = i;
+    if (threadIdx.x == 0) {
+        double s = 0.0;
+        for (int i = 0; i < N; ++i) s = __dadd_rn(s, mean[i]);
+        *w.xm = __ddiv_rn(s, (double)N);
+        *w.e = -1;
+    }
+}
+
+// One thread per resample over the m live models `list` (ascending).  With `stat` (step k): T*_b(M_k) = max over i of
+// (zbar_b - z_bi) / s_i (0 where s_i = 0), counted into *count when >= *stat.  Then zbar_b of the set without *e (all
+// of `list` when *e < 0): the sum of z_bj over the kept j, ascending, over their number.
+constexpr int MCS_ROWS_THREADS = 64;         // T_max passes: small CTAs, so that B = 10^4 resamples or ~10^3 models
+constexpr int MCS_VAR_THREADS = 32;          // spread over every SM rather than a few
+
+__global__ void __launch_bounds__(MCS_ROWS_THREADS)
+mcs_max_rows_kernel(const double* __restrict__ z, int64_t ld_z, int64_t n_boot, const int* __restrict__ list, int m,
+                    McsMaxWs w, const double* __restrict__ stat, unsigned long long* __restrict__ count) {
+    __shared__ int red[MCS_ROWS_THREADS / 32];
+    const int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int e = *w.e;
+    bool hit = false;
+    if (b < n_boot) {
+        const double* row = z + b * ld_z;
+        const double zb = w.zbar[b];
+        double acc = 0.0, mx = -INFINITY;
+        for (int p = 0; p < m; ++p) {
+            const int j = list[p];
+            const double v = row[j];
+            if (stat) {
+                const double sj = w.s[j];
+                mx = fmax(mx, sj > 0.0 ? __ddiv_rn(__dsub_rn(zb, v), sj) : 0.0);
+            }
+            if (j != e) acc = __dadd_rn(acc, v);
+        }
+        w.zbar[b] = __ddiv_rn(acc, (double)(e >= 0 ? m - 1 : m));
+        hit = stat && mx >= *stat;
+    }
+    if (!stat) return;
+    const unsigned bal = __ballot_sync(FULL, hit);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = __popc(bal);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int s = 0;
+        for (int v = 0; v < MCS_ROWS_THREADS / 32; ++v) s += red[v];
+        if (s) atomicAdd(count, (unsigned long long)s);
+    }
+}
+
+// One thread per live model i = list[p]: v_i = (sum over b ascending of (zbar_b - z_bi)^2) / B, s_i = sqrt(v_i),
+// t_i = (xbar_M - mean_i) / s_i with the zero-variance rule.
+__global__ void __launch_bounds__(MCS_VAR_THREADS)
+mcs_max_var_kernel(const double* __restrict__ z, int64_t ld_z, int64_t n_boot, const int* __restrict__ list, int m,
+                   const double* __restrict__ mean, McsMaxWs w) {
+    const int p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= m) return;
+    const int i = list[p];
+    double acc = 0.0;
+#pragma unroll 8
+    for (int64_t b = 0; b < n_boot; ++b) {
+        const double df = __dsub_rn(w.zbar[b], z[b * ld_z + i]);
+        acc = __dadd_rn(acc, __dmul_rn(df, df));
+    }
+    const double s = __dsqrt_rn(__ddiv_rn(acc, (double)n_boot));
+    w.s[i] = s;
+    w.tv[i] = mcs_t(__dsub_rn(*w.xm, mean[i]), s);
+}
+
+// Step k in one CTA: e = argmax of t over `list` (lowest index on ties), order[k], stat[k]; `next` = list without e;
+// xbar_M of `next`.
+__global__ void __launch_bounds__(MCS_ORDER_THREADS)
+mcs_max_step_kernel(const int* __restrict__ list, int m, const double* __restrict__ mean, McsMaxWs w, int k,
+                    int* __restrict__ next, int32_t* __restrict__ order, double* __restrict__ stat) {
+    __shared__ double red_v[MCS_ORDER_THREADS / 32];
+    __shared__ int red_i[MCS_ORDER_THREADS / 32];
+    __shared__ int e_s;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    double v = -INFINITY;
+    int bi = 0x7fffffff;
+    for (int p = threadIdx.x; p < m; p += blockDim.x) {
+        const int i = list[p];
+        if (mcs_better(w.tv[i], i, v, bi)) { v = w.tv[i]; bi = i; }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const double ov = shfl_xor_d(v, o);
+        const int oi = __shfl_xor_sync(FULL, bi, o);
+        if (mcs_better(ov, oi, v, bi)) { v = ov; bi = oi; }
+    }
+    if (lane == 0) { red_v[warp] = v; red_i[warp] = bi; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        for (int u = 1; u < MCS_ORDER_THREADS / 32; ++u)
+            if (mcs_better(red_v[u], red_i[u], v, bi)) { v = red_v[u]; bi = red_i[u]; }
+        order[k] = bi;
+        stat[k] = v;
+        *w.e = bi;
+        e_s = bi;
+    }
+    __syncthreads();
+    const int e = e_s;
+    for (int p = threadIdx.x; p < m; p += blockDim.x) {
+        const int i = list[p];
+        if (i < e) next[p] = i;
+        else if (i > e) next[p - 1] = i;
+    }
+    if (threadIdx.x == 0) {
+        double s = 0.0;
+        for (int p = 0; p < m; ++p)
+            if (list[p] != e) s = __dadd_rn(s, mean[list[p]]);
+        *w.xm = __ddiv_rn(s, (double)(m - 1));
+        if (m == 2) order[k + 1] = list[0] == e ? list[1] : list[0];
+    }
+}
+
+static int mcs_check_n(int N, const char* fn) {
+    B200BT_REQUIRE(N >= 2, B200BT_EINVAL, "%s: need at least 2 models (N = %d)", fn, N);
+    B200BT_REQUIRE(N <= MCS_MAX_N, B200BT_ELIMIT, "%s: at most %d models (N = %d)", fn, MCS_MAX_N, N);
+    return B200BT_OK;
+}
+
+static int mcs_check_budget(int64_t need_or_neg, int64_t max_bytes, const char* fn) {
+    B200BT_REQUIRE(need_or_neg >= 0 && need_or_neg <= max_bytes, B200BT_ELIMIT,
+                   "%s: %lld bytes of [B][N] / [N][N] buffers exceed the budget of %lld", fn, (long long)need_or_neg,
+                   (long long)max_bytes);
+    return B200BT_OK;
+}
+
+// a * b * 8 bytes, or -1 when it does not fit int64
+static int64_t mcs_bytes(int64_t a, int64_t b) {
+    if (a < 0 || b < 0 || (b > 0 && a > (INT64_MAX / 8) / b)) return -1;
+    return a * b * 8;
+}
+
+static int64_t mcs_sum(int64_t a, int64_t b) { return a < 0 || b < 0 || a > INT64_MAX - b ? -1 : a + b; }
 
 }  // namespace b200bt
 
@@ -658,5 +1135,193 @@ extern "C" int b200bt_spa_bootstrap(const double* d, int64_t ld, int N, int T, u
     B200BT_LAUNCH_CHECK("spa_bootstrap");
     spa_decode_kernel<<<(unsigned)((n_out + 255) / 256), 256, 0, st>>>(o, n_out);
     B200BT_LAUNCH_CHECK("spa_bootstrap decode");
+    return B200BT_OK;
+}
+
+extern "C" int b200bt_boot_means(const double* d, int64_t ld, int N, int T, uint64_t q32, int64_t n_boot, uint64_t seed,
+                                 uint64_t boot_offset, const double* center_or_null, double* out, int64_t ld_out,
+                                 int64_t max_bytes, b200bt_stream_t stream) {
+    B200BT_REQUIRE(out, B200BT_EINVAL, "boot_means: null pointer");
+    int rc = spa_check(d, ld, N, T, "boot_means");
+    if (rc) return rc;
+    B200BT_REQUIRE(N <= MCS_MAX_N, B200BT_ELIMIT, "boot_means: at most %d trials (N = %d)", MCS_MAX_N, N);
+    B200BT_REQUIRE(q32 >= 1 && q32 <= (1ull << 32), B200BT_EINVAL, "boot_means: q32 = %llu outside [1, 2^32]",
+                   (unsigned long long)q32);
+    B200BT_REQUIRE(n_boot >= 1, B200BT_EINVAL, "boot_means: n_boot = %lld", (long long)n_boot);
+    B200BT_REQUIRE(ld_out >= N, B200BT_EINVAL, "boot_means: ld_out = %lld below N = %d", (long long)ld_out, N);
+    rc = mcs_check_budget(mcs_bytes(n_boot, ld_out), max_bytes, "boot_means");
+    if (rc) return rc;
+    rc = check_device();
+    if (rc) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    const int64_t tiles = ((int64_t)N + SPA_TILE - 1) / SPA_TILE;
+    const int64_t want = (8 * (int64_t)device_sm_count() + tiles - 1) / tiles;
+    const int64_t ny = std::max<int64_t>(1, std::min<int64_t>({want, (n_boot + SPA_WARPS - 1) / SPA_WARPS, 65535}));
+    const int64_t per_cta = (n_boot + ny - 1) / ny;
+    const dim3 grid((unsigned)tiles, (unsigned)((n_boot + per_cta - 1) / per_cta));
+    if (T <= SPA_STAGE_T) {
+        const size_t smem = (size_t)SPA_TILE * T * sizeof(double);
+        rc = cuda_status(cudaFuncSetAttribute(boot_means_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                              (int)smem), "boot_means: cudaFuncSetAttribute");
+        if (rc) return rc;
+        boot_means_kernel<true><<<grid, SPA_WARPS * 32, smem, st>>>(d, ld, N, T, q32, n_boot, per_cta, seed, boot_offset,
+                                                                    center_or_null, out, ld_out);
+    } else {
+        boot_means_kernel<false><<<grid, SPA_WARPS * 32, 0, st>>>(d, ld, N, T, q32, n_boot, per_cta, seed, boot_offset,
+                                                                  center_or_null, out, ld_out);
+    }
+    B200BT_LAUNCH_CHECK("boot_means");
+    return B200BT_OK;
+}
+
+extern "C" int b200bt_autocov(const double* d, int64_t ld, int N, int T, int K, double* out, double* mean_or_null,
+                              b200bt_stream_t stream) {
+    B200BT_REQUIRE(out, B200BT_EINVAL, "autocov: null pointer");
+    int rc = spa_check(d, ld, N, T, "autocov");
+    if (rc) return rc;
+    B200BT_REQUIRE(K >= 0 && K < T, B200BT_EINVAL, "autocov: lags 0..K need 0 <= K < T (K = %d, T = %d)", K, T);
+    rc = check_device();
+    if (rc) return rc;
+    const size_t smem = (size_t)T * sizeof(double);
+    rc = cuda_status(cudaFuncSetAttribute(autocov_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),
+                     "autocov: cudaFuncSetAttribute");
+    if (rc) return rc;
+    autocov_kernel<<<(unsigned)N, SPA_MOM_THREADS, smem, (cudaStream_t)stream>>>(d, ld, T, K, out, mean_or_null);
+    B200BT_LAUNCH_CHECK("autocov");
+    return B200BT_OK;
+}
+
+extern "C" int b200bt_mcs_pairwise(const double* zeta, int64_t ld_z, int N, int64_t n_boot, double* s2,
+                                   int64_t max_bytes, b200bt_stream_t stream) {
+    B200BT_REQUIRE(zeta && s2, B200BT_EINVAL, "mcs_pairwise: null pointer");
+    int rc = mcs_check_n(N, "mcs_pairwise");
+    if (rc) return rc;
+    B200BT_REQUIRE(n_boot >= 1, B200BT_EINVAL, "mcs_pairwise: n_boot = %lld", (long long)n_boot);
+    B200BT_REQUIRE(ld_z >= N, B200BT_EINVAL, "mcs_pairwise: ld_z = %lld below N = %d", (long long)ld_z, N);
+    rc = mcs_check_budget(mcs_sum(mcs_bytes(n_boot, ld_z), mcs_bytes(N, N)), max_bytes, "mcs_pairwise");
+    if (rc) return rc;
+    rc = check_device();
+    if (rc) return rc;
+    const int tiles = (N + MCS_TILE - 1) / MCS_TILE;
+    mcs_pairwise_kernel<<<(unsigned)(tiles * (tiles + 1) / 2), MCS_THREADS, 0, (cudaStream_t)stream>>>(zeta, ld_z, N,
+                                                                                                      n_boot, tiles, s2);
+    B200BT_LAUNCH_CHECK("mcs_pairwise");
+    return B200BT_OK;
+}
+
+extern "C" int b200bt_mcs_range_stats(const double* mean, int N, int64_t n_boot_total, double* w, double* t,
+                                      int64_t max_bytes, b200bt_stream_t stream) {
+    B200BT_REQUIRE(mean && w && t, B200BT_EINVAL, "mcs_range_stats: null pointer");
+    int rc = mcs_check_n(N, "mcs_range_stats");
+    if (rc) return rc;
+    B200BT_REQUIRE(n_boot_total >= 1, B200BT_EINVAL, "mcs_range_stats: n_boot_total = %lld", (long long)n_boot_total);
+    rc = mcs_check_budget(mcs_bytes(2 * (int64_t)N, N), max_bytes, "mcs_range_stats");
+    if (rc) return rc;
+    rc = check_device();
+    if (rc) return rc;
+    const int64_t n = (int64_t)N * N;
+    mcs_range_stats_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(mean, N, (double)n_boot_total,
+                                                                                        w, t);
+    B200BT_LAUNCH_CHECK("mcs_range_stats");
+    return B200BT_OK;
+}
+
+extern "C" int b200bt_mcs_range_order(const double* t, const double* rho, int N, int32_t* order, double* stat,
+                                      double* rho_rank, int64_t max_bytes, b200bt_stream_t stream) {
+    B200BT_REQUIRE(t && rho && order && stat && rho_rank, B200BT_EINVAL, "mcs_range_order: null pointer");
+    int rc = mcs_check_n(N, "mcs_range_order");
+    if (rc) return rc;
+    B200BT_REQUIRE(rho_rank != rho, B200BT_EINVAL, "mcs_range_order: rho_rank may alias t but not rho");
+    rc = mcs_check_budget(mcs_bytes((rho_rank == t ? 2 : 3) * (int64_t)N, N), max_bytes, "mcs_range_order");
+    if (rc) return rc;
+    rc = check_device();
+    if (rc) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t smem = (size_t)N * 13;
+    rc = cuda_status(cudaFuncSetAttribute(mcs_range_order_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),
+                     "mcs_range_order: cudaFuncSetAttribute");
+    if (rc) return rc;
+    mcs_range_order_kernel<<<1, MCS_ORDER_THREADS, smem, st>>>(t, N, order, stat);
+    B200BT_LAUNCH_CHECK("mcs_range_order");
+    const int64_t n = (int64_t)N * N;
+    mcs_rank_rho_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(rho, order, N, rho_rank);
+    B200BT_LAUNCH_CHECK("mcs_range_order rank rho");
+    return B200BT_OK;
+}
+
+extern "C" int b200bt_mcs_range_boot(const double* zeta, int64_t ld_z, int N, int64_t n_boot, const int32_t* order,
+                                     const double* rho_rank, const double* stat, double* rmax, uint64_t* count,
+                                     int64_t max_bytes, b200bt_stream_t stream) {
+    B200BT_REQUIRE(zeta && order && rho_rank && stat && rmax && count, B200BT_EINVAL, "mcs_range_boot: null pointer");
+    int rc = mcs_check_n(N, "mcs_range_boot");
+    if (rc) return rc;
+    B200BT_REQUIRE(n_boot >= 1, B200BT_EINVAL, "mcs_range_boot: n_boot = %lld", (long long)n_boot);
+    B200BT_REQUIRE(ld_z >= N, B200BT_EINVAL, "mcs_range_boot: ld_z = %lld below N = %d", (long long)ld_z, N);
+    rc = mcs_check_budget(mcs_sum(mcs_sum(mcs_bytes(n_boot, ld_z), mcs_bytes(n_boot, N)), mcs_bytes(N, N)), max_bytes,
+                          "mcs_range_boot");
+    if (rc) return rc;
+    rc = check_device();
+    if (rc) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    const int64_t slab = (int64_t)65535 * MCS_TILE;           // resamples per launch (grid.y)
+    for (int64_t lo = 0; lo < n_boot; lo += slab) {
+        const int64_t nb = std::min(slab, n_boot - lo);
+        const dim3 grid((unsigned)((N + MCS_TILE - 1) / MCS_TILE), (unsigned)((nb + MCS_TILE - 1) / MCS_TILE));
+        mcs_range_boot_kernel<<<grid, MCS_THREADS, 0, st>>>(zeta + lo * ld_z, ld_z, N, nb, order, rho_rank, rmax + lo * N);
+        B200BT_LAUNCH_CHECK("mcs_range_boot");
+    }
+    const size_t smem = (size_t)N * sizeof(int);
+    rc = cuda_status(cudaFuncSetAttribute(mcs_range_count_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),
+                     "mcs_range_boot: cudaFuncSetAttribute");
+    if (rc) return rc;
+    const int64_t ctas = std::min<int64_t>(2 * (int64_t)device_sm_count(), (n_boot + 7) / 8);
+    mcs_range_count_kernel<<<(unsigned)ctas, MCS_THREADS, smem, st>>>(rmax, N, n_boot, stat,
+                                                                     reinterpret_cast<unsigned long long*>(count));
+    B200BT_LAUNCH_CHECK("mcs_range_boot count");
+    return B200BT_OK;
+}
+
+extern "C" int64_t b200bt_mcs_max_workspace_bytes(int N, int64_t n_boot) {
+    if (N < 2 || N > MCS_MAX_N || n_boot < 1 || n_boot > (INT64_MAX >> 4)) return 0;
+    return mcs_max_ws_layout(N, n_boot, nullptr, nullptr);
+}
+
+extern "C" int b200bt_mcs_max(const double* zeta, int64_t ld_z, int N, int64_t n_boot, const double* mean, void* workspace,
+                              int64_t workspace_bytes, int32_t* order, double* stat, uint64_t* count, int64_t max_bytes,
+                              b200bt_stream_t stream) {
+    B200BT_REQUIRE(zeta && mean && workspace && order && stat && count, B200BT_EINVAL, "mcs_max: null pointer");
+    int rc = mcs_check_n(N, "mcs_max");
+    if (rc) return rc;
+    B200BT_REQUIRE(n_boot >= 1, B200BT_EINVAL, "mcs_max: n_boot = %lld", (long long)n_boot);
+    B200BT_REQUIRE(ld_z >= N, B200BT_EINVAL, "mcs_max: ld_z = %lld below N = %d", (long long)ld_z, N);
+    rc = mcs_check_budget(mcs_bytes(n_boot, ld_z), max_bytes, "mcs_max");
+    if (rc) return rc;
+    const int64_t need = b200bt_mcs_max_workspace_bytes(N, n_boot);
+    B200BT_REQUIRE(workspace_bytes >= need, B200BT_EINVAL, "mcs_max: workspace too small (%lld < %lld)",
+                   (long long)workspace_bytes, (long long)need);
+    B200BT_REQUIRE(((uintptr_t)workspace & 15) == 0, B200BT_EINVAL, "mcs_max: workspace must be 16-byte aligned");
+    rc = check_device();
+    if (rc) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    McsMaxWs w;
+    mcs_max_ws_layout(N, n_boot, &w, (char*)workspace);
+    unsigned long long* cnt = reinterpret_cast<unsigned long long*>(count);
+    const unsigned rows_grid = (unsigned)((n_boot + MCS_ROWS_THREADS - 1) / MCS_ROWS_THREADS);
+    mcs_max_init_kernel<<<1, 1024, 0, st>>>(mean, N, w);
+    B200BT_LAUNCH_CHECK("mcs_max init");
+    mcs_max_rows_kernel<<<rows_grid, MCS_ROWS_THREADS, 0, st>>>(zeta, ld_z, n_boot, w.list0, N, w, nullptr, nullptr);
+    B200BT_LAUNCH_CHECK("mcs_max rows");
+    for (int k = 0; k + 1 < N; ++k) {
+        const int m = N - k;
+        int* cur = (k & 1) ? w.list1 : w.list0;
+        int* nxt = (k & 1) ? w.list0 : w.list1;
+        mcs_max_var_kernel<<<(unsigned)((m + MCS_VAR_THREADS - 1) / MCS_VAR_THREADS), MCS_VAR_THREADS, 0, st>>>(
+            zeta, ld_z, n_boot, cur, m, mean, w);
+        B200BT_LAUNCH_CHECK("mcs_max var");
+        mcs_max_step_kernel<<<1, MCS_ORDER_THREADS, 0, st>>>(cur, m, mean, w, k, nxt, order, stat);
+        B200BT_LAUNCH_CHECK("mcs_max step");
+        mcs_max_rows_kernel<<<rows_grid, MCS_ROWS_THREADS, 0, st>>>(zeta, ld_z, n_boot, cur, m, w, stat + k, cnt + k);
+        B200BT_LAUNCH_CHECK("mcs_max rows");
+    }
     return B200BT_OK;
 }

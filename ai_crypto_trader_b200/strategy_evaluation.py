@@ -492,7 +492,7 @@ class StrategyEvaluationSystem:
             return {}
 
     def data_snooping(self, population: List[Dict], market: MarketData, benchmark: Optional[Dict] = None,
-                      n_boot: int = 10_000, block_len: float = 10.0, alpha: float = 0.05, seed: int = 0,
+                      n_boot: int = 10_000, block_len=10.0, alpha: float = 0.05, seed: int = 0,
                       sweep: Optional[PopulationSweep] = None) -> Dict:
         """Is the best of `population` really better than `benchmark` once the search over the population is accounted
         for?  White's Reality Check, Hansen's SPA and Romano and Wolf's StepM (overfitting.spa) on the per-day PnL of
@@ -520,4 +520,36 @@ class StrategyEvaluationSystem:
             return res
         except Exception as e:        # reference convention: log, return an empty result
             logger.error("Error testing a population for data snooping: %s", e)
+            return {}
+
+    def model_confidence_set(self, population: List[Dict], market: MarketData, incumbent: Optional[Dict] = None,
+                             alpha: float = 0.10, statistic: str = "R", n_boot: int = 10_000, block_len=10.0,
+                             seed: int = 0, sweep: Optional[PopulationSweep] = None) -> Dict:
+        """Which individuals of `population` cannot be told apart from the best?  Hansen, Lunde and Nason's Model
+        Confidence Set (overfitting.mcs) at level `alpha` on the per-day PnL of every individual's book
+        (PopulationSweep.daily_pnl).  The models are the distinct decoded individuals; `incumbent`, the running
+        strategy's parameter dict, is swept on the same calendar and added as one more model.
+
+        Returns mcs()'s result with p_values, included, mean and model_of expanded to `population` order; its rows are
+        the distinct individuals, then the incumbent (row n_trials - 1), and elimination_order indexes them.  Rows with
+        the same book, such as individuals whose differing genes never change a trade, are one model and share one
+        p-value.  Also first_day, and incumbent {p_value, included}: is the running strategy still among the best?
+        Errors: logged, {} returned (the reference's convention)."""
+        from .overfitting import mcs
+        try:
+            sweep = sweep or PopulationSweep(market, optimization_goals=self.optimization_goals)
+            _, unique, expand = sweep._unique(population)
+            book, _, first_day = sweep.daily_pnl(unique)
+            if incumbent is not None:
+                book = torch.cat([book, sweep.daily_pnl([incumbent])[0]], dim=0)
+            res = mcs(book, alpha=alpha, statistic=statistic, n_boot=n_boot, block_len=block_len, seed=seed)
+            idx = np.arange(len(population)) if expand is None else np.asarray(expand)
+            if incumbent is not None:
+                res["incumbent"] = dict(p_value=float(res["p_values"][-1]), included=bool(res["included"][-1]))
+            for k in ("p_values", "included", "mean", "model_of"):
+                res[k] = res[k][idx]
+            res["first_day"] = first_day
+            return res
+        except Exception as e:        # reference convention: log, return an empty result
+            logger.error("Error computing the model confidence set of a population: %s", e)
             return {}

@@ -602,6 +602,84 @@ int b200bt_spa_bootstrap(const double* d, int64_t ld, int N, int T, uint64_t q32
                          uint64_t boot_offset, int n_stats, const double* shift, const double* scale, double* out,
                          b200bt_stream_t stream);
 
+/* Model Confidence Set (Hansen, Lunde and Nason 2011) of N models on the stationary bootstrap of b200bt_spa_bootstrap.
+ * x: device float64 [N][ld >= T], one per-day PnL row per model, finite.  The loss is the negated PnL, so the best model
+ * has the highest mean.  Arithmetic as b200bt_spa_*: correctly rounded float64, no FMA contraction, every sum in the
+ * ascending order stated from +0.0; every max is order-free.  So a NumPy restatement with the same loops matches bit for
+ * bit, whatever the launch geometry or the split of the resamples over calls.
+ *   xbar_k = (sum_t x[k][t]) / T                        (t ascending; b200bt_spa_moments' mean)
+ *   m*[b][k] = (sum_t x[k][theta_b(t)]) / T              (t ascending; theta_b the index stream of b200bt_spa_bootstrap
+ *                                                         for the same seed, gid = boot_offset + b, T and q32)
+ *   zeta[b][k] = m*[b][k] - xbar_k                       (stored resample-major, [B][ld_z >= N])
+ * T_R: sigma2_ij = (sum_b (zeta_bj - zeta_bi)^2) / B    (b ascending over all B resamples, 0 .. B-1)
+ *      sigma_ij = sqrt(sigma2_ij), rho_ij = 1.0 / sigma_ij (a correctly rounded division, not a reciprocal
+ *      approximation), t_ij = (xbar_j - xbar_i) / sigma_ij
+ *      T_R(M) = max over i, j in M of t_ij; e_R(M) = argmax over i in M of (max over j in M of t_ij), lowest index on ties
+ *      T*_R,b(M) = max over i, j in M of |zeta_bj - zeta_bi| * rho_ij
+ * T_max: zbar_b(M) = (sum over j in M, ascending j, of zeta_bj) / m     (m = |M|)
+ *      v_i(M) = (sum_b (zbar_b - zeta_bi)^2) / B (b ascending); s_i = sqrt(v_i)
+ *      xbar_M = (sum over j in M, ascending j, of xbar_j) / m; t_i = (xbar_M - xbar_i) / s_i
+ *      T_max(M) = max over i in M of t_i; e_max(M) = the argmax, lowest index on ties
+ *      T*_b(M) = max over i in M of (zbar_b - zeta_bi) / s_i
+ * Zero variance (sigma_ij = 0 or s_i = 0, whether the squares underflowed or not): t = 0 when the means are equal (the
+ * difference is +-0), +inf or -inf with the sign of the difference otherwise; the pair or model adds 0 to every
+ * bootstrap maximum (rho_ij = 0; the T_max term is 0).
+ * Copies: these entries take the models as given.  Under T_R exact copies tie (t = 0, rho = 0) but leave one step
+ * apart.  Under T_max a set's mean can differ from the copies' common value by rounding, so a step over copies of a
+ * non-zero row compares rounding residues and can remove some copies at p = 0 while others stay.  Pass distinct rows:
+ * overfitting.mcs makes byte-identical rows one model before it calls these entries.
+ * Elimination: M_0 = all N models; step k = 0 .. N-2 removes e_k from M_k.  count[k] = #{b : T*_b(M_k) >= T(M_k)}: the
+ * count is >= (not the strict > of b200bt_spa_bootstrap's tests), so under T_R, and under T_max for all-zero rows, N
+ * identical rows give count B at every step (with a strict count they would all leave at p = 0).  The host forms p_k = count[k] / B and the MCS p-values.
+ * Limits: 2 <= N <= 16384 (ELIMIT above, EINVAL below), n_boot >= 1, ld_z >= N, T as b200bt_spa_* (EINVAL for null
+ * pointers and bad strides, before the device check).  max_bytes: the [B][N] and [N][N] float64 buffers an entry reads
+ * or writes, counted with their strides, must total at most max_bytes, else ELIMIT.
+ *
+ * b200bt_boot_means (1 <= N <= 16384): out[b][k] at out + b * ld_out + k (ld_out >= N) = m*[b][k] - center[k], or m*[b][k]
+ * when center_or_null is NULL, for resamples b = 0 .. n_boot-1 (gid = boot_offset + b).  b200bt_spa_bootstrap's
+ * schedule and gather function, so m* is the very value whose maximum that entry takes.  Budget: n_boot * ld_out * 8.
+ * b200bt_autocov (1 <= N < 2^31): per row, c_t = x_t - xbar and out[k][i] = (sum_{t=0}^{T-1-i} c_t * c_{t+i}) / T for
+ * i = 0 .. K, 0 <= K < T (EINVAL otherwise): b200bt_spa_moments' gamma_i bit for bit; out: [N][K+1]; mean_or_null gets
+ * xbar.  One CTA per row, T * 8 bytes of shared memory.
+ * b200bt_mcs_pairwise: s2[i][j] (i < j, at s2 + i * N + j) += sum over this call's rows b of zeta (ascending) of
+ * (zeta_bj - zeta_bi)^2; other entries untouched.  Zero s2 before the first call; calls over consecutive resample ranges
+ * continue the ascending sum, so any split gives the same bits.  One CTA per upper (64 x 64) tile pair, 16 resamples
+ * staged per step, 4 x 4 accumulators per thread.  Budget: n_boot * ld_z * 8 + N * N * 8.
+ * b200bt_mcs_range_stats: from s2 in w over n_boot_total resamples, w becomes rho (symmetric, 0 on the diagonal) and t
+ * gets t_ij at t + i * N + j (0 on the diagonal).  Budget: 2 * N * N * 8.
+ * b200bt_mcs_range_order: the T_R elimination: order[k] = e_k (int32 [N], the last survivor last), stat[k] = T_R(M_k)
+ * (float64 [N-1]); then rho_rank[r][c] = rho[order[r]][order[c]] for c > r, 0 otherwise.  rho_rank may alias t (which it
+ * then overwrites), not rho.  One CTA keeps each live row's max and its column in shared memory (13 N bytes) and rescans
+ * only the rows whose column was just eliminated.  Budget: 2 or 3 (t not aliased) * N * N * 8.
+ * b200bt_mcs_range_boot: for this call's rows b of zeta (original model order), R_b(r) = max over c > r of
+ * |zeta_b,order[c] - zeta_b,order[r]| * rho_rank[r][c] into rmax [n_boot][N], then count[k] (uint64 [N-1]) += #{b :
+ * max over r >= k of R_b(r) >= stat[k]}: T*_R,b(M_k) = max over r >= k of R_b(r).  Calls over a split of the resamples
+ * add up to the counts of one call.  One CTA per (64-resample, 64-rank) tile; O(B N^2 / 2).  Budget: n_boot * ld_z * 8 +
+ * n_boot * N * 8 + N * N * 8.
+ * b200bt_mcs_max: the whole T_max elimination over zeta [n_boot][ld_z] (every resample in one call): order, stat (as
+ * above) and count[k] (uint64 [N-1], added to) for k = 0 .. N-2.  Per step three launches: v_i and t_i (a thread per
+ * live model, b ascending), the argmax (one CTA), and the maxima, count and next zbar (a thread per resample).
+ * Workspace: device, 16-byte aligned, b200bt_mcs_max_workspace_bytes(N, n_boot) bytes (0 outside the limits).  Budget:
+ * n_boot * ld_z * 8. */
+int b200bt_boot_means(const double* d, int64_t ld, int N, int T, uint64_t q32, int64_t n_boot, uint64_t seed,
+                      uint64_t boot_offset, const double* center_or_null, double* out, int64_t ld_out, int64_t max_bytes,
+                      b200bt_stream_t stream);
+int b200bt_autocov(const double* d, int64_t ld, int N, int T, int K, double* out, double* mean_or_null,
+                   b200bt_stream_t stream);
+int b200bt_mcs_pairwise(const double* zeta, int64_t ld_z, int N, int64_t n_boot, double* s2, int64_t max_bytes,
+                        b200bt_stream_t stream);
+int b200bt_mcs_range_stats(const double* mean, int N, int64_t n_boot_total, double* w, double* t, int64_t max_bytes,
+                           b200bt_stream_t stream);
+int b200bt_mcs_range_order(const double* t, const double* rho, int N, int32_t* order, double* stat, double* rho_rank,
+                           int64_t max_bytes, b200bt_stream_t stream);
+int b200bt_mcs_range_boot(const double* zeta, int64_t ld_z, int N, int64_t n_boot, const int32_t* order,
+                          const double* rho_rank, const double* stat, double* rmax, uint64_t* count, int64_t max_bytes,
+                          b200bt_stream_t stream);
+int64_t b200bt_mcs_max_workspace_bytes(int N, int64_t n_boot);
+int b200bt_mcs_max(const double* zeta, int64_t ld_z, int N, int64_t n_boot, const double* mean, void* workspace,
+                   int64_t workspace_bytes, int32_t* order, double* stat, uint64_t* count, int64_t max_bytes,
+                   b200bt_stream_t stream);
+
 /* ---- portfolio risk (SURVEY 8-f4) -------------------------------------------------------------------
  * Replaces the numeric core of services/portfolio_risk_service.py. */
 

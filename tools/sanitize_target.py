@@ -20,7 +20,7 @@ from ai_crypto_trader_b200.sweep import MarketData, PopulationSweep
 from oracle import indicators_ref, sim_oracle
 
 legs = sys.argv[1:] or ["sweep", "mc", "joint", "indicators", "pareto", "regime", "dca", "grid_service", "rl",
-                        "volume_profile", "market_monitor", "spa"]
+                        "volume_profile", "market_monitor", "spa", "mcs"]
 torch.cuda.set_device(0)
 
 if "sweep" in legs:
@@ -238,3 +238,21 @@ if "spa" in legs:
         assert got["reality_check"] == want["reality_check"] and np.array_equal(got["stepm"]["rejected"],
                                                                                 want["stepm"]["rejected"]), (N, T)
     print("spa ok: p-values and StepM sets equal the restatement", flush=True)
+
+if "mcs" in legs:
+    # model confidence set: staged and L2 bootstrap means, a partial 64-model tile, split resamples (T_R), the T_max
+    # step loop, copies and all-zero rows; orders and p-values checked against the exact restatement
+    sys.path.insert(0, str(Path(__file__).resolve().parents[1] / "tests"))
+    import mcs_ref
+    from ai_crypto_trader_b200.overfitting import mcs, optimal_block_length
+    rng = np.random.default_rng(7)
+    for N, T, stat, max_bytes in ((70, 90, "R", 2 * 70 * 70 * 8 + 2 * 70 * 8 * 16), (9, 800, "max", 1 << 30)):
+        x = rng.normal(0.0, 1.0, (N, T)) + np.linspace(-0.2, 0.2, N)[:, None]
+        x[1] = 0.0
+        x[2] = 0.0
+        got = mcs(torch.from_numpy(x).cuda(), statistic=stat, n_boot=40, block_len=4.0, seed=2, max_bytes=max_bytes)
+        want = mcs_ref.mcs_exact(x, 0.1, stat, 40, 4.0, 2)
+        assert np.array_equal(got["elimination_order"], want["elimination_order"]) and np.array_equal(
+            got["p_values"], want["p_values"]), (N, T, stat)
+    optimal_block_length(torch.from_numpy(x).cuda())
+    print("mcs ok: orders and p-values equal the restatement", flush=True)
